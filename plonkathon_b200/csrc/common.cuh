@@ -78,7 +78,7 @@ struct Context {
   cudaEvent_t copy_done[4] = {nullptr, nullptr, nullptr, nullptr};
   int sm_count = 132;
   std::map<int, std::unique_ptr<NttPlan>> plans;  // key: log_n * 2 + inverse
-  DevBuf scratch[8];                               // reusable temporaries
+  DevBuf scratch[10];                              // reusable temporaries
   DevBuf msm_aff[6];                               // batched-affine bucket accumulation (msm.cu)
   Comm* comm = nullptr;                            // multi-GPU: this rank's communicator (comm.cuh), or null
   DevBuf gather;                                   // receive buffer of the sharded transforms' allgather

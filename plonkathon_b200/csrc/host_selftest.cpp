@@ -6,7 +6,9 @@
 #include "msm_digits.cuh"
 #include "modinv.cuh"
 #include "msm_bucket.cuh"
+#include "msm_sort.cuh"
 #include "ntt_shard.cuh"
+#include <algorithm>
 #include <vector>
 #include <cstring>
 using namespace pb200;
@@ -135,17 +137,11 @@ int hs_curve_op(int op, const uint32_t* acc_in, const uint32_t* other, int other
   return 0;
 }
 
-// The whole bucket pipeline of msm.cu on the CPU, every thread body run in a loop: signed-digit slicing, histogram,
-// padded scan, counting-sort scatter, rounds of batched affine additions (msm_bucket.cuh), recursive bucket reduction,
-// bucket-range offset and window Horner.  points: n canonical affine points (16 words each); scalars: batch * n
-// canonical scalars; fixed_base != 0 builds the window table 2^(c w) P_i first (batch <= 4 scalar vectors share it).
-// [lo, hi): the bucket magnitudes this "rank" owns.  out: one canonical affine point (+ identity flag) per scalar
-// vector: the rank's partial sum.  Returns the number of accumulation rounds that did work, -1 on bad input.
-int hs_msm_pipeline(const uint32_t* points, uint32_t n, const uint32_t* scalars, uint32_t batch, uint32_t c,
-                    int fixed_base, uint32_t lo, uint32_t hi, uint32_t B, uint32_t g0, uint32_t* out, uint8_t* out_inf) {
-  if (!n || !batch || batch > 4 || (!fixed_base && batch != 1) || c < 1 || c > 16 || B < 2 || B > PB_AFF_BMAX) return -1;
-  if (g0 < 2 || (g0 & (g0 - 1))) return -1;
-  MsmGeom g;
+}  // extern "C"
+
+// MSM geometry of a call.  [lo, hi): the bucket magnitudes this "rank" owns; hi = 0xffffffff - log_g (log_g < 16)
+// instead selects the strided shard of rank lo out of 2^log_g.  false on bad input.
+static bool msm_geom(uint32_t n, uint32_t batch, uint32_t c, int fixed_base, uint32_t lo, uint32_t hi, MsmGeom& g) {
   g.c = c;
   g.W = (256 + c - 1) / c;
   g.half = 1u << (c - 1);
@@ -159,15 +155,163 @@ int hs_msm_pipeline(const uint32_t* points, uint32_t n, const uint32_t* scalars,
     g.own_rank = lo;
     g.lo = 0;
     g.nloc = g.half >> g.own_log;
-    if (!g.nloc || lo >= (1u << g.own_log)) return -1;
+    if (!g.nloc || lo >= (1u << g.own_log)) return false;
   } else {
     if (hi > g.half) hi = g.half;
-    if (lo >= hi) return -1;
+    if (lo >= hi) return false;
     g.lo = lo;
     g.nloc = hi - lo;
   }
   g.sets = fixed_base ? batch : g.W;
   g.nb = g.sets * g.nloc;
+  return true;
+}
+
+// k_scan_tile_sums + k_scan_tiles + k_scan_apply of msm.cu: off = exclusive prefix of the (padded) counts, counts
+// zeroed; *max_out = the largest raw count
+static void host_scan(uint32_t* cnt, uint32_t len, uint32_t pad, uint32_t* off, uint32_t* max_out) {
+  uint32_t run = 0, m = 0;
+  for (uint32_t b = 0; b < len; b++) {
+    off[b] = run;
+    run += (cnt[b] + pad) & ~pad;
+    m = std::max(m, cnt[b]);
+    cnt[b] = 0;
+  }
+  off[len] = run;
+  if (max_out) *max_out = m;
+}
+
+// The sort of msm_run_batch (msm_sort.cuh) on the CPU: every kernel's blocks one after the other, each block as a
+// loop over its phases, each phase as a loop over the block's nt threads.  Out: counts (nb raw counts + the max),
+// off (nb + 1), sorted (off[nb] + 2 positions, unused ones PB_MSM_PAD).
+static void host_msm_sort(const MsmGeom& g, const std::vector<Fr>& sc, uint32_t n, uint32_t pad, uint32_t lb,
+                          uint32_t T, uint32_t spb, uint32_t bin_nt, uint32_t chunk_nt, std::vector<uint32_t>& counts,
+                          std::vector<uint32_t>& off, std::vector<uint32_t>& sorted) {
+  const uint32_t nbins = ((g.nb - 1) >> lb) + 1;
+  const uint32_t batch = g.fixed_base ? g.batch : 1;
+  std::vector<uint32_t> bin_cnt(nbins, 0), bin_off(nbins + 1), chunk_first(nbins + 1);
+  std::vector<SortEntry> binned((size_t)n * g.W * batch);
+  counts.assign(g.nb + 1, 0);
+  off.assign(g.nb + 1, 0);
+  SortArgs a;
+  for (uint32_t k = 0; k < 4; k++) a.sb.p[k] = k < batch ? sc.data() + (size_t)k * n : nullptr;
+  a.n = n;
+  a.from_mont = 0;
+  a.g = g;
+  a.lb = lb;
+  a.nbins = nbins;
+  a.T = T;
+  a.bin_cnt = bin_cnt.data();
+  a.bin_off = bin_off.data();
+  a.binned = binned.data();
+  a.chunk_first = chunk_first.data();
+  a.counts = counts.data();
+  a.offsets = off.data();
+  a.sorted = nullptr;
+  a.spb = spb;
+  std::vector<uint32_t> sh_cnt(std::max(nbins, 1u << lb)), sh_loc(sh_cnt.size()), sh_base(sh_cnt.size()), runs;
+  std::vector<SortEntry> bin_stage_buf((size_t)spb * g.W);
+  std::vector<uint32_t> chunk_stage_buf(T);
+  // the block scan of the placement kernels: runs[t] = exclusive prefix of the threads' scan_part_sum; the total
+  auto block_scan = [&](uint32_t len, uint32_t nt) {
+    runs.assign(nt, 0);
+    uint32_t run = 0;
+    for (uint32_t t = 0; t < nt; t++) { runs[t] = run; run += scan_part_sum(sh_cnt.data(), len, t, nt); }
+    return run;
+  };
+  const uint32_t bin_blocks = (n + spb - 1) / spb;
+  // k_msm_bin_count
+  for (uint32_t k = 0; k < batch; k++)
+    for (uint32_t bx = 0; bx < bin_blocks; bx++) {
+      for (uint32_t t = 0; t < bin_nt; t++) sort_zero(sh_cnt.data(), nbins, t, bin_nt);
+      for (uint32_t t = 0; t < bin_nt; t++) bin_hist(a, bx, k, t, bin_nt, sh_cnt.data());
+      for (uint32_t t = 0; t < bin_nt; t++) bin_flush(a, t, bin_nt, sh_cnt.data());
+    }
+  host_scan(bin_cnt.data(), nbins, 0, bin_off.data(), nullptr);
+  // k_msm_bin_scatter; blocks in reverse order, so the bins' ranges are not filled in walk order
+  for (uint32_t k = batch; k-- > 0;)
+    for (uint32_t bx = bin_blocks; bx-- > 0;) {
+      for (uint32_t t = 0; t < bin_nt; t++) sort_zero(sh_cnt.data(), nbins, t, bin_nt);
+      for (uint32_t t = 0; t < bin_nt; t++) bin_hist(a, bx, k, t, bin_nt, sh_cnt.data());
+      const uint32_t total = block_scan(nbins, bin_nt);
+      for (uint32_t t = 0; t < bin_nt; t++)
+        bin_reserve(a, t, bin_nt, runs[t], sh_cnt.data(), sh_loc.data(), sh_base.data());
+      for (uint32_t t = 0; t < bin_nt; t++) bin_stage(a, bx, k, t, bin_nt, sh_cnt.data(), sh_loc.data(), bin_stage_buf.data());
+      for (uint32_t t = 0; t < bin_nt; t++)
+        bin_copy_out(a, t, bin_nt, total, sh_loc.data(), sh_base.data(), bin_stage_buf.data());
+    }
+  // k_msm_chunk_map
+  {
+    std::vector<uint32_t> sums(256);
+    for (uint32_t t = 0; t < 256; t++) sums[t] = chunk_map_sum(a, t);
+    uint32_t run = 0;
+    for (uint32_t t = 0; t < 256; t++) { const uint32_t s = sums[t]; sums[t] = run; run += s; }
+    for (uint32_t t = 0; t < 256; t++) chunk_map_write(a, t, sums[t], run);
+  }
+  // the chunk kernels, with a grid of `grid` blocks walking the chunks grid-stride
+  const uint32_t grid = 3;
+  SortChunk ch;
+  for (uint32_t bx = 0; bx < grid; bx++)
+    for (uint32_t c = bx; chunk_locate(a, c, ch); c += grid) {
+      for (uint32_t t = 0; t < chunk_nt; t++) sort_zero(sh_cnt.data(), ch.nkeys, t, chunk_nt);
+      for (uint32_t t = 0; t < chunk_nt; t++) chunk_hist(a, ch, t, chunk_nt, sh_cnt.data());
+      for (uint32_t t = 0; t < chunk_nt; t++) chunk_flush(a, ch, t, chunk_nt, sh_cnt.data());
+    }
+  host_scan(counts.data(), g.nb, pad, off.data(), &counts[g.nb]);
+  sorted.assign(off[g.nb] + 2, PB_MSM_PAD);
+  a.sorted = sorted.data();
+  for (uint32_t bx = grid; bx-- > 0;)
+    for (uint32_t c = bx; chunk_locate(a, c, ch); c += grid) {
+      for (uint32_t t = 0; t < chunk_nt; t++) sort_zero(sh_cnt.data(), ch.nkeys, t, chunk_nt);
+      for (uint32_t t = 0; t < chunk_nt; t++) chunk_hist(a, ch, t, chunk_nt, sh_cnt.data());
+      const uint32_t total = block_scan(ch.nkeys, chunk_nt);
+      for (uint32_t t = 0; t < chunk_nt; t++)
+        chunk_reserve(a, ch, t, chunk_nt, runs[t], sh_cnt.data(), sh_loc.data(), sh_base.data());
+      for (uint32_t t = 0; t < chunk_nt; t++) chunk_stage(a, ch, t, chunk_nt, sh_cnt.data(), sh_loc.data(), chunk_stage_buf.data());
+      for (uint32_t t = 0; t < chunk_nt; t++)
+        chunk_copy_out(a, ch, t, chunk_nt, sh_loc.data(), sh_base.data(), chunk_stage_buf.data());
+      if (total != ch.hi - ch.lo) abort();
+    }
+}
+
+extern "C" {
+// The sort alone: scalars: batch * n canonical scalars; geometry as hs_msm_pipeline; lb: key bits per bin
+// (0xffffffff: what msm.cu picks), T: entries per chunk, spb: scalars per bin-kernel block (0: what msm.cu picks),
+// bin_nt / chunk_nt: threads per block of the bin / chunk kernels.  Writes counts (nb + 1: raw counts, then the
+// max), off (nb + 1) and sorted[0 .. off[nb]) (at most cap words).  Returns nb, -1 on bad input.
+int hs_msm_sort(const uint32_t* scalars, uint32_t n, uint32_t batch, uint32_t c, int fixed_base, uint32_t lo,
+                uint32_t hi, uint32_t pad, uint32_t lb, uint32_t T, uint32_t spb, uint32_t bin_nt, uint32_t chunk_nt,
+                uint32_t* counts_out, uint32_t* off_out, uint32_t* sorted_out, uint32_t cap) {
+  if (!n || !batch || batch > 4 || (!fixed_base && batch != 1) || c < 1 || c > 16 || !T || !bin_nt || !chunk_nt)
+    return -1;
+  MsmGeom g;
+  if (!msm_geom(n, batch, c, fixed_base, lo, hi, g)) return -1;
+  if (lb == 0xffffffffu) lb = sort_default_lb(g.nb);
+  if (((g.nb - 1) >> lb) >= PB_SORT_MAX_BINS || (1u << lb) > PB_SORT_MAX_BIN_KEYS) return -1;
+  if (!spb) spb = PB_SORT_BIN_STAGE / g.W;
+  std::vector<Fr> sc((size_t)batch * n);
+  for (size_t i = 0; i < sc.size(); i++) sc[i] = ld<Fr>(scalars + 8 * i);
+  std::vector<uint32_t> counts, off, sorted;
+  host_msm_sort(g, sc, n, pad ? 1 : 0, lb, T, spb, bin_nt, chunk_nt, counts, off, sorted);
+  if (off[g.nb] > cap) return -1;
+  memcpy(counts_out, counts.data(), counts.size() * 4);
+  memcpy(off_out, off.data(), off.size() * 4);
+  memcpy(sorted_out, sorted.data(), (size_t)off[g.nb] * 4);
+  return (int)g.nb;
+}
+
+// The whole bucket pipeline of msm.cu on the CPU, every thread body run in a loop: signed-digit slicing, the
+// two-level counting sort, rounds of batched affine additions (msm_bucket.cuh), recursive bucket reduction,
+// bucket-range offset and window Horner.  points: n canonical affine points (16 words each); scalars: batch * n
+// canonical scalars; fixed_base != 0 builds the window table 2^(c w) P_i first (batch <= 4 scalar vectors share it).
+// [lo, hi): the bucket magnitudes this "rank" owns.  out: one canonical affine point (+ identity flag) per scalar
+// vector: the rank's partial sum.  Returns the number of accumulation rounds that did work, -1 on bad input.
+int hs_msm_pipeline(const uint32_t* points, uint32_t n, const uint32_t* scalars, uint32_t batch, uint32_t c,
+                    int fixed_base, uint32_t lo, uint32_t hi, uint32_t B, uint32_t g0, uint32_t* out, uint8_t* out_inf) {
+  if (!n || !batch || batch > 4 || (!fixed_base && batch != 1) || c < 1 || c > 16 || B < 2 || B > PB_AFF_BMAX) return -1;
+  if (g0 < 2 || (g0 & (g0 - 1))) return -1;
+  MsmGeom g;
+  if (!msm_geom(n, batch, c, fixed_base, lo, hi, g)) return -1;
   // point table
   std::vector<G1Affine> tab(fixed_base ? (size_t)g.W * n : n);
   for (uint32_t i = 0; i < n; i++) {
@@ -184,33 +328,11 @@ int hs_msm_pipeline(const uint32_t* points, uint32_t n, const uint32_t* scalars,
       }
   std::vector<Fr> sc((size_t)batch * n);
   for (size_t i = 0; i < sc.size(); i++) sc[i] = ld<Fr>(scalars + 8 * i);
-  // histogram, padded scan, scatter
-  std::vector<uint32_t> counts(g.nb + 1, 0), off(g.nb + 1, 0), cursors(g.nb, 0);
-  for (uint32_t k = 0; k < batch; k++)
-    for (uint32_t i = 0; i < n; i++) {
-      DigitWalk dw(sc.data() + (size_t)k * n, i, 0);
-      for (uint32_t w = 0; w < g.W; w++) {
-        uint32_t neg, d = dw.next(w, g, neg);
-        if (!d) continue;
-        uint32_t key = msm_bucket_key(g, k, w, d);
-        if (key != 0xffffffffu) counts[key]++;
-      }
-    }
-  uint32_t maxc = 0;
-  for (uint32_t b = 0; b < g.nb; b++) { off[b + 1] = off[b] + ((counts[b] + 1) & ~1u); maxc = std::max(maxc, counts[b]); }
-  counts[g.nb] = maxc;
-  std::vector<uint32_t> sorted(off[g.nb] + 2, PB_MSM_PAD);
-  for (uint32_t k = 0; k < batch; k++)
-    for (uint32_t i = 0; i < n; i++) {
-      DigitWalk dw(sc.data() + (size_t)k * n, i, 0);
-      for (uint32_t w = 0; w < g.W; w++) {
-        uint32_t neg, d = dw.next(w, g, neg);
-        if (!d) continue;
-        uint32_t key = msm_bucket_key(g, k, w, d);
-        if (key == 0xffffffffu) continue;
-        sorted[off[key] + cursors[key]++] = (uint32_t)((uint64_t)w * g.point_stride + i) | (neg << 31);
-      }
-    }
+  // the two-level counting sort of msm.cu, padded, with the launch's bin width, chunk size and block sizes
+  std::vector<uint32_t> counts, off, sorted;
+  host_msm_sort(g, sc, n, 1, sort_default_lb(g.nb), PB_SORT_CHUNK, PB_SORT_BIN_STAGE / g.W, PB_SORT_BIN_THREADS,
+                PB_SORT_CHUNK_THREADS, counts, off, sorted);
+  const uint32_t maxc = counts[g.nb];
   // accumulation rounds
   const uint64_t positions = (uint64_t)n * g.W * batch + g.nb, s_bound = positions / 2;
   std::vector<G1Affine> pts(s_bound + 1);

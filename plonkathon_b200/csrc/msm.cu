@@ -3,10 +3,12 @@
 // Replaces curve.py:38-111 (`ec_lincomb` -> `lincomb` -> `multisubset`) and the MSM half of
 // setup.py:66-72 (`Setup.commit`).  The result sum_i s_i * P_i is algorithm-independent, so the
 // reference's bit-sliced power-set method is replaced by:
-//   1. signed-digit window slicing of every scalar (c-bit windows, digits in [-2^(c-1), 2^(c-1)]),
-//      with a global histogram of bucket loads                                  (k_msm_histogram)
-//   2. exclusive scan of the histogram                                           (k_scan_*)
-//   3. counting-sort scatter of (point index, sign) by bucket                    (k_msm_scatter)
+//   1. signed-digit window slicing of every scalar (c-bit windows, digits in [-2^(c-1), 2^(c-1)]), with
+//      per-block shared-memory histograms over coarse bins of buckets, and their scan  (k_msm_bin_count, k_scan_*)
+//   2. scatter of (bucket, point index | sign) into the bins                     (k_msm_bin_scatter)
+//   3. counting sort of every bin by bucket, in chunks: shared-memory histograms added into the bucket counts,
+//      exclusive scan, placement           (k_msm_chunk_map, k_msm_chunk_count, k_scan_*, k_msm_chunk_place)
+//      No step does a global atomic per entry or stores into a write front larger than L2 (msm_sort.cuh).
 //   4. load-balanced bucket accumulation over fixed segments of the sorted entries: XYZZ accumulator += affine
 //      point (8M+2S, no inversion), SIMT-uniform loop                            (k_msm_seg_accumulate)
 //      + stitching of buckets that cross a segment boundary, block trees for heavy ones, piece-wise for buckets of
@@ -32,6 +34,7 @@
 #include "comm.cuh"
 #include "msm_bucket.cuh"
 #include "msm_digits.cuh"
+#include "msm_sort.cuh"
 
 namespace pb200 {
 
@@ -47,29 +50,10 @@ __device__ __forceinline__ G1Affine ld_affine(const G1Affine* p) {
   return r;
 }
 
-// counts[bucket]++ for every non-zero digit whose bucket this launch owns
-__global__ void k_msm_histogram(ScalarBatch sb, uint64_t n, int from_mont, MsmGeom g, uint32_t* counts) {
-  uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const uint32_t k = blockIdx.y;
-  DigitWalk dw(sb.p[k], i, from_mont);
-  for (uint32_t w = 0; w < g.W; w++) {
-    uint32_t neg, d = dw.next(w, g, neg);
-    if (!d) continue;
-    const uint32_t key = msm_bucket_key(g, k, w, d);
-    if (key != 0xffffffffu) atomicAdd(&counts[key], 1u);
-  }
-}
-
-// ---- exclusive scan of the bucket histogram (3 small kernels) ---------------------------------
-// offsets[0..nb] from counts[0..nb-1]; counts are zeroed on the way out (reused as scatter cursors, which the
-// scatter leaves equal to the counts again).  pad != 0 rounds every count up to even, so all offsets are even
-// (the slot layout of msm_bucket.cuh).
-#define PB_SCAN_TILE 2048  // entries per block (256 threads x 8)
-
-__device__ __forceinline__ uint32_t block_exclusive_scan_256(uint32_t v, uint32_t* sh, uint32_t* total) {
-  // 256 threads; returns exclusive prefix of v across the block, *total = block sum
-  uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+// exclusive prefix of v across the block (a multiple of 32 threads, at most 1024), *total = block sum;
+// sh: one word per warp
+__device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t v, uint32_t* sh, uint32_t* total) {
+  const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
   uint32_t x = v;
   for (int d = 1; d < 32; d <<= 1) {
     uint32_t y = __shfl_up_sync(0xffffffffu, x, d);
@@ -78,19 +62,91 @@ __device__ __forceinline__ uint32_t block_exclusive_scan_256(uint32_t v, uint32_
   if (lane == 31) sh[wid] = x;
   __syncthreads();
   if (wid == 0) {
-    uint32_t w = lane < 8 ? sh[lane] : 0;
-    for (int d = 1; d < 8; d <<= 1) {
+    uint32_t w = lane < nw ? sh[lane] : 0;
+    for (int d = 1; d < 32; d <<= 1) {
       uint32_t y = __shfl_up_sync(0xffffffffu, w, d);
       if ((int)lane >= d) w += y;
     }
-    if (lane < 8) sh[lane] = w;  // inclusive warp totals
+    if (lane < nw) sh[lane] = w;  // inclusive warp totals
   }
   __syncthreads();
   uint32_t base = wid ? sh[wid - 1] : 0;
-  *total = sh[7];
+  *total = sh[nw - 1];
   __syncthreads();
   return base + x - v;
 }
+
+// ---- two-level counting sort of the bucket entries (msm_sort.cuh holds the thread bodies) -----------------------
+__global__ void __launch_bounds__(PB_SORT_BIN_THREADS) k_msm_bin_count(SortArgs a) {
+  __shared__ uint32_t sh_cnt[PB_SORT_MAX_BINS];
+  const uint32_t t = threadIdx.x, nt = blockDim.x;
+  sort_zero(sh_cnt, a.nbins, t, nt);
+  __syncthreads();
+  bin_hist(a, blockIdx.x, blockIdx.y, t, nt, sh_cnt);
+  __syncthreads();
+  bin_flush(a, t, nt, sh_cnt);
+}
+
+// dynamic shared memory: the stage, PB_SORT_BIN_STAGE entries
+__global__ void __launch_bounds__(PB_SORT_BIN_THREADS) k_msm_bin_scatter(SortArgs a) {
+  __shared__ uint32_t sh_cnt[PB_SORT_MAX_BINS], sh_loc[PB_SORT_MAX_BINS], sh_base[PB_SORT_MAX_BINS], sh_scan[32];
+  extern __shared__ SortEntry stage[];
+  const uint32_t t = threadIdx.x, nt = blockDim.x;
+  sort_zero(sh_cnt, a.nbins, t, nt);
+  __syncthreads();
+  bin_hist(a, blockIdx.x, blockIdx.y, t, nt, sh_cnt);
+  __syncthreads();
+  uint32_t total;
+  const uint32_t run = block_exclusive_scan(scan_part_sum(sh_cnt, a.nbins, t, nt), sh_scan, &total);
+  bin_reserve(a, t, nt, run, sh_cnt, sh_loc, sh_base);
+  __syncthreads();
+  bin_stage(a, blockIdx.x, blockIdx.y, t, nt, sh_cnt, sh_loc, stage);
+  __syncthreads();
+  bin_copy_out(a, t, nt, total, sh_loc, sh_base, stage);
+}
+
+__global__ void __launch_bounds__(PB_SORT_CHUNK_THREADS) k_msm_chunk_count(SortArgs a) {
+  __shared__ uint32_t sh_cnt[PB_SORT_MAX_BIN_KEYS];
+  const uint32_t t = threadIdx.x, nt = blockDim.x;
+  SortChunk ch;
+  for (uint32_t c = blockIdx.x; chunk_locate(a, c, ch); c += gridDim.x) {
+    sort_zero(sh_cnt, ch.nkeys, t, nt);
+    __syncthreads();
+    chunk_hist(a, ch, t, nt, sh_cnt);
+    __syncthreads();
+    chunk_flush(a, ch, t, nt, sh_cnt);
+    __syncthreads();
+  }
+}
+
+// dynamic shared memory: the stage, PB_SORT_CHUNK values
+__global__ void __launch_bounds__(PB_SORT_CHUNK_THREADS) k_msm_chunk_place(SortArgs a) {
+  __shared__ uint32_t sh_cnt[PB_SORT_MAX_BIN_KEYS], sh_loc[PB_SORT_MAX_BIN_KEYS], sh_base[PB_SORT_MAX_BIN_KEYS],
+      sh_scan[32];
+  extern __shared__ uint32_t stage_vals[];
+  const uint32_t t = threadIdx.x, nt = blockDim.x;
+  SortChunk ch;
+  for (uint32_t c = blockIdx.x; chunk_locate(a, c, ch); c += gridDim.x) {
+    sort_zero(sh_cnt, ch.nkeys, t, nt);
+    __syncthreads();
+    chunk_hist(a, ch, t, nt, sh_cnt);
+    __syncthreads();
+    uint32_t total;
+    const uint32_t run = block_exclusive_scan(scan_part_sum(sh_cnt, ch.nkeys, t, nt), sh_scan, &total);
+    chunk_reserve(a, ch, t, nt, run, sh_cnt, sh_loc, sh_base);
+    __syncthreads();
+    chunk_stage(a, ch, t, nt, sh_cnt, sh_loc, stage_vals);
+    __syncthreads();
+    chunk_copy_out(a, ch, t, nt, sh_loc, sh_base, stage_vals);
+    __syncthreads();
+  }
+}
+
+// ---- exclusive scan of a count array (3 small kernels): the bins and the buckets of the sort ---------------------
+// offsets[0..nb] from counts[0..nb-1]; counts are zeroed on the way out (reused as cursors by the next placement
+// kernel, which leaves them equal to the counts again).  pad != 0 rounds every count up to even, so all offsets are
+// even (the slot layout of msm_bucket.cuh).
+#define PB_SCAN_TILE 2048  // entries per block (256 threads x 8)
 
 __global__ void __launch_bounds__(256) k_scan_tile_sums(const uint32_t* counts, uint32_t nb, uint32_t pad,
                                                         uint32_t* tile_sums, uint32_t* max_out) {
@@ -104,7 +160,7 @@ __global__ void __launch_bounds__(256) k_scan_tile_sums(const uint32_t* counts, 
       s += (c + pad) & ~pad;
     }
   uint32_t total;
-  block_exclusive_scan_256(s, sh, &total);
+  block_exclusive_scan(s, sh, &total);
   if (threadIdx.x == 0) tile_sums[blockIdx.x] = total;
   if (max_out) {  // largest bucket of the launch (decides how many accumulation rounds do work)
     for (int d = 16; d > 0; d >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, d));
@@ -120,7 +176,7 @@ __global__ void __launch_bounds__(256) k_scan_tiles(uint32_t* tile_sums, uint32_
   uint32_t s = 0;
   for (uint32_t i = lo; i < hi; i++) s += tile_sums[i];
   uint32_t total;
-  uint32_t run = block_exclusive_scan_256(s, sh, &total);
+  uint32_t run = block_exclusive_scan(s, sh, &total);
   for (uint32_t i = lo; i < hi; i++) {
     uint32_t c = tile_sums[i];
     tile_sums[i] = run;
@@ -137,43 +193,19 @@ __global__ void __launch_bounds__(256) k_scan_apply(uint32_t* counts, uint32_t n
   uint32_t s = 0;
   for (int k = 0; k < 8; k++) { c[k] = base + k < nb ? (counts[base + k] + pad) & ~pad : 0; s += c[k]; }
   uint32_t total;
-  uint32_t run = tile_sums[blockIdx.x] + block_exclusive_scan_256(s, sh, &total);
+  uint32_t run = tile_sums[blockIdx.x] + block_exclusive_scan(s, sh, &total);
   for (int k = 0; k < 8; k++) {
     if (base + k < nb) { offsets[base + k] = run; counts[base + k] = 0; }
     run += c[k];
   }
 }
 
-// sorted[offsets[key] + cursor++] = point index | sign << 31
-// A scalar's windows are handled eight at a time: all their cursor atomics are in flight together before the
-// first returned position is needed (the kernel is bound by the latency of those atomics, not by their number).
-__global__ void k_msm_scatter(ScalarBatch sb, uint64_t n, int from_mont, MsmGeom g, const uint32_t* offsets,
-                              uint32_t* cursors, uint32_t* sorted) {
-  uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const uint32_t k = blockIdx.y;
-  DigitWalk dw(sb.p[k], i, from_mont);
-  for (uint32_t w0 = 0; w0 < g.W; w0 += 8) {
-    uint32_t key[8], val[8], pos[8];
-#pragma unroll
-    for (int j = 0; j < 8; j++) {
-      key[j] = 0xffffffffu;
-      const uint32_t w = w0 + j;
-      if (w < g.W) {
-        uint32_t neg, d = dw.next(w, g, neg);
-        if (d) {
-          key[j] = msm_bucket_key(g, k, w, d);
-          val[j] = (uint32_t)((uint64_t)w * g.point_stride + i) | (neg << 31);
-        }
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < 8; j++)
-      if (key[j] != 0xffffffffu) pos[j] = __ldg(offsets + key[j]) + atomicAdd(&cursors[key[j]], 1u);
-#pragma unroll
-    for (int j = 0; j < 8; j++)
-      if (key[j] != 0xffffffffu) sorted[pos[j]] = val[j];
-  }
+// one block: the first chunk of every bin (at most 256 x 8 = PB_SORT_MAX_BINS bins)
+__global__ void __launch_bounds__(256) k_msm_chunk_map(SortArgs a) {
+  __shared__ uint32_t sh[8];
+  uint32_t total;
+  const uint32_t run = block_exclusive_scan(chunk_map_sum(a, threadIdx.x), sh, &total);
+  chunk_map_write(a, threadIdx.x, run, total);
 }
 
 // ---- batched-affine bucket accumulation (msm_bucket.cuh holds the thread bodies) -----------------------------
@@ -639,19 +671,59 @@ void msm_run_batch(Context* ctx, const G1Affine* points, uint64_t n, const Fr* c
   ctx->msm_aff[1].ensure((size_t)8192 * 4);
   uint32_t* tile_sums = ctx->msm_aff[1].as<uint32_t>();
 
+  // two-level sort (msm_sort.cuh): at most PB_SORT_MAX_BINS bins of 2^lb consecutive bucket keys
+  const uint32_t lb = sort_default_lb(g.nb);
+  PB_CHECK((1u << lb) <= PB_SORT_MAX_BIN_KEYS, "too many buckets for the sort");
+  DevBuf& binned = ctx->scratch[8];
+  DevBuf& bin_tab = ctx->scratch[9];
+  binned.ensure(entries * sizeof(SortEntry));
+  bin_tab.ensure((size_t)3 * (PB_SORT_MAX_BINS + 1) * 4);
+  SortArgs sa;
+  sa.sb = sb;
+  sa.n = n;
+  sa.from_mont = scalars_mont ? 1 : 0;
+  sa.g = g;
+  sa.lb = lb;
+  sa.nbins = ((g.nb - 1) >> lb) + 1;
+  sa.T = PB_SORT_CHUNK;
+  uint32_t* bin_cnt = bin_tab.as<uint32_t>();
+  uint32_t* bin_off = bin_cnt + PB_SORT_MAX_BINS + 1;
+  sa.bin_cnt = bin_cnt;
+  sa.bin_off = bin_off;
+  sa.binned = binned.as<SortEntry>();
+  sa.chunk_first = bin_off + PB_SORT_MAX_BINS + 1;
+  sa.counts = counts.as<uint32_t>();
+  sa.offsets = offsets.as<uint32_t>();
+  sa.sorted = sorted.as<uint32_t>();
+  sa.spb = PB_SORT_BIN_STAGE / g.W;
+  const dim3 bin_grid((unsigned)((n + sa.spb - 1) / sa.spb), batch);
+  // the chunk kernels walk the chunks grid-stride: (entries / T + bins) is a bound, the real count is on the device
+  const uint64_t chunk_bound = entries / PB_SORT_CHUNK + sa.nbins;
+  const uint32_t count_grid = (uint32_t)std::min<uint64_t>((uint64_t)ctx->sm_count * 4, chunk_bound);
+  const uint32_t place_grid = (uint32_t)std::min<uint64_t>((uint64_t)ctx->sm_count * 2, chunk_bound);
+  const size_t bin_stage_bytes = PB_SORT_BIN_STAGE * sizeof(SortEntry), chunk_stage_bytes = PB_SORT_CHUNK * 4;
+  // (a per-device setting: set on every call, as contexts of several devices may share the process)
+  PB_CUDA(cudaFuncSetAttribute(k_msm_bin_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bin_stage_bytes));
+  PB_CUDA(cudaFuncSetAttribute(k_msm_chunk_place, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)chunk_stage_bytes));
+
   cudaStream_t st = ctx->stream;
   ctx->time_begin(2);
   PB_CUDA(cudaMemsetAsync(counts.p, 0, (size_t)g.nb * 4 + 16, st));
+  PB_CUDA(cudaMemsetAsync(bin_cnt, 0, (size_t)sa.nbins * 4, st));
   if (pad) PB_CUDA(cudaMemsetAsync(sorted.p, 0xff, positions * 4, st));
-  unsigned blocks = (unsigned)((n + 127) / 128);
-  k_msm_histogram<<<dim3(blocks, batch), 128, 0, st>>>(sb, n, scalars_mont ? 1 : 0, g, counts.as<uint32_t>());
+  k_msm_bin_count<<<bin_grid, PB_SORT_BIN_THREADS, 0, st>>>(sa);
+  k_scan_tile_sums<<<1, 256, 0, st>>>(bin_cnt, sa.nbins, 0, tile_sums, nullptr);
+  k_scan_tiles<<<1, 256, 0, st>>>(tile_sums, 1, bin_off + sa.nbins);
+  k_scan_apply<<<1, 256, 0, st>>>(bin_cnt, sa.nbins, 0, tile_sums, bin_off);
+  k_msm_bin_scatter<<<bin_grid, PB_SORT_BIN_THREADS, bin_stage_bytes, st>>>(sa);
+  k_msm_chunk_map<<<1, 256, 0, st>>>(sa);
+  k_msm_chunk_count<<<count_grid, PB_SORT_CHUNK_THREADS, 0, st>>>(sa);
   k_scan_tile_sums<<<n_tiles, 256, 0, st>>>(counts.as<uint32_t>(), g.nb, pad, tile_sums, max_cnt);
   k_scan_tiles<<<1, 256, 0, st>>>(tile_sums, n_tiles, offsets.as<uint32_t>() + g.nb);
   k_scan_apply<<<n_tiles, 256, 0, st>>>(counts.as<uint32_t>(), g.nb, pad, tile_sums, offsets.as<uint32_t>());
-  k_msm_scatter<<<dim3(blocks, batch), 128, 0, st>>>(sb, n, scalars_mont ? 1 : 0, g, offsets.as<uint32_t>(),
-                                                     counts.as<uint32_t>(), sorted.as<uint32_t>());
+  k_msm_chunk_place<<<place_grid, PB_SORT_CHUNK_THREADS, chunk_stage_bytes, st>>>(sa);
   ctx->time_end(2);
-  ctx->launches += 5;
+  ctx->launches += 11;
 
   ReduceArgs ra;
   ra.pts = nullptr; ra.off = offsets.as<uint32_t>(); ra.cnt = counts.as<uint32_t>(); ra.xb = nullptr;
