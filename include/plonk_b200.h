@@ -132,6 +132,13 @@ int pb200_srs_commit_coeffs_host(pb200_ctx* ctx, pb200_srs* srs, const uint8_t* 
  * Converts them to coefficients and to a cached 4n coset extension in HBM. */
 int pb200_prover_create(pb200_ctx* ctx, pb200_srs* srs, unsigned log_n, const uint8_t* const* h_pk,
                         pb200_prover** out);
+/* Custom gates: the gate constraint gains  sum_k Q_k * a^i_k * b^j_k * c^l_k.  n_custom <= 4 terms; h_exps = 3 bytes
+ * (i, j, l) per term, total degree 2 or 3, never (1, 1, 0) (QM's term), no triple twice; h_custom = n_custom pointers
+ * to the selector columns Q_k (2^log_n Lagrange values, canonical).  The proof keeps its 768-byte form; the
+ * verification key gains one commitment per term.  n_custom = 0 is pb200_prover_create. */
+int pb200_prover_create_custom(pb200_ctx* ctx, pb200_srs* srs, unsigned log_n, const uint8_t* const* h_pk,
+                               unsigned n_custom, const uint8_t* h_exps, const uint8_t* const* h_custom,
+                               pb200_prover** out);
 void pb200_prover_destroy(pb200_prover* p);
 /* prover.py:51-84  prove(witness): h_A/h_B/h_C = wire values per row (prover.py:97-103), h_public = the
  * public input values in order (prover.py:57-62; the library negates them).  Writes the canonical 768-byte
@@ -183,6 +190,10 @@ int pb200_srs_commit_coeffs_sharded(pb200_ctx* ctx, pb200_srs* srs, const void* 
  * inputs and gets the same 768 bytes.  A failing check (the reference's asserts) fails on every rank alike. */
 int pb200_prover_create_sharded(pb200_ctx* ctx, pb200_srs* srs, unsigned log_n, const uint8_t* const* h_pk,
                                 pb200_prover** out);
+/* pb200_prover_create_custom for one proof across the ranks */
+int pb200_prover_create_custom_sharded(pb200_ctx* ctx, pb200_srs* srs, unsigned log_n, const uint8_t* const* h_pk,
+                                       unsigned n_custom, const uint8_t* h_exps, const uint8_t* const* h_custom,
+                                       pb200_prover** out);
 /* Operator-level shards with a caller-side join (tests, other transports): the partial sum over the SRS powers
  * [first, first+count) and the bucket magnitudes [bucket_lo, bucket_hi) of pb200_srs_bucket_count's range, as one
  * XYZZ point (128 bytes, Montgomery limbs); pb200_g1_combine_partials_host adds such partials. */

@@ -71,6 +71,8 @@ def _load():
         "pb200_srs_commit_coeffs_host": (I, [V, V, V, U64, V, P(I)]),
         "pb200_srs_commit_coeffs": (I, [V, V, V, U64, I, V, P(I)]),
         "pb200_prover_create": (I, [V, V, U, V, P(V)]),
+        "pb200_prover_create_custom": (I, [V, V, U, V, U, V, V, P(V)]),
+        "pb200_prover_create_custom_sharded": (I, [V, V, U, V, U, V, V, P(V)]),
         "pb200_prover_destroy": (None, [V]),
         "pb200_prover_prove": (I, [V, V, V, V, V, U64, V]),
         "pb200_prover_prove_device": (I, [V, V, V, V, V, U64, V]),

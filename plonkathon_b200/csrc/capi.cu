@@ -40,7 +40,8 @@ void msm_run(Context* ctx, const G1Affine* points, uint64_t n, const Fr* scalars
              bool fixed_base, uint64_t point_stride, uint8_t* out_xy, int* is_identity);
 void affine_to_mont(Context* ctx, const G1Affine* in, G1Affine* out, uint64_t n);
 // prover.cu
-Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h_pk, bool sharded);
+Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h_pk, int n_custom,
+                      const uint8_t* h_exps, const uint8_t* const* h_custom, bool sharded);
 void prover_destroy(Prover* p);
 void prover_prove(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t* hC, const uint8_t* h_public,
                   uint64_t n_public, uint8_t* out768, bool wires_on_device);
@@ -418,14 +419,26 @@ int pb200_srs_commit_coeffs(pb200_ctx* ctx, pb200_srs* srs, const void* d_coeffs
 
 int pb200_prover_create(pb200_ctx* ctx, pb200_srs* srs, unsigned log_n, const uint8_t* const* h_pk,
                         pb200_prover** out) {
-  PB_API_BEGIN PB_ON_CTX(C(ctx));
-  *out = reinterpret_cast<pb200_prover*>(prover_create(C(ctx), reinterpret_cast<Srs*>(srs), (int)log_n, h_pk, false));
-  PB_API_END
+  return pb200_prover_create_custom(ctx, srs, log_n, h_pk, 0, nullptr, nullptr, out);
 }
 int pb200_prover_create_sharded(pb200_ctx* ctx, pb200_srs* srs, unsigned log_n, const uint8_t* const* h_pk,
                                 pb200_prover** out) {
+  return pb200_prover_create_custom_sharded(ctx, srs, log_n, h_pk, 0, nullptr, nullptr, out);
+}
+int pb200_prover_create_custom(pb200_ctx* ctx, pb200_srs* srs, unsigned log_n, const uint8_t* const* h_pk,
+                               unsigned n_custom, const uint8_t* h_exps, const uint8_t* const* h_custom,
+                               pb200_prover** out) {
   PB_API_BEGIN PB_ON_CTX(C(ctx));
-  *out = reinterpret_cast<pb200_prover*>(prover_create(C(ctx), reinterpret_cast<Srs*>(srs), (int)log_n, h_pk, true));
+  *out = reinterpret_cast<pb200_prover*>(prover_create(C(ctx), reinterpret_cast<Srs*>(srs), (int)log_n, h_pk,
+                                                       (int)n_custom, h_exps, h_custom, false));
+  PB_API_END
+}
+int pb200_prover_create_custom_sharded(pb200_ctx* ctx, pb200_srs* srs, unsigned log_n, const uint8_t* const* h_pk,
+                                       unsigned n_custom, const uint8_t* h_exps, const uint8_t* const* h_custom,
+                                       pb200_prover** out) {
+  PB_API_BEGIN PB_ON_CTX(C(ctx));
+  *out = reinterpret_cast<pb200_prover*>(prover_create(C(ctx), reinterpret_cast<Srs*>(srs), (int)log_n, h_pk,
+                                                       (int)n_custom, h_exps, h_custom, true));
   PB_API_END
 }
 void pb200_prover_destroy(pb200_prover* p) { prover_destroy(reinterpret_cast<Prover*>(p)); }

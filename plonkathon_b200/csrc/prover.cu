@@ -117,9 +117,9 @@ __global__ void k_count_noncanonical(const Fr* v, uint64_t n, uint32_t* bad) {
   if (!lt) atomicAdd(bad, 1u);
 }
 
-// prover.py:108-116: A*QL + B*QR + A*B*QM + C*QO + PI + QC == 0 on every row
+// prover.py:108-116: A*QL + B*QR + A*B*QM + C*QO + PI + QC (+ sum_k Q_k m_k(A, B, C)) == 0 on every row
 __global__ void k_gate_check(const Fr* A, const Fr* B, const Fr* C, const Fr* QL, const Fr* QR, const Fr* QM,
-                             const Fr* QO, const Fr* QC, const Fr* PI, uint64_t n, uint32_t* bad) {
+                             const Fr* QO, const Fr* QC, const Fr* PI, CustomTerms ct, uint64_t n, uint32_t* bad) {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   Fr a = ldg_fr(A + i), b = ldg_fr(B + i), c = ldg_fr(C + i);
@@ -128,6 +128,7 @@ __global__ void k_gate_check(const Fr* A, const Fr* B, const Fr* C, const Fr* QL
   s = fp_add(s, fp_mul(fp_mul(a, b), ldg_fr(QM + i)));
   s = fp_add(s, fp_mul(c, ldg_fr(QO + i)));
   s = fp_add(s, fp_add(ldg_fr(PI + i), ldg_fr(QC + i)));
+  s = custom_gate_sum(ct, i, a, b, c, s);
   if (!s.is_zero()) atomicAdd(bad, 1u);
 }
 
@@ -359,6 +360,7 @@ struct QuotientArgs {
   int pi_cnt;
   const Fr* pi_basis[8];
   Fr pi_coef[8];
+  CustomTerms custom;                                  // extended custom selectors (this rank's slice)
 };
 __global__ void __launch_bounds__(128) k_quotient(QuotientArgs q, Fr* T) {
   uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -376,6 +378,7 @@ __global__ void __launch_bounds__(128) k_quotient(QuotientArgs q, Fr* T) {
     pi = ldg_fr(q.PI + j);
   }
   gate = fp_add(gate, fp_add(pi, ldg_fr(q.QC + j)));
+  gate = custom_gate_sum(q.custom, j, a, b, c, gate);
   Fr ag = fp_add(a, q.gamma), bg = fp_add(b, q.gamma), cg = fp_add(c, q.gamma);
   Fr bx = fp_mul(q.beta, ldg_fr(q.X + j));
   Fr bx2 = fp_dbl(bx), bx3 = fp_add(bx2, bx);
@@ -412,7 +415,7 @@ __global__ void __launch_bounds__(128) k_horner_strided(EvalArgs a, Fr* H) {
 
 // ---- coefficient-space linear combination: out[k] = sum_i w[i] * vec[i][k] (+ c0 at k == 0) -----------------
 // indices [first, first + n) of the result (a slab of a sharded round 5; first = 0, n = everything on one device)
-struct LinCombArgs { const Fr* vec[16]; Fr w[16]; Fr c0; int count; uint64_t n, first; };
+struct LinCombArgs { const Fr* vec[20]; Fr w[20]; Fr c0; int count; uint64_t n, first; };
 __global__ void __launch_bounds__(128) k_lincomb(LinCombArgs a, Fr* out) {
   uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= a.n) return;
@@ -456,9 +459,31 @@ static void upload_mont(Context* ctx, DevBuf& dst, const uint8_t* h, uint64_t n)
 
 Comm* ctx_comm(Context* ctx);
 
-// h_pk: 8 vectors (QM QL QR QO QC S1 S2 S3), each n x 32 bytes canonical (compiler/program.py:10-30).
+// Custom term exponents (i, j, l) -> the wires of the monomial.  Degree 1 duplicates QL / QR / QO, degree 4 would need
+// a fourth quotient piece, (1, 1, 0) is QM's term, and a repeated triple is one term split in two.
+static void set_custom_terms(Prover* P, int n_custom, const uint8_t* h_exps) {
+  PB_CHECK(n_custom >= 0 && n_custom <= PB_MAX_CUSTOM, "at most 4 custom gate terms");
+  PB_CHECK(n_custom == 0 || h_exps, "custom gate terms need their exponents");
+  for (int k = 0; k < n_custom; k++) {
+    const uint8_t* e = h_exps + 3 * k;
+    const int deg = e[0] + e[1] + e[2];
+    PB_CHECK(deg >= 2 && deg <= 3, "custom gate term must have total degree 2 or 3");
+    PB_CHECK(!(e[0] == 1 && e[1] == 1 && e[2] == 0), "custom gate term (1, 1, 0) duplicates QM");
+    for (int k2 = 0; k2 < k; k2++)
+      PB_CHECK(memcmp(e, h_exps + 3 * k2, 3) != 0, "custom gate terms must have distinct exponents");
+    int s = 0;
+    for (int w = 0; w < 3; w++)
+      for (int t = 0; t < e[w]; t++) P->custom_f[k][s++] = (uint8_t)w;
+    if (s == 2) P->custom_f[k][2] = 3;
+  }
+  P->n_custom = n_custom;
+}
+
+// h_pk: 8 vectors (QM QL QR QO QC S1 S2 S3), each n x 32 bytes canonical (compiler/program.py:10-30); h_custom:
+// n_custom more selector vectors of the same shape, with their exponents h_exps (3 bytes per term).
 // sharded: one proof across the ranks of the context's communicator (see Prover in prover.cuh).
-Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h_pk, bool sharded) {
+Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h_pk, int n_custom,
+                      const uint8_t* h_exps, const uint8_t* const* h_custom, bool sharded) {
   auto P = std::make_unique<Prover>();
   P->ctx = ctx;
   P->srs = srs;
@@ -467,6 +492,8 @@ Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h
   P->n = n;
   PB_CHECK(log_n >= 1 && log_n <= 26, "group order must be 2^k, 1 <= k <= 26");
   PB_CHECK(n <= srs_size(srs), "Not enough powers in setup");
+  set_custom_terms(P.get(), n_custom, h_exps);
+  PB_CHECK(n_custom == 0 || h_custom, "custom gate terms need their selector columns");
   if (sharded) {
     Comm* cm = ctx_comm(ctx);
     P->world = comm_world(cm);
@@ -520,8 +547,8 @@ Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h
     ctx->launches += 3;
     PB_CUDA(cudaStreamSynchronize(st));
   }
-  for (int k = 0; k < 8; k++) {
-    upload_mont(ctx, P->sel_lag[k], h_pk[k], n);
+  for (int k = 0; k < Prover::CUSTOM0 + n_custom; k++) {
+    upload_mont(ctx, P->sel_lag[k], k < Prover::CUSTOM0 ? h_pk[k] : h_custom[k - Prover::CUSTOM0], n);
     P->sel_coeff[k].alloc(n * 32);
     ntt_run(ctx, P->sel_lag[k].as<Fr>(), P->sel_coeff[k].as<Fr>(), log_n, true, n, nullptr, nullptr);
     P->sel_ext[k].alloc(ne * 32);
@@ -695,7 +722,8 @@ void prover_round1(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_
   k_gate_check<<<PB_GRID(n, 128), 0, st>>>(P->lag[0].as<Fr>(), P->lag[1].as<Fr>(), P->lag[2].as<Fr>(),
                                           P->sel_lag[Prover::QL].as<Fr>(), P->sel_lag[Prover::QR].as<Fr>(),
                                           P->sel_lag[Prover::QM].as<Fr>(), P->sel_lag[Prover::QO].as<Fr>(),
-                                          P->sel_lag[Prover::QC].as<Fr>(), P->pi_lag.as<Fr>(), n, P->flags.as<uint32_t>());
+                                          P->sel_lag[Prover::QC].as<Fr>(), P->pi_lag.as<Fr>(), P->custom_terms(P->sel_lag),
+                                          n, P->flags.as<uint32_t>());
   ctx->launches++;
   if (wires_on_device || P->world > 1) interpolate(P, abc_lag, abc_coeff, 3);
   // public inputs: few of them -> PI is a short combination of cached Lagrange-basis vectors (no transforms);
@@ -806,6 +834,7 @@ void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c) {
   q.QM = P->sel_ext[Prover::QM].as<Fr>(); q.QL = P->sel_ext[Prover::QL].as<Fr>(); q.QR = P->sel_ext[Prover::QR].as<Fr>();
   q.QO = P->sel_ext[Prover::QO].as<Fr>(); q.QC = P->sel_ext[Prover::QC].as<Fr>();
   q.S1 = P->sel_ext[Prover::S1].as<Fr>(); q.S2 = P->sel_ext[Prover::S2].as<Fr>(); q.S3 = P->sel_ext[Prover::S3].as<Fr>();
+  q.custom = P->custom_terms(P->sel_ext);
   q.L0 = P->l0_ext.as<Fr>(); q.X = P->xs.as<Fr>();
   for (int k = 0; k < 4; k++) q.zh_inv[k] = P->zh_inv[k];
   q.alpha = P->alpha; q.alpha2 = fp_sqr(P->alpha); q.beta = P->beta; q.gamma = P->gamma; q.one = Fr::one();
@@ -932,6 +961,8 @@ void prover_round5(Prover* P, const Fr& v_c) {
   add(P->sel_coeff[Prover::QM].as<Fr>(), fp_mul(a, b));
   add(P->sel_coeff[Prover::QO].as<Fr>(), c);
   add(P->sel_coeff[Prover::QC].as<Fr>(), one);
+  for (int t = 0; t < P->n_custom; t++)                                // m_t(a, b, c) Q_t
+    add(P->sel_coeff[Prover::CUSTOM0 + t].as<Fr>(), custom_monomial(a, b, c, P->custom_f[t]));
   add(P->coeff[3].as<Fr>(), fp_add(c1, al2l0));                        // Z
   add(P->sel_coeff[Prover::S3].as<Fr>(), fp_neg(fp_mul(c2, be)));
   add(P->tq.as<Fr>(), fp_neg(zh_ev));                                  // T1

@@ -14,6 +14,41 @@ void srs_msm_batch_sharded(Context* ctx, Srs* srs, const Fr* const* d_scalars, u
                            bool scalars_mont, uint8_t* out_xy, int* is_identity);
 uint32_t srs_bucket_count(Srs* s);
 
+// Custom gate terms: the gate constraint gains sum_k Q_k a^i_k b^j_k c^l_k, total degree 2 or 3 (so T stays below
+// degree 3n and the proof keeps its shape).  A term is stored as the wires of its monomial: 2 or 3 of {0 a, 1 b, 2 c},
+// unused slots 3.
+#define PB_MAX_CUSTOM 4
+struct CustomTerms {
+  const Fr* Q[PB_MAX_CUSTOM];
+  uint8_t f[PB_MAX_CUSTOM][3];
+  int count;
+};
+// m_k(a, b, c) with degree - 1 products; the wires are selected by value so a, b, c stay in registers
+PB_HD Fr custom_monomial(const Fr& a, const Fr& b, const Fr& c, const uint8_t* f) {
+  auto pick = [&](uint8_t w) -> Fr { return w == 0 ? a : (w == 1 ? b : c); };
+  Fr m = fp_mul(pick(f[0]), pick(f[1]));
+  if (f[2] < 3) m = fp_mul(m, pick(f[2]));
+  return m;
+}
+// sum_k Q_k[i] m_k(a, b, c), unrolled over the PB_MAX_CUSTOM slots so the kernel parameters are indexed statically
+// (a dynamic index would copy them to local memory); count == 0 costs one uniform branch
+#ifdef __CUDACC__
+__device__ __forceinline__ Fr custom_gate_sum(const CustomTerms& t, uint64_t i, const Fr& a, const Fr& b, const Fr& c,
+                                              Fr acc) {
+#pragma unroll
+  for (int k = 0; k < PB_MAX_CUSTOM; k++) {
+    if (k >= t.count) break;
+    const uint4* q = reinterpret_cast<const uint4*>(t.Q[k] + i);
+    uint4 lo = __ldg(q), hi = __ldg(q + 1);
+    Fr s;
+    s.v[0] = lo.x; s.v[1] = lo.y; s.v[2] = lo.z; s.v[3] = lo.w;
+    s.v[4] = hi.x; s.v[5] = hi.y; s.v[6] = hi.z; s.v[7] = hi.w;
+    acc = fp_add(acc, fp_mul(custom_monomial(a, b, c, t.f[k]), s));
+  }
+  return acc;
+}
+#endif
+
 struct Proof {
   uint8_t pts[9][64];    // a_1 b_1 c_1 z_1 t_lo t_mid t_hi W_z W_zw  (canonical LE x||y)
   uint8_t evals[6][32];  // a b c s1 s2 z_shifted (canonical LE)
@@ -36,9 +71,11 @@ struct Prover {
   uint64_t zw_shift = 4; // Z(w x_j) = Z-extension at local index j + 4 / world ...
   bool zw_separate = false;  // ... or, when 4 % world != 0, a separately extended vector (ext[5])
   // per-circuit (all Montgomery)
-  DevBuf sel_coeff[8];   // QM QL QR QO QC S1 S2 S3, coefficient form
-  DevBuf sel_lag[8];     // same, Lagrange values (QM..QC for the gate check, S1..S3 for round 2)
-  DevBuf sel_ext[8];     // same, on this rank's slice of the fixed 4n coset
+  DevBuf sel_coeff[8 + PB_MAX_CUSTOM];   // QM QL QR QO QC S1 S2 S3, then the custom selectors; coefficient form
+  DevBuf sel_lag[8 + PB_MAX_CUSTOM];     // same, Lagrange values (QM..QC and custom for the gate check, S1..S3 for round 2)
+  DevBuf sel_ext[8 + PB_MAX_CUSTOM];     // same, on this rank's slice of the fixed 4n coset
+  int n_custom = 0;
+  uint8_t custom_f[PB_MAX_CUSTOM][3];    // monomial wires of each custom term (CustomTerms::f)
   DevBuf roots;          // w^i, i < n
   DevBuf gpow;           // (g mu^rank)^i, i < n     (coset shift on load)
   DevBuf gpow_w;         // (g mu^(rank+4))^i, i < n (only when zw_separate)
@@ -67,7 +104,18 @@ struct Prover {
   std::vector<Fr> pub_neg;        // -public_i, Montgomery (host)
   Proof proof;
 
-  enum { QM = 0, QL, QR, QO, QC, S1, S2, S3 };
+  enum { QM = 0, QL, QR, QO, QC, S1, S2, S3, CUSTOM0 };
+
+  // the custom selectors from one of the per-circuit caches
+  CustomTerms custom_terms(const DevBuf* sel) const {
+    CustomTerms t;
+    t.count = n_custom;
+    for (int k = 0; k < PB_MAX_CUSTOM; k++) {
+      t.Q[k] = k < n_custom ? sel[CUSTOM0 + k].as<Fr>() : nullptr;
+      for (int s = 0; s < 3; s++) t.f[k][s] = custom_f[k][s];
+    }
+    return t;
+  }
 
   // several commitments in one pass over the SRS (out: count * 64 bytes, contiguous)
   void commit_batch(const Fr* const* d_coeffs, uint32_t count, uint64_t m, uint8_t* out_xy) {

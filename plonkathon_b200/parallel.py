@@ -119,11 +119,12 @@ class ShardedProver(Prover):
     same bytes.  Every rank must make the same calls with the same inputs (the collectives inside are matched
     pairwise); the context needs a communicator (``init_comm``)."""
     _CREATE = "pb200_prover_create_sharded"
+    _CREATE_CUSTOM = "pb200_prover_create_custom_sharded"
 
     @classmethod
-    def from_arrays(cls, setup, group_order, pk_arrays, group=None, ctx=None):
+    def from_arrays(cls, setup, group_order, pk_arrays, group=None, ctx=None, custom=()):
         init_comm(ctx or setup.ctx, group)
-        return super().from_arrays(setup, group_order, pk_arrays, ctx=ctx)
+        return super().from_arrays(setup, group_order, pk_arrays, ctx=ctx, custom=custom)
 
     def __init__(self, setup, program, group=None):
         init_comm(setup.ctx, group)

@@ -16,6 +16,7 @@ import numpy as np
 
 from . import _lib
 from .curve import Scalar
+from .custom_gates import split_terms
 from .field import CURVE_ORDER, FIELD_MODULUS, FQ
 from .poly import Basis, _log2_exact, scalars_to_bytes
 from .transcript import Message1, Message2, Message3, Message4, Message5, Transcript
@@ -90,6 +91,7 @@ def _raise(err: _lib.PlonkB200Error):
 
 class Prover:
     _CREATE = "pb200_prover_create"
+    _CREATE_CUSTOM = "pb200_prover_create_custom"
 
     def __init__(self, setup, program):
         """prover.py:45-49."""
@@ -101,27 +103,40 @@ class Prover:
         self._create(setup, self.group_order, cols)
 
     @classmethod
-    def from_arrays(cls, setup, group_order: int, pk_arrays: dict, ctx=None):
+    def from_arrays(cls, setup, group_order: int, pk_arrays: dict, ctx=None, custom=()):
         """pk_arrays: QM QL QR QO QC S1 S2 S3 -> list of ints or (n,32) uint8 little-endian arrays.
         ``ctx``: run this prover on another context (stream + scratch) of the same device than the setup's; the SRS
-        is shared read-only, so several provers can be driven concurrently from different host threads."""
+        is shared read-only, so several provers can be driven concurrently from different host threads.
+        ``custom``: up to 4 custom gate terms ``((i, j, l), column)``, each adding ``Q_k a^i b^j c^l`` to the gate
+        constraint (plonkathon_b200/custom_gates.py); ValueError for a malformed term."""
         self = cls.__new__(cls)
         self.group_order = group_order
         self.setup = setup
         self.program = None
         self.pk = None
         cols = {k: _as_le_rows(pk_arrays[k], group_order) for k in PK_ORDER}
-        self._create(setup, group_order, cols, ctx)
+        self._create(setup, group_order, cols, ctx, custom)
         return self
 
-    def _create(self, setup, n, cols, ctx=None):
+    def _create(self, setup, n, cols, ctx=None, custom=()):
+        exps, ccols = split_terms(custom, n)  # before any device work: a malformed term is a ValueError
         self.ctx = ctx or setup.ctx
         self._log_n = _log2_exact(n)
+        self.custom_exponents = exps
         keep = [c if isinstance(c, bytes) else c.tobytes() for c in (cols[k] for k in PK_ORDER)]
         arr = (ctypes.c_char_p * 8)(*keep)
         h = ctypes.c_void_p()
-        create = getattr(_lib.lib(), self._CREATE)  # the multi-GPU prover creates its sharded counterpart
-        _lib.check(create(self.ctx.handle, setup._srs, self._log_n, ctypes.cast(arr, ctypes.c_void_p), ctypes.byref(h)))
+        if exps:
+            ckeep = [_as_le_rows(col, n).tobytes() for col in ccols]
+            carr = (ctypes.c_char_p * len(ckeep))(*ckeep)
+            ebytes = bytes(x for e in exps for x in e)
+            create = getattr(_lib.lib(), self._CREATE_CUSTOM)
+            _lib.check(create(self.ctx.handle, setup._srs, self._log_n, ctypes.cast(arr, ctypes.c_void_p), len(exps),
+                              ebytes, ctypes.cast(carr, ctypes.c_void_p), ctypes.byref(h)))
+        else:
+            create = getattr(_lib.lib(), self._CREATE)  # the multi-GPU prover creates its sharded counterpart
+            _lib.check(create(self.ctx.handle, setup._srs, self._log_n, ctypes.cast(arr, ctypes.c_void_p),
+                              ctypes.byref(h)))
         self._h = h
 
     def __del__(self):

@@ -10,7 +10,9 @@ from typing import Optional
 from . import _lib
 from .curve import G2, Scalar, _pt_bytes, _pt_from, g2_mul
 from .field import CURVE_ORDER, FIELD_MODULUS, FQ, FQ2
+from .custom_gates import split_terms
 from .poly import Basis, Polynomial, _log2_exact
+from .prover import _as_le_rows
 from .verifier import VerificationKey  # noqa: F401  (re-exported: the reference's setup.py imports it too)
 
 SETUP_FILE_G1_STARTPOS = 80  # setup.py:11
@@ -198,14 +200,16 @@ class Setup:
             h = self._lagrange[n]
         return h
 
-    def verification_key_arrays(self, group_order: int, pk_arrays: dict) -> VerificationKey:
+    def verification_key_arrays(self, group_order: int, pk_arrays: dict, custom=()) -> VerificationKey:
         """``verification_key`` for circuits that exist only as arrays (``Prover.from_arrays``): QM..S3 as
-        (n,32) uint8 little-endian Lagrange values in host memory."""
+        (n,32) uint8 little-endian Lagrange values in host memory.  ``custom``: the circuit's custom gate terms
+        ``((i, j, l), column)`` as given to ``Prover.from_arrays``; each column is committed too."""
         import numpy as np
         log_n = _log2_exact(group_order)
-        pts = []
-        for k in ("QM", "QL", "QR", "QO", "QC", "S1", "S2", "S3"):
-            col = np.ascontiguousarray(pk_arrays[k]).view(np.uint8).reshape(-1, 32)
+        exps, ccols = split_terms(custom, group_order)
+
+        def commit_host(col):
+            col = np.ascontiguousarray(col).view(np.uint8).reshape(-1, 32)
             assert col.shape[0] == group_order
             out = ctypes.create_string_buffer(64)
             ident = ctypes.c_int(0)
@@ -216,8 +220,11 @@ class Setup:
             else:
                 _lib.check(_lib.lib().pb200_srs_commit_lagrange_host(
                     self.ctx.handle, self._srs, col.ctypes.data_as(ctypes.c_void_p), log_n, out, ctypes.byref(ident)))
-            pts.append(_pt_from(out.raw, ident.value))
-        return VerificationKey(group_order, *pts, self.X2, Scalar.root_of_unity(group_order))
+            return _pt_from(out.raw, ident.value)
+
+        pts = [commit_host(pk_arrays[k]) for k in ("QM", "QL", "QR", "QO", "QC", "S1", "S2", "S3")]
+        terms = tuple((e, commit_host(_as_le_rows(col, group_order))) for e, col in zip(exps, ccols))
+        return VerificationKey(group_order, *pts, self.X2, Scalar.root_of_unity(group_order), terms)
 
     def verification_key(self, pk) -> VerificationKey:
         """setup.py:75-77."""

@@ -10,7 +10,7 @@ tests/test_synthetic_vs_reference.py checks this against the reference compiler 
 from __future__ import annotations
 
 import random
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 
 import numpy as np
 
@@ -36,6 +36,8 @@ class ArrayCircuit:
     n_public: int
     values: list  # value of every variable id
     text: list  # the same circuit in the reference's constraint language (small sizes only)
+    # custom gate terms ((i, j, l), selector values per row), plonkathon_b200/custom_gates.py
+    custom: list = field(default_factory=list)
 
     def wires_values(self):
         val = self.values
@@ -85,10 +87,15 @@ def permutation_polys(wire_L, wire_R, wire_O, group_order: int, n_constraints: i
 
 
 def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: float = 1.0,
-                  with_text: bool = False) -> ArrayCircuit:
+                  with_text: bool = False, custom=()) -> ArrayCircuit:
     """Deterministic synthetic circuit with 2^log_n rows: ``n_public`` public-input rows, then a chain of
     multiplication / addition / add-constant gates whose operands are drawn from recently produced
-    variables (so the permutation is non-trivial and the witness values are pseudo-random field elements)."""
+    variables (so the permutation is non-trivial and the witness values are pseudo-random field elements).
+
+    ``custom``: exponent triples (i, j, l) of custom gate terms; rows using them are mixed into the chain (see
+    ``_custom_row``).  Without it the random draws, and so the circuit, are exactly those of a plain circuit."""
+    from .custom_gates import check_exponents
+    custom = check_exponents(custom)
     n = 1 << log_n
     rng = random.Random(seed)
     m = max(n_public + 1, int(n * fill))
@@ -98,6 +105,7 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
     wR = np.full(n, -1, dtype=np.int64)
     wO = np.full(n, -1, dtype=np.int64)
     QL, QR, QM, QO, QC = ([0] * n for _ in range(5))
+    QK = [[0] * n for _ in custom]
     text = []
 
     def name(i):
@@ -124,9 +132,13 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
         if first:  # make sure the private seeds are used so every variable appears in some cell
             ia, ib = n_public, n_public + 1
             first = False
-        kind = rng.randrange(3)
+        kind = rng.randrange(3 + len(custom))
         out = nv
-        if kind == 0 or ia == ib:  # c <== a * b : M = -1, O = 1
+        if kind >= 3:
+            ic = rng.randrange(lo, nv)
+            k = rng.randrange(0, 1 << 30)
+            _custom_row(custom[kind - 3], QK[kind - 3], row, (ia, ib, ic), k, values, (wL, wR, wO), (QL, QO, QC))
+        elif kind == 0 or ia == ib:  # c <== a * b : M = -1, O = 1
             values.append(values[ia] * values[ib] % R)
             wL[row], wR[row], wO[row] = ia, ib, out
             QM[row], QO[row] = R - 1, 1
@@ -147,7 +159,35 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
             if with_text:
                 text.append("%s <== %s + %d" % (name(out), name(ia), k))
         row += 1
-    return ArrayCircuit(n, m, wL, wR, wO, QL, QR, QM, QO, QC, n_public, values, text)
+    return ArrayCircuit(n, m, wL, wR, wO, QL, QR, QM, QO, QC, n_public, values, text, list(zip(custom, QK)))
+
+
+def _custom_row(exps, Q, row, operands, k, values, wires, sel):
+    """One row using the custom term a^i b^j c^l (selector column Q).  The wires of the monomial take the operands;
+    the output goes on the first wire the term does not use:
+      * l == 0:          c <== a^i b^j + k        (Q = -1, QO = 1, QC = -k), e.g. c = a^2 b, c = a^3 + k;
+      * l > 0, i == 0:   a <== b^j c^l + k        (Q = -1, QL = 1, QC = -k), e.g. a = c^3 + k;
+      * i, l > 0:        a^i b^j c^l == its value (Q = 1, QC = -value), e.g. the three-wire constraint a b c = k.
+    A wire outside the term and the output carries an operand with a zero selector."""
+    i, j, l = exps
+    wL, wR, wO = wires
+    QL, QO, QC = sel
+    ia, ib, ic = operands
+    val = lambda v, e: pow(values[v], e, R)  # noqa: E731
+    out = len(values)
+    if l == 0:
+        values.append((val(ia, i) * val(ib, j) + k) % R)
+        wL[row], wR[row], wO[row] = ia, (ib if j else ia), out
+        Q[row], QO[row], QC[row] = R - 1, 1, (R - k) % R
+    elif i == 0:
+        values.append((val(ib, j) * val(ic, l) + k) % R)
+        wL[row], wR[row], wO[row] = out, (ib if j else ic), ic
+        Q[row], QL[row], QC[row] = R - 1, 1, (R - k) % R
+    else:
+        prod = val(ia, i) * val(ib, j) * val(ic, l) % R
+        wL[row], wR[row], wO[row] = ia, ib, ic
+        Q[row], QC[row] = 1, (R - prod) % R
+        values.append(prod)  # keeps one new variable per row (unused by any cell)
 
 
 def circuit_arrays(c: ArrayCircuit):
@@ -160,3 +200,10 @@ def circuit_arrays(c: ArrayCircuit):
           "S1": to_le(S1), "S2": to_le(S2), "S3": to_le(S3)}
     A, B, C = c.wires_values()
     return pk, to_le(A), to_le(B), to_le(C), c.public_values()
+
+
+def custom_arrays(c: ArrayCircuit):
+    """-> the circuit's custom gate terms as ``((i, j, l), (n,32) uint8 array)``, ready for ``Prover.from_arrays(...,
+    custom=)`` and ``Setup.verification_key_arrays(..., custom=)``"""
+    return [(e, np.frombuffer(b"".join(int(x).to_bytes(32, "little") for x in col), dtype=np.uint8).reshape(-1, 32).copy())
+            for e, col in c.custom]

@@ -14,6 +14,7 @@ from dataclasses import dataclass
 
 from .curve import G1, G2, Scalar, ec_lincomb, g1_neg, g2_add, g2_mul, pairing_product_is_one
 from . import _lib
+from .custom_gates import monomial
 from .field import CURVE_ORDER, FIELD_MODULUS
 from .transcript import Transcript
 
@@ -45,6 +46,12 @@ class VerificationKey:
     S3: object
     X_2: object
     w: Scalar
+    # custom gate terms ((i, j, l), commitment to Q_k), in the prover's order (plonkathon_b200/custom_gates.py)
+    custom: tuple = ()
+
+    def _custom_terms(self, a, b, c):
+        """the custom gates' part of the linearisation: sum_k m_k(a, b, c) [Q_k]"""
+        return [(pt, monomial(e, a, b, c)) for e, pt in self.custom]
 
     # ---- shared by both routines: steps 4-7 of the paper's verifier
     def _common(self, group_order: int, pf, public):
@@ -90,7 +97,7 @@ class VerificationKey:
         zeta_n = zeta ** group_order
         # [D] = [r] - r0 + u [z]
         d_pt = ec_lincomb([
-            (self.Qm, a * b), (self.Ql, a), (self.Qr, b), (self.Qo, c), (self.Qc, 1),
+            (self.Qm, a * b), (self.Ql, a), (self.Qr, b), (self.Qo, c), (self.Qc, 1), *self._custom_terms(a, b, c),
             (proof["z_1"], (a + beta * zeta + gamma) * (b + beta * 2 * zeta + gamma) * (c + beta * 3 * zeta + gamma)
              * alpha + l0_ev * alpha * alpha + u),
             (self.S3, -perm_bar * beta),
@@ -125,6 +132,7 @@ class VerificationKey:
         r_pt = ec_lincomb([
             # gate constraint with the wire values fixed to their evaluations
             (self.Qm, a * b), (self.Ql, a), (self.Qr, b), (self.Qo, c), (self.Qc, 1), (G1, pi_ev),
+            *self._custom_terms(a, b, c),
             # permutation argument: Z(X) keeps its commitment, S3(X) too, everything else is a number
             (proof["z_1"], (a + beta * zeta + gamma) * (b + beta * 2 * zeta + gamma) * (c + beta * 3 * zeta + gamma) * alpha),
             (self.S3, -sigma_bar * alpha * beta), (G1, -sigma_bar * alpha * (c + gamma)),
