@@ -5,8 +5,10 @@
 // (x = X/ZZ, y = Y/ZZZ, ZZ^3 = ZZZ^2; identity <=> ZZ == 0) so an affine point is added with
 // 8 mul + 2 sqr and no inversion; a single inversion happens in g1_to_affine at the very end.
 // Formulas: the standard madd-2008-s / add-2008-s / dbl-2008-s-1 sets for short Weierstrass curves
-// with a = 0.  All coordinates are Montgomery-form Fq, fully reduced.  All exceptional cases the
-// reference's tests reach are handled: identity operands, P + P (doubling), P + (-P).
+// with a = 0.  All coordinates are Montgomery-form Fq, fully reduced; inside an addition the intermediates are lazy
+// (field.cuh: in [0, 2p)), which saves the final subtraction of most products, and Y3's difference of two products
+// takes one reduction.  All exceptional cases the reference's tests reach are handled: identity operands, P + P
+// (doubling), P + (-P).
 #pragma once
 #include "field.cuh"
 
@@ -41,7 +43,8 @@ PB_HD void g1_double_affine(G1XYZZ& acc, const G1Affine& p) {
   Fq M = fp_sqr(p.x);
   M = fp_add(fp_dbl(M), M);
   Fq X3 = fp_sub(fp_sqr(M), fp_dbl(S));
-  acc.Y = fp_sub(fp_mul(M, fp_sub(S, X3)), fp_mul(W, p.y));
+  acc.Y = fp_mul2_lazy(M, fp_sub(S, X3), W, fp_neg_lazy(p.y));  // M (S - X3) - W y: all factors <= p
+  fp_reduce_once(acc.Y);
   acc.X = X3;
   acc.ZZ = V;
   acc.ZZZ = W;
@@ -56,10 +59,30 @@ PB_HD void g1_double(G1XYZZ& a) {
   Fq M = fp_sqr(a.X);
   M = fp_add(fp_dbl(M), M);
   Fq X3 = fp_sub(fp_sqr(M), fp_dbl(S));
-  a.Y = fp_sub(fp_mul(M, fp_sub(S, X3)), fp_mul(W, a.Y));
+  a.Y = fp_mul2_lazy(M, fp_sub(S, X3), W, fp_neg_lazy(a.Y));
+  fp_reduce_once(a.Y);
   a.X = X3;
   a.ZZ = fp_mul(V, a.ZZ);
   a.ZZZ = fp_mul(W, a.ZZZ);
+}
+
+// The common part of the additions: from Pd = U2 - U1 (nonzero mod p) and Rd = S2 - S1,
+//   PP = Pd^2, PPP = Pd PP, Q = U1 PP, X3 = Rd^2 - PPP - 2Q, Y3 = Rd (Q - X3) - S1 PPP,
+//   ZZ3 = Z2 PP, ZZZ3 = Z3 PPP   (Z2, Z3: ZZ1 and ZZZ1, times ZZ2 and ZZZ2 in a full addition).
+// Ranges, with p < 0.19 R: U1, S1 canonical; U2, S2 lazy products of canonical values (< 1.19p), so Pd, Rd =
+// fp_sub(U2 or S2, canonical) < 1.19p; Z2, Z3 < 1.19p.  Then PP < 1.27p, PPP < 1.29p, Q < 1.24p, and Q - X3 < 1.24p,
+// so Rd (Q - X3) + (p - S1) PPP < 2.77p^2 < pR and Y3 needs one reduction.  All four outputs leave canonical.
+// The order (each factor used up as early as possible) keeps the accumulation kernel within 128 registers.
+PB_HD void g1_add_tail(const Fq& U1, const Fq& S1, const Fq& Pd, const Fq& Rd, const Fq& Z2, const Fq& Z3, G1XYZZ& r) {
+  const Fq PP = fp_sqr_lazy(Pd);
+  r.ZZ = fp_mul(Z2, PP);
+  const Fq PPP = fp_mul_lazy(Pd, PP);
+  r.ZZZ = fp_mul(Z3, PPP);
+  const Fq Q = fp_mul_lazy(U1, PP);
+  r.X = fp_sub_lazy(fp_sub_lazy(fp_sub_lazy(fp_sqr_lazy(Rd), PPP), Q), Q);
+  fp_reduce_once(r.X);
+  r.Y = fp_mul2_lazy(Rd, fp_sub(Q, r.X), fp_neg_lazy(S1), PPP);
+  fp_reduce_once(r.Y);
 }
 
 // acc += p (p affine, never the identity)
@@ -68,23 +91,18 @@ PB_HD void g1_add_mixed(G1XYZZ& acc, const G1Affine& p) {
     acc = g1_from_affine(p);
     return;
   }
-  Fq U2 = fp_mul(p.x, acc.ZZ);
-  Fq S2 = fp_mul(p.y, acc.ZZZ);
+  Fq U2 = fp_mul_lazy(p.x, acc.ZZ);
+  Fq S2 = fp_mul_lazy(p.y, acc.ZZZ);
   Fq Pd = fp_sub(U2, acc.X);
   Fq Rd = fp_sub(S2, acc.Y);
-  if (Pd.is_zero()) {
-    if (Rd.is_zero()) g1_double_affine(acc, p);
+  if (fp_is_zero_lazy(Pd)) {
+    if (fp_is_zero_lazy(Rd)) g1_double_affine(acc, p);
     else acc = G1XYZZ::identity();
     return;
   }
-  Fq PP = fp_sqr(Pd);
-  Fq PPP = fp_mul(Pd, PP);
-  Fq Q = fp_mul(acc.X, PP);
-  Fq X3 = fp_sub(fp_sub(fp_sqr(Rd), PPP), fp_dbl(Q));
-  acc.Y = fp_sub(fp_mul(Rd, fp_sub(Q, X3)), fp_mul(acc.Y, PPP));
-  acc.X = X3;
-  acc.ZZ = fp_mul(acc.ZZ, PP);
-  acc.ZZZ = fp_mul(acc.ZZZ, PPP);
+  G1XYZZ r;
+  g1_add_tail(acc.X, acc.Y, Pd, Rd, acc.ZZ, acc.ZZZ, r);
+  acc = r;
 }
 
 // acc += p with (almost) uniform control flow for SIMT execution: every lane runs the same 8M + 2S
@@ -92,29 +110,24 @@ PB_HD void g1_add_mixed(G1XYZZ& acc, const G1Affine& p) {
 // the rare P == +-Q cases branch.
 PB_HD void g1_add_mixed_uniform(G1XYZZ& acc, const G1Affine& p) {
   const bool was_inf = acc.is_inf();
-  Fq U2 = fp_mul(p.x, acc.ZZ);
-  Fq S2 = fp_mul(p.y, acc.ZZZ);
+  Fq U2 = fp_mul_lazy(p.x, acc.ZZ);
+  Fq S2 = fp_mul_lazy(p.y, acc.ZZZ);
   Fq Pd = fp_sub(U2, acc.X);
   Fq Rd = fp_sub(S2, acc.Y);
-  if (!was_inf && Pd.is_zero()) {
-    if (Rd.is_zero()) g1_double_affine(acc, p);
+  if (!was_inf && fp_is_zero_lazy(Pd)) {
+    if (fp_is_zero_lazy(Rd)) g1_double_affine(acc, p);
     else acc = G1XYZZ::identity();
     return;
   }
-  Fq PP = fp_sqr(Pd);
-  Fq PPP = fp_mul(Pd, PP);
-  Fq Q = fp_mul(acc.X, PP);
-  Fq X3 = fp_sub(fp_sub(fp_sqr(Rd), PPP), fp_dbl(Q));
-  Fq Y3 = fp_sub(fp_mul(Rd, fp_sub(Q, X3)), fp_mul(acc.Y, PPP));
-  Fq ZZ3 = fp_mul(acc.ZZ, PP);
-  Fq ZZZ3 = fp_mul(acc.ZZZ, PPP);
+  G1XYZZ r;
+  g1_add_tail(acc.X, acc.Y, Pd, Rd, acc.ZZ, acc.ZZZ, r);
   const Fq one = Fq::one();
 #pragma unroll
   for (int i = 0; i < 8; i++) {
-    acc.X.v[i] = was_inf ? p.x.v[i] : X3.v[i];
-    acc.Y.v[i] = was_inf ? p.y.v[i] : Y3.v[i];
-    acc.ZZ.v[i] = was_inf ? one.v[i] : ZZ3.v[i];
-    acc.ZZZ.v[i] = was_inf ? one.v[i] : ZZZ3.v[i];
+    acc.X.v[i] = was_inf ? p.x.v[i] : r.X.v[i];
+    acc.Y.v[i] = was_inf ? p.y.v[i] : r.Y.v[i];
+    acc.ZZ.v[i] = was_inf ? one.v[i] : r.ZZ.v[i];
+    acc.ZZZ.v[i] = was_inf ? one.v[i] : r.ZZZ.v[i];
   }
 }
 
@@ -126,24 +139,19 @@ PB_HD void g1_add(G1XYZZ& acc, const G1XYZZ& q) {
     return;
   }
   Fq U1 = fp_mul(acc.X, q.ZZ);
-  Fq U2 = fp_mul(q.X, acc.ZZ);
+  Fq U2 = fp_mul_lazy(q.X, acc.ZZ);
   Fq S1 = fp_mul(acc.Y, q.ZZZ);
-  Fq S2 = fp_mul(q.Y, acc.ZZZ);
+  Fq S2 = fp_mul_lazy(q.Y, acc.ZZZ);
   Fq Pd = fp_sub(U2, U1);
   Fq Rd = fp_sub(S2, S1);
-  if (Pd.is_zero()) {
-    if (Rd.is_zero()) g1_double(acc);
+  if (fp_is_zero_lazy(Pd)) {
+    if (fp_is_zero_lazy(Rd)) g1_double(acc);
     else acc = G1XYZZ::identity();
     return;
   }
-  Fq PP = fp_sqr(Pd);
-  Fq PPP = fp_mul(Pd, PP);
-  Fq Q = fp_mul(U1, PP);
-  Fq X3 = fp_sub(fp_sub(fp_sqr(Rd), PPP), fp_dbl(Q));
-  acc.Y = fp_sub(fp_mul(Rd, fp_sub(Q, X3)), fp_mul(S1, PPP));
-  acc.X = X3;
-  acc.ZZ = fp_mul(fp_mul(acc.ZZ, q.ZZ), PP);
-  acc.ZZZ = fp_mul(fp_mul(acc.ZZZ, q.ZZZ), PPP);
+  G1XYZZ r;
+  g1_add_tail(U1, S1, Pd, Rd, fp_mul_lazy(acc.ZZ, q.ZZ), fp_mul_lazy(acc.ZZZ, q.ZZZ), r);
+  acc = r;
 }
 
 // acc += q with select-based handling of identity operands (one instruction stream for all lanes, so two
@@ -151,29 +159,24 @@ PB_HD void g1_add(G1XYZZ& acc, const G1XYZZ& q) {
 PB_HD void g1_add_uniform(G1XYZZ& acc, const G1XYZZ& q) {
   const bool a_inf = acc.is_inf(), q_inf = q.is_inf();
   Fq U1 = fp_mul(acc.X, q.ZZ);
-  Fq U2 = fp_mul(q.X, acc.ZZ);
+  Fq U2 = fp_mul_lazy(q.X, acc.ZZ);
   Fq S1 = fp_mul(acc.Y, q.ZZZ);
-  Fq S2 = fp_mul(q.Y, acc.ZZZ);
+  Fq S2 = fp_mul_lazy(q.Y, acc.ZZZ);
   Fq Pd = fp_sub(U2, U1);
   Fq Rd = fp_sub(S2, S1);
-  if (!a_inf && !q_inf && Pd.is_zero()) {
-    if (Rd.is_zero()) g1_double(acc);
+  if (!a_inf && !q_inf && fp_is_zero_lazy(Pd)) {
+    if (fp_is_zero_lazy(Rd)) g1_double(acc);
     else acc = G1XYZZ::identity();
     return;
   }
-  Fq PP = fp_sqr(Pd);
-  Fq PPP = fp_mul(Pd, PP);
-  Fq Q = fp_mul(U1, PP);
-  Fq X3 = fp_sub(fp_sub(fp_sqr(Rd), PPP), fp_dbl(Q));
-  Fq Y3 = fp_sub(fp_mul(Rd, fp_sub(Q, X3)), fp_mul(S1, PPP));
-  Fq ZZ3 = fp_mul(fp_mul(acc.ZZ, q.ZZ), PP);
-  Fq ZZZ3 = fp_mul(fp_mul(acc.ZZZ, q.ZZZ), PPP);
+  G1XYZZ r;
+  g1_add_tail(U1, S1, Pd, Rd, fp_mul_lazy(acc.ZZ, q.ZZ), fp_mul_lazy(acc.ZZZ, q.ZZZ), r);
 #pragma unroll
   for (int i = 0; i < 8; i++) {
-    acc.X.v[i] = q_inf ? acc.X.v[i] : (a_inf ? q.X.v[i] : X3.v[i]);
-    acc.Y.v[i] = q_inf ? acc.Y.v[i] : (a_inf ? q.Y.v[i] : Y3.v[i]);
-    acc.ZZ.v[i] = q_inf ? acc.ZZ.v[i] : (a_inf ? q.ZZ.v[i] : ZZ3.v[i]);
-    acc.ZZZ.v[i] = q_inf ? acc.ZZZ.v[i] : (a_inf ? q.ZZZ.v[i] : ZZZ3.v[i]);
+    acc.X.v[i] = q_inf ? acc.X.v[i] : (a_inf ? q.X.v[i] : r.X.v[i]);
+    acc.Y.v[i] = q_inf ? acc.Y.v[i] : (a_inf ? q.Y.v[i] : r.Y.v[i]);
+    acc.ZZ.v[i] = q_inf ? acc.ZZ.v[i] : (a_inf ? q.ZZ.v[i] : r.ZZ.v[i]);
+    acc.ZZZ.v[i] = q_inf ? acc.ZZZ.v[i] : (a_inf ? q.ZZZ.v[i] : r.ZZZ.v[i]);
   }
 }
 

@@ -13,6 +13,10 @@
 // mad.lo.cc / madc.hi.cc pairs, which ptxas fuses into one IMAD.WIDE.U32.X each
 // (136 IMAD-class instructions per product; checked with cuobjdump -sass).
 //
+// For the group law (curve.cuh) there are cheaper variants: a dedicated squaring (36 partial products instead of
+// 64, then the reduction), products that skip the final subtraction and return a value in [0, 2p), and the sum of
+// two products with one reduction.  fp_mul itself, which the NTT and the quotient use, is unchanged.
+//
 // Every PTX instruction is wrapped in a tiny function that has a host emulation with an explicit
 // carry flag, so the identical limb-level algorithm is unit-tested on the CPU
 // (tests/test_host_arith.py via csrc/host_selftest.cpp) before it ever runs on a GPU.
@@ -266,6 +270,18 @@ inline Fp<P> fp_mul_host64(const Fp<P>& a, const Fp<P>& b) {
 }
 #endif
 
+// last CIOS step had U = Y, V = X:  T / 2^32 = X + (Y >> 32) + (w != 0)
+template <class P>
+PB_HD Fp<P> fp_cios_final(const uint32_t* X, const uint32_t* Y, uint32_t w) {
+  Fp<P> r;
+  (void)add_cc(w, 0xffffffffu);
+  r.v[0] = addc_cc(X[0], Y[1]);
+#pragma unroll
+  for (int i = 1; i < 7; i++) r.v[i] = addc_cc(X[i], Y[i + 1]);
+  r.v[7] = addc(X[7], 0u);
+  return r;
+}
+
 template <class P>
 PB_HD Fp<P> fp_mul(const Fp<P>& a, const Fp<P>& b) {
 #if !defined(__CUDA_ARCH__) && defined(PB_HOST_FAST_MUL)
@@ -280,20 +296,280 @@ PB_HD Fp<P> fp_mul(const Fp<P>& a, const Fp<P>& b) {
   fp_cios_step<P, false>(Y, X, w, a.v, b.v[5]);
   fp_cios_step<P, false>(X, Y, w, a.v, b.v[6]);
   fp_cios_step<P, false>(Y, X, w, a.v, b.v[7]);
-  // last step had U = Y, V = X:  T / 2^32 = X + (Y >> 32) + (w != 0)
-  Fp<P> r;
-  (void)add_cc(w, 0xffffffffu);
-  r.v[0] = addc_cc(X[0], Y[1]);
-#pragma unroll
-  for (int i = 1; i < 7; i++) r.v[i] = addc_cc(X[i], Y[i + 1]);
-  r.v[7] = addc(X[7], 0u);
+  Fp<P> r = fp_cios_final<P>(X, Y, w);
   fp_reduce_once(r);
   return r;
 #endif
 }
 
+// ---- redundant ("lazy") representation ---------------------------------------------------------
+// Both moduli satisfy 4p < R = 2^256 (p < 0.19 R), which gives the bounds below.  A lazy value is any
+// integer in [0, 2p) congruent to the element; it is not unique (x and x + p), so it never leaves the
+// function that made it: everything stored or compared is made canonical with fp_reduce_once.
+//
+// Montgomery reduction of T < p * R returns (T + m p) / R < 2p.  CIOS on a, b in [0, 2p) has
+// T = a b < 4p^2 < p R, so dropping the final subtraction leaves a lazy result; fp_mul is this plus
+// fp_reduce_once.
 template <class P>
-PB_HD Fp<P> fp_sqr(const Fp<P>& a) { return fp_mul(a, a); }
+PB_HD Fp<P> fp_mul_lazy(const Fp<P>& a, const Fp<P>& b) {
+#if !defined(__CUDA_ARCH__) && defined(PB_HOST_FAST_MUL)
+  return fp_mul_host64(a, b);  // canonical, so also a valid lazy result
+#else
+  uint32_t X[8], Y[8], w;
+  fp_cios_step<P, true>(X, Y, w, a.v, b.v[0]);
+  fp_cios_step<P, false>(Y, X, w, a.v, b.v[1]);
+  fp_cios_step<P, false>(X, Y, w, a.v, b.v[2]);
+  fp_cios_step<P, false>(Y, X, w, a.v, b.v[3]);
+  fp_cios_step<P, false>(X, Y, w, a.v, b.v[4]);
+  fp_cios_step<P, false>(Y, X, w, a.v, b.v[5]);
+  fp_cios_step<P, false>(X, Y, w, a.v, b.v[6]);
+  fp_cios_step<P, false>(Y, X, w, a.v, b.v[7]);
+  return fp_cios_final<P>(X, Y, w);
+#endif
+}
+
+// 2p, limb i
+template <class P>
+PB_HD constexpr uint32_t fp_2p(int i) { return (P::p(i) << 1) | (i ? P::p(i - 1) >> 31 : 0u); }
+
+// a - b for a, b in [0, 2p): adds 2p on borrow, result in [0, 2p)
+template <class P>
+PB_HD Fp<P> fp_sub_lazy(const Fp<P>& a, const Fp<P>& b) {
+  Fp<P> r;
+  r.v[0] = sub_cc(a.v[0], b.v[0]);
+#pragma unroll
+  for (int i = 1; i < 8; i++) r.v[i] = subc_cc(a.v[i], b.v[i]);
+  uint32_t mask = subc(0u, 0u);  // all ones if a < b
+  r.v[0] = add_cc(r.v[0], fp_2p<P>(0) & mask);
+#pragma unroll
+  for (int i = 1; i < 7; i++) r.v[i] = addc_cc(r.v[i], fp_2p<P>(i) & mask);
+  r.v[7] = addc(r.v[7], fp_2p<P>(7) & mask);
+  return r;
+}
+// (fp_sub is also exact for a in [0, 2p) and b in [0, p): it adds p on borrow, so the result is in [0, max(a, p)).)
+
+// p - a for a in [0, p]: result in [0, p], congruent to -a (p for a == 0, unlike fp_neg)
+template <class P>
+PB_HD Fp<P> fp_neg_lazy(const Fp<P>& a) {
+  Fp<P> r;
+  r.v[0] = sub_cc(P::p(0), a.v[0]);
+#pragma unroll
+  for (int i = 1; i < 7; i++) r.v[i] = subc_cc(P::p(i), a.v[i]);
+  r.v[7] = subc(P::p(7), a.v[7]);
+  return r;
+}
+
+// a == 0 mod p for a in [0, 2p): a is 0 or p
+template <class P>
+PB_HD bool fp_is_zero_lazy(const Fp<P>& a) {
+  uint32_t z = 0, q = 0;
+#pragma unroll
+  for (int i = 0; i < 8; i++) { z |= a.v[i]; q |= a.v[i] ^ P::p(i); }
+  return z == 0 || q == 0;
+}
+
+// One CIOS step fed two rows: T += a * b + c * d (b, d: one limb each of the second factors), then one
+// reduction row.  Same state and role swap as fp_cios_step; the second row adds into the accumulators
+// without a shift, its carry out of limb 7 going to V limb 7 as the reduction rows do.
+template <class P, bool FIRST>
+PB_HD void fp_cios_step2(uint32_t* U, uint32_t* V, uint32_t& w, const uint32_t* a, uint32_t b, const uint32_t* c,
+                         uint32_t d) {
+  if (FIRST) {
+#pragma unroll
+    for (int j = 0; j < 8; j += 2) {
+      U[j] = mul_lo(a[j], b);
+      U[j + 1] = mul_hi(a[j], b);
+      V[j] = mul_lo(a[j + 1], b);
+      V[j + 1] = mul_hi(a[j + 1], b);
+    }
+    w = 0;
+  } else {
+    (void)add_cc(w, 0xffffffffu);  // CF = (w != 0)
+    U[0] = madc_lo_cc(a[0], b, U[0]);
+    U[1] = madc_hi_cc(a[0], b, U[1]);
+#pragma unroll
+    for (int j = 2; j < 8; j += 2) {
+      U[j] = madc_lo_cc(a[j], b, U[j]);
+      U[j + 1] = madc_hi_cc(a[j], b, U[j + 1]);
+    }
+    uint32_t c1 = addc(0u, 0u);
+    w = V[1];
+    V[0] = mad_lo_cc(a[1], b, V[2]);
+    V[1] = madc_hi_cc(a[1], b, V[3]);
+    V[2] = madc_lo_cc(a[3], b, V[4]);
+    V[3] = madc_hi_cc(a[3], b, V[5]);
+    V[4] = madc_lo_cc(a[5], b, V[6]);
+    V[5] = madc_hi_cc(a[5], b, V[7]);
+    V[6] = madc_lo_cc(a[7], b, 0u);
+    V[7] = madc_hi(a[7], b, c1);
+  }
+  fp_mad_row<P>(V, c + 1, d);
+  fp_mad_row<P>(U, c, d);
+  V[7] = addc(V[7], 0u);
+  uint32_t m = mul_lo(U[0] + w, P::NP0);
+  fp_mad_row_mod<P, 1>(V, m);
+  fp_mad_row_mod<P, 0>(U, m);
+  V[7] = addc(V[7], 0u);
+}
+
+// Sum of two products with one reduction: (a b + c d) / R mod p, lazy.  Needs a b + c d < p R, which holds
+// e.g. when a, b, c, d < 2p and one factor of each product is below p (then a b + c d < 4p^2).
+// Negate one operand (fp_neg_lazy / fp_sub_lazy) to get a difference of products.
+template <class P>
+PB_HD Fp<P> fp_mul2_lazy(const Fp<P>& a, const Fp<P>& b, const Fp<P>& c, const Fp<P>& d) {
+#if !defined(__CUDA_ARCH__) && defined(PB_HOST_FAST_MUL)
+  return fp_add(fp_mul_host64(a, b), fp_mul_host64(c, d));
+#else
+  uint32_t X[8], Y[8], w;
+  fp_cios_step2<P, true>(X, Y, w, a.v, b.v[0], c.v, d.v[0]);
+  fp_cios_step2<P, false>(Y, X, w, a.v, b.v[1], c.v, d.v[1]);
+  fp_cios_step2<P, false>(X, Y, w, a.v, b.v[2], c.v, d.v[2]);
+  fp_cios_step2<P, false>(Y, X, w, a.v, b.v[3], c.v, d.v[3]);
+  fp_cios_step2<P, false>(X, Y, w, a.v, b.v[4], c.v, d.v[4]);
+  fp_cios_step2<P, false>(Y, X, w, a.v, b.v[5], c.v, d.v[5]);
+  fp_cios_step2<P, false>(X, Y, w, a.v, b.v[6], c.v, d.v[6]);
+  fp_cios_step2<P, false>(Y, X, w, a.v, b.v[7], c.v, d.v[7]);
+  return fp_cios_final<P>(X, Y, w);
+#endif
+}
+
+// ---- squaring ----------------------------------------------------------------------------------
+// The 512-bit square T = 2 * sum_{i<j} a_i a_j 2^(32(i+j)) + sum_i a_i^2 2^(64i) (28 + 8 partial products instead of
+// 64), then Montgomery reduction of T.  The off-diagonal products go to two accumulators by the parity of i + j so
+// every product lands on an aligned register pair: E[k] holds weight 2^(32k), O[k] weight 2^(32(k+1)).  Row i
+// (multiplier a_i) is one carry chain into each; where a chain ends below a limb an earlier row wrote, its carry
+// goes one limb up, into a limb no earlier row reached (the schedule is fixed, see the row comments).
+
+// acc[2k..] += x[0] y, x[2] y, ... (n products, pairs at acc, acc + 2, ..); returns with CC.CF = carry out
+PB_HD void fp_sqr_chain(uint32_t* acc, const uint32_t* x, uint32_t y, int n) {
+  acc[0] = mad_lo_cc(x[0], y, acc[0]);
+  acc[1] = madc_hi_cc(x[0], y, acc[1]);
+#pragma unroll
+  for (int k = 1; k < n; k++) {
+    acc[2 * k] = madc_lo_cc(x[2 * k], y, acc[2 * k]);
+    acc[2 * k + 1] = madc_hi_cc(x[2 * k], y, acc[2 * k + 1]);
+  }
+}
+
+// T (16 limbs) = a^2 for a < 2^256
+PB_HD void fp_sqr_wide(uint32_t* T, const uint32_t* a) {
+  uint32_t E[16], O[16];
+#pragma unroll
+  for (int k = 0; k < 16; k++) { E[k] = 0; O[k] = 0; }
+  // row 0: E limbs 2..7, O limbs 0..7 (weights 1..8); both top limbs were 0, no carry out
+  fp_sqr_chain(E + 2, a + 2, a[0], 3);
+  fp_sqr_chain(O + 0, a + 1, a[0], 4);
+  // row 1: E 4..9 (new top); O weights 3..8, carry to weight 9
+  fp_sqr_chain(E + 4, a + 3, a[1], 3);
+  fp_sqr_chain(O + 2, a + 2, a[1], 3);
+  O[8] = addc(0u, 0u);
+  // row 2: E 6..9, carry to 10; O weights 5..10 (new top)
+  fp_sqr_chain(E + 6, a + 4, a[2], 2);
+  E[10] = addc(0u, 0u);
+  fp_sqr_chain(O + 4, a + 3, a[2], 3);
+  // row 3: E 8..11 (new top); O weights 7..10, carry to 11
+  fp_sqr_chain(E + 8, a + 5, a[3], 2);
+  fp_sqr_chain(O + 6, a + 4, a[3], 2);
+  O[10] = addc(0u, 0u);
+  // row 4: E 10..11, carry to 12; O weights 9..12 (new top)
+  fp_sqr_chain(E + 10, a + 6, a[4], 1);
+  E[12] = addc(0u, 0u);
+  fp_sqr_chain(O + 8, a + 5, a[4], 2);
+  // row 5: E 12..13 (new top); O weights 11..12, carry to 13
+  fp_sqr_chain(E + 12, a + 7, a[5], 1);
+  fp_sqr_chain(O + 10, a + 6, a[5], 1);
+  O[12] = addc(0u, 0u);
+  // row 6: O weights 13..14 (new top)
+  fp_sqr_chain(O + 12, a + 7, a[6], 1);
+  // S = E + O (weights 1..15), T = 2 S + diagonal
+  uint32_t S[16];
+  S[0] = 0;
+  S[1] = O[0];
+  S[2] = add_cc(E[2], O[1]);
+#pragma unroll
+  for (int k = 3; k < 14; k++) S[k] = addc_cc(E[k], O[k - 1]);
+  S[14] = addc_cc(O[13], 0u);
+  S[15] = addc(0u, 0u);
+  S[1] = add_cc(S[1], S[1]);
+#pragma unroll
+  for (int k = 2; k < 15; k++) S[k] = addc_cc(S[k], S[k]);
+  S[15] = addc(S[15], S[15]);
+  T[0] = mad_lo_cc(a[0], a[0], 0u);
+  T[1] = madc_hi_cc(a[0], a[0], S[1]);
+#pragma unroll
+  for (int i = 1; i < 7; i++) {
+    T[2 * i] = madc_lo_cc(a[i], a[i], S[2 * i]);
+    T[2 * i + 1] = madc_hi_cc(a[i], a[i], S[2 * i + 1]);
+  }
+  T[14] = madc_lo_cc(a[7], a[7], S[14]);
+  T[15] = madc_hi(a[7], a[7], S[15]);
+}
+
+// One reduction-only CIOS step (no product row): same state and role swap as fp_cios_step.  FIRST starts from
+// U = the value, V = 0.  Otherwise the pending carry (old w != 0) enters the reduction row of U as its carry-in
+// instead of being propagated through U, and the shift of V by one limb pair is plain register renaming.
+template <class P, bool FIRST>
+PB_HD void fp_redc_step(uint32_t* U, uint32_t* V, uint32_t& w) {
+  uint32_t cf = 0;
+  if (FIRST) {
+#pragma unroll
+    for (int j = 0; j < 8; j++) V[j] = 0;
+    w = 0;
+  } else {
+    cf = w != 0;
+    w = V[1];
+#pragma unroll
+    for (int j = 0; j < 6; j++) V[j] = V[j + 2];
+    V[6] = 0;
+    V[7] = 0;
+  }
+  const uint32_t m = mul_lo(U[0] + w + cf, P::NP0);
+  fp_mad_row_mod<P, 1>(V, m);
+  (void)add_cc(cf, 0xffffffffu);  // CF = cf
+  U[0] = madc_lo_cc(P::p(0), m, U[0]);
+  U[1] = madc_hi_cc(P::p(0), m, U[1]);
+#pragma unroll
+  for (int j = 2; j < 8; j += 2) {
+    U[j] = madc_lo_cc(P::p(j), m, U[j]);
+    U[j + 1] = madc_hi_cc(P::p(j), m, U[j + 1]);
+  }
+  V[7] = addc(V[7], 0u);
+}
+
+// a^2 / R mod p, lazy, for a in [0, 2p).  T = a^2 = T_lo + R T_hi; the result is (T_lo + m p) / R + T_hi with
+// (T_lo + m p) / R <= p and T_hi < 4p^2 / R < 0.76 p, so it is below 2p.
+template <class P>
+PB_HD Fp<P> fp_sqr_lazy(const Fp<P>& a) {
+#if !defined(__CUDA_ARCH__) && defined(PB_HOST_FAST_MUL)
+  return fp_mul_host64(a, a);
+#else
+  uint32_t T[16], Y[8], w;
+  fp_sqr_wide(T, a.v);
+  uint32_t* X = T;  // U of the first step: T_lo, reduced in place
+  fp_redc_step<P, true>(X, Y, w);
+  fp_redc_step<P, false>(Y, X, w);
+  fp_redc_step<P, false>(X, Y, w);
+  fp_redc_step<P, false>(Y, X, w);
+  fp_redc_step<P, false>(X, Y, w);
+  fp_redc_step<P, false>(Y, X, w);
+  fp_redc_step<P, false>(X, Y, w);
+  fp_redc_step<P, false>(Y, X, w);
+  Fp<P> r = fp_cios_final<P>(X, Y, w);
+  r.v[0] = add_cc(r.v[0], T[8]);
+#pragma unroll
+  for (int i = 1; i < 7; i++) r.v[i] = addc_cc(r.v[i], T[8 + i]);
+  r.v[7] = addc(r.v[7], T[15]);
+  return r;
+#endif
+}
+
+// a^2: the dedicated squaring, fully reduced (bit-identical to fp_mul(a, a))
+template <class P>
+PB_HD Fp<P> fp_sqr(const Fp<P>& a) {
+  Fp<P> r = fp_sqr_lazy(a);
+  fp_reduce_once(r);
+  return r;
+}
 
 template <class P>
 PB_HD Fp<P> fp_to_mont(const Fp<P>& a) { return fp_mul(a, Fp<P>::r2()); }

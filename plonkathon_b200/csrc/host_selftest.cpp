@@ -35,11 +35,95 @@ int hs_field_op(int field, int op, const uint32_t* a, const uint32_t* b, uint32_
       case 8: r = fp_sqr(x); break;                              \
       case 9: r = fp_inv_gcd(x); break;                          \
       case 10: r = fp_inv_plain_gcd(x); break;                   \
+      case 11: r = fp_mul_lazy(x, y); break;                     \
+      case 12: r = fp_sqr_lazy(x); break;                        \
+      case 13: r = fp_sub_lazy(x, y); break;                     \
+      case 14: r = fp_neg_lazy(x); break;                        \
+      case 15: r = fp_is_zero_lazy(x) ? F::one() : F::zero(); break; \
       default: return -1;                                        \
     }                                                            \
     st(out, r);                                                  \
   }
   if (field == 0) RUN(Fr) else RUN(Fq)
+#undef RUN
+  return 0;
+}
+
+// redc(a b + c d) without the final subtraction (fp_mul2_lazy)
+int hs_field_mul2(int field, const uint32_t* a, const uint32_t* b, const uint32_t* c, const uint32_t* d, uint32_t* out) {
+  if (field == 0) st(out, fp_mul2_lazy(ld<Fr>(a), ld<Fr>(b), ld<Fr>(c), ld<Fr>(d)));
+  else st(out, fp_mul2_lazy(ld<Fq>(a), ld<Fq>(b), ld<Fq>(c), ld<Fq>(d)));
+  return 0;
+}
+}  // extern "C"
+
+// The group law as it was written before the lazily reduced primitives (canonical products, fp_sqr = fp_mul(a, a),
+// two reductions for Y3): the reference the shipped formulas must match limb for limb, since both keep every
+// coordinate they return canonical.
+static Fq ref_sqr(const Fq& a) { return fp_mul(a, a); }
+static void ref_double(G1XYZZ& a) {
+  if (a.is_inf()) return;
+  Fq U = fp_dbl(a.Y), V = ref_sqr(U), W = fp_mul(U, V), S = fp_mul(a.X, V), M = ref_sqr(a.X);
+  M = fp_add(fp_dbl(M), M);
+  Fq X3 = fp_sub(ref_sqr(M), fp_dbl(S));
+  a.Y = fp_sub(fp_mul(M, fp_sub(S, X3)), fp_mul(W, a.Y));
+  a.X = X3;
+  a.ZZ = fp_mul(V, a.ZZ);
+  a.ZZZ = fp_mul(W, a.ZZZ);
+}
+static void ref_add_mixed(G1XYZZ& acc, const G1Affine& p) {
+  if (acc.is_inf()) { acc = g1_from_affine(p); return; }
+  Fq U2 = fp_mul(p.x, acc.ZZ), S2 = fp_mul(p.y, acc.ZZZ), Pd = fp_sub(U2, acc.X), Rd = fp_sub(S2, acc.Y);
+  if (Pd.is_zero()) {
+    if (Rd.is_zero()) { acc = g1_from_affine(p); ref_double(acc); }
+    else acc = G1XYZZ::identity();
+    return;
+  }
+  Fq PP = ref_sqr(Pd), PPP = fp_mul(Pd, PP), Q = fp_mul(acc.X, PP);
+  Fq X3 = fp_sub(fp_sub(ref_sqr(Rd), PPP), fp_dbl(Q));
+  acc.Y = fp_sub(fp_mul(Rd, fp_sub(Q, X3)), fp_mul(acc.Y, PPP));
+  acc.X = X3;
+  acc.ZZ = fp_mul(acc.ZZ, PP);
+  acc.ZZZ = fp_mul(acc.ZZZ, PPP);
+}
+static void ref_add(G1XYZZ& acc, const G1XYZZ& q) {
+  if (q.is_inf()) return;
+  if (acc.is_inf()) { acc = q; return; }
+  Fq U1 = fp_mul(acc.X, q.ZZ), U2 = fp_mul(q.X, acc.ZZ), S1 = fp_mul(acc.Y, q.ZZZ), S2 = fp_mul(q.Y, acc.ZZZ);
+  Fq Pd = fp_sub(U2, U1), Rd = fp_sub(S2, S1);
+  if (Pd.is_zero()) {
+    if (Rd.is_zero()) ref_double(acc);
+    else acc = G1XYZZ::identity();
+    return;
+  }
+  Fq PP = ref_sqr(Pd), PPP = fp_mul(Pd, PP), Q = fp_mul(U1, PP);
+  Fq X3 = fp_sub(fp_sub(ref_sqr(Rd), PPP), fp_dbl(Q));
+  acc.Y = fp_sub(fp_mul(Rd, fp_sub(Q, X3)), fp_mul(S1, PPP));
+  acc.X = X3;
+  acc.ZZ = fp_mul(fp_mul(acc.ZZ, q.ZZ), PP);
+  acc.ZZZ = fp_mul(fp_mul(acc.ZZZ, q.ZZZ), PPP);
+}
+
+extern "C" {
+// hs_curve_op's ops 0, 1, 2, 4, 5 by the reference formulas above (4 and 5 are the same sums as 0 and 1)
+int hs_curve_op_ref(int op, const uint32_t* acc_in, const uint32_t* other, int other_inf, uint32_t* out) {
+  G1XYZZ acc;
+  memcpy(&acc, acc_in, sizeof(acc));
+  if (op == 0 || op == 4) {
+    G1Affine p;
+    memcpy(&p.x, other, 32);
+    memcpy(&p.y, other + 8, 32);
+    if (!other_inf) ref_add_mixed(acc, p);
+  } else if (op == 1 || op == 5) {
+    G1XYZZ q;
+    memcpy(&q, other, sizeof(q));
+    ref_add(acc, q);
+  } else if (op == 2) {
+    ref_double(acc);
+  } else {
+    return -1;
+  }
+  memcpy(out, &acc, sizeof(acc));
   return 0;
 }
 

@@ -252,7 +252,8 @@ __device__ __forceinline__ uint32_t upper_bound_u32(const uint32_t* a, uint32_t 
   return lo;
 }
 
-__global__ void __launch_bounds__(128) k_msm_seg_accumulate(const G1Affine* points, const uint32_t* offsets,
+// (128, 4): at most 128 registers, so 4 blocks fit an SM; unbounded, ptxas takes 134 and only 3 fit
+__global__ void __launch_bounds__(128, 4) k_msm_seg_accumulate(const G1Affine* points, const uint32_t* offsets,
                                                             const uint32_t* sorted, uint32_t nb, uint32_t L,
                                                             G1XYZZ* buckets, G1XYZZ* slots, uint32_t* slot_bucket,
                                                             uint32_t* own_slot) {

@@ -275,29 +275,24 @@ struct SR {
 // acc += p when take (select-based: one instruction stream for all lanes; only P == +-Q branches)
 PB_HD void g1_add_mixed_sel(G1XYZZ& acc, const G1Affine& p, bool take) {
   const bool was_inf = acc.is_inf();
-  Fq U2 = fp_mul(p.x, acc.ZZ);
-  Fq S2 = fp_mul(p.y, acc.ZZZ);
+  Fq U2 = fp_mul_lazy(p.x, acc.ZZ);
+  Fq S2 = fp_mul_lazy(p.y, acc.ZZZ);
   Fq Pd = fp_sub(U2, acc.X);
   Fq Rd = fp_sub(S2, acc.Y);
-  if (take && !was_inf && Pd.is_zero()) {
-    if (Rd.is_zero()) g1_double_affine(acc, p);
+  if (take && !was_inf && fp_is_zero_lazy(Pd)) {
+    if (fp_is_zero_lazy(Rd)) g1_double_affine(acc, p);
     else acc = G1XYZZ::identity();
     return;
   }
-  Fq PP = fp_sqr(Pd);
-  Fq PPP = fp_mul(Pd, PP);
-  Fq Q = fp_mul(acc.X, PP);
-  Fq X3 = fp_sub(fp_sub(fp_sqr(Rd), PPP), fp_dbl(Q));
-  Fq Y3 = fp_sub(fp_mul(Rd, fp_sub(Q, X3)), fp_mul(acc.Y, PPP));
-  Fq ZZ3 = fp_mul(acc.ZZ, PP);
-  Fq ZZZ3 = fp_mul(acc.ZZZ, PPP);
+  G1XYZZ r;
+  g1_add_tail(acc.X, acc.Y, Pd, Rd, acc.ZZ, acc.ZZZ, r);
   const Fq one = Fq::one();
 #pragma unroll
   for (int i = 0; i < 8; i++) {
-    acc.X.v[i] = !take ? acc.X.v[i] : (was_inf ? p.x.v[i] : X3.v[i]);
-    acc.Y.v[i] = !take ? acc.Y.v[i] : (was_inf ? p.y.v[i] : Y3.v[i]);
-    acc.ZZ.v[i] = !take ? acc.ZZ.v[i] : (was_inf ? one.v[i] : ZZ3.v[i]);
-    acc.ZZZ.v[i] = !take ? acc.ZZZ.v[i] : (was_inf ? one.v[i] : ZZZ3.v[i]);
+    acc.X.v[i] = !take ? acc.X.v[i] : (was_inf ? p.x.v[i] : r.X.v[i]);
+    acc.Y.v[i] = !take ? acc.Y.v[i] : (was_inf ? p.y.v[i] : r.Y.v[i]);
+    acc.ZZ.v[i] = !take ? acc.ZZ.v[i] : (was_inf ? one.v[i] : r.ZZ.v[i]);
+    acc.ZZZ.v[i] = !take ? acc.ZZZ.v[i] : (was_inf ? one.v[i] : r.ZZZ.v[i]);
   }
 }
 
