@@ -160,8 +160,13 @@ int pb200_prover_round5(pb200_prover* p, const uint8_t* v, uint8_t* h_w_xy /*2*6
 
 /* The round state the reference keeps on `self` (read by its own sanity asserts, prover.py:108-116, 137-145,
  * 215-219), copied out in canonical form to a device buffer of 2^log_n elements: which = 0 A, 1 B, 2 C, 3 Z, 4 PI
- * (Lagrange values), 5 T1, 6 T2, 7 T3 (coefficients).  Valid after the round that produces them. */
+ * (Lagrange values), 5 T1, 6 T2, 7 T3 (coefficients).  Valid after the round that produces them.  In zero-knowledge
+ * mode which = 5..7 is an error (the blinded pieces have more than 2^log_n coefficients); 0..4 are unchanged. */
 int pb200_prover_read_vector(pb200_prover* p, int which, void* d_out);
+/* Zero-knowledge mode for every later proof of this prover: enable != 0 blinds per PLONK paper (11 scalars).
+ * h_blinders == NULL: fresh scalars from the OS CSPRNG for every proof; otherwise 11 x 32-byte canonical Fr used for
+ * every proof (reproducible tests).  Errors: SRS shorter than n + 6, n < 8, a sharded prover, unreduced blinders. */
+int pb200_prover_set_zk(pb200_prover* p, int enable, const uint8_t* h_blinders);
 /* canonical 768-byte proof of the last rounds run on this prover (Proof.flatten() order, prover.py:18-35) */
 int pb200_prover_serialize(pb200_prover* p, uint8_t* h_proof768);
 

@@ -82,6 +82,7 @@ def _load():
         "pb200_prover_round4": (I, [V, V, V]),
         "pb200_prover_round5": (I, [V, V, V]),
         "pb200_prover_serialize": (I, [V, V]),
+        "pb200_prover_set_zk": (I, [V, I, V]),
         "pb200_g1_combine_partials_host": (I, [V, U, V, P(I)]),
         "pb200_transcript_create": (I, [V, ctypes.c_size_t, P(V)]),
         "pb200_transcript_destroy": (None, [V]),

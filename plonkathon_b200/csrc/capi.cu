@@ -52,6 +52,7 @@ void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c);
 void prover_round4(Prover* P, const Fr& zeta_c);
 void prover_round5(Prover* P, const Fr& v_c);
 void prover_serialize(const Prover* P, uint8_t* out768);
+void prover_set_zk(Prover* P, bool enable, const uint8_t* h_blinders);
 void g1_combine_partials_host(const G1XYZZ* parts, uint32_t count, uint8_t* out_xy, int* is_identity);
 void host_join_bucket_shards(const SR* all, uint32_t world, uint32_t sets, uint32_t nloc, G1XYZZ* out);
 void host_join_bucket_shards_strided(const SR* all, uint32_t world, uint32_t sets, G1XYZZ* out);
@@ -500,11 +501,20 @@ int pb200_prover_read_vector(pb200_prover* p, int which, void* d_out) {
   switch (which) {
     case 0: case 1: case 2: case 3: src = P->lag[which].as<Fr>(); break;   // A B C Z, Lagrange values
     case 4: src = P->pi_lag.as<Fr>(); break;                               // PI, Lagrange values
-    case 5: case 6: case 7: src = P->tq.as<Fr>() + (uint64_t)(which - 5) * P->n; break;  // T1 T2 T3, coefficients
+    case 5: case 6: case 7:  // T1 T2 T3, coefficients
+      PB_CHECK(!P->zk, "T1, T2, T3 are not n-coefficient vectors in zero-knowledge mode (the blinded pieces have n + 1, "
+                       "n + 1 and n + 6 coefficients)");
+      src = P->tq.as<Fr>() + (uint64_t)(which - 5) * P->n;
+      break;
     default: PB_CHECK(false, "unknown prover vector");
   }
   fr_from_mont(P->ctx, src, (Fr*)d_out, P->n);
   PB_CUDA(cudaStreamSynchronize(P->ctx->stream));
+  PB_API_END
+}
+int pb200_prover_set_zk(pb200_prover* p, int enable, const uint8_t* h_blinders) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  prover_set_zk(reinterpret_cast<Prover*>(p), enable != 0, h_blinders);
   PB_API_END
 }
 int pb200_prover_serialize(pb200_prover* p, uint8_t* h_proof768) {

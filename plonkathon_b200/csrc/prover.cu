@@ -17,6 +17,11 @@
 //     (X - zeta*w) are done on an n-point coset (quotient degree n-2 < n).
 // The reference's run-time invariants are kept as checks that fail the call: gate satisfaction
 // (prover.py:108-116), Z_n == 1 (prover.py:132), deg T < 3n (prover.py:205-208).
+// Zero-knowledge mode (prover_set_zk, one GPU) blinds A, B, C, Z and the quotient pieces as in the PLONK paper; the
+// proof keeps its 15 fields and the verifier does not change.  See "zero knowledge" below.
+#include <cerrno>
+#include <sys/random.h>
+
 #include "common.cuh"
 #include "comm.cuh"
 #include "transcript.cuh"
@@ -362,11 +367,25 @@ struct QuotientArgs {
   Fr pi_coef[8];
   CustomTerms custom;                                  // extended custom selectors (this rank's slice)
 };
-__global__ void __launch_bounds__(128) k_quotient(QuotientArgs q, Fr* T) {
+// Zero knowledge: A'(x) = A(x) + (b1 x + b2) Z_H(x) (B', C' likewise), Z'(x) = Z(x) + (b7 x^2 + b8 x + b9) Z_H(x) and
+// Z'(w x) = Z(w x) + (b7 w^2 x^2 + b8 w x + b9) Z_H(x), since Z_H(w x) = Z_H(x).  Z_H takes four values on the coset, so
+// the blinders come pre-multiplied by each of them: w[k] = Z_H class k times
+//   (b1, b2, b3, b4, b5, b6,  b7, b8, b9,  b7 w^2, b8 w, b9)
+// and a point costs 7 products.  A separate parameter after T, so the plain kernel's parameters keep their offsets.
+struct ZkCoset { Fr w[4][12]; };
+template <bool ZK>
+__global__ void __launch_bounds__(128) k_quotient(QuotientArgs q, Fr* T, ZkCoset zk) {
   uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= q.n4) return;
   uint64_t jw = j + q.zw_shift >= q.n4 ? j + q.zw_shift - q.n4 : j + q.zw_shift;
   Fr a = ldg_fr(q.A + j), b = ldg_fr(q.B + j), c = ldg_fr(q.C + j);
+  if constexpr (ZK) {
+    const uint32_t k = (uint32_t)(j * q.world + q.rank) & 3;
+    const Fr x = ldg_fr(q.X + j);
+    a = fp_add(a, fp_add(fp_mul(zk.w[k][0], x), zk.w[k][1]));
+    b = fp_add(b, fp_add(fp_mul(zk.w[k][2], x), zk.w[k][3]));
+    c = fp_add(c, fp_add(fp_mul(zk.w[k][4], x), zk.w[k][5]));
+  }
   Fr gate = fp_mul(a, ldg_fr(q.QL + j));
   gate = fp_add(gate, fp_mul(b, ldg_fr(q.QR + j)));
   gate = fp_add(gate, fp_mul(fp_mul(a, b), ldg_fr(q.QM + j)));
@@ -383,6 +402,12 @@ __global__ void __launch_bounds__(128) k_quotient(QuotientArgs q, Fr* T) {
   Fr bx = fp_mul(q.beta, ldg_fr(q.X + j));
   Fr bx2 = fp_dbl(bx), bx3 = fp_add(bx2, bx);
   Fr z = ldg_fr(q.Z + j), zw = ldg_fr(q.Zw + jw);
+  if constexpr (ZK) {
+    const uint32_t k = (uint32_t)(j * q.world + q.rank) & 3;
+    const Fr x = ldg_fr(q.X + j);
+    z = fp_add(z, fp_add(fp_mul(fp_add(fp_mul(zk.w[k][6], x), zk.w[k][7]), x), zk.w[k][8]));
+    zw = fp_add(zw, fp_add(fp_mul(fp_add(fp_mul(zk.w[k][9], x), zk.w[k][10]), x), zk.w[k][11]));
+  }
   Fr p1 = fp_mul(fp_mul(fp_mul(fp_add(ag, bx), fp_add(bg, bx2)), fp_add(cg, bx3)), z);
   Fr p2 = fp_mul(fp_mul(fp_mul(fp_add(ag, fp_mul(q.beta, ldg_fr(q.S1 + j))), fp_add(bg, fp_mul(q.beta, ldg_fr(q.S2 + j)))),
                         fp_add(cg, fp_mul(q.beta, ldg_fr(q.S3 + j)))),
@@ -445,6 +470,18 @@ __global__ void k_scale_by4(Fr* v, uint64_t n4, Four m, uint32_t world, uint32_t
 __global__ void k_negate(Fr* v, uint64_t n) {
   uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j < n) v[j] = fp_neg(v[j]);
+}
+
+// One blinded coefficient vector: out[k] = (k < n_in ? in[k] : 0) + lo[k] (k < 3) + hi[k - n] (n <= k < n + 3),
+// k < n_out.  With n >= 8 the two patches never meet.
+struct ZkPatch { Fr lo[3], hi[3]; };
+__global__ void k_zk_blind(const Fr* in, uint64_t n_in, uint64_t n, ZkPatch p, uint64_t n_out, Fr* out) {
+  uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n_out) return;
+  Fr v = k < n_in ? ldg_fr(in + k) : Fr::zero();
+  if (k < 3) v = fp_add(v, p.lo[k]);
+  else if (k >= n && k < n + 3) v = fp_add(v, p.hi[k - n]);
+  out[k] = v;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -533,6 +570,7 @@ Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h
   Fr cur = gn;
   for (int k = 0; k < 4; k++) {
     zh.v[k] = fp_sub(cur, one);
+    P->zh[k] = zh.v[k];
     P->zh_inv[k] = fp_inv(zh.v[k]);
     cur = fp_mul(cur, i4);
   }
@@ -636,6 +674,106 @@ static void store_canonical(uint8_t* dst, const Fr& mont) {
   memcpy(dst, c.v, 32);
 }
 
+// ---- zero knowledge -----------------------------------------------------------------------------------------------
+// The blinding of the PLONK paper (eprint 2019/953, prover rounds 1-3), b1..b11 = zk_b[0..10], Z_H = X^n - 1:
+//   A' = A + (b1 X + b2) Z_H,  B' = B + (b3 X + b4) Z_H,  C' = C + (b5 X + b6) Z_H,  Z' = Z + (b7 X^2 + b8 X + b9) Z_H,
+//   T = (gate + alpha perm + alpha^2 L0 (Z' - 1)) / Z_H of degree <= 3n + 5, cut at n and 2n, then
+//   T1' = T1 + b10 X^n,  T2' = T2 - b10 + b11 X^n,  T3' = T3 - b11   (T1' + X^n T2' + X^2n T3' = T).
+// On H every blinded polynomial equals the unblinded one, so rounds 1-2 check the same witness; commitments, openings
+// and round 5 use the blinded polynomials, evaluations are corrected on the host.  The verifier does not change.
+
+// Fresh blinders from the OS CSPRNG: 64 bytes per scalar, reduced mod r (bias below 2^-250).  No other source: a failed
+// read fails the proof.
+static void zk_random_blinders(Fr* out_mont, int count) {
+  std::vector<uint8_t> buf((size_t)count * 64);
+  size_t got = 0;
+  while (got < buf.size()) {
+    ssize_t r = getrandom(buf.data() + got, buf.size() - got, 0);
+    if (r < 0) {
+      PB_CHECK(errno == EINTR, "zero-knowledge blinders: getrandom() failed (no fallback source is used)");
+      continue;
+    }
+    got += (size_t)r;
+  }
+  const Fr m = Fr::modulus();
+  auto reduce = [&](Fr x) {  // x < 2^256 < 6 r: subtract r while x >= r
+    for (;;) {
+      bool ge = true;
+      for (int i = 7; i >= 0; i--)
+        if (x.v[i] != m.v[i]) { ge = x.v[i] > m.v[i]; break; }
+      if (!ge) return x;
+      uint64_t borrow = 0;
+      for (int i = 0; i < 8; i++) {
+        uint64_t d = (uint64_t)x.v[i] - m.v[i] - borrow;
+        x.v[i] = (uint32_t)d;
+        borrow = (d >> 32) & 1;
+      }
+    }
+  };
+  for (int k = 0; k < count; k++) {
+    Fr lo, hi;
+    memcpy(lo.v, buf.data() + 64 * k, 32);
+    memcpy(hi.v, buf.data() + 64 * k + 32, 32);
+    // lo + hi 2^256 mod r: fp_to_mont(hi) = hi R mod r with R = 2^256, and the sum is canonical
+    Fr v = fp_add(reduce(lo), fp_to_mont(reduce(hi)));
+    out_mont[k] = fp_to_mont(v);
+  }
+  std::fill(buf.begin(), buf.end(), 0);
+}
+
+void prover_set_zk(Prover* P, bool enable, const uint8_t* h_blinders) {
+  if (!enable) {
+    P->zk = P->zk_fixed = false;
+    for (auto& b : P->zk_coeff) b.release();
+    for (auto& b : P->zk_t) b.release();
+    return;
+  }
+  PB_CHECK(P->world == 1, "zero-knowledge proving is not available on the sharded prover (one GPU only)");
+  PB_CHECK(P->n >= 8, "zero-knowledge proving needs n >= 8 rows: the blinded quotient has degree 3n + 5 < 4n");
+  PB_CHECK(srs_size(P->srs) >= P->n + 6,
+           "Not enough powers in setup: zero-knowledge proving needs n + 6 powers (T3' has n + 6 coefficients)");
+  if (h_blinders) {
+    const Fr m = Fr::modulus();
+    for (int k = 0; k < Prover::ZK_BLINDERS; k++) {
+      Fr b;
+      memcpy(b.v, h_blinders + 32 * k, 32);
+      bool lt = false;
+      for (int i = 7; i >= 0; i--)
+        if (b.v[i] != m.v[i]) { lt = b.v[i] < m.v[i]; break; }
+      PB_CHECK(lt, "zero-knowledge blinder not reduced below the field modulus");
+      P->zk_fixed_b[k] = b;
+    }
+  }
+  const size_t bytes = (P->n + Prover::ZK_PAD) * 32;
+  for (auto& b : P->zk_coeff) b.ensure(bytes);
+  for (auto& b : P->zk_t) b.ensure(bytes);
+  for (auto& b : P->tmp) b.ensure(bytes);  // round 5 works on n + 8 coefficients
+  P->zk_fixed = h_blinders != nullptr;
+  P->zk = true;
+}
+
+static void zk_draw_blinders(Prover* P) {
+  if (P->zk_fixed) {
+    for (int k = 0; k < Prover::ZK_BLINDERS; k++) P->zk_b[k] = fp_to_mont(P->zk_fixed_b[k]);
+  } else {
+    zk_random_blinders(P->zk_b, Prover::ZK_BLINDERS);
+  }
+}
+
+// out (n + 8, zero padded) = in (n_in coefficients) + c(X) Z_H(X) with c = c[0] + c[1] X + ... (deg < 3)
+static void zk_blind(Prover* P, const Fr* in, uint64_t n_in, const ZkPatch& p, Fr* out) {
+  const uint64_t len = P->n + Prover::ZK_PAD;
+  k_zk_blind<<<PB_GRID(len, 256), 0, P->ctx->stream>>>(in, n_in, P->n, p, len, out);
+  P->ctx->launches++;
+}
+static ZkPatch zh_multiple(std::initializer_list<Fr> c) {
+  ZkPatch p;
+  for (int i = 0; i < 3; i++) p.lo[i] = p.hi[i] = Fr::zero();
+  int i = 0;
+  for (const Fr& x : c) { p.lo[i] = fp_neg(x); p.hi[i] = x; i++; }
+  return p;
+}
+
 // cached per prover: basis_i[j] = L_i(x_j) on the fixed coset for the first `count` rows
 static void ensure_pi_basis(Prover* P, int count) {
   Context* ctx = P->ctx;
@@ -668,6 +806,7 @@ void prover_round1(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_
   const uint64_t n = P->n;
   cudaStream_t st = ctx->stream;
   PB_CHECK(n_public <= n, "more public inputs than rows");
+  if (P->zk) zk_draw_blinders(P);  // here, so the whole-proof call and the round-by-round path behave alike
   if (ctx->aux_stream) {
     // a previous proof that failed a check may have left coset extensions running on the side stream: everything
     // this proof writes is ordered after them
@@ -749,6 +888,14 @@ void prover_round1(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_
   PB_CHECK(fl[1] == 0, "wire value not reduced below the field modulus (canonical 32-byte little-endian expected)");
   PB_CHECK(fl[0] == 0, "AssertionError: witness does not satisfy the gate constraints (prover.py:108-116)");
   if (P->overlap) launch_coset_ext_async(P, 0, 3, 0);
+  if (P->zk) {  // A' B' C': n + 2 coefficients
+    const Fr* b = P->zk_b;
+    for (int k = 0; k < 3; k++)
+      zk_blind(P, P->coeff[k].as<Fr>(), n, zh_multiple({b[2 * k + 1], b[2 * k]}), P->zk_coeff[k].as<Fr>());
+    const Fr* abc[3] = {P->zk_coeff[0].as<Fr>(), P->zk_coeff[1].as<Fr>(), P->zk_coeff[2].as<Fr>()};
+    P->commit_batch(abc, 3, n + 2, P->proof.pts[0]);
+    return;
+  }
   const Fr* abc[3] = {P->coeff[0].as<Fr>(), P->coeff[1].as<Fr>(), P->coeff[2].as<Fr>()};
   P->commit_batch(abc, 3, n, P->proof.pts[0]);
 }
@@ -803,6 +950,12 @@ void prover_round2(Prover* P, const Fr& beta_c, const Fr& gamma_c) {
   PB_CUDA(cudaStreamSynchronize(st));
   PB_CHECK(total == Fr::one(), "AssertionError: permutation grand product does not close, Z_n != 1 (prover.py:132)");
   if (P->overlap) launch_coset_ext_async(P, 3, 1, 1);
+  if (P->zk) {  // Z': n + 3 coefficients
+    const Fr* b = P->zk_b;
+    zk_blind(P, P->coeff[3].as<Fr>(), n, zh_multiple({b[8], b[7], b[6]}), P->zk_coeff[3].as<Fr>());
+    P->commit(P->zk_coeff[3].as<Fr>(), n + 3, P->proof.pts[3]);
+    return;
+  }
   P->commit(P->coeff[3].as<Fr>(), n, P->proof.pts[3]);
 }
 
@@ -840,7 +993,17 @@ void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c) {
   q.alpha = P->alpha; q.alpha2 = fp_sqr(P->alpha); q.beta = P->beta; q.gamma = P->gamma; q.one = Fr::one();
   q.n4 = ne;
   Fr* t_evals = P->world > 1 ? P->tq_loc.as<Fr>() : P->tq.as<Fr>();
-  k_quotient<<<PB_GRID(ne, 128), 0, st>>>(q, t_evals);
+  ZkCoset zk{};
+  if (P->zk) {
+    const Fr* b = P->zk_b;
+    const Fr w = fr_root_of_unity(P->log_n);
+    const Fr per[12] = {b[0], b[1], b[2], b[3], b[4], b[5], b[6], b[7], b[8], fp_mul(b[6], fp_sqr(w)), fp_mul(b[7], w), b[8]};
+    for (int k = 0; k < 4; k++)
+      for (int i = 0; i < 12; i++) zk.w[k][i] = fp_mul(per[i], P->zh[k]);
+    k_quotient<true><<<PB_GRID(ne, 128), 0, st>>>(q, t_evals, zk);
+  } else {
+    k_quotient<false><<<PB_GRID(ne, 128), 0, st>>>(q, t_evals, zk);
+  }
   ctx->launches++;
   PB_CUDA(cudaMemsetAsync(P->flags.p, 0, 64, st));
   if (P->world > 1) {
@@ -853,8 +1016,22 @@ void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c) {
   } else {
     // back to coefficients: ifft(4n) then * g^-i (poly.py:169-177 with the fixed coset)
     ntt_run(ctx, P->tq.as<Fr>(), P->tq.as<Fr>(), P->log_n + 2, true, n4, nullptr, P->ginv_pow.as<Fr>());
-    k_count_nonzero<<<PB_GRID(n, 256), 0, st>>>(P->tq.as<Fr>() + 3 * n, n, P->flags.as<uint32_t>());
+    const uint64_t top = P->zk ? 3 * n + 6 : 3 * n;  // zero knowledge: deg T <= 3n + 5
+    k_count_nonzero<<<PB_GRID(n4 - top, 256), 0, st>>>(P->tq.as<Fr>() + top, n4 - top, P->flags.as<uint32_t>());
     ctx->launches++;
+  }
+  if (P->zk) {
+    PB_CHECK(read_flag(P, 0) == 0,
+             "AssertionError: quotient has degree >= 3n + 6 (zero-knowledge mode; prover.py:205-208)");
+    // the pieces overlap in tq once blinded (T1' reaches X^n), so each gets its own buffer; one commitment pass
+    const Fr* t = P->tq.as<Fr>();
+    const Fr b10 = P->zk_b[9], b11 = P->zk_b[10], zero = Fr::zero();
+    zk_blind(P, t, n, ZkPatch{{zero, zero, zero}, {b10, zero, zero}}, P->zk_t[0].as<Fr>());
+    zk_blind(P, t + n, n, ZkPatch{{fp_neg(b10), zero, zero}, {b11, zero, zero}}, P->zk_t[1].as<Fr>());
+    zk_blind(P, t + 2 * n, n + 6, ZkPatch{{fp_neg(b11), zero, zero}, {zero, zero, zero}}, P->zk_t[2].as<Fr>());
+    const Fr* t123[3] = {P->zk_t[0].as<Fr>(), P->zk_t[1].as<Fr>(), P->zk_t[2].as<Fr>()};
+    P->commit_batch(t123, 3, n + 6, P->proof.pts[4]);
+    return;
   }
   PB_CHECK(read_flag(P, 0) == 0, "AssertionError: quotient has degree >= 3n (prover.py:205-208)");
   const Fr* t123[3] = {P->tq.as<Fr>(), P->tq.as<Fr>() + n, P->tq.as<Fr>() + 2 * n};
@@ -871,6 +1048,14 @@ void prover_round4(Prover* P, const Fr& zeta_c) {
   Fr xs[7] = {P->zeta, P->zeta, P->zeta, P->zeta, P->zeta, zw, P->zeta};
   Fr out[7];
   eval_polys(P, P->pi_sparse ? 6 : 7, polys, xs, out);
+  if (P->zk) {
+    // the blinded polynomials at their points: A'(zeta) = A(zeta) + (b1 zeta + b2)(zeta^n - 1), ...,
+    // Z'(zeta w) = Z(zeta w) + (b7 (zeta w)^2 + b8 zeta w + b9)(zeta^n - 1)
+    const Fr* b = P->zk_b;
+    const Fr zh = fp_sub(fp_pow_u64(P->zeta, P->n), Fr::one());
+    for (int k = 0; k < 3; k++) out[k] = fp_add(out[k], fp_mul(fp_add(fp_mul(b[2 * k], P->zeta), b[2 * k + 1]), zh));
+    out[5] = fp_add(out[5], fp_mul(fp_add(fp_mul(fp_add(fp_mul(b[6], zw), b[7]), zw), b[8]), zh));
+  }
   for (int k = 0; k < 6; k++) { P->ev[k] = out[k]; store_canonical(P->proof.evals[k], out[k]); }
   if (P->pi_sparse) {
     // PI(zeta) = sum_i (-pub_i) w^i (zeta^n - 1) / (n (zeta - w^i)), one shared inversion (host arithmetic)
@@ -903,9 +1088,11 @@ void prover_round4(Prover* P, const Fr& zeta_c) {
 // divides the slab of coefficients [r n/G, (r+1) n/G) -- `num` needs to be valid on that slab only --; the slab sums
 // are exchanged with a 32-byte allgather (the sums of the slabs above are the slab's carry), the quotient slabs with
 // one bulk allgather, so every rank ends up with the full quotient for its share of the commitment.
-static void divide_linear(Prover* P, const Fr* num, Fr* out, const Fr& point, Fr* pow_buf, Fr* invpow_buf) {
+// len: coefficients of num (P->n, or n + 8 for the blinded numerators of zero-knowledge mode, which runs on one device)
+static void divide_linear(Prover* P, const Fr* num, Fr* out, const Fr& point, Fr* pow_buf, Fr* invpow_buf,
+                          uint64_t len) {
   Context* ctx = P->ctx;
-  const uint64_t n = P->n / (uint64_t)P->world, lo = n * (uint64_t)P->rank;
+  const uint64_t n = len / (uint64_t)P->world, lo = n * (uint64_t)P->rank;
   cudaStream_t st = ctx->stream;
   const Fr point_inv = fp_inv(point);
   launch_powers(ctx, pow_buf + lo, n, point, fp_pow_u64(point, lo));
@@ -953,9 +1140,21 @@ void prover_round5(Prover* P, const Fr& v_c) {
   Fr al2l0 = fp_mul(fp_sqr(al), l0_ev);
   Fr v2 = fp_sqr(v), v3 = fp_mul(v2, v), v4 = fp_sqr(v2), v5 = fp_mul(v4, v);
   // W_z numerator = R + v(A - a) + v^2(B - b) + v^3(C - c) + v^4(S1 - s1) + v^5(S2 - s2), R per SURVEY App. D
-  LinCombArgs L;
+  // zero knowledge: Z, T1..T3, A, B, C are the blinded vectors (n + 8 coefficients, zero padded); coefficients [n, n + 8)
+  // of the numerator come from those alone (tail)
+  const bool zk = P->zk;
+  const Fr* wire[3];
+  for (int i = 0; i < 3; i++) wire[i] = zk ? P->zk_coeff[i].as<Fr>() : P->coeff[i].as<Fr>();
+  const Fr* zpoly = zk ? P->zk_coeff[3].as<Fr>() : P->coeff[3].as<Fr>();
+  const Fr* tpiece[3];
+  for (int i = 0; i < 3; i++) tpiece[i] = zk ? P->zk_t[i].as<Fr>() : P->tq.as<Fr>() + (uint64_t)i * n;
+  LinCombArgs L, tail;
   int k = 0;
-  auto add = [&](const Fr* vec, const Fr& w) { L.vec[k] = vec; L.w[k] = w; k++; };
+  tail.count = 0;
+  auto add = [&](const Fr* vec, const Fr& w, bool blinded = false) {
+    L.vec[k] = vec; L.w[k] = w; k++;
+    if (blinded) { tail.vec[tail.count] = vec; tail.w[tail.count] = w; tail.count++; }
+  };
   add(P->sel_coeff[Prover::QL].as<Fr>(), a);
   add(P->sel_coeff[Prover::QR].as<Fr>(), b);
   add(P->sel_coeff[Prover::QM].as<Fr>(), fp_mul(a, b));
@@ -963,14 +1162,14 @@ void prover_round5(Prover* P, const Fr& v_c) {
   add(P->sel_coeff[Prover::QC].as<Fr>(), one);
   for (int t = 0; t < P->n_custom; t++)                                // m_t(a, b, c) Q_t
     add(P->sel_coeff[Prover::CUSTOM0 + t].as<Fr>(), custom_monomial(a, b, c, P->custom_f[t]));
-  add(P->coeff[3].as<Fr>(), fp_add(c1, al2l0));                        // Z
+  add(zpoly, fp_add(c1, al2l0), true);                                 // Z
   add(P->sel_coeff[Prover::S3].as<Fr>(), fp_neg(fp_mul(c2, be)));
-  add(P->tq.as<Fr>(), fp_neg(zh_ev));                                  // T1
-  add(P->tq.as<Fr>() + n, fp_neg(fp_mul(zh_ev, zn)));                  // T2
-  add(P->tq.as<Fr>() + 2 * n, fp_neg(fp_mul(zh_ev, fp_sqr(zn))));      // T3
-  add(P->coeff[0].as<Fr>(), v);
-  add(P->coeff[1].as<Fr>(), v2);
-  add(P->coeff[2].as<Fr>(), v3);
+  add(tpiece[0], fp_neg(zh_ev), true);                                 // T1
+  add(tpiece[1], fp_neg(fp_mul(zh_ev, zn)), true);                     // T2
+  add(tpiece[2], fp_neg(fp_mul(zh_ev, fp_sqr(zn))), true);             // T3
+  add(wire[0], v, true);
+  add(wire[1], v2, true);
+  add(wire[2], v3, true);
   add(P->sel_coeff[Prover::S1].as<Fr>(), v4);
   add(P->sel_coeff[Prover::S2].as<Fr>(), v5);
   L.count = k;
@@ -989,21 +1188,30 @@ void prover_round5(Prover* P, const Fr& v_c) {
   PB_CUDA(cudaMemsetAsync(P->flags.p, 0, 64, st));
   k_lincomb<<<PB_GRID(L.n, 128), 0, st>>>(L, wz);
   ctx->launches++;
+  const uint64_t len = zk ? n + Prover::ZK_PAD : n;  // numerator coefficients
+  if (zk) {
+    tail.c0 = Fr::zero();
+    tail.n = Prover::ZK_PAD;
+    tail.first = n;
+    k_lincomb<<<PB_GRID(tail.n, 128), 0, st>>>(tail, wz);
+    ctx->launches++;
+  }
   Fr* wz_q = P->tmp[1].as<Fr>();
-  divide_linear(P, wz, wz_q, zeta, P->tmp[2].as<Fr>(), P->tmp[3].as<Fr>());
+  divide_linear(P, wz, wz_q, zeta, P->tmp[2].as<Fr>(), P->tmp[3].as<Fr>(), len);
   // W_zw numerator = Z - z_shifted_eval
   LinCombArgs M;
-  M.vec[0] = P->coeff[3].as<Fr>(); M.w[0] = one; M.count = 1; M.c0 = fp_neg(zw);
-  M.n = L.n; M.first = L.first;
+  M.vec[0] = zpoly; M.w[0] = one; M.count = 1; M.c0 = fp_neg(zw);
+  M.n = zk ? len : L.n; M.first = L.first;
   Fr* wzw = P->tmp[0].as<Fr>();  // the W_z numerator is no longer needed
   k_lincomb<<<PB_GRID(M.n, 128), 0, st>>>(M, wzw);
   ctx->launches++;
   Fr* wzw_q = P->tmp[4].as<Fr>();
-  divide_linear(P, wzw, wzw_q, fp_mul(zeta, fr_root_of_unity(P->log_n)), P->tmp[2].as<Fr>(), P->tmp[3].as<Fr>());
+  divide_linear(P, wzw, wzw_q, fp_mul(zeta, fr_root_of_unity(P->log_n)), P->tmp[2].as<Fr>(), P->tmp[3].as<Fr>(), len);
   PB_CHECK(read_flag(P, 0) == 0,
            "AssertionError: opening numerator is not divisible by (X - point) (prover.py:267,288,299)");
   const Fr* ws[2] = {wz_q, wzw_q};
-  P->commit_batch(ws, 2, n, P->proof.pts[7]);
+  // zero knowledge: W_z has n + 5 coefficients (numerator n + 6), W_zw n + 2; the rest of the buffers is zero
+  P->commit_batch(ws, 2, zk ? n + 5 : n, P->proof.pts[7]);
 }
 
 // canonical 768-byte proof: Proof.flatten() order (prover.py:18-35), G1 as x||y, every integer 32-byte

@@ -83,6 +83,7 @@ struct Prover {
   DevBuf xs;             // x_j, j < n_ext
   DevBuf l0_ext;         // L0 on the slice
   Fr g, g_inv, zh_inv[4];
+  Fr zh[4];              // Z_H(x_j) = x_j^n - 1 for j mod 4 (Montgomery)
   // per-proof state
   DevBuf lag[4];         // A B C Z Lagrange
   DevBuf coeff[5];       // a b c z pi coefficients
@@ -102,6 +103,16 @@ struct Prover {
   bool pi_sparse = false;
   std::vector<DevBuf> pi_basis;   // L_i on the slice (n_ext each), i < 8
   std::vector<Fr> pub_neg;        // -public_i, Montgomery (host)
+  // Zero knowledge (one GPU only): the blinding of the PLONK paper with 11 scalars b1..b11 per proof.  The unblinded
+  // n-coefficient vectors above stay as they are (the coset extensions read them; k_quotient adds the Z_H multiples);
+  // the blinded vectors, which are longer than n, live in their own zero-padded buffers of n + 8 elements.
+  static const int ZK_BLINDERS = 11, ZK_PAD = 8;
+  bool zk = false;
+  bool zk_fixed = false;          // the same blinders for every proof (zk_fixed_b) instead of fresh OS randomness
+  Fr zk_fixed_b[ZK_BLINDERS];     // canonical
+  Fr zk_b[ZK_BLINDERS];           // this proof's b1..b11, Montgomery (drawn when round 1 starts)
+  DevBuf zk_coeff[4];             // A' B' C' (n + 2 coefficients) Z' (n + 3)
+  DevBuf zk_t[3];                 // T1' T2' (n + 1 coefficients) T3' (n + 6)
   Proof proof;
 
   enum { QM = 0, QL, QR, QO, QC, S1, S2, S3, CUSTOM0 };

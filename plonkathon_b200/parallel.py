@@ -130,6 +130,12 @@ class ShardedProver(Prover):
         init_comm(setup.ctx, group)
         super().__init__(setup, program)
 
+    def set_zk(self, enable: bool = True, blinders=None):
+        """Zero-knowledge proving runs on one GPU only (``Prover.set_zk``)."""
+        if enable:
+            raise ValueError("zero-knowledge proving is not available on the sharded prover (one GPU only)")
+        super().set_zk(False)
+
 
 # ------------------------------------------------------------------------------------------------
 # operators (BASELINE.json metric: Fr-NTT elems/s and G1-MSM pts/s at 1/2/4/8 GPUs)

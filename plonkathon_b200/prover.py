@@ -258,9 +258,33 @@ class Prover:
     PI = property(lambda self: self._state(4, Basis.LAGRANGE), doc="prover.py:57-63 (after round_1)")
     # T1, T2, T3 are Lagrange-basis Polynomials in the reference (prover.py:209-219): the forward transform of the
     # three coefficient thirds the library keeps (after round_3)
-    T1 = property(lambda self: self._state(5, Basis.MONOMIAL).fft(ctx=self.ctx))
-    T2 = property(lambda self: self._state(6, Basis.MONOMIAL).fft(ctx=self.ctx))
-    T3 = property(lambda self: self._state(7, Basis.MONOMIAL).fft(ctx=self.ctx))
+    def _piece(self, which: int, name: str):
+        if getattr(self, "zk", False):
+            raise RuntimeError("%s is not available in zero-knowledge mode: the blinded quotient pieces have n + 1, "
+                               "n + 1 and n + 6 coefficients, so they have no n-value Lagrange form" % name)
+        return self._state(which, Basis.MONOMIAL).fft(ctx=self.ctx)
+
+    T1 = property(lambda self: self._piece(5, "T1"))
+    T2 = property(lambda self: self._piece(6, "T2"))
+    T3 = property(lambda self: self._piece(7, "T3"))
+
+    # ------------------------------------------------------------------ zero knowledge
+    def set_zk(self, enable: bool = True, blinders=None):
+        """Zero-knowledge mode for every later proof: A, B, C, Z and the quotient pieces are blinded as in the PLONK
+        paper (eprint 2019/953), with 11 scalars b1..b11 per proof.  The proof keeps its 768 bytes and the verifier does
+        not change.  ``blinders=None``: fresh scalars from the OS CSPRNG for every proof; otherwise 11 integers in
+        [0, r) used for every proof (reproducible tests only: fixed blinders reveal the witness to whoever knows them).
+        Needs n >= 8 and an SRS of at least n + 6 powers; the sharded prover has no zero-knowledge mode."""
+        raw = None
+        if enable and blinders is not None:
+            blinders = [int(b) for b in blinders]
+            if len(blinders) != 11:
+                raise ValueError("zero knowledge takes 11 blinders b1..b11, got %d" % len(blinders))
+            if any(not 0 <= b < CURVE_ORDER for b in blinders):
+                raise ValueError("zero-knowledge blinders must lie in [0, r)")
+            raw = b"".join(b.to_bytes(32, "little") for b in blinders)
+        _lib.check(_lib.lib().pb200_prover_set_zk(self._h, 1 if enable else 0, raw))
+        self.zk = bool(enable)
 
     def _commitments(self, first_slot: int, count: int, raw: bytes):
         """commitments a round produced"""
