@@ -170,6 +170,26 @@ int pb200_prover_set_zk(pb200_prover* p, int enable, const uint8_t* h_blinders);
 /* canonical 768-byte proof of the last rounds run on this prover (Proof.flatten() order, prover.py:18-35) */
 int pb200_prover_serialize(pb200_prover* p, uint8_t* h_proof768);
 
+/* Lookups: a plookup argument over one fixed table of three columns.  Called once, before the first proof.
+ * h_qk: n x 32 bytes, q_K in {0, 1} per row; h_t1..h_t3: table_rows x 32 bytes each (canonical LE), 1 <= table_rows
+ * <= n, padded to n by repeating the last row.  A row with q_K = 1 claims that (a, b, c) is a row of the table.
+ * Errors: malformed input, a sharded prover, a prover in zero-knowledge mode, a second call.
+ * On a lookup prover pb200_prover_prove, _prove_device, _serialize, _round2 and _round4 return an error: a proof has
+ * 13 points and 12 scalars (1216 bytes) and is made by the entry points below.  Round 1, 3 and 5 are unchanged. */
+int pb200_prover_set_lookup(pb200_prover* p, const uint8_t* h_qk, const uint8_t* h_t1, const uint8_t* h_t2,
+                            const uint8_t* h_t3, uint64_t table_rows);
+/* step 1L, after round 1 and the challenge eta: commitments f_1 h1_1 h2_1 */
+int pb200_prover_round_lookup(pb200_prover* p, const uint8_t* eta, uint8_t* h_fh_xy /*3*64*/);
+/* round 2 with the lookup challenges: commitments z_1 z2_1 */
+int pb200_prover_round2_lookup(pb200_prover* p, const uint8_t* beta, const uint8_t* gamma, const uint8_t* delta,
+                               const uint8_t* epsilon, uint8_t* h_zz2_xy /*2*64*/);
+/* round 4: the 6 plain evaluations, then f, t, t(zeta w), h2, h1(zeta w), z2(zeta w) */
+int pb200_prover_round4_lookup(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals /*12*32*/);
+/* the whole proof: 768 plain bytes, then f_1 h1_1 h2_1 z2_1, then the six lookup evaluations (1216 bytes) */
+int pb200_prover_prove_lookup(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
+                              const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof1216);
+int pb200_prover_serialize_lookup(pb200_prover* p, uint8_t* h_proof1216);
+
 /* ---- multi-GPU: one process per GPU, one communicator per context (SURVEY.md 8(e)) -------------------------
  * The library issues its data-path collectives itself, on the context's stream, through NCCL (bound at run time
  * from the libnccl.so.2 the process has loaded; the single-GPU entry points work without it).  Rendezvous stays

@@ -83,6 +83,12 @@ def _load():
         "pb200_prover_round5": (I, [V, V, V]),
         "pb200_prover_serialize": (I, [V, V]),
         "pb200_prover_set_zk": (I, [V, I, V]),
+        "pb200_prover_set_lookup": (I, [V, V, V, V, V, U64]),
+        "pb200_prover_round_lookup": (I, [V, V, V]),
+        "pb200_prover_round2_lookup": (I, [V, V, V, V, V, V]),
+        "pb200_prover_round4_lookup": (I, [V, V, V]),
+        "pb200_prover_prove_lookup": (I, [V, V, V, V, V, U64, V]),
+        "pb200_prover_serialize_lookup": (I, [V, V]),
         "pb200_g1_combine_partials_host": (I, [V, U, V, P(I)]),
         "pb200_transcript_create": (I, [V, ctypes.c_size_t, P(V)]),
         "pb200_transcript_destroy": (None, [V]),

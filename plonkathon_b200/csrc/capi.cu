@@ -53,6 +53,13 @@ void prover_round4(Prover* P, const Fr& zeta_c);
 void prover_round5(Prover* P, const Fr& v_c);
 void prover_serialize(const Prover* P, uint8_t* out768);
 void prover_set_zk(Prover* P, bool enable, const uint8_t* h_blinders);
+void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* const* h_tab, uint64_t rows);
+void prover_round_lookup(Prover* P, const Fr& eta_c);
+void prover_round2_lookup(Prover* P, const Fr& beta_c, const Fr& gamma_c, const Fr& delta_c, const Fr& epsilon_c);
+void prover_round4_lookup(Prover* P, const Fr& zeta_c);
+void prover_prove_lookup(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t* hC, const uint8_t* h_public,
+                         uint64_t n_public, uint8_t* out1216);
+void prover_serialize_lookup(const Prover* P, uint8_t* out1216);
 void g1_combine_partials_host(const G1XYZZ* parts, uint32_t count, uint8_t* out_xy, int* is_identity);
 void host_join_bucket_shards(const SR* all, uint32_t world, uint32_t sets, uint32_t nloc, G1XYZZ* out);
 void host_join_bucket_shards_strided(const SR* all, uint32_t world, uint32_t sets, G1XYZZ* out);
@@ -76,6 +83,10 @@ static thread_local std::string g_err;
   }
 
 static Context* C(pb200_ctx* c) { return reinterpret_cast<Context*>(c); }
+
+// the 768-byte entry points (and the plain round 2 / round 4) on a prover with a lookup table
+#define PB_NOT_LOOKUP(P, entry)                                                                       \
+  PB_CHECK(!(P)->lk, "this prover has a lookup argument: its proofs have 1216 bytes; use " entry)
 
 // Every entry point that touches the GPU runs on its context's device, whatever device the calling host thread had
 // current (contexts on several GPUs in one process, provers driven from worker threads); the previous device is
@@ -447,12 +458,14 @@ void pb200_prover_destroy(pb200_prover* p) { prover_destroy(reinterpret_cast<Pro
 int pb200_prover_prove(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                        const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof768) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  PB_NOT_LOOKUP(reinterpret_cast<Prover*>(p), "pb200_prover_prove_lookup");
   prover_prove(reinterpret_cast<Prover*>(p), h_A, h_B, h_C, h_public, n_public, h_proof768, false);
   PB_API_END
 }
 int pb200_prover_prove_device(pb200_prover* p, const void* d_A, const void* d_B, const void* d_C,
                               const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof768) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  PB_NOT_LOOKUP(reinterpret_cast<Prover*>(p), "pb200_prover_prove_lookup (wires in host memory)");
   prover_prove(reinterpret_cast<Prover*>(p), (const uint8_t*)d_A, (const uint8_t*)d_B, (const uint8_t*)d_C, h_public,
                n_public, h_proof768, true);
   PB_API_END
@@ -468,6 +481,7 @@ int pb200_prover_round1(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B,
 int pb200_prover_round2(pb200_prover* p, const uint8_t* beta, const uint8_t* gamma, uint8_t* h_z_xy) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   Prover* P = reinterpret_cast<Prover*>(p);
+  PB_NOT_LOOKUP(P, "pb200_prover_round2_lookup");
   prover_round2(P, load_fr_canonical(beta), load_fr_canonical(gamma));
   memcpy(h_z_xy, P->proof.pts[3], 64);
   PB_API_END
@@ -482,6 +496,7 @@ int pb200_prover_round3(pb200_prover* p, const uint8_t* alpha, const uint8_t* ff
 int pb200_prover_round4(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   Prover* P = reinterpret_cast<Prover*>(p);
+  PB_NOT_LOOKUP(P, "pb200_prover_round4_lookup");
   prover_round4(P, load_fr_canonical(zeta));
   memcpy(h_evals, P->proof.evals[0], 6 * 32);
   PB_API_END
@@ -519,7 +534,53 @@ int pb200_prover_set_zk(pb200_prover* p, int enable, const uint8_t* h_blinders) 
 }
 int pb200_prover_serialize(pb200_prover* p, uint8_t* h_proof768) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  PB_NOT_LOOKUP(reinterpret_cast<Prover*>(p), "pb200_prover_serialize_lookup");
   prover_serialize(reinterpret_cast<Prover*>(p), h_proof768);
+  PB_API_END
+}
+int pb200_prover_set_lookup(pb200_prover* p, const uint8_t* h_qk, const uint8_t* h_t1, const uint8_t* h_t2,
+                            const uint8_t* h_t3, uint64_t table_rows) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  const uint8_t* tab[3] = {h_t1, h_t2, h_t3};
+  prover_set_lookup(reinterpret_cast<Prover*>(p), h_qk, tab, table_rows);
+  PB_API_END
+}
+int pb200_prover_round_lookup(pb200_prover* p, const uint8_t* eta, uint8_t* h_fh_xy) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  prover_round_lookup(P, load_fr_canonical(eta));
+  memcpy(h_fh_xy, P->lk_pts[0], 3 * 64);
+  PB_API_END
+}
+int pb200_prover_round2_lookup(pb200_prover* p, const uint8_t* beta, const uint8_t* gamma, const uint8_t* delta,
+                               const uint8_t* epsilon, uint8_t* h_zz2_xy) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  prover_round2_lookup(P, load_fr_canonical(beta), load_fr_canonical(gamma), load_fr_canonical(delta),
+                       load_fr_canonical(epsilon));
+  memcpy(h_zz2_xy, P->proof.pts[3], 64);
+  memcpy(h_zz2_xy + 64, P->lk_pts[3], 64);
+  PB_API_END
+}
+int pb200_prover_round4_lookup(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  prover_round4_lookup(P, load_fr_canonical(zeta));
+  memcpy(h_evals, P->proof.evals[0], 6 * 32);
+  memcpy(h_evals + 6 * 32, P->lk_evals[0], 6 * 32);
+  PB_API_END
+}
+int pb200_prover_prove_lookup(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
+                              const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof1216) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  prover_prove_lookup(reinterpret_cast<Prover*>(p), h_A, h_B, h_C, h_public, n_public, h_proof1216);
+  PB_API_END
+}
+int pb200_prover_serialize_lookup(pb200_prover* p, uint8_t* h_proof1216) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  PB_CHECK(P->lk, "this prover has no lookup table: use pb200_prover_serialize (768 bytes)");
+  prover_serialize_lookup(P, h_proof1216);
   PB_API_END
 }
 int pb200_g1_combine_partials_host(const uint8_t* h_xyzz, unsigned count, uint8_t* h_out_xy, int* is_identity) {

@@ -19,6 +19,7 @@
 // (prover.py:108-116), Z_n == 1 (prover.py:132), deg T < 3n (prover.py:205-208).
 // Zero-knowledge mode (prover_set_zk, one GPU) blinds A, B, C, Z and the quotient pieces as in the PLONK paper; the
 // proof keeps its 15 fields and the verifier does not change.  See "zero knowledge" below.
+#include <algorithm>
 #include <cerrno>
 #include <sys/random.h>
 
@@ -450,6 +451,16 @@ __global__ void __launch_bounds__(128) k_lincomb(LinCombArgs a, Fr* out) {
   out[k] = acc;
 }
 
+// the same, added to out: the lookup terms of round 5 (the plain batch already takes up to 19 of the 20 slots)
+__global__ void __launch_bounds__(128) k_lincomb_add(LinCombArgs a, Fr* out) {
+  uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= a.n) return;
+  k += a.first;
+  Fr acc = k == 0 ? a.c0 : Fr::zero();
+  for (int i = 0; i < a.count; i++) acc = fp_add(acc, fp_mul(a.w[i], ldg_fr(a.vec[i] + k)));
+  out[k] = fp_add(out[k], acc);
+}
+
 // den[j] = shift * roots[j] - point    (the n-point coset x_j = shift * w^j minus the opening point)
 __global__ void k_coset_minus(const Fr* roots, Fr shift, Fr point, uint64_t n, Fr* den) {
   uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -482,6 +493,124 @@ __global__ void k_zk_blind(const Fr* in, uint64_t n_in, uint64_t n, ZkPatch p, u
   if (k < 3) v = fp_add(v, p.lo[k]);
   else if (k >= n && k < n + 3) v = fp_add(v, p.hi[k - n]);
   out[k] = v;
+}
+
+// ---- lookups (plookup, cyclic alternating split) ------------------------------------------------------------------
+// exclusive scan of a uint32 count array (msm.cu): offsets[0..nb) and the total at offsets[nb]; counts are zeroed
+#define PB_SCAN_TILE 2048
+__global__ void k_scan_tile_sums(const uint32_t* counts, uint32_t nb, uint32_t pad, uint32_t* tile_sums, uint32_t* max_out);
+__global__ void k_scan_tiles(uint32_t* tile_sums, uint32_t n_tiles, uint32_t* total_out);
+__global__ void k_scan_apply(uint32_t* counts, uint32_t nb, uint32_t pad, const uint32_t* tile_sums, uint32_t* offsets);
+
+// the order of the sorted table copy: (t1, t2, t3) lexicographically, each by Montgomery limbs from the top
+PB_HD int lookup_cmp(const Fr* x, const Fr& a, const Fr& b, const Fr& c) {
+  const Fr* y[3] = {&a, &b, &c};
+  for (int w = 0; w < 3; w++)
+    for (int l = 7; l >= 0; l--)
+      if (x[w].v[l] != y[w]->v[l]) return x[w].v[l] < y[w]->v[l] ? -1 : 1;
+  return 0;
+}
+
+// j_i: for a lookup row (q_K = 1) the lowest table index of a row equal to (a_i, b_i, c_i) -- the first of the equal rows
+// in the sorted copy, which keeps table order among them --, else 0.  A row not in the table: the lowest such i goes to
+// *missing.
+__global__ void __launch_bounds__(128) k_lookup_index(const Fr* A, const Fr* B, const Fr* C, const Fr* QK, const Fr* keys,
+                                                      const uint32_t* keys_idx, uint64_t rows, uint64_t n, uint32_t* j_out,
+                                                      uint32_t* missing) {
+  uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  if (ldg_fr(QK + i).is_zero()) { j_out[i] = 0; return; }
+  const Fr a = ldg_fr(A + i), b = ldg_fr(B + i), c = ldg_fr(C + i);
+  uint64_t lo = 0, hi = rows;
+  while (lo < hi) {
+    uint64_t mid = (lo + hi) / 2;
+    if (lookup_cmp(keys + 3 * mid, a, b, c) < 0) lo = mid + 1;
+    else hi = mid;
+  }
+  if (lo < rows && lookup_cmp(keys + 3 * lo, a, b, c) == 0) {
+    j_out[i] = keys_idx[lo];
+  } else {
+    j_out[i] = 0;
+    atomicMin(missing, (uint32_t)i);
+  }
+}
+
+// histogram of j over the n table entries.  Every non-lookup row has j = 0, so equal keys are first merged within the
+// warp: one atomic per distinct key per warp instead of one per row on a single counter.
+__global__ void __launch_bounds__(256) k_lookup_hist(const uint32_t* j, uint64_t n, uint32_t* cnt) {
+  uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t key = i < n ? j[i] : 0xffffffffu;
+  const uint32_t peers = __match_any_sync(0xffffffffu, key);
+  if (key != 0xffffffffu && (int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(cnt + key, (uint32_t)__popc(peers));
+}
+
+// s (2n positions) is the table in order, entry j taking 1 + cnt_j positions from start_j = j + off_j on: position p
+// belongs to the last entry with start_j <= p.  Each position finds its entry by binary search, so no thread writes a run.
+__global__ void __launch_bounds__(256) k_lookup_place(const uint32_t* off, uint64_t n, uint32_t* sidx) {
+  uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= 2 * n) return;
+  uint64_t lo = 0, hi = n;  // first entry with start > p
+  while (lo < hi) {
+    uint64_t mid = (lo + hi) / 2;
+    if (mid + off[mid] <= p) lo = mid + 1;
+    else hi = mid;
+  }
+  sidx[p] = (uint32_t)(lo - 1);
+}
+
+// t = t1 + eta t2 + eta^2 t3, then f_i = t[j_i], h1_i = s_2i, h2_i = s_2i+1
+__global__ void k_lookup_compress(const Fr* t1, const Fr* t2, const Fr* t3, Fr eta, Fr eta2, uint64_t n, Fr* t) {
+  uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) t[i] = fp_add(ldg_fr(t1 + i), fp_add(fp_mul(eta, ldg_fr(t2 + i)), fp_mul(eta2, ldg_fr(t3 + i))));
+}
+__global__ void k_lookup_gather(const Fr* t, const uint32_t* j, const uint32_t* sidx, uint64_t n, Fr* f, Fr* h1, Fr* h2) {
+  uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  f[i] = ldg_fr(t + j[i]);
+  h1[i] = ldg_fr(t + sidx[2 * i]);
+  h2[i] = ldg_fr(t + sidx[2 * i + 1]);
+}
+
+// per-row numerator / denominator of Z2 (indices wrap at n):
+//   (1+d)(e+f_i)(e(1+d)+t_i+d t_i+1)  /  (e(1+d)+h1_i+d h2_i)(e(1+d)+h2_i+d h1_i+1)
+struct LookupChallenges { Fr delta, eps, one_d, eps_one_d; };
+__global__ void k_lookup_z2_terms(const Fr* t, const Fr* f, const Fr* h1, const Fr* h2, LookupChallenges ch, uint64_t n,
+                                  Fr* num, Fr* den) {
+  uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint64_t i1 = i + 1 == n ? 0 : i + 1;
+  const Fr x1 = ldg_fr(h1 + i), x2 = ldg_fr(h2 + i);
+  num[i] = fp_mul(fp_mul(ch.one_d, fp_add(ch.eps, ldg_fr(f + i))),
+                  fp_add(fp_add(ch.eps_one_d, ldg_fr(t + i)), fp_mul(ch.delta, ldg_fr(t + i1))));
+  den[i] = fp_mul(fp_add(fp_add(ch.eps_one_d, x1), fp_mul(ch.delta, x2)),
+                  fp_add(fp_add(ch.eps_one_d, x2), fp_mul(ch.delta, ldg_fr(h1 + i1))));
+}
+
+// the three lookup terms of the quotient, added to the plain quotient's evaluations on the 4n coset (one GPU):
+//   a3 q_K (A + eta B + eta^2 C - F)
+// + a4 [Z2 (1+d)(e+F)(e(1+d) + T + d T(wX)) - Z2(wX)(e(1+d) + H1 + d H2)(e(1+d) + H2 + d H1(wX))]
+// + a5 L0 (Z2 - 1),   all over Z_H.  X -> wX is index + 4 on the coset, as for Z.
+struct LookupQuotientArgs {
+  const Fr *A, *B, *C, *QK, *T, *F, *H1, *H2, *Z2, *L0;
+  Fr zh_inv[4];
+  Fr eta, eta2, delta, eps, one_d, eps_one_d, alpha3, alpha4, alpha5, one;
+  uint64_t n4;
+};
+__global__ void __launch_bounds__(128) k_quotient_lookup(LookupQuotientArgs q, Fr* out) {
+  uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= q.n4) return;
+  const uint64_t jw = j + 4 >= q.n4 ? j + 4 - q.n4 : j + 4;
+  const Fr f = ldg_fr(q.F + j);
+  Fr w = fp_add(ldg_fr(q.A + j), fp_add(fp_mul(q.eta, ldg_fr(q.B + j)), fp_mul(q.eta2, ldg_fr(q.C + j))));
+  Fr acc = fp_mul(q.alpha3, fp_mul(ldg_fr(q.QK + j), fp_sub(w, f)));
+  const Fr z2 = ldg_fr(q.Z2 + j), h1 = ldg_fr(q.H1 + j), h2 = ldg_fr(q.H2 + j);
+  Fr p1 = fp_mul(fp_mul(fp_mul(z2, q.one_d), fp_add(q.eps, f)),
+                 fp_add(fp_add(q.eps_one_d, ldg_fr(q.T + j)), fp_mul(q.delta, ldg_fr(q.T + jw))));
+  Fr p2 = fp_mul(fp_mul(ldg_fr(q.Z2 + jw), fp_add(fp_add(q.eps_one_d, h1), fp_mul(q.delta, h2))),
+                 fp_add(fp_add(q.eps_one_d, h2), fp_mul(q.delta, ldg_fr(q.H1 + jw))));
+  acc = fp_add(acc, fp_mul(q.alpha4, fp_sub(p1, p2)));
+  acc = fp_add(acc, fp_mul(q.alpha5, fp_mul(fp_sub(z2, q.one), ldg_fr(q.L0 + j))));
+  out[j] = fp_add(out[j], fp_mul(acc, q.zh_inv[j & 3]));
 }
 
 // ------------------------------------------------------------------------------------------
@@ -729,6 +858,7 @@ void prover_set_zk(Prover* P, bool enable, const uint8_t* h_blinders) {
     return;
   }
   PB_CHECK(P->world == 1, "zero-knowledge proving is not available on the sharded prover (one GPU only)");
+  PB_CHECK(!P->lk, "zero-knowledge mode does not combine with lookups");
   PB_CHECK(P->n >= 8, "zero-knowledge proving needs n >= 8 rows: the blinded quotient has degree 3n + 5 < 4n");
   PB_CHECK(srs_size(P->srs) >= P->n + 6,
            "Not enough powers in setup: zero-knowledge proving needs n + 6 powers (T3' has n + 6 coefficients)");
@@ -773,6 +903,175 @@ static ZkPatch zh_multiple(std::initializer_list<Fr> c) {
   for (const Fr& x : c) { p.lo[i] = fp_neg(x); p.hi[i] = x; i++; }
   return p;
 }
+
+// ---- lookups ------------------------------------------------------------------------------------------------------
+// plookup (eprint 2020/315) in the cyclic, alternating-split form of PlonKup (eprint 2022/086).  A boolean selector q_K
+// marks the rows whose (a, b, c) must be a row of one fixed table (t1, t2, t3).  Per proof, with t = t1 + eta t2 +
+// eta^2 t3: f_i = t[j_i] (j_i the lowest matching table index, 0 on other rows); s (2n) is t in table order with every
+// entry followed by one copy per row that looks it up; h1 = s[0::2], h2 = s[1::2]; Z2 is the grand product of
+// k_lookup_z2_terms.  The quotient gains k_quotient_lookup's three terms (degree <= 3n); round 5 opens F, T, H2 at
+// zeta and T, H1, Z2 at zeta w.  The index, histogram and placement do not depend on eta and run in round 1.
+
+static bool fr_is_canonical(const Fr& a) {
+  const Fr m = Fr::modulus();
+  for (int i = 7; i >= 0; i--)
+    if (a.v[i] != m.v[i]) return a.v[i] < m.v[i];
+  return false;
+}
+
+void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* const* h_tab, uint64_t rows) {
+  Context* ctx = P->ctx;
+  const uint64_t n = P->n;
+  PB_CHECK(P->world == 1, "lookups are not available on the sharded prover (one GPU only)");
+  PB_CHECK(!P->zk, "lookups do not combine with zero-knowledge mode");
+  PB_CHECK(!P->lk, "the lookup table is already set (set it once, before the first proof)");
+  PB_CHECK(h_qk && h_tab && h_tab[0] && h_tab[1] && h_tab[2], "lookups need q_K and three table columns");
+  PB_CHECK(rows >= 1, "the lookup table is empty");
+  PB_CHECK(rows <= n, "the lookup table has more rows than the circuit");
+  // q_K: 0 or 1 on every row
+  for (uint64_t i = 0; i < n; i++) {
+    const uint8_t* e = h_qk + 32 * i;
+    bool ok = e[0] <= 1;
+    for (int k = 1; k < 32 && ok; k++) ok = e[k] == 0;
+    PB_CHECK(ok, "q_K must be 0 or 1 on every row");
+  }
+  // the table, padded to n rows by repeating its last row, in Montgomery form
+  std::vector<Fr> tab[3];
+  for (int w = 0; w < 3; w++) {
+    tab[w].resize(n);
+    for (uint64_t r = 0; r < n; r++) {
+      Fr x;
+      memcpy(x.v, h_tab[w] + 32 * std::min(r, rows - 1), 32);
+      PB_CHECK(fr_is_canonical(x), "lookup table value not reduced below the field modulus");
+      tab[w][r] = fp_to_mont(x);
+    }
+  }
+  std::vector<uint32_t> order(rows);
+  for (uint64_t r = 0; r < rows; r++) order[r] = (uint32_t)r;
+  std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) {
+    const Fr kx[3] = {tab[0][x], tab[1][x], tab[2][x]};
+    return lookup_cmp(kx, tab[0][y], tab[1][y], tab[2][y]) < 0;
+  });
+  std::vector<Fr> keys(3 * rows);
+  for (uint64_t r = 0; r < rows; r++)
+    for (int w = 0; w < 3; w++) keys[3 * r + w] = tab[w][order[r]];
+  cudaStream_t st = ctx->stream;
+  P->lk_keys.alloc(keys.size() * 32);
+  P->lk_keys_idx.alloc(rows * 4);
+  PB_CUDA(cudaMemcpyAsync(P->lk_keys.p, keys.data(), keys.size() * 32, cudaMemcpyHostToDevice, st));
+  PB_CUDA(cudaMemcpyAsync(P->lk_keys_idx.p, order.data(), rows * 4, cudaMemcpyHostToDevice, st));
+  for (int w = 0; w < 3; w++) {
+    P->lk_tab[w].alloc(n * 32);
+    PB_CUDA(cudaMemcpyAsync(P->lk_tab[w].p, tab[w].data(), n * 32, cudaMemcpyHostToDevice, st));
+  }
+  upload_mont(ctx, P->lk_qk_lag, h_qk, n);
+  P->lk_qk_coeff.alloc(n * 32);
+  ntt_run(ctx, P->lk_qk_lag.as<Fr>(), P->lk_qk_coeff.as<Fr>(), P->log_n, true, n, nullptr, nullptr);
+  P->lk_qk_ext.alloc(P->n_ext * 32);
+  coset_extend(P, st, nullptr, P->lk_qk_coeff.as<Fr>(), P->lk_qk_ext.as<Fr>(), P->gpow.as<Fr>());
+  P->lk_j.alloc(n * 4);
+  P->lk_cnt.alloc(n * 4);
+  P->lk_off.alloc((n + 1) * 4);
+  P->lk_sidx.alloc(2 * n * 4);
+  for (int k = 0; k < Prover::LK_VECS; k++) {
+    P->lk_lag[k].alloc(n * 32);
+    P->lk_coeff[k].alloc(n * 32);
+    P->lk_ext[k].alloc(P->n_ext * 32);
+  }
+  PB_CUDA(cudaStreamSynchronize(st));  // the host copies die here
+  P->lk_rows = rows;
+  P->lk = true;
+}
+
+// round 1: table index of every row, the histogram over the table entries and each position's entry in s
+static void lookup_index(Prover* P) {
+  Context* ctx = P->ctx;
+  const uint64_t n = P->n;
+  cudaStream_t st = ctx->stream;
+  uint32_t* missing = P->flags.as<uint32_t>() + 2;
+  PB_CUDA(cudaMemsetAsync(missing, 0xff, 4, st));
+  k_lookup_index<<<PB_GRID(n, 128), 0, st>>>(P->lag[0].as<Fr>(), P->lag[1].as<Fr>(), P->lag[2].as<Fr>(),
+                                            P->lk_qk_lag.as<Fr>(), P->lk_keys.as<Fr>(), P->lk_keys_idx.as<uint32_t>(),
+                                            P->lk_rows, n, P->lk_j.as<uint32_t>(), missing);
+  PB_CUDA(cudaMemsetAsync(P->lk_cnt.p, 0, n * 4, st));
+  k_lookup_hist<<<PB_GRID(n, 256), 0, st>>>(P->lk_j.as<uint32_t>(), n, P->lk_cnt.as<uint32_t>());
+  const uint32_t n_tiles = (uint32_t)((n + PB_SCAN_TILE - 1) / PB_SCAN_TILE);
+  ctx->scratch[0].ensure((size_t)n_tiles * 4);
+  uint32_t* tiles = ctx->scratch[0].as<uint32_t>();
+  uint32_t* off = P->lk_off.as<uint32_t>();
+  k_scan_tile_sums<<<n_tiles, 256, 0, st>>>(P->lk_cnt.as<uint32_t>(), (uint32_t)n, 0, tiles, nullptr);
+  k_scan_tiles<<<1, 256, 0, st>>>(tiles, n_tiles, off + n);
+  k_scan_apply<<<n_tiles, 256, 0, st>>>(P->lk_cnt.as<uint32_t>(), (uint32_t)n, 0, tiles, off);
+  k_lookup_place<<<PB_GRID(2 * n, 256), 0, st>>>(off, n, P->lk_sidx.as<uint32_t>());
+  ctx->launches += 6;
+  const uint32_t row = read_flag(P, 2);
+  PB_CHECK(row == 0xffffffffu,
+           ("AssertionError: lookup row " + std::to_string(row) + " is not in the table").c_str());
+}
+
+// step 1L: t, f, h1, h2 from eta, and one commitment pass over f, h1, h2
+void prover_round_lookup(Prover* P, const Fr& eta_c) {
+  Context* ctx = P->ctx;
+  const uint64_t n = P->n;
+  cudaStream_t st = ctx->stream;
+  PB_CHECK(P->lk, "this prover has no lookup table (pb200_prover_set_lookup)");
+  P->eta = fp_to_mont(eta_c);
+  Fr* v[Prover::LK_VECS];
+  for (int k = 0; k < Prover::LK_VECS; k++) v[k] = P->lk_lag[k].as<Fr>();
+  k_lookup_compress<<<PB_GRID(n, 256), 0, st>>>(P->lk_tab[0].as<Fr>(), P->lk_tab[1].as<Fr>(), P->lk_tab[2].as<Fr>(),
+                                               P->eta, fp_sqr(P->eta), n, v[Prover::LK_T]);
+  k_lookup_gather<<<PB_GRID(n, 256), 0, st>>>(v[Prover::LK_T], P->lk_j.as<uint32_t>(), P->lk_sidx.as<uint32_t>(), n,
+                                             v[Prover::LK_F], v[Prover::LK_H1], v[Prover::LK_H2]);
+  ctx->launches += 2;
+  const Fr* lag[4] = {v[Prover::LK_T], v[Prover::LK_F], v[Prover::LK_H1], v[Prover::LK_H2]};
+  Fr* coeff[4] = {P->lk_coeff[Prover::LK_T].as<Fr>(), P->lk_coeff[Prover::LK_F].as<Fr>(),
+                  P->lk_coeff[Prover::LK_H1].as<Fr>(), P->lk_coeff[Prover::LK_H2].as<Fr>()};
+  interpolate(P, lag, coeff, 4);
+  const Fr* fh[3] = {coeff[1], coeff[2], coeff[3]};
+  P->commit_batch(fh, 3, n, P->lk_pts[0]);
+}
+
+// round 2 of a lookup proof, after Z: the grand product Z2, then one commitment pass over Z and Z2
+static void lookup_round2(Prover* P) {
+  Context* ctx = P->ctx;
+  const uint64_t n = P->n;
+  cudaStream_t st = ctx->stream;
+  const Fr one = Fr::one();
+  LookupChallenges ch;
+  ch.delta = P->delta;
+  ch.eps = P->epsilon;
+  ch.one_d = fp_add(one, P->delta);
+  ch.eps_one_d = fp_mul(P->epsilon, ch.one_d);
+  Fr* num = P->tmp[2].as<Fr>();
+  Fr* den = P->tmp[3].as<Fr>();
+  k_lookup_z2_terms<<<PB_GRID(n, 128), 0, st>>>(P->lk_lag[Prover::LK_T].as<Fr>(), P->lk_lag[Prover::LK_F].as<Fr>(),
+                                               P->lk_lag[Prover::LK_H1].as<Fr>(), P->lk_lag[Prover::LK_H2].as<Fr>(), ch, n,
+                                               num, den);
+  uint64_t T = (n + PB_BATCH_CH - 1) / PB_BATCH_CH;
+  k_batch_div<<<PB_GRID(T, 128), 0, st>>>(num, den, num, n, T);
+  uint32_t n_tiles = (uint32_t)((n + PB_PROD_TILE - 1) / PB_PROD_TILE);
+  ctx->scratch[0].ensure((size_t)(n_tiles + 1) * 32);
+  Fr* tiles = ctx->scratch[0].as<Fr>();
+  k_prod_tiles<<<n_tiles, 256, 0, st>>>(num, n, tiles);
+  k_prod_scan_tiles<<<1, 256, 0, st>>>(tiles, n_tiles, tiles + n_tiles);
+  k_prod_apply<<<n_tiles, 256, 0, st>>>(num, n, tiles, nullptr, P->lk_lag[Prover::LK_Z2].as<Fr>());
+  ctx->launches += 5;
+  Fr total;
+  PB_CUDA(cudaMemcpyAsync(&total, tiles + n_tiles, 32, cudaMemcpyDeviceToHost, st));
+  const Fr* zl = P->lk_lag[Prover::LK_Z2].as<Fr>();
+  Fr* zc = P->lk_coeff[Prover::LK_Z2].as<Fr>();
+  interpolate(P, &zl, &zc, 1);
+  PB_CUDA(cudaStreamSynchronize(st));
+  PB_CHECK(total == one, "AssertionError: lookup grand product does not close, Z2_n != 1");
+  const Fr* zz[2] = {P->coeff[3].as<Fr>(), zc};
+  uint8_t out[2][64];
+  P->commit_batch(zz, 2, n, out[0]);
+  memcpy(P->proof.pts[3], out[0], 64);
+  memcpy(P->lk_pts[3], out[1], 64);
+}
+
+void prover_round2_lookup(Prover* P, const Fr& beta_c, const Fr& gamma_c, const Fr& delta_c, const Fr& epsilon_c);
+void prover_round4_lookup(Prover* P, const Fr& zeta_c);
 
 // cached per prover: basis_i[j] = L_i(x_j) on the fixed coset for the first `count` rows
 static void ensure_pi_basis(Prover* P, int count) {
@@ -887,6 +1186,7 @@ void prover_round1(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_
   PB_CUDA(cudaStreamSynchronize(st));
   PB_CHECK(fl[1] == 0, "wire value not reduced below the field modulus (canonical 32-byte little-endian expected)");
   PB_CHECK(fl[0] == 0, "AssertionError: witness does not satisfy the gate constraints (prover.py:108-116)");
+  if (P->lk) lookup_index(P);
   if (P->overlap) launch_coset_ext_async(P, 0, 3, 0);
   if (P->zk) {  // A' B' C': n + 2 coefficients
     const Fr* b = P->zk_b;
@@ -956,7 +1256,18 @@ void prover_round2(Prover* P, const Fr& beta_c, const Fr& gamma_c) {
     P->commit(P->zk_coeff[3].as<Fr>(), n + 3, P->proof.pts[3]);
     return;
   }
+  if (P->lk) {  // Z2, and Z with it in one commitment pass
+    lookup_round2(P);
+    return;
+  }
   P->commit(P->coeff[3].as<Fr>(), n, P->proof.pts[3]);
+}
+
+void prover_round2_lookup(Prover* P, const Fr& beta_c, const Fr& gamma_c, const Fr& delta_c, const Fr& epsilon_c) {
+  PB_CHECK(P->lk, "this prover has no lookup table (pb200_prover_set_lookup)");
+  P->delta = fp_to_mont(delta_c);
+  P->epsilon = fp_to_mont(epsilon_c);
+  prover_round2(P, beta_c, gamma_c);
 }
 
 // ---- round 3 (prover.py:154-226) -------------------------------------------------------------------------
@@ -1005,6 +1316,23 @@ void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c) {
     k_quotient<false><<<PB_GRID(ne, 128), 0, st>>>(q, t_evals, zk);
   }
   ctx->launches++;
+  if (P->lk) {  // one GPU: the slice is the whole 4n coset
+    for (int k = 0; k < Prover::LK_VECS; k++)
+      coset_extend(P, st, nullptr, P->lk_coeff[k].as<Fr>(), P->lk_ext[k].as<Fr>(), P->gpow.as<Fr>());
+    LookupQuotientArgs lq;
+    lq.A = q.A; lq.B = q.B; lq.C = q.C; lq.QK = P->lk_qk_ext.as<Fr>(); lq.L0 = q.L0;
+    lq.T = P->lk_ext[Prover::LK_T].as<Fr>(); lq.F = P->lk_ext[Prover::LK_F].as<Fr>();
+    lq.H1 = P->lk_ext[Prover::LK_H1].as<Fr>(); lq.H2 = P->lk_ext[Prover::LK_H2].as<Fr>();
+    lq.Z2 = P->lk_ext[Prover::LK_Z2].as<Fr>();
+    for (int k = 0; k < 4; k++) lq.zh_inv[k] = P->zh_inv[k];
+    lq.eta = P->eta; lq.eta2 = fp_sqr(P->eta); lq.delta = P->delta; lq.eps = P->epsilon;
+    lq.one_d = fp_add(Fr::one(), P->delta); lq.eps_one_d = fp_mul(P->epsilon, lq.one_d);
+    lq.alpha3 = fp_mul(q.alpha2, P->alpha); lq.alpha4 = fp_sqr(q.alpha2); lq.alpha5 = fp_mul(lq.alpha4, P->alpha);
+    lq.one = Fr::one();
+    lq.n4 = ne;
+    k_quotient_lookup<<<PB_GRID(ne, 128), 0, st>>>(lq, t_evals);
+    ctx->launches++;
+  }
   PB_CUDA(cudaMemsetAsync(P->flags.p, 0, 64, st));
   if (P->world > 1) {
     // slab-sharded inverse over the 4n coset: the local inverse transform of the slice, ONE allgather, then the
@@ -1083,6 +1411,19 @@ void prover_round4(Prover* P, const Fr& zeta_c) {
   }
 }
 
+// round 4 of a lookup proof: the six plain evaluations, then F, T at zeta, T at zeta w, H2 at zeta, H1 and Z2 at zeta w
+void prover_round4_lookup(Prover* P, const Fr& zeta_c) {
+  PB_CHECK(P->lk, "this prover has no lookup table (pb200_prover_set_lookup)");
+  prover_round4(P, zeta_c);
+  const Fr z = P->zeta, zw = fp_mul(P->zeta, fr_root_of_unity(P->log_n));
+  const Fr* polys[6] = {P->lk_coeff[Prover::LK_F].as<Fr>(), P->lk_coeff[Prover::LK_T].as<Fr>(),
+                        P->lk_coeff[Prover::LK_T].as<Fr>(), P->lk_coeff[Prover::LK_H2].as<Fr>(),
+                        P->lk_coeff[Prover::LK_H1].as<Fr>(), P->lk_coeff[Prover::LK_Z2].as<Fr>()};
+  const Fr xs[6] = {z, z, zw, z, zw, zw};
+  eval_polys(P, 6, polys, xs, P->lk_ev);
+  for (int k = 0; k < 6; k++) store_canonical(P->lk_evals[k], P->lk_ev[k]);
+}
+
 // (num coefficients, n) / (X - point) -> quotient coefficients (out != num), remainder dropped.
 // Coefficient-space synthetic division as a weighted suffix sum (see k_sufsum_*).  One proof across G ranks: rank r
 // divides the slab of coefficients [r n/G, (r+1) n/G) -- `num` needs to be valid on that slab only --; the slab sums
@@ -1148,13 +1489,15 @@ void prover_round5(Prover* P, const Fr& v_c) {
   const Fr* zpoly = zk ? P->zk_coeff[3].as<Fr>() : P->coeff[3].as<Fr>();
   const Fr* tpiece[3];
   for (int i = 0; i < 3; i++) tpiece[i] = zk ? P->zk_t[i].as<Fr>() : P->tq.as<Fr>() + (uint64_t)i * n;
-  LinCombArgs L, tail;
+  LinCombArgs L, tail, lkp;
   int k = 0;
   tail.count = 0;
+  lkp.count = 0;
   auto add = [&](const Fr* vec, const Fr& w, bool blinded = false) {
     L.vec[k] = vec; L.w[k] = w; k++;
     if (blinded) { tail.vec[tail.count] = vec; tail.w[tail.count] = w; tail.count++; }
   };
+  auto add_lookup = [&](const Fr* vec, const Fr& w) { lkp.vec[lkp.count] = vec; lkp.w[lkp.count] = w; lkp.count++; };
   add(P->sel_coeff[Prover::QL].as<Fr>(), a);
   add(P->sel_coeff[Prover::QR].as<Fr>(), b);
   add(P->sel_coeff[Prover::QM].as<Fr>(), fp_mul(a, b));
@@ -1172,6 +1515,31 @@ void prover_round5(Prover* P, const Fr& v_c) {
   add(wire[2], v3, true);
   add(P->sel_coeff[Prover::S1].as<Fr>(), v4);
   add(P->sel_coeff[Prover::S2].as<Fr>(), v5);
+  // lookups: q_K, Z2 and H1 keep their commitments in the linearisation; F, T, H2 join the batch at zeta (a second
+  // pass, k_lincomb_add)
+  if (P->lk) {
+    const Fr &fe = P->lk_ev[0], &te = P->lk_ev[1], &tw = P->lk_ev[2], &h2e = P->lk_ev[3], &h1w = P->lk_ev[4],
+             &z2w = P->lk_ev[5];
+    const Fr &eta = P->eta, &de = P->delta, &ep = P->epsilon;
+    const Fr od = fp_add(one, de), eod = fp_mul(ep, od);
+    const Fr al2 = fp_sqr(al), al3 = fp_mul(al2, al), al4 = fp_sqr(al2), al5 = fp_mul(al4, al);
+    const Fr v6 = fp_mul(v5, v), v7 = fp_mul(v6, v), v8 = fp_mul(v7, v);
+    const Fr abc = fp_add(a, fp_add(fp_mul(eta, b), fp_mul(fp_sqr(eta), c)));
+    const Fr hw = fp_add(fp_add(eod, h2e), fp_mul(de, h1w));       // e(1+d) + h2 + d h1(zeta w)
+    const Fr az2 = fp_mul(al4, z2w);
+    add_lookup(P->lk_qk_coeff.as<Fr>(), fp_mul(al3, fp_sub(abc, fe)));
+    add_lookup(P->lk_coeff[Prover::LK_Z2].as<Fr>(),
+        fp_add(fp_mul(fp_mul(fp_mul(al4, od), fp_add(ep, fe)), fp_add(fp_add(eod, te), fp_mul(de, tw))),
+               fp_mul(al5, l0_ev)));
+    add_lookup(P->lk_coeff[Prover::LK_H1].as<Fr>(), fp_neg(fp_mul(az2, hw)));
+    add_lookup(P->lk_coeff[Prover::LK_F].as<Fr>(), v6);
+    add_lookup(P->lk_coeff[Prover::LK_T].as<Fr>(), v7);
+    add_lookup(P->lk_coeff[Prover::LK_H2].as<Fr>(), v8);
+    // -a4 z2w (e(1+d) + d h2) hw - a5 L0(zeta) - v^6 f - v^7 t - v^8 h2
+    Fr c = fp_neg(fp_mul(fp_mul(az2, fp_add(eod, fp_mul(de, h2e))), hw));
+    c = fp_sub(c, fp_mul(al5, l0_ev));
+    lkp.c0 = fp_sub(c, fp_add(fp_mul(v6, fe), fp_add(fp_mul(v7, te), fp_mul(v8, h2e))));
+  }
   L.count = k;
   L.n = n / (uint64_t)P->world;          // one proof across G ranks: every rank builds (and divides) its slab only
   L.first = L.n * (uint64_t)P->rank;
@@ -1188,6 +1556,12 @@ void prover_round5(Prover* P, const Fr& v_c) {
   PB_CUDA(cudaMemsetAsync(P->flags.p, 0, 64, st));
   k_lincomb<<<PB_GRID(L.n, 128), 0, st>>>(L, wz);
   ctx->launches++;
+  if (P->lk) {
+    lkp.n = L.n;
+    lkp.first = L.first;
+    k_lincomb_add<<<PB_GRID(lkp.n, 128), 0, st>>>(lkp, wz);
+    ctx->launches++;
+  }
   const uint64_t len = zk ? n + Prover::ZK_PAD : n;  // numerator coefficients
   if (zk) {
     tail.c0 = Fr::zero();
@@ -1202,6 +1576,13 @@ void prover_round5(Prover* P, const Fr& v_c) {
   LinCombArgs M;
   M.vec[0] = zpoly; M.w[0] = one; M.count = 1; M.c0 = fp_neg(zw);
   M.n = zk ? len : L.n; M.first = L.first;
+  if (P->lk) {  // + v (T - t(zeta w)) + v^2 (H1 - h1(zeta w)) + v^3 (Z2 - z2(zeta w))
+    M.vec[1] = P->lk_coeff[Prover::LK_T].as<Fr>(); M.w[1] = v;
+    M.vec[2] = P->lk_coeff[Prover::LK_H1].as<Fr>(); M.w[2] = v2;
+    M.vec[3] = P->lk_coeff[Prover::LK_Z2].as<Fr>(); M.w[3] = v3;
+    M.count = 4;
+    M.c0 = fp_sub(M.c0, fp_add(fp_mul(v, P->lk_ev[2]), fp_add(fp_mul(v2, P->lk_ev[4]), fp_mul(v3, P->lk_ev[5]))));
+  }
   Fr* wzw = P->tmp[0].as<Fr>();  // the W_z numerator is no longer needed
   k_lincomb<<<PB_GRID(M.n, 128), 0, st>>>(M, wzw);
   ctx->launches++;
@@ -1250,6 +1631,54 @@ void prover_prove(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t
   Fr v = tr.get_and_append_challenge("v");
   prover_round5(P, v);
   prover_serialize(P, out768);
+}
+
+// 1216-byte lookup proof: the 768 plain bytes, then f_1 h1_1 h2_1 z2_1, then the six lookup evaluations
+void prover_serialize_lookup(const Prover* P, uint8_t* out1216) {
+  auto be = [](uint8_t* dst, const uint8_t* le) { for (int i = 0; i < 32; i++) dst[i] = le[31 - i]; };
+  prover_serialize(P, out1216);
+  uint8_t* o = out1216 + 768;
+  for (int k = 0; k < 4; k++) { be(o, P->lk_pts[k]); be(o + 32, P->lk_pts[k] + 32); o += 64; }
+  for (int k = 0; k < 6; k++) { be(o, P->lk_evals[k]); o += 32; }
+}
+
+void prover_prove_lookup(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t* hC, const uint8_t* h_public,
+                         uint64_t n_public, uint8_t* out1216) {
+  PB_CUDA(cudaSetDevice(P->ctx->device));
+  PB_CHECK(P->lk, "this prover has no lookup table (pb200_prover_set_lookup)");
+  Transcript tr("plonk");
+  prover_round1(P, hA, hB, hC, h_public, n_public, false);
+  tr.append_point_le("a_1", P->proof.pts[0]);
+  tr.append_point_le("b_1", P->proof.pts[1]);
+  tr.append_point_le("c_1", P->proof.pts[2]);
+  Fr beta = tr.get_and_append_challenge("beta");
+  Fr gamma = tr.get_and_append_challenge("gamma");
+  Fr eta = tr.get_and_append_challenge("eta");
+  prover_round_lookup(P, eta);
+  tr.append_point_le("f_1", P->lk_pts[0]);
+  tr.append_point_le("h1_1", P->lk_pts[1]);
+  tr.append_point_le("h2_1", P->lk_pts[2]);
+  Fr delta = tr.get_and_append_challenge("delta");
+  Fr epsilon = tr.get_and_append_challenge("epsilon");
+  prover_round2_lookup(P, beta, gamma, delta, epsilon);
+  tr.append_point_le("z_1", P->proof.pts[3]);
+  tr.append_point_le("z2_1", P->lk_pts[3]);
+  Fr alpha = tr.get_and_append_challenge("alpha");
+  Fr cof = tr.get_and_append_challenge("fft_cofactor");
+  prover_round3(P, alpha, cof);
+  tr.append_point_le("t_lo_1", P->proof.pts[4]);
+  tr.append_point_le("t_mid_1", P->proof.pts[5]);
+  tr.append_point_le("t_hi_1", P->proof.pts[6]);
+  Fr zeta = tr.get_and_append_challenge("zeta");
+  prover_round4_lookup(P, zeta);
+  static const char* ev_labels[6] = {"a_eval", "b_eval", "c_eval", "s1_eval", "s2_eval", "z_shifted_eval"};
+  for (int k = 0; k < 6; k++) tr.append_scalar_le(ev_labels[k], P->proof.evals[k]);
+  static const char* lk_labels[6] = {"f_eval", "t_eval", "t_shifted_eval", "h2_eval", "h1_shifted_eval",
+                                     "z2_shifted_eval"};
+  for (int k = 0; k < 6; k++) tr.append_scalar_le(lk_labels[k], P->lk_evals[k]);
+  Fr v = tr.get_and_append_challenge("v");
+  prover_round5(P, v);
+  prover_serialize_lookup(P, out1216);
 }
 
 }  // namespace pb200

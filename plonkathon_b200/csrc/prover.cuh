@@ -113,6 +113,27 @@ struct Prover {
   Fr zk_b[ZK_BLINDERS];           // this proof's b1..b11, Montgomery (drawn when round 1 starts)
   DevBuf zk_coeff[4];             // A' B' C' (n + 2 coefficients) Z' (n + 3)
   DevBuf zk_t[3];                 // T1' T2' (n + 1 coefficients) T3' (n + 6)
+  // Lookup argument (prover_set_lookup, one GPU): plookup over one fixed table of three columns, see "lookups" in
+  // prover.cu.  The proof gains f_1 h1_1 h2_1 z2_1 and six evaluations (1216 bytes).
+  enum { LK_T = 0, LK_F, LK_H1, LK_H2, LK_Z2, LK_VECS };
+  bool lk = false;
+  uint64_t lk_rows = 0;                // table rows before padding
+  DevBuf lk_qk_coeff, lk_qk_ext;       // q_K: coefficients, on the 4n coset
+  DevBuf lk_qk_lag;                    // q_K Lagrange values (Montgomery 0 / 1)
+  DevBuf lk_tab[3];                    // t1 t2 t3, Lagrange, padded to n by repeating the last row
+  DevBuf lk_keys;                      // the table rows sorted by their Montgomery limbs (3 Fr per row) ...
+  DevBuf lk_keys_idx;                  // ... and their original indices (uint32); equal rows keep table order
+  DevBuf lk_j;                         // per row: table index j_i (uint32, n)
+  DevBuf lk_cnt;                       // rows per table entry (uint32, n), zeroed by the scan
+  DevBuf lk_off;                       // exclusive scan of lk_cnt (uint32, n + 1)
+  DevBuf lk_sidx;                      // per position of s: its table entry (uint32, 2n)
+  DevBuf lk_lag[LK_VECS];              // T F H1 H2 Z2: Lagrange values ...
+  DevBuf lk_coeff[LK_VECS];            // ... coefficients ...
+  DevBuf lk_ext[LK_VECS];              // ... on the 4n coset
+  Fr eta, delta, epsilon;              // Montgomery
+  Fr lk_ev[6];                         // f, t, t(zeta w), h2, h1(zeta w), z2(zeta w) at their points (Montgomery)
+  uint8_t lk_pts[4][64];               // f_1 h1_1 h2_1 z2_1 (canonical LE x||y)
+  uint8_t lk_evals[6][32];             // canonical LE
   Proof proof;
 
   enum { QM = 0, QL, QR, QO, QC, S1, S2, S3, CUSTOM0 };

@@ -1,0 +1,66 @@
+"""Lookups: a plookup argument over one fixed table of three columns.
+
+A circuit with lookups has a boolean selector column q_K and a table (t1, t2, t3) of 1..n rows, padded to n rows by
+repeating its last row.  A row i with q_K[i] = 1 claims that (a_i, b_i, c_i) is a row of the table; the table's rows
+keep the order the user gives them and may repeat.  The argument is plookup (eprint 2020/315) in the cyclic,
+alternating-split form of PlonKup (eprint 2022/086); DESIGN.md describes it.  A lookup proof has 13 G1 points and 12
+scalars (1216 bytes, ``LookupProof``).
+
+Here: the checks on a lookup argument as users give it, ``(q_K, (t1, t2, t3))``, shared by ``Prover.from_arrays``,
+``Setup.verification_key_arrays`` and ``synthetic.build_circuit``.  Out of scope, and refused: zero knowledge with
+lookups, the sharded prover, more than one table, tables wider than three columns."""
+from __future__ import annotations
+
+import numpy as np
+
+from .field import CURVE_ORDER
+
+PROOF_BYTES = 1216
+
+
+def _column_ints(col) -> list:
+    """a column as Python ints: a list / tuple of ints, or an (m,32) uint8 / (m,8) uint32 little-endian array"""
+    if isinstance(col, np.ndarray) and col.dtype != object:
+        raw = np.ascontiguousarray(col).view(np.uint8).reshape(-1, 32).tobytes()
+        return [int.from_bytes(raw[i:i + 32], "little") for i in range(0, len(raw), 32)]
+    return [int(x.n) if hasattr(x, "n") else int(x) for x in col]
+
+
+def check_lookup(lookup, group_order: int):
+    """``lookup = (q_K, (t1, t2, t3))`` -> (q_K as n ints, [t1, t2, t3] as lists of ints, table rows).
+    ValueError for a q_K that is not 0/1 or not n rows long, an empty table, a table longer than n, columns of
+    unequal length, fewer or more than three columns, or a value >= r."""
+    try:
+        qk, table = lookup
+    except (TypeError, ValueError):
+        raise ValueError("lookup must be (q_K, (t1, t2, t3))") from None
+    qk = _column_ints(qk)
+    if len(qk) != group_order:
+        raise ValueError("q_K has %d rows, expected %d" % (len(qk), group_order))
+    if any(x not in (0, 1) for x in qk):
+        raise ValueError("q_K must be 0 or 1 on every row")
+    table = list(table)
+    if len(table) != 3:
+        raise ValueError("a lookup table has exactly three columns (t1, t2, t3), got %d" % len(table))
+    cols = [_column_ints(c) for c in table]
+    rows = len(cols[0])
+    if any(len(c) != rows for c in cols):
+        raise ValueError("lookup table columns of unequal length: %s" % [len(c) for c in cols])
+    if rows == 0:
+        raise ValueError("the lookup table is empty")
+    if rows > group_order:
+        raise ValueError("the lookup table has %d rows, more than the circuit's %d" % (rows, group_order))
+    if any(not 0 <= x < CURVE_ORDER for c in cols for x in c):
+        raise ValueError("lookup table values must lie in [0, r)")
+    return qk, cols, rows
+
+
+def padded_table(cols, group_order: int):
+    """the three columns padded to n rows by repeating their last row"""
+    return [c + [c[-1]] * (group_order - len(c)) for c in cols]
+
+
+def to_le_rows(ints) -> np.ndarray:
+    """ints -> contiguous (m,32) uint8 little-endian"""
+    raw = b"".join(int(x).to_bytes(32, "little") for x in ints)
+    return np.frombuffer(raw, dtype=np.uint8).reshape(-1, 32).copy()

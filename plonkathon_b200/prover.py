@@ -17,6 +17,7 @@ import numpy as np
 from . import _lib
 from .curve import Scalar
 from .custom_gates import split_terms
+from .lookup import PROOF_BYTES as LOOKUP_PROOF_BYTES, check_lookup, padded_table, to_le_rows
 from .field import CURVE_ORDER, FIELD_MODULUS, FQ
 from .poly import Basis, _log2_exact, scalars_to_bytes
 from .transcript import Message1, Message2, Message3, Message4, Message5, Transcript
@@ -65,6 +66,56 @@ class Proof:
                    Message4(*[Scalar(x) for x in w[14:20]]), Message5(pt(20), pt(22)))
 
 
+LOOKUP_FIELDS = ("f_1", "h1_1", "h2_1", "z2_1", "f_eval", "t_eval", "t_shifted_eval", "h2_eval", "h1_shifted_eval",
+                 "z2_shifted_eval")
+
+
+@dataclass
+class LookupProof:
+    """A proof with a lookup argument (plonkathon_b200/lookup.py): the plain proof's 15 fields and 10 more, 13 G1 points
+    and 12 scalars.  Byte order: the plain fields in ``Proof.flatten()`` order, then f_1 h1_1 h2_1 z2_1, then the six
+    lookup evaluations in transcript order -- 1216 bytes, encoded as the plain proof."""
+    plain: Proof
+    f_1: object
+    h1_1: object
+    h2_1: object
+    z2_1: object
+    f_eval: Scalar
+    t_eval: Scalar
+    t_shifted_eval: Scalar
+    h2_eval: Scalar
+    h1_shifted_eval: Scalar
+    z2_shifted_eval: Scalar
+
+    def flatten(self):
+        out = self.plain.flatten()
+        out.update((k, getattr(self, k)) for k in LOOKUP_FIELDS)
+        return out
+
+    def to_bytes(self) -> bytes:
+        out = bytearray(self.plain.to_bytes())
+        for k in LOOKUP_FIELDS:
+            v = getattr(self, k)
+            if isinstance(v, tuple):
+                out += v[0].n.to_bytes(32, "big") + v[1].n.to_bytes(32, "big")
+            else:
+                out += v.n.to_bytes(32, "big")
+        return bytes(out)
+
+    @classmethod
+    def from_bytes(cls, raw: bytes) -> "LookupProof":
+        """Inverse of to_bytes; ValueError for a word that is not reduced (coordinates below q, scalars below r)."""
+        if len(raw) != LOOKUP_PROOF_BYTES:
+            raise ValueError("a lookup proof has %d bytes, got %d" % (LOOKUP_PROOF_BYTES, len(raw)))
+        plain = Proof.from_bytes(raw[:768])
+        w = [int.from_bytes(raw[i:i + 32], "big") for i in range(768, LOOKUP_PROOF_BYTES, 32)]
+        for k, x in enumerate(w):
+            if x >= (CURVE_ORDER if k >= 8 else FIELD_MODULUS):
+                raise ValueError("non-canonical proof encoding (word %d is not reduced)" % (24 + k))
+        pt = lambda k: (FQ(w[k]), FQ(w[k + 1]))  # noqa: E731
+        return cls(plain, pt(0), pt(2), pt(4), pt(6), *[Scalar(x) for x in w[8:14]])
+
+
 def _as_le_rows(values, n) -> np.ndarray:
     """list of ints / Scalars, or an (m,32) uint8 / (m,8) uint32 array -> contiguous (n,32) uint8, zero padded."""
     if isinstance(values, np.ndarray):
@@ -103,12 +154,16 @@ class Prover:
         self._create(setup, self.group_order, cols)
 
     @classmethod
-    def from_arrays(cls, setup, group_order: int, pk_arrays: dict, ctx=None, custom=()):
+    def from_arrays(cls, setup, group_order: int, pk_arrays: dict, ctx=None, custom=(), lookup=None):
         """pk_arrays: QM QL QR QO QC S1 S2 S3 -> list of ints or (n,32) uint8 little-endian arrays.
         ``ctx``: run this prover on another context (stream + scratch) of the same device than the setup's; the SRS
         is shared read-only, so several provers can be driven concurrently from different host threads.
         ``custom``: up to 4 custom gate terms ``((i, j, l), column)``, each adding ``Q_k a^i b^j c^l`` to the gate
-        constraint (plonkathon_b200/custom_gates.py); ValueError for a malformed term."""
+        constraint (plonkathon_b200/custom_gates.py); ValueError for a malformed term.
+        ``lookup``: ``(q_K, (t1, t2, t3))``, a lookup argument over one table of three columns
+        (plonkathon_b200/lookup.py); ``prove_arrays`` then returns a 1216-byte ``LookupProof``.  ValueError for a
+        malformed argument; the library refuses it on the sharded prover."""
+        lk = check_lookup(lookup, group_order) if lookup is not None else None  # before any device work
         self = cls.__new__(cls)
         self.group_order = group_order
         self.setup = setup
@@ -116,7 +171,15 @@ class Prover:
         self.pk = None
         cols = {k: _as_le_rows(pk_arrays[k], group_order) for k in PK_ORDER}
         self._create(setup, group_order, cols, ctx, custom)
+        if lk is not None:
+            self._set_lookup(*lk)
         return self
+
+    def _set_lookup(self, qk, cols, rows):
+        keep = [to_le_rows(qk)] + [to_le_rows(c) for c in cols]
+        ptr = [k.ctypes.data_as(ctypes.c_void_p) for k in keep]
+        _lib.check(_lib.lib().pb200_prover_set_lookup(self._h, *ptr, rows))
+        self.lookup = True
 
     def _create(self, setup, n, cols, ctx=None, custom=()):
         exps, ccols = split_terms(custom, n)  # before any device work: a malformed term is a ValueError
@@ -149,13 +212,16 @@ class Prover:
 
     # ------------------------------------------------------------------ array-level fast path
     def prove_arrays(self, A, B, C, public) -> bytes:
-        """One C-ABI call for the whole proof (rounds 1-5 + transcript); returns the canonical 768 bytes."""
+        """One C-ABI call for the whole proof (rounds 1-5 + transcript); returns the canonical 768 bytes, or the
+        1216 bytes of a ``LookupProof`` on a prover with a lookup argument."""
         n = self.group_order
         a, b, c = (_as_le_rows(v, n) for v in (A, B, C))
         pub = _as_le_rows(public, len(public)) if len(public) else np.zeros((0, 32), dtype=np.uint8)
-        out = ctypes.create_string_buffer(768)
+        lookup = getattr(self, "lookup", False)
+        out = ctypes.create_string_buffer(LOOKUP_PROOF_BYTES if lookup else 768)
+        prove = _lib.lib().pb200_prover_prove_lookup if lookup else _lib.lib().pb200_prover_prove
         try:
-            _lib.check(_lib.lib().pb200_prover_prove(
+            _lib.check(prove(
                 self._h, a.ctypes.data_as(ctypes.c_void_p), b.ctypes.data_as(ctypes.c_void_p),
                 c.ctypes.data_as(ctypes.c_void_p), pub.ctypes.data_as(ctypes.c_void_p), pub.shape[0], out))
         except _lib.PlonkB200Error as e:

@@ -11,6 +11,7 @@ from . import _lib
 from .curve import G2, Scalar, _pt_bytes, _pt_from, g2_mul
 from .field import CURVE_ORDER, FIELD_MODULUS, FQ, FQ2
 from .custom_gates import split_terms
+from .lookup import check_lookup, padded_table, to_le_rows
 from .poly import Basis, Polynomial, _log2_exact
 from .prover import _as_le_rows
 from .verifier import VerificationKey  # noqa: F401  (re-exported: the reference's setup.py imports it too)
@@ -200,13 +201,16 @@ class Setup:
             h = self._lagrange[n]
         return h
 
-    def verification_key_arrays(self, group_order: int, pk_arrays: dict, custom=()) -> VerificationKey:
+    def verification_key_arrays(self, group_order: int, pk_arrays: dict, custom=(), lookup=None) -> VerificationKey:
         """``verification_key`` for circuits that exist only as arrays (``Prover.from_arrays``): QM..S3 as
         (n,32) uint8 little-endian Lagrange values in host memory.  ``custom``: the circuit's custom gate terms
-        ``((i, j, l), column)`` as given to ``Prover.from_arrays``; each column is committed too."""
+        ``((i, j, l), column)`` as given to ``Prover.from_arrays``; each column is committed too.  ``lookup``:
+        ``(q_K, (t1, t2, t3))`` as given to ``Prover.from_arrays``; the key gains [q_K], [t1], [t2], [t3] (the table
+        padded to n rows), the identity for a constant-zero column."""
         import numpy as np
         log_n = _log2_exact(group_order)
         exps, ccols = split_terms(custom, group_order)
+        lk = check_lookup(lookup, group_order) if lookup is not None else None
 
         def commit_host(col):
             col = np.ascontiguousarray(col).view(np.uint8).reshape(-1, 32)
@@ -224,7 +228,11 @@ class Setup:
 
         pts = [commit_host(pk_arrays[k]) for k in ("QM", "QL", "QR", "QO", "QC", "S1", "S2", "S3")]
         terms = tuple((e, commit_host(_as_le_rows(col, group_order))) for e, col in zip(exps, ccols))
-        return VerificationKey(group_order, *pts, self.X2, Scalar.root_of_unity(group_order), terms)
+        lk_pts = ()
+        if lk is not None:
+            qk, cols, _rows = lk
+            lk_pts = tuple(commit_host(to_le_rows(c)) for c in [qk] + padded_table(cols, group_order))
+        return VerificationKey(group_order, *pts, self.X2, Scalar.root_of_unity(group_order), terms, lk_pts)
 
     def verification_key(self, pk) -> VerificationKey:
         """setup.py:75-77."""

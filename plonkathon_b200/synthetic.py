@@ -38,6 +38,8 @@ class ArrayCircuit:
     text: list  # the same circuit in the reference's constraint language (small sizes only)
     # custom gate terms ((i, j, l), selector values per row), plonkathon_b200/custom_gates.py
     custom: list = field(default_factory=list)
+    # lookup argument (q_K per row, (t1, t2, t3)), plonkathon_b200/lookup.py; () without lookups
+    lookup: tuple = ()
 
     def wires_values(self):
         val = self.values
@@ -87,16 +89,25 @@ def permutation_polys(wire_L, wire_R, wire_O, group_order: int, n_constraints: i
 
 
 def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: float = 1.0,
-                  with_text: bool = False, custom=()) -> ArrayCircuit:
+                  with_text: bool = False, custom=(), lookup=None) -> ArrayCircuit:
     """Deterministic synthetic circuit with 2^log_n rows: ``n_public`` public-input rows, then a chain of
     multiplication / addition / add-constant gates whose operands are drawn from recently produced
     variables (so the permutation is non-trivial and the witness values are pseudo-random field elements).
 
     ``custom``: exponent triples (i, j, l) of custom gate terms; rows using them are mixed into the chain (see
-    ``_custom_row``).  Without it the random draws, and so the circuit, are exactly those of a plain circuit."""
+    ``_custom_row``).  Without it the random draws, and so the circuit, are exactly those of a plain circuit.
+
+    ``lookup``: a table ``(t1, t2, t3)``; lookup rows are mixed into the chain as one more kind of row (a quarter of
+    the rows without custom terms): the wires take a random table row as three new variables, q_K = 1 and every gate
+    selector is 0, and later gates use those variables like any other (copy constraints).  Without it the random
+    draws are unchanged."""
     from .custom_gates import check_exponents
+    from .lookup import check_lookup
     custom = check_exponents(custom)
     n = 1 << log_n
+    if lookup is not None:
+        _, table, rows = check_lookup(([0] * n, lookup), n)
+        QKl = [0] * n
     rng = random.Random(seed)
     m = max(n_public + 1, int(n * fill))
     m = min(m, n)
@@ -132,9 +143,14 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
         if first:  # make sure the private seeds are used so every variable appears in some cell
             ia, ib = n_public, n_public + 1
             first = False
-        kind = rng.randrange(3 + len(custom))
+        kind = rng.randrange(3 + len(custom) + (lookup is not None))
         out = nv
-        if kind >= 3:
+        if lookup is not None and kind == 3 + len(custom):  # (a, b, c) = a table row, q_K = 1
+            r = rng.randrange(rows)
+            values.extend(table[w][r] for w in range(3))
+            wL[row], wR[row], wO[row] = nv, nv + 1, nv + 2
+            QKl[row] = 1
+        elif kind >= 3:
             ic = rng.randrange(lo, nv)
             k = rng.randrange(0, 1 << 30)
             _custom_row(custom[kind - 3], QK[kind - 3], row, (ia, ib, ic), k, values, (wL, wR, wO), (QL, QO, QC))
@@ -159,7 +175,8 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
             if with_text:
                 text.append("%s <== %s + %d" % (name(out), name(ia), k))
         row += 1
-    return ArrayCircuit(n, m, wL, wR, wO, QL, QR, QM, QO, QC, n_public, values, text, list(zip(custom, QK)))
+    lk = (QKl, tuple(table)) if lookup is not None else ()
+    return ArrayCircuit(n, m, wL, wR, wO, QL, QR, QM, QO, QC, n_public, values, text, list(zip(custom, QK)), lk)
 
 
 def _custom_row(exps, Q, row, operands, k, values, wires, sel):
@@ -207,3 +224,9 @@ def custom_arrays(c: ArrayCircuit):
     custom=)`` and ``Setup.verification_key_arrays(..., custom=)``"""
     return [(e, np.frombuffer(b"".join(int(x).to_bytes(32, "little") for x in col), dtype=np.uint8).reshape(-1, 32).copy())
             for e, col in c.custom]
+
+
+def lookup_arrays(c: ArrayCircuit):
+    """-> the circuit's lookup argument ``(q_K, (t1, t2, t3))``, ready for ``Prover.from_arrays(..., lookup=)`` and
+    ``Setup.verification_key_arrays(..., lookup=)``"""
+    return c.lookup[0], c.lookup[1]

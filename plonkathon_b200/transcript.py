@@ -20,6 +20,18 @@ SCHEDULE = {
     5: (("W_z_1", "W_zw_1"), "point", ("u",)),
 }
 
+# The same table for a proof with a lookup argument (plonkathon_b200/lookup.py): step 1 also draws eta, step 1L absorbs
+# the lookup commitments, round 2 absorbs Z2 beside Z and round 4 the six lookup evaluations after the plain ones.
+LOOKUP_SCHEDULE = {
+    "1": (("a_1", "b_1", "c_1"), "point", ("beta", "gamma", "eta")),
+    "1L": (("f_1", "h1_1", "h2_1"), "point", ("delta", "epsilon")),
+    "2": (("z_1", "z2_1"), "point", ("alpha", "fft_cofactor")),
+    "3": (("t_lo_1", "t_mid_1", "t_hi_1"), "point", ("zeta",)),
+    "4": (("a_eval", "b_eval", "c_eval", "s1_eval", "s2_eval", "z_shifted_eval", "f_eval", "t_eval", "t_shifted_eval",
+           "h2_eval", "h1_shifted_eval", "z2_shifted_eval"), "scalar", ("v",)),
+    "5": (("W_z_1", "W_zw_1"), "point", ("u",)),
+}
+
 # Message1 .. Message5: plain records with exactly the reference's field names and order
 Message1, Message2, Message3, Message4, Message5 = (
     make_dataclass("Message%d" % rnd, [(name, object) for name in SCHEDULE[rnd][0]]) for rnd in sorted(SCHEDULE))
@@ -77,6 +89,17 @@ class Transcript:
             absorb(name.encode(), getattr(message, name))
         drawn = tuple(self.get_and_append_challenge(c.encode()) for c in challenges)
         return drawn if len(drawn) > 1 else drawn[0]
+
+    def replay(self, schedule: dict, values: dict) -> dict:
+        """every step of ``schedule`` in order over ``values`` (field name -> point or scalar); -> {label: challenge}"""
+        drawn = {}
+        for fields, kind, challenges in schedule.values():
+            absorb = self.append_point if kind == "point" else self.append_scalar
+            for name in fields:
+                absorb(name.encode(), values[name])
+            for c in challenges:
+                drawn[c] = self.get_and_append_challenge(c.encode())
+        return drawn
 
     def round_1(self, message):
         return self._round(1, message)

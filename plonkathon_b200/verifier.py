@@ -16,7 +16,7 @@ from .curve import G1, G2, Scalar, ec_lincomb, g1_neg, g2_add, g2_mul, pairing_p
 from . import _lib
 from .custom_gates import monomial
 from .field import CURVE_ORDER, FIELD_MODULUS
-from .transcript import Transcript
+from .transcript import LOOKUP_SCHEDULE, Transcript
 
 
 def _lagrange_terms_at(group_order: int, values, x: Scalar) -> Scalar:
@@ -48,6 +48,9 @@ class VerificationKey:
     w: Scalar
     # custom gate terms ((i, j, l), commitment to Q_k), in the prover's order (plonkathon_b200/custom_gates.py)
     custom: tuple = ()
+    # lookup argument (plonkathon_b200/lookup.py): ([q_K], [t1], [t2], [t3]), the identity (None) for a zero column;
+    # () for a circuit without lookups
+    lookup: tuple = ()
 
     def _custom_terms(self, a, b, c):
         """the custom gates' part of the linearisation: sum_k m_k(a, b, c) [Q_k]"""
@@ -75,12 +78,20 @@ class VerificationKey:
                 return False
         return True
 
+    def _matches(self, pf) -> bool:
+        """a lookup key takes lookup proofs only, a plain key plain proofs only"""
+        from .prover import LookupProof
+        return bool(self.lookup) == isinstance(pf, LookupProof)
+
     def verify_proof(self, group_order: int, pf, public=[]) -> bool:
         """verifier.py:40-73: the batched form -- one pairing equation, the linearisation commitment never
-        formed on its own.  Malformed proofs (points off the curve, the identity) are rejected, not raised."""
-        if not self._well_formed(pf):
+        formed on its own.  Malformed proofs (points off the curve, the identity) are rejected, not raised; so is a
+        plain proof against a lookup key and the reverse."""
+        if not self._matches(pf) or not self._well_formed(pf):
             return False
         try:
+            if self.lookup:
+                return self._verify_lookup(group_order, pf, public, batched=True)
             return self._verify_batched(group_order, pf, public)
         except _lib.PlonkB200Error:
             return False
@@ -114,9 +125,11 @@ class VerificationKey:
     def verify_proof_unoptimized(self, group_order: int, pf, public=[]) -> bool:
         """verifier.py:76-92: rebuild the commitment to the prover's linearisation polynomial R (R(zeta) == 0),
         then check the opening at zeta and the opening of Z at zeta*w separately."""
-        if not self._well_formed(pf):
+        if not self._matches(pf) or not self._well_formed(pf):
             return False
         try:
+            if self.lookup:
+                return self._verify_lookup(group_order, pf, public, batched=False)
             return self._verify_unoptimized(group_order, pf, public)
         except _lib.PlonkB200Error:
             return False
@@ -153,6 +166,68 @@ class VerificationKey:
         z_open = ec_lincomb([(proof["z_1"], 1), (G1, -zw)])
         x_minus_zeta_w = g2_add(self.X_2, g2_mul(G2, -(zeta * root)))
         return pairing_product_is_one([(z_open, G2), (g1_neg(proof["W_zw_1"]), x_minus_zeta_w)])
+
+    # ---- lookup proofs (plonkathon_b200/lookup.py, DESIGN.md): both routines, selected by ``batched``
+    def _verify_lookup(self, group_order: int, pf, public, batched: bool) -> bool:
+        n = group_order
+        proof = pf.flatten()
+        ch = Transcript(b"plonk").replay(LOOKUP_SCHEDULE, proof)
+        beta, gamma, eta, delta, eps = ch["beta"], ch["gamma"], ch["eta"], ch["delta"], ch["epsilon"]
+        alpha, zeta, v, u = ch["alpha"], ch["zeta"], ch["v"], ch["u"]
+        zh_ev = zeta ** n - 1
+        l0_ev = zh_ev / ((zeta - 1) * n)
+        pi_ev = _lagrange_terms_at(n, [-int(x) % CURVE_ORDER for x in public], zeta)
+        a, b, c = proof["a_eval"], proof["b_eval"], proof["c_eval"]
+        s1, s2, zw = proof["s1_eval"], proof["s2_eval"], proof["z_shifted_eval"]
+        fe, te, tw = proof["f_eval"], proof["t_eval"], proof["t_shifted_eval"]
+        h2e, h1w, z2w = proof["h2_eval"], proof["h1_shifted_eval"], proof["z2_shifted_eval"]
+        root = Scalar.root_of_unity(n)
+        zeta_n = zeta ** n
+        a2 = alpha * alpha
+        a3, a4 = a2 * alpha, a2 * a2
+        a5 = a4 * alpha
+        od = delta + 1
+        eod = eps * od
+        hw = eod + h2e + delta * h1w
+        qk, t1, t2, t3 = self.lookup
+        sigma_bar = (a + beta * s1 + gamma) * (b + beta * s2 + gamma) * zw
+        # the linearisation R without its constant, and the constant r0 (R(zeta) == 0)
+        r_terms = [
+            (self.Qm, a * b), (self.Ql, a), (self.Qr, b), (self.Qo, c), (self.Qc, 1), *self._custom_terms(a, b, c),
+            (proof["z_1"], (a + beta * zeta + gamma) * (b + beta * 2 * zeta + gamma) * (c + beta * 3 * zeta + gamma)
+             * alpha + l0_ev * a2),
+            (self.S3, -sigma_bar * alpha * beta),
+            (proof["t_lo_1"], -zh_ev), (proof["t_mid_1"], -zh_ev * zeta_n), (proof["t_hi_1"], -zh_ev * zeta_n * zeta_n),
+            # alpha^3 q_K (a + eta b + eta^2 c - f)
+            (qk, a3 * (a + eta * b + eta * eta * c - fe)),
+            # alpha^4 [Z2 (1+d)(e+f)(e(1+d) + t + d t_w) - z2_w (e(1+d) + H1 + d h2) hw] + alpha^5 L0 (Z2 - 1)
+            (proof["z2_1"], a4 * od * (eps + fe) * (eod + te + delta * tw) + a5 * l0_ev),
+            (proof["h1_1"], -a4 * z2w * hw),
+        ]
+        r0 = (pi_ev - l0_ev * a2 - sigma_bar * alpha * (c + gamma) - a4 * z2w * (eod + delta * h2e) * hw
+              - a5 * l0_ev)
+        v2, v3, v4, v5 = v ** 2, v ** 3, v ** 4, v ** 5
+        v6, v7, v8 = v5 * v, v5 * v2, v5 * v3
+        at_zeta = [(proof["a_1"], v), (proof["b_1"], v2), (proof["c_1"], v3), (self.S1, v4), (self.S2, v5),
+                   (proof["f_1"], v6), (proof["h2_1"], v8)]
+        t_parts = [(t1, Scalar(1)), (t2, eta), (t3, eta * eta)]  # [T] = [t1] + eta [t2] + eta^2 [t3]
+        e_zeta = v * a + v2 * b + v3 * c + v4 * s1 + v5 * s2 + v6 * fe + v7 * te + v8 * h2e
+        e_zw = zw + v * tw + v2 * h1w + v3 * z2w
+        if batched:
+            d_pt = ec_lincomb(r_terms + [(proof["z_1"], u), (proof["z2_1"], u * v3), (proof["h1_1"], u * v2)]
+                              + [(p, k * (v7 + u * v)) for p, k in t_parts] + at_zeta)
+            e_scalar = -r0 + e_zeta + u * e_zw
+            lhs = ec_lincomb([(proof["W_z_1"], 1), (proof["W_zw_1"], u)])
+            rhs = ec_lincomb([(proof["W_z_1"], zeta), (proof["W_zw_1"], u * zeta * root), (d_pt, 1), (G1, -e_scalar)])
+            return pairing_product_is_one([(lhs, self.X_2), (g1_neg(rhs), G2)])
+        batch = ec_lincomb(r_terms + [(G1, r0)] + at_zeta + [(p, k * v7) for p, k in t_parts] + [(G1, -e_zeta)])
+        x_minus_zeta = g2_add(self.X_2, g2_mul(G2, -zeta))
+        if not pairing_product_is_one([(batch, G2), (g1_neg(proof["W_z_1"]), x_minus_zeta)]):
+            return False
+        shifted = ec_lincomb([(proof["z_1"], 1), (proof["h1_1"], v2), (proof["z2_1"], v3)]
+                             + [(p, k * v) for p, k in t_parts] + [(G1, -e_zw)])
+        x_minus_zeta_w = g2_add(self.X_2, g2_mul(G2, -(zeta * root)))
+        return pairing_product_is_one([(shifted, G2), (g1_neg(proof["W_zw_1"]), x_minus_zeta_w)])
 
     def compute_challenges(self, proof):
         """verifier.py:95-106: replay the prover's transcript over the proof's five messages."""
