@@ -44,22 +44,19 @@ Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h
                       const uint8_t* h_exps, const uint8_t* const* h_custom, bool sharded);
 void prover_destroy(Prover* p);
 void prover_prove(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t* hC, const uint8_t* h_public,
-                  uint64_t n_public, uint8_t* out768, bool wires_on_device);
+                  uint64_t n_public, uint8_t* out, bool wires_on_device);
 void prover_round1(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t* hC, const uint8_t* h_public,
                    uint64_t n_public, bool wires_on_device);
 void prover_round2(Prover* P, const Fr& beta_c, const Fr& gamma_c);
 void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c);
 void prover_round4(Prover* P, const Fr& zeta_c);
 void prover_round5(Prover* P, const Fr& v_c);
-void prover_serialize(const Prover* P, uint8_t* out768);
+void prover_serialize(const Prover* P, uint8_t* out);
 void prover_set_zk(Prover* P, bool enable, const uint8_t* h_blinders);
 void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* const* h_tab, uint64_t rows);
 void prover_round_lookup(Prover* P, const Fr& eta_c);
 void prover_round2_lookup(Prover* P, const Fr& beta_c, const Fr& gamma_c, const Fr& delta_c, const Fr& epsilon_c);
 void prover_round4_lookup(Prover* P, const Fr& zeta_c);
-void prover_prove_lookup(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t* hC, const uint8_t* h_public,
-                         uint64_t n_public, uint8_t* out1216);
-void prover_serialize_lookup(const Prover* P, uint8_t* out1216);
 void g1_combine_partials_host(const G1XYZZ* parts, uint32_t count, uint8_t* out_xy, int* is_identity);
 void host_join_bucket_shards(const SR* all, uint32_t world, uint32_t sets, uint32_t nloc, G1XYZZ* out);
 void host_join_bucket_shards_strided(const SR* all, uint32_t world, uint32_t sets, G1XYZZ* out);
@@ -105,13 +102,7 @@ struct DeviceGuard {
 static Fr load_fr_canonical(const uint8_t* h) {
   Fr a;
   memcpy(a.v, h, 32);
-  // reject non-canonical input
-  Fr m = Fr::modulus();
-  bool lt = false;
-  for (int i = 7; i >= 0; i--) {
-    if (a.v[i] != m.v[i]) { lt = a.v[i] < m.v[i]; break; }
-  }
-  PB_CHECK(lt, "Fr value not reduced below the modulus");
+  PB_CHECK(fp_is_canonical(a), "Fr value not reduced below the modulus");
   return a;
 }
 
@@ -573,14 +564,16 @@ int pb200_prover_round4_lookup(pb200_prover* p, const uint8_t* zeta, uint8_t* h_
 int pb200_prover_prove_lookup(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                               const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof1216) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  prover_prove_lookup(reinterpret_cast<Prover*>(p), h_A, h_B, h_C, h_public, n_public, h_proof1216);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  PB_CHECK(P->lk, "this prover has no lookup table (pb200_prover_set_lookup)");
+  prover_prove(P, h_A, h_B, h_C, h_public, n_public, h_proof1216, false);
   PB_API_END
 }
 int pb200_prover_serialize_lookup(pb200_prover* p, uint8_t* h_proof1216) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   Prover* P = reinterpret_cast<Prover*>(p);
   PB_CHECK(P->lk, "this prover has no lookup table: use pb200_prover_serialize (768 bytes)");
-  prover_serialize_lookup(P, h_proof1216);
+  prover_serialize(P, h_proof1216);
   PB_API_END
 }
 int pb200_g1_combine_partials_host(const uint8_t* h_xyzz, unsigned count, uint8_t* h_out_xy, int* is_identity) {
@@ -655,12 +648,7 @@ int pb200_transcript_get_and_append_challenge(pb200_transcript* t, const uint8_t
 static Fq load_fq_canonical(const uint8_t* h) {
   Fq a;
   memcpy(a.v, h, 32);
-  Fq m = Fq::modulus();
-  bool lt = false;
-  for (int i = 7; i >= 0; i--) {
-    if (a.v[i] != m.v[i]) { lt = a.v[i] < m.v[i]; break; }
-  }
-  PB_CHECK(lt, "Fq value not reduced below the modulus");
+  PB_CHECK(fp_is_canonical(a), "Fq value not reduced below the modulus");
   return fp_to_mont(a);
 }
 static G2Affine load_g2(const uint8_t* h, bool inf) {

@@ -107,6 +107,15 @@ struct alignas(16) Fp {
   PB_HD bool operator!=(const Fp& b) const { return !(*this == b); }
 };
 
+// a < p: a is the canonical (fully reduced) representative of its value
+template <class P>
+PB_HD bool fp_is_canonical(const Fp<P>& a) {
+  const Fp<P> m = Fp<P>::modulus();
+  for (int i = 7; i >= 0; i--)
+    if (a.v[i] != m.v[i]) return a.v[i] < m.v[i];
+  return false;
+}
+
 // r = a - p if a >= p else a     (a < 2p < 2^256)
 template <class P>
 PB_HD void fp_reduce_once(Fp<P>& a) {

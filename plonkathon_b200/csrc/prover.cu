@@ -102,25 +102,14 @@ __device__ __forceinline__ Fr ldg_fr(const Fr* p) {
 static Fr load_fr_checked(const uint8_t* h) {
   Fr a;
   memcpy(a.v, h, 32);
-  const Fr m = Fr::modulus();
-  bool lt = false;
-  for (int i = 7; i >= 0; i--) {
-    if (a.v[i] != m.v[i]) { lt = a.v[i] < m.v[i]; break; }
-  }
-  PB_CHECK(lt, "public input not reduced below the field modulus");
+  PB_CHECK(fp_is_canonical(a), "public input not reduced below the field modulus");
   return a;
 }
 
 // wire values arrive canonical (< r): a value >= r would silently become a different field element in fp_to_mont
 __global__ void k_count_noncanonical(const Fr* v, uint64_t n, uint32_t* bad) {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const Fr x = ldg_fr(v + i), m = Fr::modulus();
-  bool lt = false;
-  for (int l = 7; l >= 0; l--) {
-    if (x.v[l] != m.v[l]) { lt = x.v[l] < m.v[l]; break; }
-  }
-  if (!lt) atomicAdd(bad, 1u);
+  if (i < n && !fp_is_canonical(ldg_fr(v + i))) atomicAdd(bad, 1u);
 }
 
 // prover.py:108-116: A*QL + B*QR + A*B*QM + C*QO + PI + QC (+ sum_k Q_k m_k(A, B, C)) == 0 on every row
@@ -187,59 +176,74 @@ __global__ void __launch_bounds__(128) k_batch_div(const Fr* num, const Fr* den,
   }
 }
 
-// ---- exclusive prefix product: Z[0] = 1, Z[i+1] = Z[i] * f[i]   (3 kernels, tiles of 256 x 8) ----
-#define PB_PROD_TILE 2048
-__device__ __forceinline__ Fr block_exclusive_prod_256(const Fr& v, Fr* sh, Fr* total) {
+// ---- exclusive scans over a monoid, 3 kernels over tiles of 256 x 8: the vector's tiles (one total per tile), the
+// tile totals (one block), then every element from its tile's start.  ScanMul is the grand product, ScanAdd the
+// suffix sum of the division below.
+#define PB_FR_TILE 2048
+struct ScanMul {
+  static __device__ __forceinline__ Fr id() { return Fr::one(); }
+  static __device__ __forceinline__ Fr op(const Fr& a, const Fr& b) { return fp_mul(a, b); }
+};
+struct ScanAdd {
+  static __device__ __forceinline__ Fr id() { return Fr::zero(); }
+  static __device__ __forceinline__ Fr op(const Fr& a, const Fr& b) { return fp_add(a, b); }
+};
+template <class Op>
+__device__ __forceinline__ Fr block_exclusive_scan_256(const Fr& v, Fr* sh, Fr* total) {
   // Hillis-Steele over 256 threads in shared memory (inclusive), then shift
   sh[threadIdx.x] = v;
   __syncthreads();
   for (int d = 1; d < 256; d <<= 1) {
     Fr x = sh[threadIdx.x];
-    Fr y = (int)threadIdx.x >= d ? sh[threadIdx.x - d] : Fr::one();
+    Fr y = (int)threadIdx.x >= d ? sh[threadIdx.x - d] : Op::id();
     __syncthreads();
-    if ((int)threadIdx.x >= d) sh[threadIdx.x] = fp_mul(x, y);
+    if ((int)threadIdx.x >= d) sh[threadIdx.x] = Op::op(x, y);
     __syncthreads();
   }
-  Fr excl = threadIdx.x ? sh[threadIdx.x - 1] : Fr::one();
+  Fr excl = threadIdx.x ? sh[threadIdx.x - 1] : Op::id();
   *total = sh[255];
   __syncthreads();
   return excl;
 }
-__global__ void __launch_bounds__(256) k_prod_tiles(const Fr* f, uint64_t n, Fr* tile_prod) {
-  __shared__ Fr sh[256];
-  uint64_t base = (uint64_t)blockIdx.x * PB_PROD_TILE + threadIdx.x * 8;
-  Fr p = Fr::one();
-  for (int k = 0; k < 8; k++) if (base + k < n) p = fp_mul(p, ldg_fr(f + base + k));
-  Fr total;
-  block_exclusive_prod_256(p, sh, &total);
-  if (threadIdx.x == 0) tile_prod[blockIdx.x] = total;
-}
-__global__ void __launch_bounds__(256) k_prod_scan_tiles(Fr* tile_prod, uint32_t n_tiles, Fr* total_out) {
+// the tile totals in place -> the exclusive scan of them, and the grand total
+template <class Op>
+__global__ void __launch_bounds__(256) k_fr_scan_tiles(Fr* tiles, uint32_t n_tiles, Fr* total_out) {
   __shared__ Fr sh[256];
   uint32_t per = (n_tiles + 255) / 256;
   uint32_t lo = threadIdx.x * per, hi = min(lo + per, n_tiles);
-  Fr p = Fr::one();
-  for (uint32_t i = lo; i < hi; i++) p = fp_mul(p, tile_prod[i]);
+  Fr p = Op::id();
+  for (uint32_t i = lo; i < hi; i++) p = Op::op(p, tiles[i]);
   Fr total;
-  Fr run = block_exclusive_prod_256(p, sh, &total);
+  Fr run = block_exclusive_scan_256<Op>(p, sh, &total);
   for (uint32_t i = lo; i < hi; i++) {
-    Fr c = tile_prod[i];
-    tile_prod[i] = run;
-    run = fp_mul(run, c);
+    Fr c = tiles[i];
+    tiles[i] = run;
+    run = Op::op(run, c);
   }
   if (threadIdx.x == 0) *total_out = total;
+}
+
+// ---- exclusive prefix product: Z[0] = 1, Z[i+1] = Z[i] * f[i] ----
+__global__ void __launch_bounds__(256) k_prod_tiles(const Fr* f, uint64_t n, Fr* tile_prod) {
+  __shared__ Fr sh[256];
+  uint64_t base = (uint64_t)blockIdx.x * PB_FR_TILE + threadIdx.x * 8;
+  Fr p = Fr::one();
+  for (int k = 0; k < 8; k++) if (base + k < n) p = fp_mul(p, ldg_fr(f + base + k));
+  Fr total;
+  block_exclusive_scan_256<ScanMul>(p, sh, &total);
+  if (threadIdx.x == 0) tile_prod[blockIdx.x] = total;
 }
 // carry (optional): the product of everything below this vector (the slabs of the lower ranks in a sharded round 2)
 __global__ void __launch_bounds__(256) k_prod_apply(const Fr* f, uint64_t n, const Fr* tile_prod, const Fr* carry, Fr* Z) {
   __shared__ Fr sh[256];
-  uint64_t base = (uint64_t)blockIdx.x * PB_PROD_TILE + threadIdx.x * 8;
+  uint64_t base = (uint64_t)blockIdx.x * PB_FR_TILE + threadIdx.x * 8;
   Fr c[8];
   Fr p = Fr::one();
   for (int k = 0; k < 8; k++) { c[k] = base + k < n ? ldg_fr(f + base + k) : Fr::one(); p = fp_mul(p, c[k]); }
   Fr total;
   Fr start = tile_prod[blockIdx.x];
   if (carry) start = fp_mul(start, ldg_fr(carry));
-  Fr run = fp_mul(start, block_exclusive_prod_256(p, sh, &total));
+  Fr run = fp_mul(start, block_exclusive_scan_256<ScanMul>(p, sh, &total));
   for (int k = 0; k < 8; k++) {
     if (base + k < n) Z[base + k] = run;
     run = fp_mul(run, c[k]);
@@ -263,47 +267,16 @@ __global__ void k_prod_carry(const Fr* totals, uint32_t world, uint32_t rank, Fr
 // ---- division by (X - z) in coefficient space ---------------------------------------------------------------
 // q_(k-1) = s_k with s_k = N_k + z s_(k+1); multiplying through by z^k turns the recurrence into a plain suffix
 // sum: s_k z^k = sum_(m >= k) N_m z^m.  So: u = N .* z^m, suffix-sum scan (additions only), multiply by z^-k.
-#define PB_SUM_TILE 2048
-__device__ __forceinline__ Fr block_exclusive_sum_256(const Fr& v, Fr* sh, Fr* total) {
-  sh[threadIdx.x] = v;
-  __syncthreads();
-  for (int d = 1; d < 256; d <<= 1) {
-    Fr x = sh[threadIdx.x];
-    Fr y = (int)threadIdx.x >= d ? sh[threadIdx.x - d] : Fr::zero();
-    __syncthreads();
-    if ((int)threadIdx.x >= d) sh[threadIdx.x] = fp_add(x, y);
-    __syncthreads();
-  }
-  Fr excl = threadIdx.x ? sh[threadIdx.x - 1] : Fr::zero();
-  *total = sh[255];
-  __syncthreads();
-  return excl;
-}
-// all three kernels walk the vector from the top: logical position i <-> index n-1-i
+// The tile and apply kernels walk the vector from the top: logical position i <-> index n-1-i
 __global__ void __launch_bounds__(256) k_sufsum_tiles(const Fr* N, const Fr* zpow, uint64_t n, Fr* tile_sum) {
   __shared__ Fr sh[256];
-  uint64_t base = (uint64_t)blockIdx.x * PB_SUM_TILE + threadIdx.x * 8;
+  uint64_t base = (uint64_t)blockIdx.x * PB_FR_TILE + threadIdx.x * 8;
   Fr p = Fr::zero();
   for (int k = 0; k < 8; k++)
     if (base + k < n) { uint64_t m = n - 1 - (base + k); p = fp_add(p, fp_mul(ldg_fr(N + m), ldg_fr(zpow + m))); }
   Fr total;
-  block_exclusive_sum_256(p, sh, &total);
+  block_exclusive_scan_256<ScanAdd>(p, sh, &total);
   if (threadIdx.x == 0) tile_sum[blockIdx.x] = total;
-}
-__global__ void __launch_bounds__(256) k_sufsum_scan_tiles(Fr* tile_sum, uint32_t n_tiles, Fr* total_out) {
-  __shared__ Fr sh[256];
-  uint32_t per = (n_tiles + 255) / 256;
-  uint32_t lo = threadIdx.x * per, hi = min(lo + per, n_tiles);
-  Fr p = Fr::zero();
-  for (uint32_t i = lo; i < hi; i++) p = fp_add(p, tile_sum[i]);
-  Fr total;
-  Fr run = block_exclusive_sum_256(p, sh, &total);
-  for (uint32_t i = lo; i < hi; i++) {
-    Fr c = tile_sum[i];
-    tile_sum[i] = run;
-    run = fp_add(run, c);
-  }
-  if (threadIdx.x == 0) *total_out = total;
 }
 // out[m-1] = z^-m * (carry + sum_(m' >= m) N_m' z^m')  for m >= 1 ; out[n-1] = carry * z^-n ; the m = 0 sum is dropped.
 // One device: carry = 0 (the m = 0 sum is N(z), the remainder).  Slab of a sharded division: N, zpow, zinvpow and out
@@ -311,7 +284,7 @@ __global__ void __launch_bounds__(256) k_sufsum_scan_tiles(Fr* tile_sum, uint32_
 __global__ void __launch_bounds__(256) k_sufsum_apply(const Fr* N, const Fr* zpow, const Fr* zinvpow, uint64_t n,
                                                       const Fr* tile_sum, const Fr* carry, Fr last_scale, Fr* out) {
   __shared__ Fr sh[256];
-  uint64_t base = (uint64_t)blockIdx.x * PB_SUM_TILE + threadIdx.x * 8;
+  uint64_t base = (uint64_t)blockIdx.x * PB_FR_TILE + threadIdx.x * 8;
   Fr c[8];
   Fr p = Fr::zero();
   for (int k = 0; k < 8; k++) {
@@ -321,7 +294,7 @@ __global__ void __launch_bounds__(256) k_sufsum_apply(const Fr* N, const Fr* zpo
   }
   const Fr cy = carry ? ldg_fr(carry) : Fr::zero();
   Fr total;
-  Fr run = fp_add(fp_add(tile_sum[blockIdx.x], cy), block_exclusive_sum_256(p, sh, &total));
+  Fr run = fp_add(fp_add(tile_sum[blockIdx.x], cy), block_exclusive_scan_256<ScanAdd>(p, sh, &total));
   for (int k = 0; k < 8; k++) {
     run = fp_add(run, c[k]);  // inclusive suffix sum at m
     if (base + k < n) {
@@ -440,8 +413,10 @@ __global__ void __launch_bounds__(128) k_horner_strided(EvalArgs a, Fr* H) {
 }
 
 // ---- coefficient-space linear combination: out[k] = sum_i w[i] * vec[i][k] (+ c0 at k == 0) -----------------
-// indices [first, first + n) of the result (a slab of a sharded round 5; first = 0, n = everything on one device)
-struct LinCombArgs { const Fr* vec[20]; Fr w[20]; Fr c0; int count; uint64_t n, first; };
+// indices [first, first + n) of the result (a slab of a sharded round 5; first = 0, n = everything on one device).
+// 26 slots: round 5's largest batch is 19 plain terms (5 gate selectors, 4 custom, Z, S3, T1-T3, A, B, C, S1, S2) and
+// 6 lookup terms.
+struct LinCombArgs { const Fr* vec[26]; Fr w[26]; Fr c0; int count; uint64_t n, first; };
 __global__ void __launch_bounds__(128) k_lincomb(LinCombArgs a, Fr* out) {
   uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= a.n) return;
@@ -451,27 +426,12 @@ __global__ void __launch_bounds__(128) k_lincomb(LinCombArgs a, Fr* out) {
   out[k] = acc;
 }
 
-// the same, added to out: the lookup terms of round 5 (the plain batch already takes up to 19 of the 20 slots)
-__global__ void __launch_bounds__(128) k_lincomb_add(LinCombArgs a, Fr* out) {
-  uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= a.n) return;
-  k += a.first;
-  Fr acc = k == 0 ? a.c0 : Fr::zero();
-  for (int i = 0; i < a.count; i++) acc = fp_add(acc, fp_mul(a.w[i], ldg_fr(a.vec[i] + k)));
-  out[k] = fp_add(out[k], acc);
-}
-
 // den[j] = shift * roots[j] - point    (the n-point coset x_j = shift * w^j minus the opening point)
 __global__ void k_coset_minus(const Fr* roots, Fr shift, Fr point, uint64_t n, Fr* den) {
   uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j < n) den[j] = fp_sub(fp_mul(shift, ldg_fr(roots + j)), point);
 }
 
-// out[j] = 1 / (n * (x_j - 1)) * (x_j^n - 1),   x_j = X[j], x_j^n = gn * i4[j & 3]
-__global__ void k_l0_num(const Fr* X, uint64_t n4, Fr n_mont, Fr one, Fr* den) {
-  uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (j < n4) den[j] = fp_mul(n_mont, fp_sub(ldg_fr(X + j), one));
-}
 struct Four { Fr v[4]; };
 // v[j] *= m[(global coset index of j) mod 4], global index = world * j + rank
 __global__ void k_scale_by4(Fr* v, uint64_t n4, Four m, uint32_t world, uint32_t rank) {
@@ -625,6 +585,30 @@ static void upload_mont(Context* ctx, DevBuf& dst, const uint8_t* h, uint64_t n)
 
 Comm* ctx_comm(Context* ctx);
 
+// cached per prover: pi_basis[i][j] = L_i(x_j) on this rank's slice of the fixed coset for the first `count` rows.
+// L0 is made when the prover is created (the quotient's L0 term); the public inputs add the rows they need.
+static void ensure_pi_basis(Prover* P, int count) {
+  Context* ctx = P->ctx;
+  const uint64_t n = P->n, ne = P->n_ext;
+  cudaStream_t st = ctx->stream;
+  if ((int)P->pi_basis.size() >= count) return;
+  Fr w = fr_root_of_unity(P->log_n);
+  DevBuf den(ne * 32);
+  for (int i = (int)P->pi_basis.size(); i < count; i++) {
+    Fr wi = fp_pow_u64(w, (uint64_t)i);
+    Four zh;  // w^i (x_j^n - 1): four values
+    for (int k = 0; k < 4; k++) zh.v[k] = fp_mul(wi, P->zh[k]);
+    P->pi_basis.emplace_back(ne * 32);
+    Fr* out = P->pi_basis.back().as<Fr>();
+    k_lagrange_den<<<PB_GRID(ne, 256), 0, st>>>(P->xs.as<Fr>(), ne, wi, fr_from_u64(n), den.as<Fr>());
+    uint64_t T = (ne + PB_BATCH_CH - 1) / PB_BATCH_CH;
+    k_batch_div<<<PB_GRID(T, 128), 0, st>>>(nullptr, den.as<Fr>(), out, ne, T);
+    k_scale_by4<<<PB_GRID(ne, 256), 0, st>>>(out, ne, zh, (uint32_t)P->world, (uint32_t)P->rank);
+    ctx->launches += 3;
+  }
+  PB_CUDA(cudaStreamSynchronize(st));
+}
+
 // Custom term exponents (i, j, l) -> the wires of the monomial.  Degree 1 duplicates QL / QR / QO, degree 4 would need
 // a fourth quotient piece, (1, 1, 0) is QM's term, and a repeated triple is one term split in two.
 static void set_custom_terms(Prover* P, int n_custom, const uint8_t* h_exps) {
@@ -693,27 +677,14 @@ Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h
   P->xs.alloc(ne * 32);
   launch_powers(ctx, P->xs.as<Fr>(), ne, fp_pow_u64(mu, G), shift);
   // Z_H on the coset takes 4 values: g^n * i^(j mod 4) - 1, i = mu^n, j the global coset index
-  Fr gn = fp_pow_u64(P->g, n);
   Fr i4 = fp_pow_u64(mu, n);
-  Four zh;
-  Fr cur = gn;
+  Fr cur = fp_pow_u64(P->g, n);
   for (int k = 0; k < 4; k++) {
-    zh.v[k] = fp_sub(cur, one);
-    P->zh[k] = zh.v[k];
-    P->zh_inv[k] = fp_inv(zh.v[k]);
+    P->zh[k] = fp_sub(cur, one);
+    P->zh_inv[k] = fp_inv(P->zh[k]);
     cur = fp_mul(cur, i4);
   }
-  // L0(x_j) = (x_j^n - 1) / (n (x_j - 1))
-  P->l0_ext.alloc(ne * 32);
-  {
-    DevBuf den(ne * 32);
-    k_l0_num<<<PB_GRID(ne, 256), 0, st>>>(P->xs.as<Fr>(), ne, fr_from_u64(n), one, den.as<Fr>());
-    uint64_t T = (ne + PB_BATCH_CH - 1) / PB_BATCH_CH;
-    k_batch_div<<<PB_GRID(T, 128), 0, st>>>(nullptr, den.as<Fr>(), P->l0_ext.as<Fr>(), ne, T);
-    k_scale_by4<<<PB_GRID(ne, 256), 0, st>>>(P->l0_ext.as<Fr>(), ne, zh, G, R);
-    ctx->launches += 3;
-    PB_CUDA(cudaStreamSynchronize(st));
-  }
+  ensure_pi_basis(P.get(), 1);  // L0, for the quotient
   for (int k = 0; k < Prover::CUSTOM0 + n_custom; k++) {
     upload_mont(ctx, P->sel_lag[k], k < Prover::CUSTOM0 ? h_pk[k] : h_custom[k - Prover::CUSTOM0], n);
     P->sel_coeff[k].alloc(n * 32);
@@ -826,11 +797,7 @@ static void zk_random_blinders(Fr* out_mont, int count) {
   }
   const Fr m = Fr::modulus();
   auto reduce = [&](Fr x) {  // x < 2^256 < 6 r: subtract r while x >= r
-    for (;;) {
-      bool ge = true;
-      for (int i = 7; i >= 0; i--)
-        if (x.v[i] != m.v[i]) { ge = x.v[i] > m.v[i]; break; }
-      if (!ge) return x;
+    while (!fp_is_canonical(x)) {
       uint64_t borrow = 0;
       for (int i = 0; i < 8; i++) {
         uint64_t d = (uint64_t)x.v[i] - m.v[i] - borrow;
@@ -838,6 +805,7 @@ static void zk_random_blinders(Fr* out_mont, int count) {
         borrow = (d >> 32) & 1;
       }
     }
+    return x;
   };
   for (int k = 0; k < count; k++) {
     Fr lo, hi;
@@ -863,14 +831,10 @@ void prover_set_zk(Prover* P, bool enable, const uint8_t* h_blinders) {
   PB_CHECK(srs_size(P->srs) >= P->n + 6,
            "Not enough powers in setup: zero-knowledge proving needs n + 6 powers (T3' has n + 6 coefficients)");
   if (h_blinders) {
-    const Fr m = Fr::modulus();
     for (int k = 0; k < Prover::ZK_BLINDERS; k++) {
       Fr b;
       memcpy(b.v, h_blinders + 32 * k, 32);
-      bool lt = false;
-      for (int i = 7; i >= 0; i--)
-        if (b.v[i] != m.v[i]) { lt = b.v[i] < m.v[i]; break; }
-      PB_CHECK(lt, "zero-knowledge blinder not reduced below the field modulus");
+      PB_CHECK(fp_is_canonical(b), "zero-knowledge blinder not reduced below the field modulus");
       P->zk_fixed_b[k] = b;
     }
   }
@@ -912,13 +876,6 @@ static ZkPatch zh_multiple(std::initializer_list<Fr> c) {
 // k_lookup_z2_terms.  The quotient gains k_quotient_lookup's three terms (degree <= 3n); round 5 opens F, T, H2 at
 // zeta and T, H1, Z2 at zeta w.  The index, histogram and placement do not depend on eta and run in round 1.
 
-static bool fr_is_canonical(const Fr& a) {
-  const Fr m = Fr::modulus();
-  for (int i = 7; i >= 0; i--)
-    if (a.v[i] != m.v[i]) return a.v[i] < m.v[i];
-  return false;
-}
-
 void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* const* h_tab, uint64_t rows) {
   Context* ctx = P->ctx;
   const uint64_t n = P->n;
@@ -942,7 +899,7 @@ void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* const* h_t
     for (uint64_t r = 0; r < n; r++) {
       Fr x;
       memcpy(x.v, h_tab[w] + 32 * std::min(r, rows - 1), 32);
-      PB_CHECK(fr_is_canonical(x), "lookup table value not reduced below the field modulus");
+      PB_CHECK(fp_is_canonical(x), "lookup table value not reduced below the field modulus");
       tab[w][r] = fp_to_mont(x);
     }
   }
@@ -1031,71 +988,71 @@ void prover_round_lookup(Prover* P, const Fr& eta_c) {
   P->commit_batch(fh, 3, n, P->lk_pts[0]);
 }
 
+// A grand product (Z of the permutation argument, Z2 of the lookup argument) from its per-row numerators and
+// denominators on this rank's slab [lo, lo + n/G) -- num and den point at the slab; num is overwritten with num / den.
+// lag (all n rows) gets the exclusive prefix product, coeff its coefficients.  One proof across G ranks: the divisions
+// and the in-slab prefix products are local; the slab products are exchanged with a 32-byte allgather (the product of
+// the lower slabs is the slab's carry) and the values with one bulk allgather.  The product over all rows must be 1:
+// `not_one` is the error otherwise.
+static void grand_product(Prover* P, Fr* num, const Fr* den, Fr* lag, Fr* coeff, const char* not_one) {
+  Context* ctx = P->ctx;
+  cudaStream_t st = ctx->stream;
+  const uint64_t ns = P->n / (uint64_t)P->world, lo = ns * (uint64_t)P->rank;
+  uint64_t T = (ns + PB_BATCH_CH - 1) / PB_BATCH_CH;
+  k_batch_div<<<PB_GRID(T, 128), 0, st>>>(num, den, num, ns, T);
+  uint32_t n_tiles = (uint32_t)((ns + PB_FR_TILE - 1) / PB_FR_TILE);
+  PB_CHECK(n_tiles <= 65536, "group order too large for the product scan");
+  ctx->scratch[0].ensure((size_t)(n_tiles + 1 + 16) * 32);
+  Fr* tiles = ctx->scratch[0].as<Fr>();
+  Fr* totals = tiles + n_tiles + 1;  // [world] slab products, then carry and grand total
+  k_prod_tiles<<<n_tiles, 256, 0, st>>>(num, ns, tiles);
+  k_fr_scan_tiles<ScanMul><<<1, 256, 0, st>>>(tiles, n_tiles, tiles + n_tiles);
+  const Fr* d_total = tiles + n_tiles;
+  if (P->world > 1) {
+    PB_CUDA(cudaMemcpyAsync(totals + P->rank, tiles + n_tiles, 32, cudaMemcpyDeviceToDevice, st));
+    comm_allgather_inplace(ctx_comm(ctx), totals, 32, st);
+    Fr* carry = totals + P->world;
+    k_prod_carry<<<1, 32, 0, st>>>(totals, (uint32_t)P->world, (uint32_t)P->rank, carry, carry + 1);
+    k_prod_apply<<<n_tiles, 256, 0, st>>>(num, ns, tiles, carry, lag + lo);
+    comm_allgather_inplace(ctx_comm(ctx), lag, ns * 32, st);
+    d_total = carry + 1;
+    ctx->launches++;
+  } else {
+    k_prod_apply<<<n_tiles, 256, 0, st>>>(num, ns, tiles, nullptr, lag);
+  }
+  ctx->launches += 4;
+  Fr total;
+  PB_CUDA(cudaMemcpyAsync(&total, d_total, 32, cudaMemcpyDeviceToHost, st));
+  const Fr* zl = lag;
+  interpolate(P, &zl, &coeff, 1);
+  PB_CUDA(cudaStreamSynchronize(st));
+  PB_CHECK(total == Fr::one(), not_one);
+}
+
 // round 2 of a lookup proof, after Z: the grand product Z2, then one commitment pass over Z and Z2
 static void lookup_round2(Prover* P) {
   Context* ctx = P->ctx;
   const uint64_t n = P->n;
   cudaStream_t st = ctx->stream;
-  const Fr one = Fr::one();
   LookupChallenges ch;
   ch.delta = P->delta;
   ch.eps = P->epsilon;
-  ch.one_d = fp_add(one, P->delta);
+  ch.one_d = fp_add(Fr::one(), P->delta);
   ch.eps_one_d = fp_mul(P->epsilon, ch.one_d);
   Fr* num = P->tmp[2].as<Fr>();
   Fr* den = P->tmp[3].as<Fr>();
   k_lookup_z2_terms<<<PB_GRID(n, 128), 0, st>>>(P->lk_lag[Prover::LK_T].as<Fr>(), P->lk_lag[Prover::LK_F].as<Fr>(),
                                                P->lk_lag[Prover::LK_H1].as<Fr>(), P->lk_lag[Prover::LK_H2].as<Fr>(), ch, n,
                                                num, den);
-  uint64_t T = (n + PB_BATCH_CH - 1) / PB_BATCH_CH;
-  k_batch_div<<<PB_GRID(T, 128), 0, st>>>(num, den, num, n, T);
-  uint32_t n_tiles = (uint32_t)((n + PB_PROD_TILE - 1) / PB_PROD_TILE);
-  ctx->scratch[0].ensure((size_t)(n_tiles + 1) * 32);
-  Fr* tiles = ctx->scratch[0].as<Fr>();
-  k_prod_tiles<<<n_tiles, 256, 0, st>>>(num, n, tiles);
-  k_prod_scan_tiles<<<1, 256, 0, st>>>(tiles, n_tiles, tiles + n_tiles);
-  k_prod_apply<<<n_tiles, 256, 0, st>>>(num, n, tiles, nullptr, P->lk_lag[Prover::LK_Z2].as<Fr>());
-  ctx->launches += 5;
-  Fr total;
-  PB_CUDA(cudaMemcpyAsync(&total, tiles + n_tiles, 32, cudaMemcpyDeviceToHost, st));
-  const Fr* zl = P->lk_lag[Prover::LK_Z2].as<Fr>();
+  ctx->launches++;
   Fr* zc = P->lk_coeff[Prover::LK_Z2].as<Fr>();
-  interpolate(P, &zl, &zc, 1);
-  PB_CUDA(cudaStreamSynchronize(st));
-  PB_CHECK(total == one, "AssertionError: lookup grand product does not close, Z2_n != 1");
+  grand_product(P, num, den, P->lk_lag[Prover::LK_Z2].as<Fr>(), zc,
+                "AssertionError: lookup grand product does not close, Z2_n != 1");
   const Fr* zz[2] = {P->coeff[3].as<Fr>(), zc};
   uint8_t out[2][64];
   P->commit_batch(zz, 2, n, out[0]);
   memcpy(P->proof.pts[3], out[0], 64);
   memcpy(P->lk_pts[3], out[1], 64);
-}
-
-void prover_round2_lookup(Prover* P, const Fr& beta_c, const Fr& gamma_c, const Fr& delta_c, const Fr& epsilon_c);
-void prover_round4_lookup(Prover* P, const Fr& zeta_c);
-
-// cached per prover: basis_i[j] = L_i(x_j) on the fixed coset for the first `count` rows
-static void ensure_pi_basis(Prover* P, int count) {
-  Context* ctx = P->ctx;
-  const uint64_t n = P->n, ne = P->n_ext;
-  cudaStream_t st = ctx->stream;
-  if ((int)P->pi_basis.size() >= count) return;
-  Fr w = fr_root_of_unity(P->log_n);
-  Fr gn = fp_pow_u64(P->g, n), i4 = fp_pow_u64(fr_root_of_unity(P->log_n + 2), n), one = Fr::one();
-  DevBuf den(ne * 32);
-  for (int i = (int)P->pi_basis.size(); i < count; i++) {
-    Fr wi = fp_pow_u64(w, (uint64_t)i);
-    Four zh;  // w^i (x_j^n - 1): four values
-    Fr cur = gn;
-    for (int k = 0; k < 4; k++) { zh.v[k] = fp_mul(wi, fp_sub(cur, one)); cur = fp_mul(cur, i4); }
-    P->pi_basis.emplace_back(ne * 32);
-    Fr* out = P->pi_basis.back().as<Fr>();
-    k_lagrange_den<<<PB_GRID(ne, 256), 0, st>>>(P->xs.as<Fr>(), ne, wi, fr_from_u64(n), den.as<Fr>());
-    uint64_t T = (ne + PB_BATCH_CH - 1) / PB_BATCH_CH;
-    k_batch_div<<<PB_GRID(T, 128), 0, st>>>(nullptr, den.as<Fr>(), out, ne, T);
-    k_scale_by4<<<PB_GRID(ne, 256), 0, st>>>(out, ne, zh, (uint32_t)P->world, (uint32_t)P->rank);
-    ctx->launches += 3;
-  }
-  PB_CUDA(cudaStreamSynchronize(st));
 }
 
 // ---- round 1 (prover.py:86-119) -------------------------------------------------------------------------
@@ -1208,47 +1165,16 @@ void prover_round2(Prover* P, const Fr& beta_c, const Fr& gamma_c) {
   P->beta = fp_to_mont(beta_c);
   P->gamma = fp_to_mont(gamma_c);
   PermChallenges ch{P->beta, P->gamma};
-  // one proof across G ranks: rank r builds the slab [r n/G, (r+1) n/G) of the grand product -- per-row terms, the
-  // batched inversion and the in-slab prefix products are local; the slab products are exchanged with a 32-byte
-  // allgather (the product of the lower slabs is the slab's carry) and the Z values with one bulk allgather
+  // one proof across G ranks: rank r builds the slab [r n/G, (r+1) n/G) of the grand product (see grand_product)
   const uint64_t ns = n / (uint64_t)P->world, lo = ns * (uint64_t)P->rank;
   Fr* num = P->tmp[0].as<Fr>() + lo;
   Fr* den = P->tmp[1].as<Fr>() + lo;
   k_perm_terms<<<PB_GRID(ns, 128), 0, st>>>(P->lag[0].as<Fr>() + lo, P->lag[1].as<Fr>() + lo, P->lag[2].as<Fr>() + lo,
                                            P->sel_lag[Prover::S1].as<Fr>() + lo, P->sel_lag[Prover::S2].as<Fr>() + lo,
                                            P->sel_lag[Prover::S3].as<Fr>() + lo, P->roots.as<Fr>() + lo, ch, ns, num, den);
-  uint64_t T = (ns + PB_BATCH_CH - 1) / PB_BATCH_CH;
-  k_batch_div<<<PB_GRID(T, 128), 0, st>>>(num, den, num, ns, T);
-  uint32_t n_tiles = (uint32_t)((ns + PB_PROD_TILE - 1) / PB_PROD_TILE);
-  PB_CHECK(n_tiles <= 65536, "group order too large for the product scan");
-  ctx->scratch[0].ensure((size_t)(n_tiles + 1 + 16) * 32);
-  Fr* tiles = ctx->scratch[0].as<Fr>();
-  Fr* totals = tiles + n_tiles + 1;  // [world] slab products, then carry and grand total
-  k_prod_tiles<<<n_tiles, 256, 0, st>>>(num, ns, tiles);
-  k_prod_scan_tiles<<<1, 256, 0, st>>>(tiles, n_tiles, tiles + n_tiles);
-  const Fr* d_total = tiles + n_tiles;
-  if (P->world > 1) {
-    PB_CUDA(cudaMemcpyAsync(totals + P->rank, tiles + n_tiles, 32, cudaMemcpyDeviceToDevice, st));
-    comm_allgather_inplace(ctx_comm(ctx), totals, 32, st);
-    Fr* carry = totals + P->world;
-    k_prod_carry<<<1, 32, 0, st>>>(totals, (uint32_t)P->world, (uint32_t)P->rank, carry, carry + 1);
-    k_prod_apply<<<n_tiles, 256, 0, st>>>(num, ns, tiles, carry, P->lag[3].as<Fr>() + lo);
-    comm_allgather_inplace(ctx_comm(ctx), P->lag[3].p, ns * 32, st);
-    d_total = carry + 1;
-    ctx->launches++;
-  } else {
-    k_prod_apply<<<n_tiles, 256, 0, st>>>(num, ns, tiles, nullptr, P->lag[3].as<Fr>());
-  }
-  ctx->launches += 5;
-  Fr total;
-  PB_CUDA(cudaMemcpyAsync(&total, d_total, 32, cudaMemcpyDeviceToHost, st));
-  {
-    const Fr* zl = P->lag[3].as<Fr>();
-    Fr* zc = P->coeff[3].as<Fr>();
-    interpolate(P, &zl, &zc, 1);
-  }
-  PB_CUDA(cudaStreamSynchronize(st));
-  PB_CHECK(total == Fr::one(), "AssertionError: permutation grand product does not close, Z_n != 1 (prover.py:132)");
+  ctx->launches++;
+  grand_product(P, num, den, P->lag[3].as<Fr>(), P->coeff[3].as<Fr>(),
+                "AssertionError: permutation grand product does not close, Z_n != 1 (prover.py:132)");
   if (P->overlap) launch_coset_ext_async(P, 3, 1, 1);
   if (P->zk) {  // Z': n + 3 coefficients
     const Fr* b = P->zk_b;
@@ -1299,7 +1225,7 @@ void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c) {
   q.QO = P->sel_ext[Prover::QO].as<Fr>(); q.QC = P->sel_ext[Prover::QC].as<Fr>();
   q.S1 = P->sel_ext[Prover::S1].as<Fr>(); q.S2 = P->sel_ext[Prover::S2].as<Fr>(); q.S3 = P->sel_ext[Prover::S3].as<Fr>();
   q.custom = P->custom_terms(P->sel_ext);
-  q.L0 = P->l0_ext.as<Fr>(); q.X = P->xs.as<Fr>();
+  q.L0 = P->pi_basis[0].as<Fr>(); q.X = P->xs.as<Fr>();
   for (int k = 0; k < 4; k++) q.zh_inv[k] = P->zh_inv[k];
   q.alpha = P->alpha; q.alpha2 = fp_sqr(P->alpha); q.beta = P->beta; q.gamma = P->gamma; q.one = Fr::one();
   q.n4 = ne;
@@ -1409,19 +1335,19 @@ void prover_round4(Prover* P, const Fr& zeta_c) {
   } else {
     P->pi_ev = out[6];
   }
+  if (P->lk) {  // the lookup evaluations: F, T at zeta, T at zeta w, H2 at zeta, H1 and Z2 at zeta w
+    const Fr* lpolys[6] = {P->lk_coeff[Prover::LK_F].as<Fr>(), P->lk_coeff[Prover::LK_T].as<Fr>(),
+                           P->lk_coeff[Prover::LK_T].as<Fr>(), P->lk_coeff[Prover::LK_H2].as<Fr>(),
+                           P->lk_coeff[Prover::LK_H1].as<Fr>(), P->lk_coeff[Prover::LK_Z2].as<Fr>()};
+    const Fr lxs[6] = {P->zeta, P->zeta, zw, P->zeta, zw, zw};
+    eval_polys(P, 6, lpolys, lxs, P->lk_ev);
+    for (int k = 0; k < 6; k++) store_canonical(P->lk_evals[k], P->lk_ev[k]);
+  }
 }
 
-// round 4 of a lookup proof: the six plain evaluations, then F, T at zeta, T at zeta w, H2 at zeta, H1 and Z2 at zeta w
 void prover_round4_lookup(Prover* P, const Fr& zeta_c) {
   PB_CHECK(P->lk, "this prover has no lookup table (pb200_prover_set_lookup)");
   prover_round4(P, zeta_c);
-  const Fr z = P->zeta, zw = fp_mul(P->zeta, fr_root_of_unity(P->log_n));
-  const Fr* polys[6] = {P->lk_coeff[Prover::LK_F].as<Fr>(), P->lk_coeff[Prover::LK_T].as<Fr>(),
-                        P->lk_coeff[Prover::LK_T].as<Fr>(), P->lk_coeff[Prover::LK_H2].as<Fr>(),
-                        P->lk_coeff[Prover::LK_H1].as<Fr>(), P->lk_coeff[Prover::LK_Z2].as<Fr>()};
-  const Fr xs[6] = {z, z, zw, z, zw, zw};
-  eval_polys(P, 6, polys, xs, P->lk_ev);
-  for (int k = 0; k < 6; k++) store_canonical(P->lk_evals[k], P->lk_ev[k]);
 }
 
 // (num coefficients, n) / (X - point) -> quotient coefficients (out != num), remainder dropped.
@@ -1438,12 +1364,12 @@ static void divide_linear(Prover* P, const Fr* num, Fr* out, const Fr& point, Fr
   const Fr point_inv = fp_inv(point);
   launch_powers(ctx, pow_buf + lo, n, point, fp_pow_u64(point, lo));
   launch_powers(ctx, invpow_buf + lo, n, point_inv, fp_pow_u64(point_inv, lo));
-  uint32_t n_tiles = (uint32_t)((n + PB_SUM_TILE - 1) / PB_SUM_TILE);
+  uint32_t n_tiles = (uint32_t)((n + PB_FR_TILE - 1) / PB_FR_TILE);
   ctx->scratch[0].ensure((size_t)(n_tiles + 1 + 16) * 32);
   Fr* tiles = ctx->scratch[0].as<Fr>();
   Fr* totals = tiles + n_tiles + 1;  // [world] slab sums, then the carry
   k_sufsum_tiles<<<n_tiles, 256, 0, st>>>(num + lo, pow_buf + lo, n, tiles);
-  k_sufsum_scan_tiles<<<1, 256, 0, st>>>(tiles, n_tiles, tiles + n_tiles);
+  k_fr_scan_tiles<ScanAdd><<<1, 256, 0, st>>>(tiles, n_tiles, tiles + n_tiles);
   if (P->world > 1) {
     PB_CUDA(cudaMemcpyAsync(totals + P->rank, tiles + n_tiles, 32, cudaMemcpyDeviceToDevice, st));
     comm_allgather_inplace(ctx_comm(ctx), totals, 32, st);
@@ -1489,15 +1415,13 @@ void prover_round5(Prover* P, const Fr& v_c) {
   const Fr* zpoly = zk ? P->zk_coeff[3].as<Fr>() : P->coeff[3].as<Fr>();
   const Fr* tpiece[3];
   for (int i = 0; i < 3; i++) tpiece[i] = zk ? P->zk_t[i].as<Fr>() : P->tq.as<Fr>() + (uint64_t)i * n;
-  LinCombArgs L, tail, lkp;
+  LinCombArgs L, tail;
   int k = 0;
   tail.count = 0;
-  lkp.count = 0;
   auto add = [&](const Fr* vec, const Fr& w, bool blinded = false) {
     L.vec[k] = vec; L.w[k] = w; k++;
     if (blinded) { tail.vec[tail.count] = vec; tail.w[tail.count] = w; tail.count++; }
   };
-  auto add_lookup = [&](const Fr* vec, const Fr& w) { lkp.vec[lkp.count] = vec; lkp.w[lkp.count] = w; lkp.count++; };
   add(P->sel_coeff[Prover::QL].as<Fr>(), a);
   add(P->sel_coeff[Prover::QR].as<Fr>(), b);
   add(P->sel_coeff[Prover::QM].as<Fr>(), fp_mul(a, b));
@@ -1515,8 +1439,15 @@ void prover_round5(Prover* P, const Fr& v_c) {
   add(wire[2], v3, true);
   add(P->sel_coeff[Prover::S1].as<Fr>(), v4);
   add(P->sel_coeff[Prover::S2].as<Fr>(), v5);
-  // lookups: q_K, Z2 and H1 keep their commitments in the linearisation; F, T, H2 join the batch at zeta (a second
-  // pass, k_lincomb_add)
+  // constant term: PI(zeta) - c2 (c + gamma) - alpha^2 L0(zeta) - v a - v^2 b - v^3 c - v^4 s1 - v^5 s2
+  Fr c0 = fp_sub(P->pi_ev, fp_mul(c2, fp_add(c, ga)));
+  c0 = fp_sub(c0, al2l0);
+  c0 = fp_sub(c0, fp_mul(v, a));
+  c0 = fp_sub(c0, fp_mul(v2, b));
+  c0 = fp_sub(c0, fp_mul(v3, c));
+  c0 = fp_sub(c0, fp_mul(v4, s1));
+  c0 = fp_sub(c0, fp_mul(v5, s2));
+  // lookups: q_K, Z2 and H1 keep their commitments in the linearisation; F, T, H2 join the batch at zeta
   if (P->lk) {
     const Fr &fe = P->lk_ev[0], &te = P->lk_ev[1], &tw = P->lk_ev[2], &h2e = P->lk_ev[3], &h1w = P->lk_ev[4],
              &z2w = P->lk_ev[5];
@@ -1527,41 +1458,27 @@ void prover_round5(Prover* P, const Fr& v_c) {
     const Fr abc = fp_add(a, fp_add(fp_mul(eta, b), fp_mul(fp_sqr(eta), c)));
     const Fr hw = fp_add(fp_add(eod, h2e), fp_mul(de, h1w));       // e(1+d) + h2 + d h1(zeta w)
     const Fr az2 = fp_mul(al4, z2w);
-    add_lookup(P->lk_qk_coeff.as<Fr>(), fp_mul(al3, fp_sub(abc, fe)));
-    add_lookup(P->lk_coeff[Prover::LK_Z2].as<Fr>(),
+    add(P->lk_qk_coeff.as<Fr>(), fp_mul(al3, fp_sub(abc, fe)));
+    add(P->lk_coeff[Prover::LK_Z2].as<Fr>(),
         fp_add(fp_mul(fp_mul(fp_mul(al4, od), fp_add(ep, fe)), fp_add(fp_add(eod, te), fp_mul(de, tw))),
                fp_mul(al5, l0_ev)));
-    add_lookup(P->lk_coeff[Prover::LK_H1].as<Fr>(), fp_neg(fp_mul(az2, hw)));
-    add_lookup(P->lk_coeff[Prover::LK_F].as<Fr>(), v6);
-    add_lookup(P->lk_coeff[Prover::LK_T].as<Fr>(), v7);
-    add_lookup(P->lk_coeff[Prover::LK_H2].as<Fr>(), v8);
+    add(P->lk_coeff[Prover::LK_H1].as<Fr>(), fp_neg(fp_mul(az2, hw)));
+    add(P->lk_coeff[Prover::LK_F].as<Fr>(), v6);
+    add(P->lk_coeff[Prover::LK_T].as<Fr>(), v7);
+    add(P->lk_coeff[Prover::LK_H2].as<Fr>(), v8);
     // -a4 z2w (e(1+d) + d h2) hw - a5 L0(zeta) - v^6 f - v^7 t - v^8 h2
-    Fr c = fp_neg(fp_mul(fp_mul(az2, fp_add(eod, fp_mul(de, h2e))), hw));
-    c = fp_sub(c, fp_mul(al5, l0_ev));
-    lkp.c0 = fp_sub(c, fp_add(fp_mul(v6, fe), fp_add(fp_mul(v7, te), fp_mul(v8, h2e))));
+    Fr lc = fp_neg(fp_mul(fp_mul(az2, fp_add(eod, fp_mul(de, h2e))), hw));
+    lc = fp_sub(lc, fp_mul(al5, l0_ev));
+    c0 = fp_add(c0, fp_sub(lc, fp_add(fp_mul(v6, fe), fp_add(fp_mul(v7, te), fp_mul(v8, h2e)))));
   }
   L.count = k;
   L.n = n / (uint64_t)P->world;          // one proof across G ranks: every rank builds (and divides) its slab only
   L.first = L.n * (uint64_t)P->rank;
-  // constant term: PI(zeta) - c2 (c + gamma) - alpha^2 L0(zeta) - v a - v^2 b - v^3 c - v^4 s1 - v^5 s2
-  Fr c0 = fp_sub(P->pi_ev, fp_mul(c2, fp_add(c, ga)));
-  c0 = fp_sub(c0, al2l0);
-  c0 = fp_sub(c0, fp_mul(v, a));
-  c0 = fp_sub(c0, fp_mul(v2, b));
-  c0 = fp_sub(c0, fp_mul(v3, c));
-  c0 = fp_sub(c0, fp_mul(v4, s1));
-  c0 = fp_sub(c0, fp_mul(v5, s2));
   L.c0 = c0;
   Fr* wz = P->tmp[0].as<Fr>();
   PB_CUDA(cudaMemsetAsync(P->flags.p, 0, 64, st));
   k_lincomb<<<PB_GRID(L.n, 128), 0, st>>>(L, wz);
   ctx->launches++;
-  if (P->lk) {
-    lkp.n = L.n;
-    lkp.first = L.first;
-    k_lincomb_add<<<PB_GRID(lkp.n, 128), 0, st>>>(lkp, wz);
-    ctx->launches++;
-  }
   const uint64_t len = zk ? n + Prover::ZK_PAD : n;  // numerator coefficients
   if (zk) {
     tail.c0 = Fr::zero();
@@ -1596,18 +1513,22 @@ void prover_round5(Prover* P, const Fr& v_c) {
 }
 
 // canonical 768-byte proof: Proof.flatten() order (prover.py:18-35), G1 as x||y, every integer 32-byte
-// big-endian exactly as the transcript absorbs it (transcript.py:62-67)
-void prover_serialize(const Prover* P, uint8_t* out768) {
+// big-endian exactly as the transcript absorbs it (transcript.py:62-67).  A lookup proof has 1216 bytes: the 768 plain
+// bytes, then f_1 h1_1 h2_1 z2_1, then the six lookup evaluations.
+void prover_serialize(const Prover* P, uint8_t* out) {
   auto be = [](uint8_t* dst, const uint8_t* le) { for (int i = 0; i < 32; i++) dst[i] = le[31 - i]; };
-  uint8_t* o = out768;
+  uint8_t* o = out;
   for (int k = 0; k < 7; k++) { be(o, P->proof.pts[k]); be(o + 32, P->proof.pts[k] + 32); o += 64; }
   for (int k = 0; k < 6; k++) { be(o, P->proof.evals[k]); o += 32; }
   for (int k = 7; k < 9; k++) { be(o, P->proof.pts[k]); be(o + 32, P->proof.pts[k] + 32); o += 64; }
+  if (!P->lk) return;
+  for (int k = 0; k < 4; k++) { be(o, P->lk_pts[k]); be(o + 32, P->lk_pts[k] + 32); o += 64; }
+  for (int k = 0; k < 6; k++) { be(o, P->lk_evals[k]); o += 32; }
 }
 
-// prover.py:51-84
+// prover.py:51-84; a prover with a lookup table runs step 1L between rounds 1 and 2 and writes the 1216-byte proof
 void prover_prove(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t* hC, const uint8_t* h_public,
-                  uint64_t n_public, uint8_t* out768, bool wires_on_device) {
+                  uint64_t n_public, uint8_t* out, bool wires_on_device) {
   PB_CUDA(cudaSetDevice(P->ctx->device));  // the calling host thread may not be the one that created the context
   Transcript tr("plonk");  // prover.py:53
   prover_round1(P, hA, hB, hC, h_public, n_public, wires_on_device);
@@ -1616,8 +1537,17 @@ void prover_prove(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t
   tr.append_point_le("c_1", P->proof.pts[2]);
   Fr beta = tr.get_and_append_challenge("beta");
   Fr gamma = tr.get_and_append_challenge("gamma");
+  if (P->lk) {
+    prover_round_lookup(P, tr.get_and_append_challenge("eta"));
+    tr.append_point_le("f_1", P->lk_pts[0]);
+    tr.append_point_le("h1_1", P->lk_pts[1]);
+    tr.append_point_le("h2_1", P->lk_pts[2]);
+    P->delta = fp_to_mont(tr.get_and_append_challenge("delta"));
+    P->epsilon = fp_to_mont(tr.get_and_append_challenge("epsilon"));
+  }
   prover_round2(P, beta, gamma);
   tr.append_point_le("z_1", P->proof.pts[3]);
+  if (P->lk) tr.append_point_le("z2_1", P->lk_pts[3]);
   Fr alpha = tr.get_and_append_challenge("alpha");
   Fr cof = tr.get_and_append_challenge("fft_cofactor");
   prover_round3(P, alpha, cof);
@@ -1628,57 +1558,14 @@ void prover_prove(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t
   prover_round4(P, zeta);
   static const char* ev_labels[6] = {"a_eval", "b_eval", "c_eval", "s1_eval", "s2_eval", "z_shifted_eval"};
   for (int k = 0; k < 6; k++) tr.append_scalar_le(ev_labels[k], P->proof.evals[k]);
+  if (P->lk) {
+    static const char* lk_labels[6] = {"f_eval", "t_eval", "t_shifted_eval", "h2_eval", "h1_shifted_eval",
+                                       "z2_shifted_eval"};
+    for (int k = 0; k < 6; k++) tr.append_scalar_le(lk_labels[k], P->lk_evals[k]);
+  }
   Fr v = tr.get_and_append_challenge("v");
   prover_round5(P, v);
-  prover_serialize(P, out768);
-}
-
-// 1216-byte lookup proof: the 768 plain bytes, then f_1 h1_1 h2_1 z2_1, then the six lookup evaluations
-void prover_serialize_lookup(const Prover* P, uint8_t* out1216) {
-  auto be = [](uint8_t* dst, const uint8_t* le) { for (int i = 0; i < 32; i++) dst[i] = le[31 - i]; };
-  prover_serialize(P, out1216);
-  uint8_t* o = out1216 + 768;
-  for (int k = 0; k < 4; k++) { be(o, P->lk_pts[k]); be(o + 32, P->lk_pts[k] + 32); o += 64; }
-  for (int k = 0; k < 6; k++) { be(o, P->lk_evals[k]); o += 32; }
-}
-
-void prover_prove_lookup(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t* hC, const uint8_t* h_public,
-                         uint64_t n_public, uint8_t* out1216) {
-  PB_CUDA(cudaSetDevice(P->ctx->device));
-  PB_CHECK(P->lk, "this prover has no lookup table (pb200_prover_set_lookup)");
-  Transcript tr("plonk");
-  prover_round1(P, hA, hB, hC, h_public, n_public, false);
-  tr.append_point_le("a_1", P->proof.pts[0]);
-  tr.append_point_le("b_1", P->proof.pts[1]);
-  tr.append_point_le("c_1", P->proof.pts[2]);
-  Fr beta = tr.get_and_append_challenge("beta");
-  Fr gamma = tr.get_and_append_challenge("gamma");
-  Fr eta = tr.get_and_append_challenge("eta");
-  prover_round_lookup(P, eta);
-  tr.append_point_le("f_1", P->lk_pts[0]);
-  tr.append_point_le("h1_1", P->lk_pts[1]);
-  tr.append_point_le("h2_1", P->lk_pts[2]);
-  Fr delta = tr.get_and_append_challenge("delta");
-  Fr epsilon = tr.get_and_append_challenge("epsilon");
-  prover_round2_lookup(P, beta, gamma, delta, epsilon);
-  tr.append_point_le("z_1", P->proof.pts[3]);
-  tr.append_point_le("z2_1", P->lk_pts[3]);
-  Fr alpha = tr.get_and_append_challenge("alpha");
-  Fr cof = tr.get_and_append_challenge("fft_cofactor");
-  prover_round3(P, alpha, cof);
-  tr.append_point_le("t_lo_1", P->proof.pts[4]);
-  tr.append_point_le("t_mid_1", P->proof.pts[5]);
-  tr.append_point_le("t_hi_1", P->proof.pts[6]);
-  Fr zeta = tr.get_and_append_challenge("zeta");
-  prover_round4_lookup(P, zeta);
-  static const char* ev_labels[6] = {"a_eval", "b_eval", "c_eval", "s1_eval", "s2_eval", "z_shifted_eval"};
-  for (int k = 0; k < 6; k++) tr.append_scalar_le(ev_labels[k], P->proof.evals[k]);
-  static const char* lk_labels[6] = {"f_eval", "t_eval", "t_shifted_eval", "h2_eval", "h1_shifted_eval",
-                                     "z2_shifted_eval"};
-  for (int k = 0; k < 6; k++) tr.append_scalar_le(lk_labels[k], P->lk_evals[k]);
-  Fr v = tr.get_and_append_challenge("v");
-  prover_round5(P, v);
-  prover_serialize_lookup(P, out1216);
+  prover_serialize(P, out);
 }
 
 }  // namespace pb200

@@ -81,7 +81,6 @@ struct Prover {
   DevBuf gpow_w;         // (g mu^(rank+4))^i, i < n (only when zw_separate)
   DevBuf ginv_pow;       // g^-i, i < 4n            (undo the shift on store)
   DevBuf xs;             // x_j, j < n_ext
-  DevBuf l0_ext;         // L0 on the slice
   Fr g, g_inv, zh_inv[4];
   Fr zh[4];              // Z_H(x_j) = x_j^n - 1 for j mod 4 (Montgomery)
   // per-proof state
@@ -101,7 +100,7 @@ struct Prover {
   // public inputs: when there are at most 8, PI is a combination of cached Lagrange-basis coset vectors
   uint64_t n_public = 0;
   bool pi_sparse = false;
-  std::vector<DevBuf> pi_basis;   // L_i on the slice (n_ext each), i < 8
+  std::vector<DevBuf> pi_basis;   // L_i on the slice (n_ext each), i < 8; always holds L0 (the quotient's L0 term)
   std::vector<Fr> pub_neg;        // -public_i, Montgomery (host)
   // Zero knowledge (one GPU only): the blinding of the PLONK paper with 11 scalars b1..b11 per proof.  The unblinded
   // n-coefficient vectors above stay as they are (the coset extensions read them; k_quotient adds the Z_H multiples);

@@ -27,6 +27,27 @@ PROOF_FIELDS = ("a_1", "b_1", "c_1", "z_1", "t_lo_1", "t_mid_1", "t_hi_1", "a_ev
                 "s1_eval", "s2_eval", "z_shifted_eval", "W_z_1", "W_zw_1")
 
 
+def _encode(values) -> bytes:
+    """a sequence of proof fields -> G1 points as x||y, every integer 32-byte big-endian"""
+    out = bytearray()
+    for v in values:
+        if isinstance(v, tuple):
+            out += v[0].n.to_bytes(32, "big") + v[1].n.to_bytes(32, "big")
+        else:
+            out += v.n.to_bytes(32, "big")
+    return bytes(out)
+
+
+def _decode_words(raw: bytes, scalar_words: range, first: int = 0) -> list:
+    """32-byte big-endian words -> ints; the words in ``scalar_words`` must be below r, the others (coordinates) below
+    q, else ValueError naming the word by its index in the proof (raw starts at word ``first``)"""
+    w = [int.from_bytes(raw[i:i + 32], "big") for i in range(0, len(raw), 32)]
+    for k, x in enumerate(w):
+        if x >= (CURVE_ORDER if k in scalar_words else FIELD_MODULUS):
+            raise ValueError("non-canonical proof encoding (word %d is not reduced)" % (first + k))
+    return w
+
+
 @dataclass
 class Proof:
     msg_1: Message1
@@ -44,23 +65,14 @@ class Proof:
 
     def to_bytes(self) -> bytes:
         """Canonical 768-byte form: flatten() order, G1 as x||y, 32-byte big-endian integers."""
-        out = bytearray()
-        for v in self.flatten().values():
-            if isinstance(v, tuple):
-                out += v[0].n.to_bytes(32, "big") + v[1].n.to_bytes(32, "big")
-            else:
-                out += v.n.to_bytes(32, "big")
-        return bytes(out)
+        return _encode(self.flatten().values())
 
     @classmethod
     def from_bytes(cls, raw: bytes) -> "Proof":
         """Inverse of to_bytes.  The encoding is canonical: coordinates must be below q and evaluations below r
         (ValueError otherwise) -- a second byte string for the same proof would make proofs malleable."""
         assert len(raw) == 768
-        w = [int.from_bytes(raw[i:i + 32], "big") for i in range(0, 768, 32)]
-        for k, x in enumerate(w):
-            if x >= (CURVE_ORDER if 14 <= k < 20 else FIELD_MODULUS):
-                raise ValueError("non-canonical proof encoding (word %d is not reduced)" % k)
+        w = _decode_words(raw, range(14, 20))
         pt = lambda k: (FQ(w[k]), FQ(w[k + 1]))  # noqa: E731
         return cls(Message1(pt(0), pt(2), pt(4)), Message2(pt(6)), Message3(pt(8), pt(10), pt(12)),
                    Message4(*[Scalar(x) for x in w[14:20]]), Message5(pt(20), pt(22)))
@@ -93,14 +105,7 @@ class LookupProof:
         return out
 
     def to_bytes(self) -> bytes:
-        out = bytearray(self.plain.to_bytes())
-        for k in LOOKUP_FIELDS:
-            v = getattr(self, k)
-            if isinstance(v, tuple):
-                out += v[0].n.to_bytes(32, "big") + v[1].n.to_bytes(32, "big")
-            else:
-                out += v.n.to_bytes(32, "big")
-        return bytes(out)
+        return _encode(self.flatten().values())
 
     @classmethod
     def from_bytes(cls, raw: bytes) -> "LookupProof":
@@ -108,10 +113,7 @@ class LookupProof:
         if len(raw) != LOOKUP_PROOF_BYTES:
             raise ValueError("a lookup proof has %d bytes, got %d" % (LOOKUP_PROOF_BYTES, len(raw)))
         plain = Proof.from_bytes(raw[:768])
-        w = [int.from_bytes(raw[i:i + 32], "big") for i in range(768, LOOKUP_PROOF_BYTES, 32)]
-        for k, x in enumerate(w):
-            if x >= (CURVE_ORDER if k >= 8 else FIELD_MODULUS):
-                raise ValueError("non-canonical proof encoding (word %d is not reduced)" % (24 + k))
+        w = _decode_words(raw[768:], range(8, 14), first=24)
         pt = lambda k: (FQ(w[k]), FQ(w[k + 1]))  # noqa: E731
         return cls(plain, pt(0), pt(2), pt(4), pt(6), *[Scalar(x) for x in w[8:14]])
 

@@ -16,7 +16,7 @@ from .curve import G1, G2, Scalar, ec_lincomb, g1_neg, g2_add, g2_mul, pairing_p
 from . import _lib
 from .custom_gates import monomial
 from .field import CURVE_ORDER, FIELD_MODULUS
-from .transcript import LOOKUP_SCHEDULE, Transcript
+from .transcript import LOOKUP_SCHEDULE, SCHEDULE, Transcript
 
 
 def _lagrange_terms_at(group_order: int, values, x: Scalar) -> Scalar:
@@ -56,15 +56,6 @@ class VerificationKey:
         """the custom gates' part of the linearisation: sum_k m_k(a, b, c) [Q_k]"""
         return [(pt, monomial(e, a, b, c)) for e, pt in self.custom]
 
-    # ---- shared by both routines: steps 4-7 of the paper's verifier
-    def _common(self, group_order: int, pf, public):
-        beta, gamma, alpha, zeta, v, u = self.compute_challenges(pf)
-        proof = pf.flatten()
-        zh_ev = zeta ** group_order - 1
-        l0_ev = zh_ev / ((zeta - 1) * group_order)
-        pi_ev = _lagrange_terms_at(group_order, [-int(x) % CURVE_ORDER for x in public], zeta)
-        return beta, gamma, alpha, zeta, v, u, proof, zh_ev, l0_ev, pi_ev
-
     @staticmethod
     def _well_formed(pf) -> bool:
         """every commitment of the proof is a point of the curve y^2 = x^3 + 3 with reduced coordinates and every
@@ -90,37 +81,9 @@ class VerificationKey:
         if not self._matches(pf) or not self._well_formed(pf):
             return False
         try:
-            if self.lookup:
-                return self._verify_lookup(group_order, pf, public, batched=True)
-            return self._verify_batched(group_order, pf, public)
+            return self._verify(group_order, pf, public, batched=True)
         except _lib.PlonkB200Error:
             return False
-
-    def _verify_batched(self, group_order: int, pf, public) -> bool:
-        beta, gamma, alpha, zeta, v, u, proof, zh_ev, l0_ev, pi_ev = self._common(group_order, pf, public)
-        a, b, c = proof["a_eval"], proof["b_eval"], proof["c_eval"]
-        s1, s2, zw = proof["s1_eval"], proof["s2_eval"], proof["z_shifted_eval"]
-        root = Scalar.root_of_unity(group_order)
-
-        perm_bar = (a + beta * s1 + gamma) * (b + beta * s2 + gamma) * alpha * zw
-        # the part of r(zeta) that needs no commitment
-        r0 = pi_ev - l0_ev * alpha * alpha - perm_bar * (c + gamma)
-        zeta_n = zeta ** group_order
-        # [D] = [r] - r0 + u [z]
-        d_pt = ec_lincomb([
-            (self.Qm, a * b), (self.Ql, a), (self.Qr, b), (self.Qo, c), (self.Qc, 1), *self._custom_terms(a, b, c),
-            (proof["z_1"], (a + beta * zeta + gamma) * (b + beta * 2 * zeta + gamma) * (c + beta * 3 * zeta + gamma)
-             * alpha + l0_ev * alpha * alpha + u),
-            (self.S3, -perm_bar * beta),
-            (proof["t_lo_1"], -zh_ev), (proof["t_mid_1"], -zh_ev * zeta_n), (proof["t_hi_1"], -zh_ev * zeta_n * zeta_n),
-        ])
-        f_pt = ec_lincomb([(d_pt, 1), (proof["a_1"], v), (proof["b_1"], v ** 2), (proof["c_1"], v ** 3),
-                           (self.S1, v ** 4), (self.S2, v ** 5)])
-        e_scalar = -r0 + v * a + v ** 2 * b + v ** 3 * c + v ** 4 * s1 + v ** 5 * s2 + u * zw
-        # e(W_z + u W_zw, [x]_2) == e(zeta W_z + u zeta w W_zw + F - E, [1]_2)
-        lhs = ec_lincomb([(proof["W_z_1"], 1), (proof["W_zw_1"], u)])
-        rhs = ec_lincomb([(proof["W_z_1"], zeta), (proof["W_zw_1"], u * zeta * root), (f_pt, 1), (G1, -e_scalar)])
-        return pairing_product_is_one([(lhs, self.X_2), (g1_neg(rhs), G2)])
 
     def verify_proof_unoptimized(self, group_order: int, pf, public=[]) -> bool:
         """verifier.py:76-92: rebuild the commitment to the prover's linearisation polynomial R (R(zeta) == 0),
@@ -128,68 +91,25 @@ class VerificationKey:
         if not self._matches(pf) or not self._well_formed(pf):
             return False
         try:
-            if self.lookup:
-                return self._verify_lookup(group_order, pf, public, batched=False)
-            return self._verify_unoptimized(group_order, pf, public)
+            return self._verify(group_order, pf, public, batched=False)
         except _lib.PlonkB200Error:
             return False
 
-    def _verify_unoptimized(self, group_order: int, pf, public) -> bool:
-        beta, gamma, alpha, zeta, v, u, proof, zh_ev, l0_ev, pi_ev = self._common(group_order, pf, public)
-        a, b, c = proof["a_eval"], proof["b_eval"], proof["c_eval"]
-        s1, s2, zw = proof["s1_eval"], proof["s2_eval"], proof["z_shifted_eval"]
-        root = Scalar.root_of_unity(group_order)
-        zeta_n = zeta ** group_order
-        sigma_bar = (a + beta * s1 + gamma) * (b + beta * s2 + gamma) * zw
-
-        r_pt = ec_lincomb([
-            # gate constraint with the wire values fixed to their evaluations
-            (self.Qm, a * b), (self.Ql, a), (self.Qr, b), (self.Qo, c), (self.Qc, 1), (G1, pi_ev),
-            *self._custom_terms(a, b, c),
-            # permutation argument: Z(X) keeps its commitment, S3(X) too, everything else is a number
-            (proof["z_1"], (a + beta * zeta + gamma) * (b + beta * 2 * zeta + gamma) * (c + beta * 3 * zeta + gamma) * alpha),
-            (self.S3, -sigma_bar * alpha * beta), (G1, -sigma_bar * alpha * (c + gamma)),
-            # (Z(X) - 1) L0(zeta)
-            (proof["z_1"], l0_ev * alpha * alpha), (G1, -l0_ev * alpha * alpha),
-            # - Z_H(zeta) (T1 + zeta^n T2 + zeta^2n T3)
-            (proof["t_lo_1"], -zh_ev), (proof["t_mid_1"], -zh_ev * zeta_n), (proof["t_hi_1"], -zh_ev * zeta_n * zeta_n),
-        ])
-        # opening at zeta of  R + v(A - a) + v^2(B - b) + v^3(C - c) + v^4(S1 - s1) + v^5(S2 - s2)
-        batch = ec_lincomb([
-            (r_pt, 1), (proof["a_1"], v), (proof["b_1"], v ** 2), (proof["c_1"], v ** 3), (self.S1, v ** 4),
-            (self.S2, v ** 5), (G1, -(v * a + v ** 2 * b + v ** 3 * c + v ** 4 * s1 + v ** 5 * s2)),
-        ])
-        x_minus_zeta = g2_add(self.X_2, g2_mul(G2, -zeta))
-        if not pairing_product_is_one([(batch, G2), (g1_neg(proof["W_z_1"]), x_minus_zeta)]):
-            return False
-        # opening of Z at zeta * w
-        z_open = ec_lincomb([(proof["z_1"], 1), (G1, -zw)])
-        x_minus_zeta_w = g2_add(self.X_2, g2_mul(G2, -(zeta * root)))
-        return pairing_product_is_one([(z_open, G2), (g1_neg(proof["W_zw_1"]), x_minus_zeta_w)])
-
-    # ---- lookup proofs (plonkathon_b200/lookup.py, DESIGN.md): both routines, selected by ``batched``
-    def _verify_lookup(self, group_order: int, pf, public, batched: bool) -> bool:
+    # ---- both routines, plain and lookup proofs: steps 4-12 of the paper's verifier
+    def _verify(self, group_order: int, pf, public, batched: bool) -> bool:
         n = group_order
         proof = pf.flatten()
-        ch = Transcript(b"plonk").replay(LOOKUP_SCHEDULE, proof)
-        beta, gamma, eta, delta, eps = ch["beta"], ch["gamma"], ch["eta"], ch["delta"], ch["epsilon"]
-        alpha, zeta, v, u = ch["alpha"], ch["zeta"], ch["v"], ch["u"]
+        ch = Transcript(b"plonk").replay(LOOKUP_SCHEDULE if self.lookup else SCHEDULE, proof)
+        beta, gamma, alpha, zeta, v, u = ch["beta"], ch["gamma"], ch["alpha"], ch["zeta"], ch["v"], ch["u"]
         zh_ev = zeta ** n - 1
         l0_ev = zh_ev / ((zeta - 1) * n)
         pi_ev = _lagrange_terms_at(n, [-int(x) % CURVE_ORDER for x in public], zeta)
         a, b, c = proof["a_eval"], proof["b_eval"], proof["c_eval"]
         s1, s2, zw = proof["s1_eval"], proof["s2_eval"], proof["z_shifted_eval"]
-        fe, te, tw = proof["f_eval"], proof["t_eval"], proof["t_shifted_eval"]
-        h2e, h1w, z2w = proof["h2_eval"], proof["h1_shifted_eval"], proof["z2_shifted_eval"]
         root = Scalar.root_of_unity(n)
         zeta_n = zeta ** n
         a2 = alpha * alpha
-        a3, a4 = a2 * alpha, a2 * a2
-        a5 = a4 * alpha
-        od = delta + 1
-        eod = eps * od
-        hw = eod + h2e + delta * h1w
-        qk, t1, t2, t3 = self.lookup
+        v2, v3, v4, v5 = v ** 2, v ** 3, v ** 4, v ** 5
         sigma_bar = (a + beta * s1 + gamma) * (b + beta * s2 + gamma) * zw
         # the linearisation R without its constant, and the constant r0 (R(zeta) == 0)
         r_terms = [
@@ -198,34 +118,50 @@ class VerificationKey:
              * alpha + l0_ev * a2),
             (self.S3, -sigma_bar * alpha * beta),
             (proof["t_lo_1"], -zh_ev), (proof["t_mid_1"], -zh_ev * zeta_n), (proof["t_hi_1"], -zh_ev * zeta_n * zeta_n),
-            # alpha^3 q_K (a + eta b + eta^2 c - f)
-            (qk, a3 * (a + eta * b + eta * eta * c - fe)),
-            # alpha^4 [Z2 (1+d)(e+f)(e(1+d) + t + d t_w) - z2_w (e(1+d) + H1 + d h2) hw] + alpha^5 L0 (Z2 - 1)
-            (proof["z2_1"], a4 * od * (eps + fe) * (eod + te + delta * tw) + a5 * l0_ev),
-            (proof["h1_1"], -a4 * z2w * hw),
         ]
-        r0 = (pi_ev - l0_ev * a2 - sigma_bar * alpha * (c + gamma) - a4 * z2w * (eod + delta * h2e) * hw
-              - a5 * l0_ev)
-        v2, v3, v4, v5 = v ** 2, v ** 3, v ** 4, v ** 5
-        v6, v7, v8 = v5 * v, v5 * v2, v5 * v3
-        at_zeta = [(proof["a_1"], v), (proof["b_1"], v2), (proof["c_1"], v3), (self.S1, v4), (self.S2, v5),
-                   (proof["f_1"], v6), (proof["h2_1"], v8)]
-        t_parts = [(t1, Scalar(1)), (t2, eta), (t3, eta * eta)]  # [T] = [t1] + eta [t2] + eta^2 [t3]
-        e_zeta = v * a + v2 * b + v3 * c + v4 * s1 + v5 * s2 + v6 * fe + v7 * te + v8 * h2e
-        e_zw = zw + v * tw + v2 * h1w + v3 * z2w
+        r0 = pi_ev - l0_ev * a2 - sigma_bar * alpha * (c + gamma)
+        # the openings at zeta and at zeta w: (commitment, batching weight), and the claimed value of each batch
+        at_zeta = [(proof["a_1"], v), (proof["b_1"], v2), (proof["c_1"], v3), (self.S1, v4), (self.S2, v5)]
+        e_zeta = v * a + v2 * b + v3 * c + v4 * s1 + v5 * s2
+        at_zw = [(proof["z_1"], Scalar(1))]
+        e_zw = zw
+        if self.lookup:
+            eta, delta, eps = ch["eta"], ch["delta"], ch["epsilon"]
+            fe, te, tw = proof["f_eval"], proof["t_eval"], proof["t_shifted_eval"]
+            h2e, h1w, z2w = proof["h2_eval"], proof["h1_shifted_eval"], proof["z2_shifted_eval"]
+            a3, a4 = a2 * alpha, a2 * a2
+            a5 = a4 * alpha
+            od = delta + 1
+            eod = eps * od
+            hw = eod + h2e + delta * h1w
+            qk, t1, t2, t3 = self.lookup
+            r_terms += [
+                # alpha^3 q_K (a + eta b + eta^2 c - f)
+                (qk, a3 * (a + eta * b + eta * eta * c - fe)),
+                # alpha^4 [Z2 (1+d)(e+f)(e(1+d) + t + d t_w) - z2_w (e(1+d) + H1 + d h2) hw] + alpha^5 L0 (Z2 - 1)
+                (proof["z2_1"], a4 * od * (eps + fe) * (eod + te + delta * tw) + a5 * l0_ev),
+                (proof["h1_1"], -a4 * z2w * hw),
+            ]
+            r0 = r0 - a4 * z2w * (eod + delta * h2e) * hw - a5 * l0_ev
+            v6, v7, v8 = v5 * v, v5 * v2, v5 * v3
+            t_parts = [(t1, Scalar(1)), (t2, eta), (t3, eta * eta)]  # [T] = [t1] + eta [t2] + eta^2 [t3]
+            at_zeta += [(proof["f_1"], v6), (proof["h2_1"], v8)] + [(p, k * v7) for p, k in t_parts]
+            e_zeta = e_zeta + v6 * fe + v7 * te + v8 * h2e
+            at_zw += [(proof["h1_1"], v2), (proof["z2_1"], v3)] + [(p, k * v) for p, k in t_parts]
+            e_zw = e_zw + v * tw + v2 * h1w + v3 * z2w
         if batched:
-            d_pt = ec_lincomb(r_terms + [(proof["z_1"], u), (proof["z2_1"], u * v3), (proof["h1_1"], u * v2)]
-                              + [(p, k * (v7 + u * v)) for p, k in t_parts] + at_zeta)
+            # e(W_z + u W_zw, [x]_2) == e(zeta W_z + u zeta w W_zw + F - E, [1]_2), F = [R] - r0 + both batches
+            f_pt = ec_lincomb(r_terms + at_zeta + [(p, u * k) for p, k in at_zw])
             e_scalar = -r0 + e_zeta + u * e_zw
             lhs = ec_lincomb([(proof["W_z_1"], 1), (proof["W_zw_1"], u)])
-            rhs = ec_lincomb([(proof["W_z_1"], zeta), (proof["W_zw_1"], u * zeta * root), (d_pt, 1), (G1, -e_scalar)])
+            rhs = ec_lincomb([(proof["W_z_1"], zeta), (proof["W_zw_1"], u * zeta * root), (f_pt, 1), (G1, -e_scalar)])
             return pairing_product_is_one([(lhs, self.X_2), (g1_neg(rhs), G2)])
-        batch = ec_lincomb(r_terms + [(G1, r0)] + at_zeta + [(p, k * v7) for p, k in t_parts] + [(G1, -e_zeta)])
+        # R's commitment formed, then the opening at zeta and the opening at zeta w, each its own pairing product
+        batch = ec_lincomb(r_terms + [(G1, r0)] + at_zeta + [(G1, -e_zeta)])
         x_minus_zeta = g2_add(self.X_2, g2_mul(G2, -zeta))
         if not pairing_product_is_one([(batch, G2), (g1_neg(proof["W_z_1"]), x_minus_zeta)]):
             return False
-        shifted = ec_lincomb([(proof["z_1"], 1), (proof["h1_1"], v2), (proof["z2_1"], v3)]
-                             + [(p, k * v) for p, k in t_parts] + [(G1, -e_zw)])
+        shifted = ec_lincomb(at_zw + [(G1, -e_zw)])
         x_minus_zeta_w = g2_add(self.X_2, g2_mul(G2, -(zeta * root)))
         return pairing_product_is_one([(shifted, G2), (g1_neg(proof["W_zw_1"]), x_minus_zeta_w)])
 
