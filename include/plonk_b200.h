@@ -178,6 +178,13 @@ int pb200_prover_serialize(pb200_prover* p, uint8_t* h_proof768);
  * 13 points and 12 scalars (1216 bytes) and is made by the entry points below.  Round 1, 3 and 5 are unchanged. */
 int pb200_prover_set_lookup(pb200_prover* p, const uint8_t* h_qk, const uint8_t* h_t1, const uint8_t* h_t2,
                             const uint8_t* h_t3, uint64_t table_rows);
+/* Lookups over several tables, told apart by a table tag (PlonKup).  The tables are concatenated into h_t1..h_t3 and
+ * h_t4 holds each table row's table id (table_rows x 32 bytes, canonical LE).  h_qtag: n x 32 bytes, Q_T = the id of
+ * the table each lookup row reads, canonical and 0 wherever q_K = 0.  A row with q_K = 1 claims that (a, b, c, Q_T)
+ * is a row of (t1, t2, t3, t4).  The same refusals as pb200_prover_set_lookup; proofs are made by the same entry
+ * points and have the same 1216 bytes.  With t4 = Q_T = 0 the proof equals pb200_prover_set_lookup's. */
+int pb200_prover_set_lookup_tagged(pb200_prover* p, const uint8_t* h_qk, const uint8_t* h_qtag, const uint8_t* h_t1,
+                                   const uint8_t* h_t2, const uint8_t* h_t3, const uint8_t* h_t4, uint64_t table_rows);
 /* step 1L, after round 1 and the challenge eta: commitments f_1 h1_1 h2_1 */
 int pb200_prover_round_lookup(pb200_prover* p, const uint8_t* eta, uint8_t* h_fh_xy /*3*64*/);
 /* round 2 with the lookup challenges: commitments z_1 z2_1 */

@@ -84,6 +84,7 @@ def _load():
         "pb200_prover_serialize": (I, [V, V]),
         "pb200_prover_set_zk": (I, [V, I, V]),
         "pb200_prover_set_lookup": (I, [V, V, V, V, V, U64]),
+        "pb200_prover_set_lookup_tagged": (I, [V, V, V, V, V, V, V, U64]),
         "pb200_prover_round_lookup": (I, [V, V, V]),
         "pb200_prover_round2_lookup": (I, [V, V, V, V, V, V]),
         "pb200_prover_round4_lookup": (I, [V, V, V]),

@@ -53,7 +53,8 @@ void prover_round4(Prover* P, const Fr& zeta_c);
 void prover_round5(Prover* P, const Fr& v_c);
 void prover_serialize(const Prover* P, uint8_t* out);
 void prover_set_zk(Prover* P, bool enable, const uint8_t* h_blinders);
-void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* const* h_tab, uint64_t rows);
+void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* h_qtag, const uint8_t* const* h_tab,
+                       uint64_t rows);
 void prover_round_lookup(Prover* P, const Fr& eta_c);
 void prover_round2_lookup(Prover* P, const Fr& beta_c, const Fr& gamma_c, const Fr& delta_c, const Fr& epsilon_c);
 void prover_round4_lookup(Prover* P, const Fr& zeta_c);
@@ -532,8 +533,16 @@ int pb200_prover_serialize(pb200_prover* p, uint8_t* h_proof768) {
 int pb200_prover_set_lookup(pb200_prover* p, const uint8_t* h_qk, const uint8_t* h_t1, const uint8_t* h_t2,
                             const uint8_t* h_t3, uint64_t table_rows) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  const uint8_t* tab[3] = {h_t1, h_t2, h_t3};
-  prover_set_lookup(reinterpret_cast<Prover*>(p), h_qk, tab, table_rows);
+  const uint8_t* tab[4] = {h_t1, h_t2, h_t3, nullptr};
+  prover_set_lookup(reinterpret_cast<Prover*>(p), h_qk, nullptr, tab, table_rows);
+  PB_API_END
+}
+int pb200_prover_set_lookup_tagged(pb200_prover* p, const uint8_t* h_qk, const uint8_t* h_qtag, const uint8_t* h_t1,
+                                   const uint8_t* h_t2, const uint8_t* h_t3, const uint8_t* h_t4, uint64_t table_rows) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  PB_CHECK(h_qtag && h_t4, "tagged lookups need Q_T and the table tag column t4");
+  const uint8_t* tab[4] = {h_t1, h_t2, h_t3, h_t4};
+  prover_set_lookup(reinterpret_cast<Prover*>(p), h_qk, h_qtag, tab, table_rows);
   PB_API_END
 }
 int pb200_prover_round_lookup(pb200_prover* p, const uint8_t* eta, uint8_t* h_fh_xy) {

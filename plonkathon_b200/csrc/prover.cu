@@ -415,8 +415,9 @@ __global__ void __launch_bounds__(128) k_horner_strided(EvalArgs a, Fr* H) {
 // ---- coefficient-space linear combination: out[k] = sum_i w[i] * vec[i][k] (+ c0 at k == 0) -----------------
 // indices [first, first + n) of the result (a slab of a sharded round 5; first = 0, n = everything on one device).
 // 26 slots: round 5's largest batch is 19 plain terms (5 gate selectors, 4 custom, Z, S3, T1-T3, A, B, C, S1, S2) and
-// 6 lookup terms.
+// 7 lookup terms (q_K, Q_T with a table tag, Z2, H1, F, T, H2).
 struct LinCombArgs { const Fr* vec[26]; Fr w[26]; Fr c0; int count; uint64_t n, first; };
+static_assert(5 + PB_MAX_CUSTOM + 10 + 7 <= 26, "round 5's largest batch must fit LinCombArgs");
 __global__ void __launch_bounds__(128) k_lincomb(LinCombArgs a, Fr* out) {
   uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= a.n) return;
@@ -462,32 +463,37 @@ __global__ void k_scan_tile_sums(const uint32_t* counts, uint32_t nb, uint32_t p
 __global__ void k_scan_tiles(uint32_t* tile_sums, uint32_t n_tiles, uint32_t* total_out);
 __global__ void k_scan_apply(uint32_t* counts, uint32_t nb, uint32_t pad, const uint32_t* tile_sums, uint32_t* offsets);
 
-// the order of the sorted table copy: (t1, t2, t3) lexicographically, each by Montgomery limbs from the top
-PB_HD int lookup_cmp(const Fr* x, const Fr& a, const Fr& b, const Fr& c) {
-  const Fr* y[3] = {&a, &b, &c};
-  for (int w = 0; w < 3; w++)
+// the order of the sorted table copy: (t1, t2, t3[, t4]) lexicographically, each by Montgomery limbs from the top.
+// width 3 for one untagged table, 4 with the table tag t4 (y[3] is read only then).  Unrolled, so y stays in registers.
+PB_HD int lookup_cmp(const Fr* x, const Fr (&y)[4], int width) {
+#pragma unroll
+  for (int w = 0; w < 4; w++) {
+    if (w == width) break;
+#pragma unroll
     for (int l = 7; l >= 0; l--)
-      if (x[w].v[l] != y[w]->v[l]) return x[w].v[l] < y[w]->v[l] ? -1 : 1;
+      if (x[w].v[l] != y[w].v[l]) return x[w].v[l] < y[w].v[l] ? -1 : 1;
+  }
   return 0;
 }
 
-// j_i: for a lookup row (q_K = 1) the lowest table index of a row equal to (a_i, b_i, c_i) -- the first of the equal rows
-// in the sorted copy, which keeps table order among them --, else 0.  A row not in the table: the lowest such i goes to
-// *missing.
-__global__ void __launch_bounds__(128) k_lookup_index(const Fr* A, const Fr* B, const Fr* C, const Fr* QK, const Fr* keys,
-                                                      const uint32_t* keys_idx, uint64_t rows, uint64_t n, uint32_t* j_out,
-                                                      uint32_t* missing) {
+// j_i: for a lookup row (q_K = 1) the lowest table index of a row equal to (a_i, b_i, c_i[, Q_T[i]]) -- the first of
+// the equal rows in the sorted copy, which keeps table order among them --, else 0.  QT == nullptr: one untagged table,
+// keys of three columns.  A row not in the table: the lowest such i goes to *missing.
+__global__ void __launch_bounds__(128) k_lookup_index(const Fr* A, const Fr* B, const Fr* C, const Fr* QK, const Fr* QT,
+                                                      const Fr* keys, const uint32_t* keys_idx, uint64_t rows, uint64_t n,
+                                                      uint32_t* j_out, uint32_t* missing) {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   if (ldg_fr(QK + i).is_zero()) { j_out[i] = 0; return; }
-  const Fr a = ldg_fr(A + i), b = ldg_fr(B + i), c = ldg_fr(C + i);
+  const int width = QT ? 4 : 3;
+  const Fr key[4] = {ldg_fr(A + i), ldg_fr(B + i), ldg_fr(C + i), QT ? ldg_fr(QT + i) : Fr::zero()};
   uint64_t lo = 0, hi = rows;
   while (lo < hi) {
     uint64_t mid = (lo + hi) / 2;
-    if (lookup_cmp(keys + 3 * mid, a, b, c) < 0) lo = mid + 1;
+    if (lookup_cmp(keys + width * mid, key, width) < 0) lo = mid + 1;
     else hi = mid;
   }
-  if (lo < rows && lookup_cmp(keys + 3 * lo, a, b, c) == 0) {
+  if (lo < rows && lookup_cmp(keys + width * lo, key, width) == 0) {
     j_out[i] = keys_idx[lo];
   } else {
     j_out[i] = 0;
@@ -518,10 +524,15 @@ __global__ void __launch_bounds__(256) k_lookup_place(const uint32_t* off, uint6
   sidx[p] = (uint32_t)(lo - 1);
 }
 
-// t = t1 + eta t2 + eta^2 t3, then f_i = t[j_i], h1_i = s_2i, h2_i = s_2i+1
-__global__ void k_lookup_compress(const Fr* t1, const Fr* t2, const Fr* t3, Fr eta, Fr eta2, uint64_t n, Fr* t) {
+// t = t1 + eta t2 + eta^2 t3 (+ eta^3 t4 with a table tag; t4 == nullptr without), then f_i = t[j_i], h1_i = s_2i,
+// h2_i = s_2i+1
+__global__ void k_lookup_compress(const Fr* t1, const Fr* t2, const Fr* t3, const Fr* t4, Fr eta, Fr eta2, Fr eta3,
+                                  uint64_t n, Fr* t) {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) t[i] = fp_add(ldg_fr(t1 + i), fp_add(fp_mul(eta, ldg_fr(t2 + i)), fp_mul(eta2, ldg_fr(t3 + i))));
+  if (i >= n) return;
+  Fr x = fp_add(ldg_fr(t1 + i), fp_add(fp_mul(eta, ldg_fr(t2 + i)), fp_mul(eta2, ldg_fr(t3 + i))));
+  if (t4) x = fp_add(x, fp_mul(eta3, ldg_fr(t4 + i)));
+  t[i] = x;
 }
 __global__ void k_lookup_gather(const Fr* t, const uint32_t* j, const uint32_t* sidx, uint64_t n, Fr* f, Fr* h1, Fr* h2) {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -547,13 +558,14 @@ __global__ void k_lookup_z2_terms(const Fr* t, const Fr* f, const Fr* h1, const 
 }
 
 // the three lookup terms of the quotient, added to the plain quotient's evaluations on the 4n coset (one GPU):
-//   a3 q_K (A + eta B + eta^2 C - F)
+//   a3 [q_K (A + eta B + eta^2 C - F) + eta^3 Q_T]
 // + a4 [Z2 (1+d)(e+F)(e(1+d) + T + d T(wX)) - Z2(wX)(e(1+d) + H1 + d H2)(e(1+d) + H2 + d H1(wX))]
-// + a5 L0 (Z2 - 1),   all over Z_H.  X -> wX is index + 4 on the coset, as for Z.
+// + a5 L0 (Z2 - 1),   all over Z_H.  X -> wX is index + 4 on the coset, as for Z.  Q_T = q_K * tag, the table id of
+// each lookup row; QT == nullptr for one untagged table (the term is zero).
 struct LookupQuotientArgs {
-  const Fr *A, *B, *C, *QK, *T, *F, *H1, *H2, *Z2, *L0;
+  const Fr *A, *B, *C, *QK, *QT, *T, *F, *H1, *H2, *Z2, *L0;
   Fr zh_inv[4];
-  Fr eta, eta2, delta, eps, one_d, eps_one_d, alpha3, alpha4, alpha5, one;
+  Fr eta, eta2, eta3, delta, eps, one_d, eps_one_d, alpha3, alpha4, alpha5, one;
   uint64_t n4;
 };
 __global__ void __launch_bounds__(128) k_quotient_lookup(LookupQuotientArgs q, Fr* out) {
@@ -562,7 +574,9 @@ __global__ void __launch_bounds__(128) k_quotient_lookup(LookupQuotientArgs q, F
   const uint64_t jw = j + 4 >= q.n4 ? j + 4 - q.n4 : j + 4;
   const Fr f = ldg_fr(q.F + j);
   Fr w = fp_add(ldg_fr(q.A + j), fp_add(fp_mul(q.eta, ldg_fr(q.B + j)), fp_mul(q.eta2, ldg_fr(q.C + j))));
-  Fr acc = fp_mul(q.alpha3, fp_mul(ldg_fr(q.QK + j), fp_sub(w, f)));
+  Fr acc = fp_mul(ldg_fr(q.QK + j), fp_sub(w, f));
+  if (q.QT) acc = fp_add(acc, fp_mul(q.eta3, ldg_fr(q.QT + j)));
+  acc = fp_mul(q.alpha3, acc);
   const Fr z2 = ldg_fr(q.Z2 + j), h1 = ldg_fr(q.H1 + j), h2 = ldg_fr(q.H2 + j);
   Fr p1 = fp_mul(fp_mul(fp_mul(z2, q.one_d), fp_add(q.eps, f)),
                  fp_add(fp_add(q.eps_one_d, ldg_fr(q.T + j)), fp_mul(q.delta, ldg_fr(q.T + jw))));
@@ -875,26 +889,43 @@ static ZkPatch zh_multiple(std::initializer_list<Fr> c) {
 // entry followed by one copy per row that looks it up; h1 = s[0::2], h2 = s[1::2]; Z2 is the grand product of
 // k_lookup_z2_terms.  The quotient gains k_quotient_lookup's three terms (degree <= 3n); round 5 opens F, T, H2 at
 // zeta and T, H1, Z2 at zeta w.  The index, histogram and placement do not depend on eta and run in round 1.
+// Several tables (PlonKup's table tag): the tables are concatenated, t4 holds each table row's table id and Q_T the id
+// of the table each lookup row reads (0 off lookup rows).  t gains eta^3 t4, the index matches (a, b, c, Q_T), the
+// quotient's alpha^3 term gains eta^3 Q_T and round 5 one slot, alpha^3 eta^3 Q_T.  With t4 = Q_T = 0 every one of
+// these terms vanishes, so one table proves the same bytes tagged or not.
 
-void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* const* h_tab, uint64_t rows) {
+// h_qtag == nullptr: one untagged table of three columns (h_tab[3] unused).  Otherwise several tables concatenated: the
+// fourth column h_tab[3] holds each table row's table id and h_qtag = Q_T the id of the table each lookup row reads,
+// zero wherever q_K = 0.  The rows are matched on (a, b, c, Q_T) and compressed with eta^3 t4 (eta^3 Q_T in the
+// quotient), so a row can only match a row of its own table.
+void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* h_qtag, const uint8_t* const* h_tab,
+                       uint64_t rows) {
   Context* ctx = P->ctx;
   const uint64_t n = P->n;
+  const bool tagged = h_qtag != nullptr;
+  const int width = tagged ? 4 : 3;
   PB_CHECK(P->world == 1, "lookups are not available on the sharded prover (one GPU only)");
   PB_CHECK(!P->zk, "lookups do not combine with zero-knowledge mode");
   PB_CHECK(!P->lk, "the lookup table is already set (set it once, before the first proof)");
   PB_CHECK(h_qk && h_tab && h_tab[0] && h_tab[1] && h_tab[2], "lookups need q_K and three table columns");
+  PB_CHECK(!tagged || h_tab[3], "tagged lookups need the table tag column t4");
   PB_CHECK(rows >= 1, "the lookup table is empty");
   PB_CHECK(rows <= n, "the lookup table has more rows than the circuit");
-  // q_K: 0 or 1 on every row
+  // q_K: 0 or 1 on every row; Q_T canonical and 0 where q_K = 0
   for (uint64_t i = 0; i < n; i++) {
     const uint8_t* e = h_qk + 32 * i;
     bool ok = e[0] <= 1;
     for (int k = 1; k < 32 && ok; k++) ok = e[k] == 0;
     PB_CHECK(ok, "q_K must be 0 or 1 on every row");
+    if (!tagged) continue;
+    Fr x;
+    memcpy(x.v, h_qtag + 32 * i, 32);
+    PB_CHECK(fp_is_canonical(x), ("Q_T on row " + std::to_string(i) + " not reduced below the field modulus").c_str());
+    PB_CHECK(e[0] == 1 || x.is_zero(), ("Q_T must be 0 where q_K = 0: row " + std::to_string(i)).c_str());
   }
   // the table, padded to n rows by repeating its last row, in Montgomery form
-  std::vector<Fr> tab[3];
-  for (int w = 0; w < 3; w++) {
+  std::vector<Fr> tab[4];
+  for (int w = 0; w < width; w++) {
     tab[w].resize(n);
     for (uint64_t r = 0; r < n; r++) {
       Fr x;
@@ -903,21 +934,24 @@ void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* const* h_t
       tab[w][r] = fp_to_mont(x);
     }
   }
+  // stable: equal rows keep table order, so the first of them in the sorted copy is the lowest table index
   std::vector<uint32_t> order(rows);
   for (uint64_t r = 0; r < rows; r++) order[r] = (uint32_t)r;
+  const Fr zero = Fr::zero();
   std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) {
-    const Fr kx[3] = {tab[0][x], tab[1][x], tab[2][x]};
-    return lookup_cmp(kx, tab[0][y], tab[1][y], tab[2][y]) < 0;
+    const Fr kx[4] = {tab[0][x], tab[1][x], tab[2][x], tagged ? tab[3][x] : zero};
+    const Fr ky[4] = {tab[0][y], tab[1][y], tab[2][y], tagged ? tab[3][y] : zero};
+    return lookup_cmp(kx, ky, width) < 0;
   });
-  std::vector<Fr> keys(3 * rows);
+  std::vector<Fr> keys(width * rows);
   for (uint64_t r = 0; r < rows; r++)
-    for (int w = 0; w < 3; w++) keys[3 * r + w] = tab[w][order[r]];
+    for (int w = 0; w < width; w++) keys[width * r + w] = tab[w][order[r]];
   cudaStream_t st = ctx->stream;
   P->lk_keys.alloc(keys.size() * 32);
   P->lk_keys_idx.alloc(rows * 4);
   PB_CUDA(cudaMemcpyAsync(P->lk_keys.p, keys.data(), keys.size() * 32, cudaMemcpyHostToDevice, st));
   PB_CUDA(cudaMemcpyAsync(P->lk_keys_idx.p, order.data(), rows * 4, cudaMemcpyHostToDevice, st));
-  for (int w = 0; w < 3; w++) {
+  for (int w = 0; w < width; w++) {
     P->lk_tab[w].alloc(n * 32);
     PB_CUDA(cudaMemcpyAsync(P->lk_tab[w].p, tab[w].data(), n * 32, cudaMemcpyHostToDevice, st));
   }
@@ -926,6 +960,13 @@ void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* const* h_t
   ntt_run(ctx, P->lk_qk_lag.as<Fr>(), P->lk_qk_coeff.as<Fr>(), P->log_n, true, n, nullptr, nullptr);
   P->lk_qk_ext.alloc(P->n_ext * 32);
   coset_extend(P, st, nullptr, P->lk_qk_coeff.as<Fr>(), P->lk_qk_ext.as<Fr>(), P->gpow.as<Fr>());
+  if (tagged) {  // Q_T as q_K: Lagrange values (the index), coefficients (round 5), the 4n coset (the quotient)
+    upload_mont(ctx, P->lk_qt_lag, h_qtag, n);
+    P->lk_qt_coeff.alloc(n * 32);
+    ntt_run(ctx, P->lk_qt_lag.as<Fr>(), P->lk_qt_coeff.as<Fr>(), P->log_n, true, n, nullptr, nullptr);
+    P->lk_qt_ext.alloc(P->n_ext * 32);
+    coset_extend(P, st, nullptr, P->lk_qt_coeff.as<Fr>(), P->lk_qt_ext.as<Fr>(), P->gpow.as<Fr>());
+  }
   P->lk_j.alloc(n * 4);
   P->lk_cnt.alloc(n * 4);
   P->lk_off.alloc((n + 1) * 4);
@@ -937,6 +978,7 @@ void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* const* h_t
   }
   PB_CUDA(cudaStreamSynchronize(st));  // the host copies die here
   P->lk_rows = rows;
+  P->lk_tagged = tagged;
   P->lk = true;
 }
 
@@ -948,8 +990,9 @@ static void lookup_index(Prover* P) {
   uint32_t* missing = P->flags.as<uint32_t>() + 2;
   PB_CUDA(cudaMemsetAsync(missing, 0xff, 4, st));
   k_lookup_index<<<PB_GRID(n, 128), 0, st>>>(P->lag[0].as<Fr>(), P->lag[1].as<Fr>(), P->lag[2].as<Fr>(),
-                                            P->lk_qk_lag.as<Fr>(), P->lk_keys.as<Fr>(), P->lk_keys_idx.as<uint32_t>(),
-                                            P->lk_rows, n, P->lk_j.as<uint32_t>(), missing);
+                                            P->lk_qk_lag.as<Fr>(), P->lk_tagged ? P->lk_qt_lag.as<Fr>() : nullptr,
+                                            P->lk_keys.as<Fr>(), P->lk_keys_idx.as<uint32_t>(), P->lk_rows, n,
+                                            P->lk_j.as<uint32_t>(), missing);
   PB_CUDA(cudaMemsetAsync(P->lk_cnt.p, 0, n * 4, st));
   k_lookup_hist<<<PB_GRID(n, 256), 0, st>>>(P->lk_j.as<uint32_t>(), n, P->lk_cnt.as<uint32_t>());
   const uint32_t n_tiles = (uint32_t)((n + PB_SCAN_TILE - 1) / PB_SCAN_TILE);
@@ -975,8 +1018,10 @@ void prover_round_lookup(Prover* P, const Fr& eta_c) {
   P->eta = fp_to_mont(eta_c);
   Fr* v[Prover::LK_VECS];
   for (int k = 0; k < Prover::LK_VECS; k++) v[k] = P->lk_lag[k].as<Fr>();
+  const Fr eta2 = fp_sqr(P->eta);
   k_lookup_compress<<<PB_GRID(n, 256), 0, st>>>(P->lk_tab[0].as<Fr>(), P->lk_tab[1].as<Fr>(), P->lk_tab[2].as<Fr>(),
-                                               P->eta, fp_sqr(P->eta), n, v[Prover::LK_T]);
+                                               P->lk_tagged ? P->lk_tab[3].as<Fr>() : nullptr, P->eta, eta2,
+                                               fp_mul(eta2, P->eta), n, v[Prover::LK_T]);
   k_lookup_gather<<<PB_GRID(n, 256), 0, st>>>(v[Prover::LK_T], P->lk_j.as<uint32_t>(), P->lk_sidx.as<uint32_t>(), n,
                                              v[Prover::LK_F], v[Prover::LK_H1], v[Prover::LK_H2]);
   ctx->launches += 2;
@@ -1247,11 +1292,12 @@ void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c) {
       coset_extend(P, st, nullptr, P->lk_coeff[k].as<Fr>(), P->lk_ext[k].as<Fr>(), P->gpow.as<Fr>());
     LookupQuotientArgs lq;
     lq.A = q.A; lq.B = q.B; lq.C = q.C; lq.QK = P->lk_qk_ext.as<Fr>(); lq.L0 = q.L0;
+    lq.QT = P->lk_tagged ? P->lk_qt_ext.as<Fr>() : nullptr;
     lq.T = P->lk_ext[Prover::LK_T].as<Fr>(); lq.F = P->lk_ext[Prover::LK_F].as<Fr>();
     lq.H1 = P->lk_ext[Prover::LK_H1].as<Fr>(); lq.H2 = P->lk_ext[Prover::LK_H2].as<Fr>();
     lq.Z2 = P->lk_ext[Prover::LK_Z2].as<Fr>();
     for (int k = 0; k < 4; k++) lq.zh_inv[k] = P->zh_inv[k];
-    lq.eta = P->eta; lq.eta2 = fp_sqr(P->eta); lq.delta = P->delta; lq.eps = P->epsilon;
+    lq.eta = P->eta; lq.eta2 = fp_sqr(P->eta); lq.eta3 = fp_mul(lq.eta2, P->eta); lq.delta = P->delta; lq.eps = P->epsilon;
     lq.one_d = fp_add(Fr::one(), P->delta); lq.eps_one_d = fp_mul(P->epsilon, lq.one_d);
     lq.alpha3 = fp_mul(q.alpha2, P->alpha); lq.alpha4 = fp_sqr(q.alpha2); lq.alpha5 = fp_mul(lq.alpha4, P->alpha);
     lq.one = Fr::one();
@@ -1459,6 +1505,7 @@ void prover_round5(Prover* P, const Fr& v_c) {
     const Fr hw = fp_add(fp_add(eod, h2e), fp_mul(de, h1w));       // e(1+d) + h2 + d h1(zeta w)
     const Fr az2 = fp_mul(al4, z2w);
     add(P->lk_qk_coeff.as<Fr>(), fp_mul(al3, fp_sub(abc, fe)));
+    if (P->lk_tagged) add(P->lk_qt_coeff.as<Fr>(), fp_mul(al3, fp_mul(fp_sqr(eta), eta)));  // alpha^3 eta^3 Q_T
     add(P->lk_coeff[Prover::LK_Z2].as<Fr>(),
         fp_add(fp_mul(fp_mul(fp_mul(al4, od), fp_add(ep, fe)), fp_add(fp_add(eod, te), fp_mul(de, tw))),
                fp_mul(al5, l0_ev)));

@@ -112,15 +112,18 @@ struct Prover {
   Fr zk_b[ZK_BLINDERS];           // this proof's b1..b11, Montgomery (drawn when round 1 starts)
   DevBuf zk_coeff[4];             // A' B' C' (n + 2 coefficients) Z' (n + 3)
   DevBuf zk_t[3];                 // T1' T2' (n + 1 coefficients) T3' (n + 6)
-  // Lookup argument (prover_set_lookup, one GPU): plookup over one fixed table of three columns, see "lookups" in
-  // prover.cu.  The proof gains f_1 h1_1 h2_1 z2_1 and six evaluations (1216 bytes).
+  // Lookup argument (prover_set_lookup, one GPU): plookup over one fixed table of three columns, or over several
+  // tables told apart by a tag column t4 and the selector Q_T, see "lookups" in prover.cu.  The proof gains f_1 h1_1
+  // h2_1 z2_1 and six evaluations (1216 bytes).
   enum { LK_T = 0, LK_F, LK_H1, LK_H2, LK_Z2, LK_VECS };
   bool lk = false;
+  bool lk_tagged = false;              // several tables: t4 and Q_T are set (and lk_keys has 4 Fr per row)
   uint64_t lk_rows = 0;                // table rows before padding
   DevBuf lk_qk_coeff, lk_qk_ext;       // q_K: coefficients, on the 4n coset
   DevBuf lk_qk_lag;                    // q_K Lagrange values (Montgomery 0 / 1)
-  DevBuf lk_tab[3];                    // t1 t2 t3, Lagrange, padded to n by repeating the last row
-  DevBuf lk_keys;                      // the table rows sorted by their Montgomery limbs (3 Fr per row) ...
+  DevBuf lk_qt_lag, lk_qt_coeff, lk_qt_ext;  // Q_T (table id per lookup row): Lagrange, coefficients, 4n coset
+  DevBuf lk_tab[4];                    // t1 t2 t3 (t4 if tagged), Lagrange, padded to n by repeating the last row
+  DevBuf lk_keys;                      // the table rows sorted by their Montgomery limbs (3 or 4 Fr per row) ...
   DevBuf lk_keys_idx;                  // ... and their original indices (uint32); equal rows keep table order
   DevBuf lk_j;                         // per row: table index j_i (uint32, n)
   DevBuf lk_cnt;                       // rows per table entry (uint32, n), zeroed by the scan

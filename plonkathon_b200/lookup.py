@@ -1,4 +1,4 @@
-"""Lookups: a plookup argument over one fixed table of three columns.
+"""Lookups: a plookup argument over fixed tables of three columns.
 
 A circuit with lookups has a boolean selector column q_K and a table (t1, t2, t3) of 1..n rows, padded to n rows by
 repeating its last row.  A row i with q_K[i] = 1 claims that (a_i, b_i, c_i) is a row of the table; the table's rows
@@ -6,9 +6,15 @@ keep the order the user gives them and may repeat.  The argument is plookup (epr
 alternating-split form of PlonKup (eprint 2022/086); DESIGN.md describes it.  A lookup proof has 13 G1 points and 12
 scalars (1216 bytes, ``LookupProof``).
 
-Here: the checks on a lookup argument as users give it, ``(q_K, (t1, t2, t3))``, shared by ``Prover.from_arrays``,
-``Setup.verification_key_arrays`` and ``synthetic.build_circuit``.  Out of scope, and refused: zero knowledge with
-lookups, the sharded prover, more than one table, tables wider than three columns."""
+Several tables (``lookups=[(q_0, (t1, t2, t3)), (q_1, ...), ...]``) are told apart by PlonKup's table tag: the tables
+are concatenated, a fourth column t4 holds each table row's id (table k has id k) and the selector Q_T the id of the
+table each lookup row reads (0 off lookup rows).  A lookup row then matches (a, b, c, Q_T) against (t1, t2, t3, t4),
+so it can only match a row of its own table: merging an XOR and an AND table without the tag would let a row meant
+for XOR pass with an AND row.
+
+Here: the checks on a lookup argument as users give it, ``(q_K, (t1, t2, t3))`` or a list of them, shared by
+``Prover.from_arrays``, ``Setup.verification_key_arrays`` and ``synthetic.build_circuit``.  Out of scope, and
+refused: zero knowledge with lookups, the sharded prover, tables wider than three columns."""
 from __future__ import annotations
 
 import numpy as np
@@ -55,8 +61,37 @@ def check_lookup(lookup, group_order: int):
     return qk, cols, rows
 
 
+def check_lookups(lookups, group_order: int):
+    """``lookups = [(q_0, (t1, t2, t3)), (q_1, ...), ...]``, one entry per table -> (q_K, Q_T as n ints each,
+    [t1, t2, t3, t4] as lists of ints over the concatenated tables, total rows).  Table k has id k: t4 is k on its rows
+    and Q_T is k where q_k = 1.  Each entry is checked as ``check_lookup`` checks ``lookup=``; ValueError also for an
+    empty list, selectors that overlap on a row (naming it) and more table rows in all than n."""
+    try:
+        lookups = list(lookups)
+    except TypeError:
+        raise ValueError("lookups must be a list of (q_K, (t1, t2, t3)), one per table") from None
+    if not lookups:
+        raise ValueError("lookups needs at least one table")
+    qk, qtag = [0] * group_order, [0] * group_order
+    cols, total = [[], [], [], []], 0
+    for k, lookup in enumerate(lookups):
+        q, tab, rows = check_lookup(lookup, group_order)
+        for i in range(group_order):
+            if q[i]:
+                if qk[i]:
+                    raise ValueError("lookup selectors overlap on row %d (tables %d and %d)" % (i, qtag[i], k))
+                qk[i], qtag[i] = 1, k
+        for w in range(3):
+            cols[w] += tab[w]
+        cols[3] += [k] * rows
+        total += rows
+    if total > group_order:
+        raise ValueError("the lookup tables have %d rows in all, more than the circuit's %d" % (total, group_order))
+    return qk, qtag, cols, total
+
+
 def padded_table(cols, group_order: int):
-    """the three columns padded to n rows by repeating their last row"""
+    """the columns padded to n rows by repeating their last row"""
     return [c + [c[-1]] * (group_order - len(c)) for c in cols]
 
 

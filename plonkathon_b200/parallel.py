@@ -122,8 +122,8 @@ class ShardedProver(Prover):
     _CREATE_CUSTOM = "pb200_prover_create_custom_sharded"
 
     @classmethod
-    def from_arrays(cls, setup, group_order, pk_arrays, group=None, ctx=None, custom=(), lookup=None):
-        if lookup is not None:
+    def from_arrays(cls, setup, group_order, pk_arrays, group=None, ctx=None, custom=(), lookup=None, lookups=None):
+        if lookup is not None or lookups is not None:
             raise ValueError("lookups are not available on the sharded prover (one GPU only)")
         init_comm(ctx or setup.ctx, group)
         return super().from_arrays(setup, group_order, pk_arrays, ctx=ctx, custom=custom)

@@ -17,7 +17,7 @@ import numpy as np
 from . import _lib
 from .curve import Scalar
 from .custom_gates import split_terms
-from .lookup import PROOF_BYTES as LOOKUP_PROOF_BYTES, check_lookup, padded_table, to_le_rows
+from .lookup import PROOF_BYTES as LOOKUP_PROOF_BYTES, check_lookup, check_lookups, padded_table, to_le_rows
 from .field import CURVE_ORDER, FIELD_MODULUS, FQ
 from .poly import Basis, _log2_exact, scalars_to_bytes
 from .transcript import Message1, Message2, Message3, Message4, Message5, Transcript
@@ -156,7 +156,7 @@ class Prover:
         self._create(setup, self.group_order, cols)
 
     @classmethod
-    def from_arrays(cls, setup, group_order: int, pk_arrays: dict, ctx=None, custom=(), lookup=None):
+    def from_arrays(cls, setup, group_order: int, pk_arrays: dict, ctx=None, custom=(), lookup=None, lookups=None):
         """pk_arrays: QM QL QR QO QC S1 S2 S3 -> list of ints or (n,32) uint8 little-endian arrays.
         ``ctx``: run this prover on another context (stream + scratch) of the same device than the setup's; the SRS
         is shared read-only, so several provers can be driven concurrently from different host threads.
@@ -164,8 +164,14 @@ class Prover:
         constraint (plonkathon_b200/custom_gates.py); ValueError for a malformed term.
         ``lookup``: ``(q_K, (t1, t2, t3))``, a lookup argument over one table of three columns
         (plonkathon_b200/lookup.py); ``prove_arrays`` then returns a 1216-byte ``LookupProof``.  ValueError for a
-        malformed argument; the library refuses it on the sharded prover."""
-        lk = check_lookup(lookup, group_order) if lookup is not None else None  # before any device work
+        malformed argument; the library refuses it on the sharded prover.
+        ``lookups``: ``[(q_0, (t1, t2, t3)), (q_1, ...), ...]``, lookups over several tables told apart by a table tag
+        (table k has id k; ``check_lookups``).  The proof is a ``LookupProof`` too.  Not together with ``lookup``."""
+        if lookup is not None and lookups is not None:
+            raise ValueError("pass either lookup= (one table) or lookups= (several tables), not both")
+        # before any device work
+        lk = check_lookup(lookup, group_order) if lookup is not None else None
+        lks = check_lookups(lookups, group_order) if lookups is not None else None
         self = cls.__new__(cls)
         self.group_order = group_order
         self.setup = setup
@@ -175,12 +181,21 @@ class Prover:
         self._create(setup, group_order, cols, ctx, custom)
         if lk is not None:
             self._set_lookup(*lk)
+        if lks is not None:
+            self._set_lookup_tagged(*lks)
         return self
 
     def _set_lookup(self, qk, cols, rows):
         keep = [to_le_rows(qk)] + [to_le_rows(c) for c in cols]
         ptr = [k.ctypes.data_as(ctypes.c_void_p) for k in keep]
         _lib.check(_lib.lib().pb200_prover_set_lookup(self._h, *ptr, rows))
+        self.lookup = True
+
+    def _set_lookup_tagged(self, qk, qtag, cols, rows):
+        """cols: t1, t2, t3, t4 (the table ids)"""
+        keep = [to_le_rows(qk), to_le_rows(qtag)] + [to_le_rows(c) for c in cols]
+        ptr = [k.ctypes.data_as(ctypes.c_void_p) for k in keep]
+        _lib.check(_lib.lib().pb200_prover_set_lookup_tagged(self._h, *ptr, rows))
         self.lookup = True
 
     def _create(self, setup, n, cols, ctx=None, custom=()):

@@ -11,7 +11,7 @@ from . import _lib
 from .curve import G2, Scalar, _pt_bytes, _pt_from, g2_mul
 from .field import CURVE_ORDER, FIELD_MODULUS, FQ, FQ2
 from .custom_gates import split_terms
-from .lookup import check_lookup, padded_table, to_le_rows
+from .lookup import check_lookup, check_lookups, padded_table, to_le_rows
 from .poly import Basis, Polynomial, _log2_exact
 from .prover import _as_le_rows
 from .verifier import VerificationKey  # noqa: F401  (re-exported: the reference's setup.py imports it too)
@@ -201,16 +201,22 @@ class Setup:
             h = self._lagrange[n]
         return h
 
-    def verification_key_arrays(self, group_order: int, pk_arrays: dict, custom=(), lookup=None) -> VerificationKey:
+    def verification_key_arrays(self, group_order: int, pk_arrays: dict, custom=(), lookup=None,
+                                lookups=None) -> VerificationKey:
         """``verification_key`` for circuits that exist only as arrays (``Prover.from_arrays``): QM..S3 as
         (n,32) uint8 little-endian Lagrange values in host memory.  ``custom``: the circuit's custom gate terms
         ``((i, j, l), column)`` as given to ``Prover.from_arrays``; each column is committed too.  ``lookup``:
         ``(q_K, (t1, t2, t3))`` as given to ``Prover.from_arrays``; the key gains [q_K], [t1], [t2], [t3] (the table
-        padded to n rows), the identity for a constant-zero column."""
+        padded to n rows), the identity for a constant-zero column.  ``lookups``: several tables as given to
+        ``Prover.from_arrays``; the key gains [q_K], [t1], [t2], [t3], [Q_T], [t4] (the tables concatenated and padded).
+        Not together with ``lookup``."""
         import numpy as np
+        if lookup is not None and lookups is not None:
+            raise ValueError("pass either lookup= (one table) or lookups= (several tables), not both")
         log_n = _log2_exact(group_order)
         exps, ccols = split_terms(custom, group_order)
         lk = check_lookup(lookup, group_order) if lookup is not None else None
+        lks = check_lookups(lookups, group_order) if lookups is not None else None
 
         def commit_host(col):
             col = np.ascontiguousarray(col).view(np.uint8).reshape(-1, 32)
@@ -232,6 +238,10 @@ class Setup:
         if lk is not None:
             qk, cols, _rows = lk
             lk_pts = tuple(commit_host(to_le_rows(c)) for c in [qk] + padded_table(cols, group_order))
+        if lks is not None:
+            qk, qtag, cols, _rows = lks
+            t1, t2, t3, t4 = padded_table(cols, group_order)
+            lk_pts = tuple(commit_host(to_le_rows(c)) for c in (qk, t1, t2, t3, qtag, t4))
         return VerificationKey(group_order, *pts, self.X2, Scalar.root_of_unity(group_order), terms, lk_pts)
 
     def verification_key(self, pk) -> VerificationKey:

@@ -40,6 +40,8 @@ class ArrayCircuit:
     custom: list = field(default_factory=list)
     # lookup argument (q_K per row, (t1, t2, t3)), plonkathon_b200/lookup.py; () without lookups
     lookup: tuple = ()
+    # lookups over several tables ((q_k per row, (t1, t2, t3)) per table, table k has id k); () without them
+    lookups: tuple = ()
 
     def wires_values(self):
         val = self.values
@@ -89,7 +91,7 @@ def permutation_polys(wire_L, wire_R, wire_O, group_order: int, n_constraints: i
 
 
 def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: float = 1.0,
-                  with_text: bool = False, custom=(), lookup=None) -> ArrayCircuit:
+                  with_text: bool = False, custom=(), lookup=None, lookups=None) -> ArrayCircuit:
     """Deterministic synthetic circuit with 2^log_n rows: ``n_public`` public-input rows, then a chain of
     multiplication / addition / add-constant gates whose operands are drawn from recently produced
     variables (so the permutation is non-trivial and the witness values are pseudo-random field elements).
@@ -100,14 +102,23 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
     ``lookup``: a table ``(t1, t2, t3)``; lookup rows are mixed into the chain as one more kind of row (a quarter of
     the rows without custom terms): the wires take a random table row as three new variables, q_K = 1 and every gate
     selector is 0, and later gates use those variables like any other (copy constraints).  Without it the random
-    draws are unchanged."""
+    draws are unchanged.
+
+    ``lookups``: a list of tables ``[(t1, t2, t3), ...]``; as ``lookup``, but each lookup row picks its table at random
+    (one more draw, only with two or more tables: ``lookups=[x]`` builds the circuit of ``lookup=x``)."""
     from .custom_gates import check_exponents
-    from .lookup import check_lookup
+    from .lookup import check_lookup, check_lookups
     custom = check_exponents(custom)
     n = 1 << log_n
+    if lookup is not None and lookups is not None:
+        raise ValueError("pass either lookup= (one table) or lookups= (several tables), not both")
+    tables = []  # (columns, rows) per table
     if lookup is not None:
-        _, table, rows = check_lookup(([0] * n, lookup), n)
-        QKl = [0] * n
+        tables = [check_lookup(([0] * n, lookup), n)[1:]]
+    if lookups is not None:
+        check_lookups([([0] * n, t) for t in lookups], n)  # each table, and their total size
+        tables = [check_lookup(([0] * n, t), n)[1:] for t in lookups]
+    QKs = [[0] * n for _ in tables]
     rng = random.Random(seed)
     m = max(n_public + 1, int(n * fill))
     m = min(m, n)
@@ -143,13 +154,15 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
         if first:  # make sure the private seeds are used so every variable appears in some cell
             ia, ib = n_public, n_public + 1
             first = False
-        kind = rng.randrange(3 + len(custom) + (lookup is not None))
+        kind = rng.randrange(3 + len(custom) + bool(tables))
         out = nv
-        if lookup is not None and kind == 3 + len(custom):  # (a, b, c) = a table row, q_K = 1
+        if tables and kind == 3 + len(custom):  # (a, b, c) = a row of table t, q_t = 1
+            t = rng.randrange(len(tables)) if len(tables) > 1 else 0
+            table, rows = tables[t]
             r = rng.randrange(rows)
             values.extend(table[w][r] for w in range(3))
             wL[row], wR[row], wO[row] = nv, nv + 1, nv + 2
-            QKl[row] = 1
+            QKs[t][row] = 1
         elif kind >= 3:
             ic = rng.randrange(lo, nv)
             k = rng.randrange(0, 1 << 30)
@@ -175,8 +188,9 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
             if with_text:
                 text.append("%s <== %s + %d" % (name(out), name(ia), k))
         row += 1
-    lk = (QKl, tuple(table)) if lookup is not None else ()
-    return ArrayCircuit(n, m, wL, wR, wO, QL, QR, QM, QO, QC, n_public, values, text, list(zip(custom, QK)), lk)
+    lk = (QKs[0], tuple(tables[0][0])) if lookup is not None else ()
+    lks = tuple((q, tuple(t)) for q, (t, _) in zip(QKs, tables)) if lookups is not None else ()
+    return ArrayCircuit(n, m, wL, wR, wO, QL, QR, QM, QO, QC, n_public, values, text, list(zip(custom, QK)), lk, lks)
 
 
 def _custom_row(exps, Q, row, operands, k, values, wires, sel):
@@ -230,3 +244,9 @@ def lookup_arrays(c: ArrayCircuit):
     """-> the circuit's lookup argument ``(q_K, (t1, t2, t3))``, ready for ``Prover.from_arrays(..., lookup=)`` and
     ``Setup.verification_key_arrays(..., lookup=)``"""
     return c.lookup[0], c.lookup[1]
+
+
+def lookups_arrays(c: ArrayCircuit):
+    """-> the circuit's lookups over several tables ``[(q_0, (t1, t2, t3)), ...]``, ready for
+    ``Prover.from_arrays(..., lookups=)`` and ``Setup.verification_key_arrays(..., lookups=)``"""
+    return list(c.lookups)

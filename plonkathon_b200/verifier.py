@@ -48,8 +48,8 @@ class VerificationKey:
     w: Scalar
     # custom gate terms ((i, j, l), commitment to Q_k), in the prover's order (plonkathon_b200/custom_gates.py)
     custom: tuple = ()
-    # lookup argument (plonkathon_b200/lookup.py): ([q_K], [t1], [t2], [t3]), the identity (None) for a zero column;
-    # () for a circuit without lookups
+    # lookup argument (plonkathon_b200/lookup.py): ([q_K], [t1], [t2], [t3]) for one table, ([q_K], [t1], [t2], [t3],
+    # [Q_T], [t4]) for several tables told apart by a tag; the identity (None) for a zero column; () without lookups
     lookup: tuple = ()
 
     def _custom_terms(self, a, b, c):
@@ -134,7 +134,14 @@ class VerificationKey:
             od = delta + 1
             eod = eps * od
             hw = eod + h2e + delta * h1w
-            qk, t1, t2, t3 = self.lookup
+            # several tables: ([q_K], [t1], [t2], [t3], [Q_T], [t4]); one table: the first four
+            qk, t1, t2, t3, *tag = self.lookup
+            eta3 = eta * eta * eta
+            t_parts = [(t1, Scalar(1)), (t2, eta), (t3, eta * eta)]  # [T] = [t1] + eta [t2] + eta^2 [t3] (+ eta^3 [t4])
+            if tag:
+                qt, t4 = tag
+                r_terms.append((qt, a3 * eta3))  # alpha^3 eta^3 Q_T
+                t_parts.append((t4, eta3))
             r_terms += [
                 # alpha^3 q_K (a + eta b + eta^2 c - f)
                 (qk, a3 * (a + eta * b + eta * eta * c - fe)),
@@ -144,7 +151,6 @@ class VerificationKey:
             ]
             r0 = r0 - a4 * z2w * (eod + delta * h2e) * hw - a5 * l0_ev
             v6, v7, v8 = v5 * v, v5 * v2, v5 * v3
-            t_parts = [(t1, Scalar(1)), (t2, eta), (t3, eta * eta)]  # [T] = [t1] + eta [t2] + eta^2 [t3]
             at_zeta += [(proof["f_1"], v6), (proof["h2_1"], v8)] + [(p, k * v7) for p, k in t_parts]
             e_zeta = e_zeta + v6 * fe + v7 * te + v8 * h2e
             at_zw += [(proof["h1_1"], v2), (proof["z2_1"], v3)] + [(p, k * v) for p, k in t_parts]
