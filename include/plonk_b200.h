@@ -173,7 +173,8 @@ int pb200_prover_serialize(pb200_prover* p, uint8_t* h_proof768);
 /* Lookups: a plookup argument over one fixed table of three columns.  Called once, before the first proof.
  * h_qk: n x 32 bytes, q_K in {0, 1} per row; h_t1..h_t3: table_rows x 32 bytes each (canonical LE), 1 <= table_rows
  * <= n, padded to n by repeating the last row.  A row with q_K = 1 claims that (a, b, c) is a row of the table.
- * Errors: malformed input, a sharded prover, a prover in zero-knowledge mode, a second call.
+ * Errors: malformed input, a sharded prover, a prover in zero-knowledge mode (set the table first, then
+ * pb200_prover_set_zk_lookup), a second call.
  * On a lookup prover pb200_prover_prove, _prove_device, _serialize, _round2 and _round4 return an error: a proof has
  * 13 points and 12 scalars (1216 bytes) and is made by the entry points below.  Round 1, 3 and 5 are unchanged. */
 int pb200_prover_set_lookup(pb200_prover* p, const uint8_t* h_qk, const uint8_t* h_t1, const uint8_t* h_t2,
@@ -196,6 +197,15 @@ int pb200_prover_round4_lookup(pb200_prover* p, const uint8_t* zeta, uint8_t* h_
 int pb200_prover_prove_lookup(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                               const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof1216);
 int pb200_prover_serialize_lookup(pb200_prover* p, uint8_t* h_proof1216);
+/* Zero-knowledge lookup proofs for every later proof of a lookup prover (one table or several): enable != 0 blinds A,
+ * B, C, Z and the quotient pieces as pb200_prover_set_zk does, and F, H1, H2, Z2 with 10 more scalars (21 in all,
+ * DESIGN.md section 1).  h_blinders == NULL: fresh scalars from the OS CSPRNG for every proof; otherwise 21 x 32-byte
+ * canonical Fr used for every proof (reproducible tests).  The proofs keep their 1216 bytes and entry points
+ * (_prove_lookup, _round_lookup, _round2_lookup, _round4_lookup, _serialize_lookup) and the verifier does not change.
+ * enable == 0, or pb200_prover_set_zk(p, 0, NULL), returns to plain lookup proofs.  Errors: a prover without a table,
+ * a sharded prover, n < 8, an SRS shorter than n + 6, unreduced blinders; a refused call leaves the prover as it was.
+ * pb200_prover_set_zk(p, 1, ...) on a lookup prover stays an error. */
+int pb200_prover_set_zk_lookup(pb200_prover* p, int enable, const uint8_t* h_blinders);
 
 /* ---- multi-GPU: one process per GPU, one communicator per context (SURVEY.md 8(e)) -------------------------
  * The library issues its data-path collectives itself, on the context's stream, through NCCL (bound at run time

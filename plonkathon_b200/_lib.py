@@ -83,6 +83,7 @@ def _load():
         "pb200_prover_round5": (I, [V, V, V]),
         "pb200_prover_serialize": (I, [V, V]),
         "pb200_prover_set_zk": (I, [V, I, V]),
+        "pb200_prover_set_zk_lookup": (I, [V, I, V]),
         "pb200_prover_set_lookup": (I, [V, V, V, V, V, U64]),
         "pb200_prover_set_lookup_tagged": (I, [V, V, V, V, V, V, V, U64]),
         "pb200_prover_round_lookup": (I, [V, V, V]),

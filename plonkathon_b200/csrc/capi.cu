@@ -53,6 +53,7 @@ void prover_round4(Prover* P, const Fr& zeta_c);
 void prover_round5(Prover* P, const Fr& v_c);
 void prover_serialize(const Prover* P, uint8_t* out);
 void prover_set_zk(Prover* P, bool enable, const uint8_t* h_blinders);
+void prover_set_zk_lookup(Prover* P, bool enable, const uint8_t* h_blinders);
 void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* h_qtag, const uint8_t* const* h_tab,
                        uint64_t rows);
 void prover_round_lookup(Prover* P, const Fr& eta_c);
@@ -522,6 +523,11 @@ int pb200_prover_read_vector(pb200_prover* p, int which, void* d_out) {
 int pb200_prover_set_zk(pb200_prover* p, int enable, const uint8_t* h_blinders) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   prover_set_zk(reinterpret_cast<Prover*>(p), enable != 0, h_blinders);
+  PB_API_END
+}
+int pb200_prover_set_zk_lookup(pb200_prover* p, int enable, const uint8_t* h_blinders) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  prover_set_zk_lookup(reinterpret_cast<Prover*>(p), enable != 0, h_blinders);
   PB_API_END
 }
 int pb200_prover_serialize(pb200_prover* p, uint8_t* h_proof768) {

@@ -568,20 +568,43 @@ struct LookupQuotientArgs {
   Fr eta, eta2, eta3, delta, eps, one_d, eps_one_d, alpha3, alpha4, alpha5, one;
   uint64_t n4;
 };
-__global__ void __launch_bounds__(128) k_quotient_lookup(LookupQuotientArgs q, Fr* out) {
+// Zero knowledge (prover_set_zk_lookup): the kernel reads the unblinded extensions and adds the Z_H multiples, as
+// k_quotient<true> does.  F' = F + (b12 X + b13) Z_H, H1' = H1 + (b14 X^2 + b15 X + b16) Z_H, H2' = H2 + (b17 X + b18) Z_H,
+// Z2' = Z2 + (b19 X^2 + b20 X + b21) Z_H, and A' + eta B' + eta^2 C' = A + eta B + eta^2 C + (e1 X + e0) Z_H with
+// e1 = b1 + eta b3 + eta^2 b5, e0 = b2 + eta b4 + eta^2 b6.  w[k] = Z_H class k times
+//   (e1, e0,  b12, b13,  b14, b15, b16,  b14 w^2, b15 w, b16,  b17, b18,  b19, b20, b21,  b19 w^2, b20 w, b21)
+// (the terms at wX use Z_H(w x) = Z_H(x)): 11 products a point.  A separate parameter after out, so the plain kernel's
+// parameters keep their offsets.
+struct ZkLookupCoset { const Fr* X; Fr w[4][18]; };
+static_assert(sizeof(LookupQuotientArgs) + sizeof(Fr*) + sizeof(ZkLookupCoset) <= 4096,
+              "k_quotient_lookup's parameters must fit the 4 KiB parameter space");
+template <bool ZK>
+__global__ void __launch_bounds__(128) k_quotient_lookup(LookupQuotientArgs q, Fr* out, ZkLookupCoset zk) {
   uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= q.n4) return;
   const uint64_t jw = j + 4 >= q.n4 ? j + 4 - q.n4 : j + 4;
-  const Fr f = ldg_fr(q.F + j);
-  Fr w = fp_add(ldg_fr(q.A + j), fp_add(fp_mul(q.eta, ldg_fr(q.B + j)), fp_mul(q.eta2, ldg_fr(q.C + j))));
+  // zero knowledge: y + (w_i x + w_i+1) or y + ((w_i x + w_i+1) x + w_i+2), the Z_H multiple of the blinded polynomial;
+  // in the plain instance both return y.  Indexed in the parameter space (a pointer to the weights would copy them)
+  const uint32_t k = (uint32_t)j & 3;
+  const Fr x = ZK ? ldg_fr(zk.X + j) : Fr::zero();
+  auto lin = [&](Fr y, int i) {
+    if constexpr (ZK) y = fp_add(y, fp_add(fp_mul(zk.w[k][i], x), zk.w[k][i + 1]));
+    return y;
+  };
+  auto quad = [&](Fr y, int i) {
+    if constexpr (ZK) y = fp_add(y, fp_add(fp_mul(fp_add(fp_mul(zk.w[k][i], x), zk.w[k][i + 1]), x), zk.w[k][i + 2]));
+    return y;
+  };
+  const Fr f = lin(ldg_fr(q.F + j), 2);
+  Fr w = lin(fp_add(ldg_fr(q.A + j), fp_add(fp_mul(q.eta, ldg_fr(q.B + j)), fp_mul(q.eta2, ldg_fr(q.C + j)))), 0);
   Fr acc = fp_mul(ldg_fr(q.QK + j), fp_sub(w, f));
   if (q.QT) acc = fp_add(acc, fp_mul(q.eta3, ldg_fr(q.QT + j)));
   acc = fp_mul(q.alpha3, acc);
-  const Fr z2 = ldg_fr(q.Z2 + j), h1 = ldg_fr(q.H1 + j), h2 = ldg_fr(q.H2 + j);
+  const Fr z2 = quad(ldg_fr(q.Z2 + j), 12), h1 = quad(ldg_fr(q.H1 + j), 4), h2 = lin(ldg_fr(q.H2 + j), 10);
   Fr p1 = fp_mul(fp_mul(fp_mul(z2, q.one_d), fp_add(q.eps, f)),
                  fp_add(fp_add(q.eps_one_d, ldg_fr(q.T + j)), fp_mul(q.delta, ldg_fr(q.T + jw))));
-  Fr p2 = fp_mul(fp_mul(ldg_fr(q.Z2 + jw), fp_add(fp_add(q.eps_one_d, h1), fp_mul(q.delta, h2))),
-                 fp_add(fp_add(q.eps_one_d, h2), fp_mul(q.delta, ldg_fr(q.H1 + jw))));
+  Fr p2 = fp_mul(fp_mul(quad(ldg_fr(q.Z2 + jw), 15), fp_add(fp_add(q.eps_one_d, h1), fp_mul(q.delta, h2))),
+                 fp_add(fp_add(q.eps_one_d, h2), fp_mul(q.delta, quad(ldg_fr(q.H1 + jw), 7))));
   acc = fp_add(acc, fp_mul(q.alpha4, fp_sub(p1, p2)));
   acc = fp_add(acc, fp_mul(q.alpha5, fp_mul(fp_sub(z2, q.one), ldg_fr(q.L0 + j))));
   out[j] = fp_add(out[j], fp_mul(acc, q.zh_inv[j & 3]));
@@ -832,39 +855,62 @@ static void zk_random_blinders(Fr* out_mont, int count) {
   std::fill(buf.begin(), buf.end(), 0);
 }
 
-void prover_set_zk(Prover* P, bool enable, const uint8_t* h_blinders) {
-  if (!enable) {
-    P->zk = P->zk_fixed = false;
-    for (auto& b : P->zk_coeff) b.release();
-    for (auto& b : P->zk_t) b.release();
-    return;
-  }
-  PB_CHECK(P->world == 1, "zero-knowledge proving is not available on the sharded prover (one GPU only)");
-  PB_CHECK(!P->lk, "zero-knowledge mode does not combine with lookups");
+// Switch zero-knowledge mode on with zk_blinders() scalars (h_blinders: that many canonical 32-byte words, or null for
+// fresh ones per proof).  Every check comes before any change, so a refused call leaves the prover as it was.
+static void zk_enable(Prover* P, const uint8_t* h_blinders) {
   PB_CHECK(P->n >= 8, "zero-knowledge proving needs n >= 8 rows: the blinded quotient has degree 3n + 5 < 4n");
   PB_CHECK(srs_size(P->srs) >= P->n + 6,
            "Not enough powers in setup: zero-knowledge proving needs n + 6 powers (T3' has n + 6 coefficients)");
-  if (h_blinders) {
-    for (int k = 0; k < Prover::ZK_BLINDERS; k++) {
-      Fr b;
-      memcpy(b.v, h_blinders + 32 * k, 32);
-      PB_CHECK(fp_is_canonical(b), "zero-knowledge blinder not reduced below the field modulus");
-      P->zk_fixed_b[k] = b;
-    }
+  const int count = P->zk_blinders();
+  Fr fixed[Prover::ZK_LK_BLINDERS];
+  for (int k = 0; h_blinders && k < count; k++) {
+    memcpy(fixed[k].v, h_blinders + 32 * k, 32);
+    PB_CHECK(fp_is_canonical(fixed[k]), "zero-knowledge blinder not reduced below the field modulus");
   }
   const size_t bytes = (P->n + Prover::ZK_PAD) * 32;
   for (auto& b : P->zk_coeff) b.ensure(bytes);
   for (auto& b : P->zk_t) b.ensure(bytes);
   for (auto& b : P->tmp) b.ensure(bytes);  // round 5 works on n + 8 coefficients
+  if (P->lk)
+    for (auto& b : P->zk_lk) b.ensure(bytes);
+  if (h_blinders) std::copy(fixed, fixed + count, P->zk_fixed_b);
   P->zk_fixed = h_blinders != nullptr;
   P->zk = true;
 }
 
+void prover_set_zk(Prover* P, bool enable, const uint8_t* h_blinders) {
+  if (!enable) {  // also ends zero-knowledge lookup proofs (prover_set_zk_lookup)
+    P->zk = P->zk_fixed = false;
+    for (auto& b : P->zk_coeff) b.release();
+    for (auto& b : P->zk_t) b.release();
+    for (auto& b : P->zk_lk) b.release();
+    return;
+  }
+  PB_CHECK(P->world == 1, "zero-knowledge proving is not available on the sharded prover (one GPU only)");
+  PB_CHECK(!P->lk, "zero-knowledge mode does not combine with lookups here: a lookup prover takes 21 blinders through "
+                   "pb200_prover_set_zk_lookup");
+  zk_enable(P, h_blinders);
+}
+
+// Zero-knowledge lookup proofs: the 11 blinders of prover_set_zk and b12..b21 for F, H1, H2 and Z2 (see "zero knowledge
+// with lookups" below).  A separate entry point because it takes another number of blinders: the size of the caller's
+// buffer never depends on the prover's state.
+void prover_set_zk_lookup(Prover* P, bool enable, const uint8_t* h_blinders) {
+  PB_CHECK(P->world == 1, "zero-knowledge proving is not available on the sharded prover (one GPU only)");
+  PB_CHECK(P->lk, "this prover has no lookup table (pb200_prover_set_lookup): use pb200_prover_set_zk");
+  if (!enable) {
+    prover_set_zk(P, false, nullptr);
+    return;
+  }
+  zk_enable(P, h_blinders);
+}
+
 static void zk_draw_blinders(Prover* P) {
+  const int count = P->zk_blinders();
   if (P->zk_fixed) {
-    for (int k = 0; k < Prover::ZK_BLINDERS; k++) P->zk_b[k] = fp_to_mont(P->zk_fixed_b[k]);
+    for (int k = 0; k < count; k++) P->zk_b[k] = fp_to_mont(P->zk_fixed_b[k]);
   } else {
-    zk_random_blinders(P->zk_b, Prover::ZK_BLINDERS);
+    zk_random_blinders(P->zk_b, count);
   }
 }
 
@@ -893,6 +939,14 @@ static ZkPatch zh_multiple(std::initializer_list<Fr> c) {
 // of the table each lookup row reads (0 off lookup rows).  t gains eta^3 t4, the index matches (a, b, c, Q_T), the
 // quotient's alpha^3 term gains eta^3 Q_T and round 5 one slot, alpha^3 eta^3 Q_T.  With t4 = Q_T = 0 every one of
 // these terms vanishes, so one table proves the same bytes tagged or not.
+// Zero knowledge with lookups (prover_set_zk_lookup): everything of plain zero-knowledge mode, and b12..b21 blind the
+// lookup polynomials the proof commits to, one scalar more than the points each is revealed at (PlonKup, 2022/086):
+//   F' = F + (b12 X + b13) Z_H,  H1' = H1 + (b14 X^2 + b15 X + b16) Z_H,  H2' = H2 + (b17 X + b18) Z_H,
+//   Z2' = Z2 + (b19 X^2 + b20 X + b21) Z_H.
+// T, q_K and Q_T are fixed or public and stay as they are.  Z2 is built from the unblinded values, as the checks are;
+// k_quotient_lookup<true> adds the Z_H multiples on the coset (A', B', C' included), round 4 corrects f, h2, h1(zeta w)
+// and z2(zeta w), and round 5 uses the blinded vectors.  deg T <= 3n + 5 still holds (the lookup products reach 2n + 6
+// after the division), so T is split as in plain zero-knowledge mode and the proof keeps its 1216 bytes.
 
 // h_qtag == nullptr: one untagged table of three columns (h_tab[3] unused).  Otherwise several tables concatenated: the
 // fourth column h_tab[3] holds each table row's table id and h_qtag = Q_T the id of the table each lookup row reads,
@@ -905,7 +959,8 @@ void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* h_qtag, co
   const bool tagged = h_qtag != nullptr;
   const int width = tagged ? 4 : 3;
   PB_CHECK(P->world == 1, "lookups are not available on the sharded prover (one GPU only)");
-  PB_CHECK(!P->zk, "lookups do not combine with zero-knowledge mode");
+  PB_CHECK(!P->zk, "lookups do not combine with zero-knowledge mode switched on first: set the table, then "
+                   "pb200_prover_set_zk_lookup");
   PB_CHECK(!P->lk, "the lookup table is already set (set it once, before the first proof)");
   PB_CHECK(h_qk && h_tab && h_tab[0] && h_tab[1] && h_tab[2], "lookups need q_K and three table columns");
   PB_CHECK(!tagged || h_tab[3], "tagged lookups need the table tag column t4");
@@ -1029,8 +1084,15 @@ void prover_round_lookup(Prover* P, const Fr& eta_c) {
   Fr* coeff[4] = {P->lk_coeff[Prover::LK_T].as<Fr>(), P->lk_coeff[Prover::LK_F].as<Fr>(),
                   P->lk_coeff[Prover::LK_H1].as<Fr>(), P->lk_coeff[Prover::LK_H2].as<Fr>()};
   interpolate(P, lag, coeff, 4);
-  const Fr* fh[3] = {coeff[1], coeff[2], coeff[3]};
-  P->commit_batch(fh, 3, n, P->lk_pts[0]);
+  if (P->zk) {  // F' H1' H2' (n + 2, n + 3, n + 2 coefficients), and T zero padded to n + 8 for round 5
+    const Fr* b = P->zk_b;
+    zk_blind(P, coeff[0], n, zh_multiple({}), P->zk_lk[Prover::LK_T].as<Fr>());
+    zk_blind(P, coeff[1], n, zh_multiple({b[12], b[11]}), P->zk_lk[Prover::LK_F].as<Fr>());
+    zk_blind(P, coeff[2], n, zh_multiple({b[15], b[14], b[13]}), P->zk_lk[Prover::LK_H1].as<Fr>());
+    zk_blind(P, coeff[3], n, zh_multiple({b[17], b[16]}), P->zk_lk[Prover::LK_H2].as<Fr>());
+  }
+  const Fr* fh[3] = {P->lk_poly(Prover::LK_F), P->lk_poly(Prover::LK_H1), P->lk_poly(Prover::LK_H2)};
+  P->commit_batch(fh, 3, P->zk ? n + 3 : n, P->lk_pts[0]);
 }
 
 // A grand product (Z of the permutation argument, Z2 of the lookup argument) from its per-row numerators and
@@ -1093,9 +1155,14 @@ static void lookup_round2(Prover* P) {
   Fr* zc = P->lk_coeff[Prover::LK_Z2].as<Fr>();
   grand_product(P, num, den, P->lk_lag[Prover::LK_Z2].as<Fr>(), zc,
                 "AssertionError: lookup grand product does not close, Z2_n != 1");
-  const Fr* zz[2] = {P->coeff[3].as<Fr>(), zc};
+  if (P->zk) {  // Z' and Z2': n + 3 coefficients each
+    const Fr* b = P->zk_b;
+    zk_blind(P, P->coeff[3].as<Fr>(), n, zh_multiple({b[8], b[7], b[6]}), P->zk_coeff[3].as<Fr>());
+    zk_blind(P, zc, n, zh_multiple({b[20], b[19], b[18]}), P->zk_lk[Prover::LK_Z2].as<Fr>());
+  }
+  const Fr* zz[2] = {P->zk ? P->zk_coeff[3].as<Fr>() : P->coeff[3].as<Fr>(), P->lk_poly(Prover::LK_Z2)};
   uint8_t out[2][64];
-  P->commit_batch(zz, 2, n, out[0]);
+  P->commit_batch(zz, 2, P->zk ? n + 3 : n, out[0]);
   memcpy(P->proof.pts[3], out[0], 64);
   memcpy(P->lk_pts[3], out[1], 64);
 }
@@ -1221,14 +1288,14 @@ void prover_round2(Prover* P, const Fr& beta_c, const Fr& gamma_c) {
   grand_product(P, num, den, P->lag[3].as<Fr>(), P->coeff[3].as<Fr>(),
                 "AssertionError: permutation grand product does not close, Z_n != 1 (prover.py:132)");
   if (P->overlap) launch_coset_ext_async(P, 3, 1, 1);
+  if (P->lk) {  // Z2, and Z with it in one commitment pass (both blinded in zero-knowledge mode)
+    lookup_round2(P);
+    return;
+  }
   if (P->zk) {  // Z': n + 3 coefficients
     const Fr* b = P->zk_b;
     zk_blind(P, P->coeff[3].as<Fr>(), n, zh_multiple({b[8], b[7], b[6]}), P->zk_coeff[3].as<Fr>());
     P->commit(P->zk_coeff[3].as<Fr>(), n + 3, P->proof.pts[3]);
-    return;
-  }
-  if (P->lk) {  // Z2, and Z with it in one commitment pass
-    lookup_round2(P);
     return;
   }
   P->commit(P->coeff[3].as<Fr>(), n, P->proof.pts[3]);
@@ -1302,7 +1369,21 @@ void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c) {
     lq.alpha3 = fp_mul(q.alpha2, P->alpha); lq.alpha4 = fp_sqr(q.alpha2); lq.alpha5 = fp_mul(lq.alpha4, P->alpha);
     lq.one = Fr::one();
     lq.n4 = ne;
-    k_quotient_lookup<<<PB_GRID(ne, 128), 0, st>>>(lq, t_evals);
+    ZkLookupCoset zl{};
+    if (P->zk) {
+      const Fr* b = P->zk_b;
+      const Fr w = fr_root_of_unity(P->log_n), w2 = fp_sqr(w);
+      const Fr e1 = fp_add(b[0], fp_add(fp_mul(lq.eta, b[2]), fp_mul(lq.eta2, b[4])));
+      const Fr e0 = fp_add(b[1], fp_add(fp_mul(lq.eta, b[3]), fp_mul(lq.eta2, b[5])));
+      const Fr per[18] = {e1,    e0,    b[11], b[12], b[13], b[14], b[15], fp_mul(b[13], w2), fp_mul(b[14], w),
+                          b[15], b[16], b[17], b[18], b[19], b[20], fp_mul(b[18], w2), fp_mul(b[19], w), b[20]};
+      zl.X = P->xs.as<Fr>();
+      for (int k = 0; k < 4; k++)
+        for (int i = 0; i < 18; i++) zl.w[k][i] = fp_mul(per[i], P->zh[k]);
+      k_quotient_lookup<true><<<PB_GRID(ne, 128), 0, st>>>(lq, t_evals, zl);
+    } else {
+      k_quotient_lookup<false><<<PB_GRID(ne, 128), 0, st>>>(lq, t_evals, zl);
+    }
     ctx->launches++;
   }
   PB_CUDA(cudaMemsetAsync(P->flags.p, 0, 64, st));
@@ -1387,6 +1468,15 @@ void prover_round4(Prover* P, const Fr& zeta_c) {
                            P->lk_coeff[Prover::LK_H1].as<Fr>(), P->lk_coeff[Prover::LK_Z2].as<Fr>()};
     const Fr lxs[6] = {P->zeta, P->zeta, zw, P->zeta, zw, zw};
     eval_polys(P, 6, lpolys, lxs, P->lk_ev);
+    if (P->zk) {  // F', H2' at zeta and H1', Z2' at zeta w, with Z_H(zeta w) = Z_H(zeta); T is not blinded
+      const Fr* b = P->zk_b;
+      const Fr zh = fp_sub(fp_pow_u64(P->zeta, P->n), Fr::one());
+      Fr* e = P->lk_ev;
+      e[0] = fp_add(e[0], fp_mul(fp_add(fp_mul(b[11], P->zeta), b[12]), zh));
+      e[3] = fp_add(e[3], fp_mul(fp_add(fp_mul(b[16], P->zeta), b[17]), zh));
+      e[4] = fp_add(e[4], fp_mul(fp_add(fp_mul(fp_add(fp_mul(b[13], zw), b[14]), zw), b[15]), zh));
+      e[5] = fp_add(e[5], fp_mul(fp_add(fp_mul(fp_add(fp_mul(b[18], zw), b[19]), zw), b[20]), zh));
+    }
     for (int k = 0; k < 6; k++) store_canonical(P->lk_evals[k], P->lk_ev[k]);
   }
 }
@@ -1504,15 +1594,16 @@ void prover_round5(Prover* P, const Fr& v_c) {
     const Fr abc = fp_add(a, fp_add(fp_mul(eta, b), fp_mul(fp_sqr(eta), c)));
     const Fr hw = fp_add(fp_add(eod, h2e), fp_mul(de, h1w));       // e(1+d) + h2 + d h1(zeta w)
     const Fr az2 = fp_mul(al4, z2w);
+    // zero knowledge: Z2', H1', F', H2' (n + 3 or n + 2 coefficients) join the tail; T stays unblinded
     add(P->lk_qk_coeff.as<Fr>(), fp_mul(al3, fp_sub(abc, fe)));
     if (P->lk_tagged) add(P->lk_qt_coeff.as<Fr>(), fp_mul(al3, fp_mul(fp_sqr(eta), eta)));  // alpha^3 eta^3 Q_T
-    add(P->lk_coeff[Prover::LK_Z2].as<Fr>(),
+    add(P->lk_poly(Prover::LK_Z2),
         fp_add(fp_mul(fp_mul(fp_mul(al4, od), fp_add(ep, fe)), fp_add(fp_add(eod, te), fp_mul(de, tw))),
-               fp_mul(al5, l0_ev)));
-    add(P->lk_coeff[Prover::LK_H1].as<Fr>(), fp_neg(fp_mul(az2, hw)));
-    add(P->lk_coeff[Prover::LK_F].as<Fr>(), v6);
-    add(P->lk_coeff[Prover::LK_T].as<Fr>(), v7);
-    add(P->lk_coeff[Prover::LK_H2].as<Fr>(), v8);
+               fp_mul(al5, l0_ev)), true);
+    add(P->lk_poly(Prover::LK_H1), fp_neg(fp_mul(az2, hw)), true);
+    add(P->lk_poly(Prover::LK_F), v6, true);
+    add(P->lk_poly(Prover::LK_T), v7);
+    add(P->lk_poly(Prover::LK_H2), v8, true);
     // -a4 z2w (e(1+d) + d h2) hw - a5 L0(zeta) - v^6 f - v^7 t - v^8 h2
     Fr lc = fp_neg(fp_mul(fp_mul(az2, fp_add(eod, fp_mul(de, h2e))), hw));
     lc = fp_sub(lc, fp_mul(al5, l0_ev));
@@ -1540,10 +1631,10 @@ void prover_round5(Prover* P, const Fr& v_c) {
   LinCombArgs M;
   M.vec[0] = zpoly; M.w[0] = one; M.count = 1; M.c0 = fp_neg(zw);
   M.n = zk ? len : L.n; M.first = L.first;
-  if (P->lk) {  // + v (T - t(zeta w)) + v^2 (H1 - h1(zeta w)) + v^3 (Z2 - z2(zeta w))
-    M.vec[1] = P->lk_coeff[Prover::LK_T].as<Fr>(); M.w[1] = v;
-    M.vec[2] = P->lk_coeff[Prover::LK_H1].as<Fr>(); M.w[2] = v2;
-    M.vec[3] = P->lk_coeff[Prover::LK_Z2].as<Fr>(); M.w[3] = v3;
+  if (P->lk) {  // + v (T - t(zeta w)) + v^2 (H1 - h1(zeta w)) + v^3 (Z2 - z2(zeta w)); zero knowledge: T zero padded
+    M.vec[1] = P->lk_poly(Prover::LK_T); M.w[1] = v;
+    M.vec[2] = P->lk_poly(Prover::LK_H1); M.w[2] = v2;
+    M.vec[3] = P->lk_poly(Prover::LK_Z2); M.w[3] = v3;
     M.count = 4;
     M.c0 = fp_sub(M.c0, fp_add(fp_mul(v, P->lk_ev[2]), fp_add(fp_mul(v2, P->lk_ev[4]), fp_mul(v3, P->lk_ev[5]))));
   }

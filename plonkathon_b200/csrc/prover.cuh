@@ -105,18 +105,23 @@ struct Prover {
   // Zero knowledge (one GPU only): the blinding of the PLONK paper with 11 scalars b1..b11 per proof.  The unblinded
   // n-coefficient vectors above stay as they are (the coset extensions read them; k_quotient adds the Z_H multiples);
   // the blinded vectors, which are longer than n, live in their own zero-padded buffers of n + 8 elements.
-  static const int ZK_BLINDERS = 11, ZK_PAD = 8;
+  // With a lookup table (prover_set_zk_lookup) there are 21 scalars: b12..b21 blind F, H1, H2 and Z2.
+  static const int ZK_BLINDERS = 11, ZK_LK_BLINDERS = 21, ZK_PAD = 8;
   bool zk = false;
   bool zk_fixed = false;          // the same blinders for every proof (zk_fixed_b) instead of fresh OS randomness
-  Fr zk_fixed_b[ZK_BLINDERS];     // canonical
-  Fr zk_b[ZK_BLINDERS];           // this proof's b1..b11, Montgomery (drawn when round 1 starts)
+  Fr zk_fixed_b[ZK_LK_BLINDERS];  // canonical
+  Fr zk_b[ZK_LK_BLINDERS];        // this proof's b1..b11 (..b21 with lookups), Montgomery (drawn when round 1 starts)
   DevBuf zk_coeff[4];             // A' B' C' (n + 2 coefficients) Z' (n + 3)
   DevBuf zk_t[3];                 // T1' T2' (n + 1 coefficients) T3' (n + 6)
+  DevBuf zk_lk[5];                // lookups: T (n, zero padded) F' H2' (n + 2) H1' Z2' (n + 3), indexed by LK_*
+  int zk_blinders() const { return lk ? ZK_LK_BLINDERS : ZK_BLINDERS; }
   // Lookup argument (prover_set_lookup, one GPU): plookup over one fixed table of three columns, or over several
   // tables told apart by a tag column t4 and the selector Q_T, see "lookups" in prover.cu.  The proof gains f_1 h1_1
   // h2_1 z2_1 and six evaluations (1216 bytes).
   enum { LK_T = 0, LK_F, LK_H1, LK_H2, LK_Z2, LK_VECS };
   bool lk = false;
+  // the coefficient vectors a lookup proof commits and opens: the unblinded lk_coeff, or zk_lk in zero-knowledge mode
+  const Fr* lk_poly(int k) const { return (zk ? zk_lk[k] : lk_coeff[k]).as<Fr>(); }
   bool lk_tagged = false;              // several tables: t4 and Q_T are set (and lk_keys has 4 Fr per row)
   uint64_t lk_rows = 0;                // table rows before padding
   DevBuf lk_qk_coeff, lk_qk_ext;       // q_K: coefficients, on the 4n coset

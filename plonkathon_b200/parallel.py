@@ -138,6 +138,10 @@ class ShardedProver(Prover):
             raise ValueError("zero-knowledge proving is not available on the sharded prover (one GPU only)")
         super().set_zk(False)
 
+    def set_zk_lookup(self, enable: bool = True, blinders=None):
+        """Zero-knowledge lookup proofs run on one GPU only (``Prover.set_zk_lookup``); so do lookups."""
+        raise ValueError("zero-knowledge lookups are not available on the sharded prover (one GPU only)")
+
 
 # ------------------------------------------------------------------------------------------------
 # operators (BASELINE.json metric: Fr-NTT elems/s and G1-MSM pts/s at 1/2/4/8 GPUs)

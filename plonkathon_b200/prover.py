@@ -369,6 +369,23 @@ class Prover:
         _lib.check(_lib.lib().pb200_prover_set_zk(self._h, 1 if enable else 0, raw))
         self.zk = bool(enable)
 
+    def set_zk_lookup(self, enable: bool = True, blinders=None):
+        """Zero-knowledge mode for the later proofs of a lookup prover (``lookup=`` or ``lookups=``): ``set_zk``'s
+        blinding and 10 more scalars for F, H1, H2 and Z2, 21 in all (DESIGN.md section 1).  The proofs keep their 1216
+        bytes and the verifier does not change.  ``blinders=None``: fresh scalars from the OS CSPRNG for every proof;
+        otherwise 21 integers in [0, r) used for every proof (reproducible tests only).  ``enable=False`` (or
+        ``set_zk(False)``) returns to plain lookup proofs.  Needs a lookup table, n >= 8 and an SRS of n + 6 powers."""
+        raw = None
+        if enable and blinders is not None:
+            blinders = [int(b) for b in blinders]
+            if len(blinders) != 21:
+                raise ValueError("zero-knowledge lookups take 21 blinders b1..b21, got %d" % len(blinders))
+            if any(not 0 <= b < CURVE_ORDER for b in blinders):
+                raise ValueError("zero-knowledge blinders must lie in [0, r)")
+            raw = b"".join(b.to_bytes(32, "little") for b in blinders)
+        _lib.check(_lib.lib().pb200_prover_set_zk_lookup(self._h, 1 if enable else 0, raw))
+        self.zk = bool(enable)
+
     def _commitments(self, first_slot: int, count: int, raw: bytes):
         """commitments a round produced"""
         return _pts(raw, count)
