@@ -163,9 +163,11 @@ int pb200_prover_round5(pb200_prover* p, const uint8_t* v, uint8_t* h_w_xy /*2*6
  * (Lagrange values), 5 T1, 6 T2, 7 T3 (coefficients).  Valid after the round that produces them.  In zero-knowledge
  * mode which = 5..7 is an error (the blinded pieces have more than 2^log_n coefficients); 0..4 are unchanged. */
 int pb200_prover_read_vector(pb200_prover* p, int which, void* d_out);
-/* Zero-knowledge mode for every later proof of this prover: enable != 0 blinds per PLONK paper (11 scalars).
- * h_blinders == NULL: fresh scalars from the OS CSPRNG for every proof; otherwise 11 x 32-byte canonical Fr used for
- * every proof (reproducible tests).  Errors: SRS shorter than n + 6, n < 8, a sharded prover, unreduced blinders. */
+/* Zero-knowledge mode for every later proof of this prover: enable != 0 blinds per PLONK paper (11 scalars; 14 on a
+ * next-row prover, see pb200_prover_create_custom_next_row).
+ * h_blinders == NULL: fresh scalars from the OS CSPRNG for every proof; otherwise 11 (14) x 32-byte canonical Fr used
+ * for every proof (reproducible tests).  Errors: SRS shorter than n + 6, n < 8, a sharded prover, unreduced blinders;
+ * on a next-row prover an SRS shorter than n + 9 and n < 16. */
 int pb200_prover_set_zk(pb200_prover* p, int enable, const uint8_t* h_blinders);
 /* canonical 768-byte proof of the last rounds run on this prover (Proof.flatten() order, prover.py:18-35) */
 int pb200_prover_serialize(pb200_prover* p, uint8_t* h_proof768);
@@ -206,6 +208,26 @@ int pb200_prover_serialize_lookup(pb200_prover* p, uint8_t* h_proof1216);
  * a sharded prover, n < 8, an SRS shorter than n + 6, unreduced blinders; a refused call leaves the prover as it was.
  * pb200_prover_set_zk(p, 1, ...) on a lookup prover stays an error. */
 int pb200_prover_set_zk_lookup(pb200_prover* p, int enable, const uint8_t* h_blinders);
+
+/* Custom gates over the next row (TurboPLONK): h_exps = 6 bytes (i, j, l, i', j', l') per term, the term
+ * Q_k * a^i b^j c^l * a(wX)^i' b(wX)^j' c(wX)^l'.  Rows are cyclic: row n - 1 reads row 0.  A term without next-row
+ * exponents keeps the rules of pb200_prover_create_custom; a term with one has total degree 1, 2 or 3.  At most 4 terms,
+ * none twice.  With at least one next-row term the prover is a next-row prover: round 4 also evaluates A, B, C at
+ * zeta w, the zeta w opening batches them with Z, and a proof has 864 bytes.  Otherwise it is the prover
+ * pb200_prover_create_custom makes.  One GPU only: there is no sharded form.
+ * On a next-row prover pb200_prover_prove, _prove_device, _serialize and _round4 return an error, and so do
+ * pb200_prover_set_lookup and _set_lookup_tagged (lookups do not combine with next-row terms).  Rounds 1, 2, 3 and 5
+ * are the plain entry points.  pb200_prover_set_zk takes 14 blinders on a next-row prover (b12..b14 give A, B, C a
+ * third blinder each) and needs n >= 16 and an SRS of n + 9 powers. */
+int pb200_prover_create_custom_next_row(pb200_ctx* ctx, pb200_srs* srs, unsigned log_n, const uint8_t* const* h_pk,
+                                        unsigned n_custom, const uint8_t* h_exps, const uint8_t* const* h_custom,
+                                        pb200_prover** out);
+/* round 4 of a next-row prover: the 6 plain evaluations, then a(zeta w), b(zeta w), c(zeta w) */
+int pb200_prover_round4_next_row(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals /*9*32*/);
+/* the whole proof: the 768 plain bytes, then a_shifted_eval, b_shifted_eval, c_shifted_eval (864 bytes) */
+int pb200_prover_prove_next_row(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
+                                const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof864);
+int pb200_prover_serialize_next_row(pb200_prover* p, uint8_t* h_proof864);
 
 /* ---- multi-GPU: one process per GPU, one communicator per context (SURVEY.md 8(e)) -------------------------
  * The library issues its data-path collectives itself, on the context's stream, through NCCL (bound at run time

@@ -91,6 +91,10 @@ def _load():
         "pb200_prover_round4_lookup": (I, [V, V, V]),
         "pb200_prover_prove_lookup": (I, [V, V, V, V, V, U64, V]),
         "pb200_prover_serialize_lookup": (I, [V, V]),
+        "pb200_prover_create_custom_next_row": (I, [V, V, U, V, U, V, V, P(V)]),
+        "pb200_prover_round4_next_row": (I, [V, V, V]),
+        "pb200_prover_prove_next_row": (I, [V, V, V, V, V, U64, V]),
+        "pb200_prover_serialize_next_row": (I, [V, V]),
         "pb200_g1_combine_partials_host": (I, [V, U, V, P(I)]),
         "pb200_transcript_create": (I, [V, ctypes.c_size_t, P(V)]),
         "pb200_transcript_destroy": (None, [V]),

@@ -41,7 +41,7 @@ void msm_run(Context* ctx, const G1Affine* points, uint64_t n, const Fr* scalars
 void affine_to_mont(Context* ctx, const G1Affine* in, G1Affine* out, uint64_t n);
 // prover.cu
 Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h_pk, int n_custom,
-                      const uint8_t* h_exps, const uint8_t* const* h_custom, bool sharded);
+                      const uint8_t* h_exps, const uint8_t* const* h_custom, bool sharded, int exp_width);
 void prover_destroy(Prover* p);
 void prover_prove(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t* hC, const uint8_t* h_public,
                   uint64_t n_public, uint8_t* out, bool wires_on_device);
@@ -86,6 +86,9 @@ static Context* C(pb200_ctx* c) { return reinterpret_cast<Context*>(c); }
 // the 768-byte entry points (and the plain round 2 / round 4) on a prover with a lookup table
 #define PB_NOT_LOOKUP(P, entry)                                                                       \
   PB_CHECK(!(P)->lk, "this prover has a lookup argument: its proofs have 1216 bytes; use " entry)
+// the 768-byte entry points (and the plain round 4) on a prover with next-row custom gate terms
+#define PB_NOT_NEXT_ROW(P, entry)                                                                     \
+  PB_CHECK(!(P)->next_row, "this prover has next-row custom gate terms: its proofs have 864 bytes; use " entry)
 
 // Every entry point that touches the GPU runs on its context's device, whatever device the calling host thread had
 // current (contexts on several GPUs in one process, provers driven from worker threads); the previous device is
@@ -435,7 +438,15 @@ int pb200_prover_create_custom(pb200_ctx* ctx, pb200_srs* srs, unsigned log_n, c
                                pb200_prover** out) {
   PB_API_BEGIN PB_ON_CTX(C(ctx));
   *out = reinterpret_cast<pb200_prover*>(prover_create(C(ctx), reinterpret_cast<Srs*>(srs), (int)log_n, h_pk,
-                                                       (int)n_custom, h_exps, h_custom, false));
+                                                       (int)n_custom, h_exps, h_custom, false, 3));
+  PB_API_END
+}
+int pb200_prover_create_custom_next_row(pb200_ctx* ctx, pb200_srs* srs, unsigned log_n, const uint8_t* const* h_pk,
+                                        unsigned n_custom, const uint8_t* h_exps, const uint8_t* const* h_custom,
+                                        pb200_prover** out) {
+  PB_API_BEGIN PB_ON_CTX(C(ctx));
+  *out = reinterpret_cast<pb200_prover*>(prover_create(C(ctx), reinterpret_cast<Srs*>(srs), (int)log_n, h_pk,
+                                                       (int)n_custom, h_exps, h_custom, false, 6));
   PB_API_END
 }
 int pb200_prover_create_custom_sharded(pb200_ctx* ctx, pb200_srs* srs, unsigned log_n, const uint8_t* const* h_pk,
@@ -443,7 +454,7 @@ int pb200_prover_create_custom_sharded(pb200_ctx* ctx, pb200_srs* srs, unsigned 
                                        pb200_prover** out) {
   PB_API_BEGIN PB_ON_CTX(C(ctx));
   *out = reinterpret_cast<pb200_prover*>(prover_create(C(ctx), reinterpret_cast<Srs*>(srs), (int)log_n, h_pk,
-                                                       (int)n_custom, h_exps, h_custom, true));
+                                                       (int)n_custom, h_exps, h_custom, true, 3));
   PB_API_END
 }
 void pb200_prover_destroy(pb200_prover* p) { prover_destroy(reinterpret_cast<Prover*>(p)); }
@@ -452,6 +463,7 @@ int pb200_prover_prove(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, 
                        const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof768) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   PB_NOT_LOOKUP(reinterpret_cast<Prover*>(p), "pb200_prover_prove_lookup");
+  PB_NOT_NEXT_ROW(reinterpret_cast<Prover*>(p), "pb200_prover_prove_next_row");
   prover_prove(reinterpret_cast<Prover*>(p), h_A, h_B, h_C, h_public, n_public, h_proof768, false);
   PB_API_END
 }
@@ -459,6 +471,7 @@ int pb200_prover_prove_device(pb200_prover* p, const void* d_A, const void* d_B,
                               const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof768) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   PB_NOT_LOOKUP(reinterpret_cast<Prover*>(p), "pb200_prover_prove_lookup (wires in host memory)");
+  PB_NOT_NEXT_ROW(reinterpret_cast<Prover*>(p), "pb200_prover_prove_next_row (wires in host memory)");
   prover_prove(reinterpret_cast<Prover*>(p), (const uint8_t*)d_A, (const uint8_t*)d_B, (const uint8_t*)d_C, h_public,
                n_public, h_proof768, true);
   PB_API_END
@@ -490,6 +503,7 @@ int pb200_prover_round4(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals) 
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   Prover* P = reinterpret_cast<Prover*>(p);
   PB_NOT_LOOKUP(P, "pb200_prover_round4_lookup");
+  PB_NOT_NEXT_ROW(P, "pb200_prover_round4_next_row");
   prover_round4(P, load_fr_canonical(zeta));
   memcpy(h_evals, P->proof.evals[0], 6 * 32);
   PB_API_END
@@ -533,6 +547,7 @@ int pb200_prover_set_zk_lookup(pb200_prover* p, int enable, const uint8_t* h_bli
 int pb200_prover_serialize(pb200_prover* p, uint8_t* h_proof768) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   PB_NOT_LOOKUP(reinterpret_cast<Prover*>(p), "pb200_prover_serialize_lookup");
+  PB_NOT_NEXT_ROW(reinterpret_cast<Prover*>(p), "pb200_prover_serialize_next_row");
   prover_serialize(reinterpret_cast<Prover*>(p), h_proof768);
   PB_API_END
 }
@@ -589,6 +604,30 @@ int pb200_prover_serialize_lookup(pb200_prover* p, uint8_t* h_proof1216) {
   Prover* P = reinterpret_cast<Prover*>(p);
   PB_CHECK(P->lk, "this prover has no lookup table: use pb200_prover_serialize (768 bytes)");
   prover_serialize(P, h_proof1216);
+  PB_API_END
+}
+int pb200_prover_round4_next_row(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  PB_CHECK(P->next_row, "this prover has no next-row custom gate terms: use pb200_prover_round4");
+  prover_round4(P, load_fr_canonical(zeta));
+  memcpy(h_evals, P->proof.evals[0], 6 * 32);
+  memcpy(h_evals + 6 * 32, P->nr_evals[0], 3 * 32);
+  PB_API_END
+}
+int pb200_prover_prove_next_row(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
+                                const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof864) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  PB_CHECK(P->next_row, "this prover has no next-row custom gate terms: use pb200_prover_prove (768 bytes)");
+  prover_prove(P, h_A, h_B, h_C, h_public, n_public, h_proof864, false);
+  PB_API_END
+}
+int pb200_prover_serialize_next_row(pb200_prover* p, uint8_t* h_proof864) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  PB_CHECK(P->next_row, "this prover has no next-row custom gate terms: use pb200_prover_serialize (768 bytes)");
+  prover_serialize(P, h_proof864);
   PB_API_END
 }
 int pb200_g1_combine_partials_host(const uint8_t* h_xyzz, unsigned count, uint8_t* h_out_xy, int* is_identity) {

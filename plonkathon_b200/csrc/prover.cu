@@ -19,6 +19,9 @@
 // (prover.py:108-116), Z_n == 1 (prover.py:132), deg T < 3n (prover.py:205-208).
 // Zero-knowledge mode (prover_set_zk, one GPU) blinds A, B, C, Z and the quotient pieces as in the PLONK paper; the
 // proof keeps its 15 fields and the verifier does not change.  See "zero knowledge" below.
+// Custom terms over the next row (Prover::next_row, one GPU) read a(wX), b(wX), c(wX): k_gate_check<true> and
+// k_quotient<ZK, true> read index + 1 (mod n) and coset index + 4, round 4 adds A, B, C at zeta w and round 5 opens them
+// there with Z; the proof gains those three evaluations (864 bytes).
 #include <algorithm>
 #include <cerrno>
 #include <sys/random.h>
@@ -112,7 +115,9 @@ __global__ void k_count_noncanonical(const Fr* v, uint64_t n, uint32_t* bad) {
   if (i < n && !fp_is_canonical(ldg_fr(v + i))) atomicAdd(bad, 1u);
 }
 
-// prover.py:108-116: A*QL + B*QR + A*B*QM + C*QO + PI + QC (+ sum_k Q_k m_k(A, B, C)) == 0 on every row
+// prover.py:108-116: A*QL + B*QR + A*B*QM + C*QO + PI + QC (+ sum_k Q_k m_k(A, B, C)) == 0 on every row.
+// NEXT: the custom terms also read the next row's wires, cyclically (row n - 1 reads row 0).
+template <bool NEXT>
 __global__ void k_gate_check(const Fr* A, const Fr* B, const Fr* C, const Fr* QL, const Fr* QR, const Fr* QM,
                              const Fr* QO, const Fr* QC, const Fr* PI, CustomTerms ct, uint64_t n, uint32_t* bad) {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -123,7 +128,12 @@ __global__ void k_gate_check(const Fr* A, const Fr* B, const Fr* C, const Fr* QL
   s = fp_add(s, fp_mul(fp_mul(a, b), ldg_fr(QM + i)));
   s = fp_add(s, fp_mul(c, ldg_fr(QO + i)));
   s = fp_add(s, fp_add(ldg_fr(PI + i), ldg_fr(QC + i)));
-  s = custom_gate_sum(ct, i, a, b, c, s);
+  if constexpr (NEXT) {
+    const uint64_t i1 = i + 1 == n ? 0 : i + 1;
+    s = custom_gate_sum_next(ct, i, a, b, c, ldg_fr(A + i1), ldg_fr(B + i1), ldg_fr(C + i1), s);
+  } else {
+    s = custom_gate_sum(ct, i, a, b, c, s);
+  }
   if (!s.is_zero()) atomicAdd(bad, 1u);
 }
 
@@ -347,13 +357,38 @@ struct QuotientArgs {
 //   (b1, b2, b3, b4, b5, b6,  b7, b8, b9,  b7 w^2, b8 w, b9)
 // and a point costs 7 products.  A separate parameter after T, so the plain kernel's parameters keep their offsets.
 struct ZkCoset { Fr w[4][12]; };
-template <bool ZK>
-__global__ void __launch_bounds__(128) k_quotient(QuotientArgs q, Fr* T, ZkCoset zk) {
+// Zero knowledge on a next-row prover: A' = A + (b12 X^2 + b1 X + b2) Z_H, B' = B + (b13 X^2 + b3 X + b4) Z_H,
+// C' = C + (b14 X^2 + b5 X + b6) Z_H, and the shifted wires A'(w x) = A(w x) + (b12 w^2 x^2 + b1 w x + b2) Z_H(x) like
+// Z'(w x).  w[k] = Z_H class k times
+//   (b12, b1, b2,  b13, b3, b4,  b14, b5, b6,  b7, b8, b9,  b7 w^2, b8 w, b9,
+//    b12 w^2, b1 w, b2,  b13 w^2, b3 w, b4,  b14 w^2, b5 w, b6)
+// and a point costs 16 products.
+struct ZkNextCoset { Fr w[4][24]; };
+template <bool ZK_NEXT> struct ZkCosetOf { using type = ZkCoset; };
+template <> struct ZkCosetOf<true> { using type = ZkNextCoset; };
+static_assert(sizeof(QuotientArgs) + sizeof(Fr*) + sizeof(ZkNextCoset) <= 4096,
+              "k_quotient's parameters must fit the 4 KiB parameter space");
+// NEXT (a next-row prover, one GPU): the custom terms also read A, B, C at w x, the coset index + zw_shift as for Z.
+template <bool ZK, bool NEXT>
+__global__ void __launch_bounds__(128) k_quotient(QuotientArgs q, Fr* T, typename ZkCosetOf<ZK && NEXT>::type zk) {
   uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= q.n4) return;
   uint64_t jw = j + q.zw_shift >= q.n4 ? j + q.zw_shift - q.n4 : j + q.zw_shift;
   Fr a = ldg_fr(q.A + j), b = ldg_fr(q.B + j), c = ldg_fr(q.C + j);
-  if constexpr (ZK) {
+  // y + ((w_i x + w_i+1) x + w_i+2), the quadratic Z_H multiple of a next-row zero-knowledge vector
+  auto quad = [&](Fr y, int i) {
+    if constexpr (ZK && NEXT) {
+      const uint32_t k = (uint32_t)j & 3;
+      const Fr x = ldg_fr(q.X + j);
+      y = fp_add(y, fp_add(fp_mul(fp_add(fp_mul(zk.w[k][i], x), zk.w[k][i + 1]), x), zk.w[k][i + 2]));
+    }
+    return y;
+  };
+  if constexpr (ZK && NEXT) {
+    a = quad(a, 0);
+    b = quad(b, 3);
+    c = quad(c, 6);
+  } else if constexpr (ZK) {
     const uint32_t k = (uint32_t)(j * q.world + q.rank) & 3;
     const Fr x = ldg_fr(q.X + j);
     a = fp_add(a, fp_add(fp_mul(zk.w[k][0], x), zk.w[k][1]));
@@ -371,12 +406,20 @@ __global__ void __launch_bounds__(128) k_quotient(QuotientArgs q, Fr* T, ZkCoset
     pi = ldg_fr(q.PI + j);
   }
   gate = fp_add(gate, fp_add(pi, ldg_fr(q.QC + j)));
-  gate = custom_gate_sum(q.custom, j, a, b, c, gate);
+  if constexpr (NEXT) {
+    const Fr an = quad(ldg_fr(q.A + jw), 15), bn = quad(ldg_fr(q.B + jw), 18), cn = quad(ldg_fr(q.C + jw), 21);
+    gate = custom_gate_sum_next(q.custom, j, a, b, c, an, bn, cn, gate);
+  } else {
+    gate = custom_gate_sum(q.custom, j, a, b, c, gate);
+  }
   Fr ag = fp_add(a, q.gamma), bg = fp_add(b, q.gamma), cg = fp_add(c, q.gamma);
   Fr bx = fp_mul(q.beta, ldg_fr(q.X + j));
   Fr bx2 = fp_dbl(bx), bx3 = fp_add(bx2, bx);
   Fr z = ldg_fr(q.Z + j), zw = ldg_fr(q.Zw + jw);
-  if constexpr (ZK) {
+  if constexpr (ZK && NEXT) {
+    z = quad(z, 9);
+    zw = quad(zw, 12);
+  } else if constexpr (ZK) {
     const uint32_t k = (uint32_t)(j * q.world + q.rank) & 3;
     const Fr x = ldg_fr(q.X + j);
     z = fp_add(z, fp_add(fp_mul(fp_add(fp_mul(zk.w[k][6], x), zk.w[k][7]), x), zk.w[k][8]));
@@ -646,31 +689,46 @@ static void ensure_pi_basis(Prover* P, int count) {
   PB_CUDA(cudaStreamSynchronize(st));
 }
 
-// Custom term exponents (i, j, l) -> the wires of the monomial.  Degree 1 duplicates QL / QR / QO, degree 4 would need
-// a fourth quotient piece, (1, 1, 0) is QM's term, and a repeated triple is one term split in two.
-static void set_custom_terms(Prover* P, int n_custom, const uint8_t* h_exps) {
+// Custom term exponents -> the factors of the monomial.  width 3: (i, j, l); width 6: (i, j, l, i', j', l'), the last
+// three on a(wX), b(wX), c(wX).  A same-row term keeps its rules: degree 1 duplicates QL / QR / QO, degree 4 would need
+// a fourth quotient piece, (1, 1, 0) is QM's term.  A term with a next-row exponent may have degree 1, 2 or 3 (no
+// selector reads the next row).  A repeated term is one term split in two.  Sets P->next_row when some term reads the
+// next row.
+static void set_custom_terms(Prover* P, int n_custom, const uint8_t* h_exps, int width) {
   PB_CHECK(n_custom >= 0 && n_custom <= PB_MAX_CUSTOM, "at most 4 custom gate terms");
   PB_CHECK(n_custom == 0 || h_exps, "custom gate terms need their exponents");
+  uint8_t six[PB_MAX_CUSTOM][6] = {};
+  bool next_row = false;
   for (int k = 0; k < n_custom; k++) {
-    const uint8_t* e = h_exps + 3 * k;
-    const int deg = e[0] + e[1] + e[2];
-    PB_CHECK(deg >= 2 && deg <= 3, "custom gate term must have total degree 2 or 3");
-    PB_CHECK(!(e[0] == 1 && e[1] == 1 && e[2] == 0), "custom gate term (1, 1, 0) duplicates QM");
+    uint8_t* e = six[k];
+    memcpy(e, h_exps + width * k, width);
+    const bool next = e[3] || e[4] || e[5];
+    const int deg = e[0] + e[1] + e[2] + e[3] + e[4] + e[5];
+    if (next) {
+      PB_CHECK(deg >= 1 && deg <= 3, "custom gate term with next-row exponents must have total degree 1, 2 or 3");
+    } else {
+      PB_CHECK(deg >= 2 && deg <= 3, "custom gate term must have total degree 2 or 3");
+      PB_CHECK(!(e[0] == 1 && e[1] == 1 && e[2] == 0), "custom gate term (1, 1, 0) duplicates QM");
+    }
     for (int k2 = 0; k2 < k; k2++)
-      PB_CHECK(memcmp(e, h_exps + 3 * k2, 3) != 0, "custom gate terms must have distinct exponents");
+      PB_CHECK(memcmp(e, six[k2], 6) != 0, "custom gate terms must have distinct exponents");
+    next_row = next_row || next;
+  }
+  for (int k = 0; k < n_custom; k++) {
     int s = 0;
-    for (int w = 0; w < 3; w++)
-      for (int t = 0; t < e[w]; t++) P->custom_f[k][s++] = (uint8_t)w;
-    if (s == 2) P->custom_f[k][2] = 3;
+    for (int w = 0; w < 6; w++)
+      for (int t = 0; t < six[k][w]; t++) P->custom_f[k][s++] = (uint8_t)w;
+    while (s < 3) P->custom_f[k][s++] = PB_FACTOR_ONE;
   }
   P->n_custom = n_custom;
+  P->next_row = next_row;
 }
 
 // h_pk: 8 vectors (QM QL QR QO QC S1 S2 S3), each n x 32 bytes canonical (compiler/program.py:10-30); h_custom:
-// n_custom more selector vectors of the same shape, with their exponents h_exps (3 bytes per term).
+// n_custom more selector vectors of the same shape, with their exponents h_exps (exp_width = 3 or 6 bytes per term).
 // sharded: one proof across the ranks of the context's communicator (see Prover in prover.cuh).
 Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h_pk, int n_custom,
-                      const uint8_t* h_exps, const uint8_t* const* h_custom, bool sharded) {
+                      const uint8_t* h_exps, const uint8_t* const* h_custom, bool sharded, int exp_width) {
   auto P = std::make_unique<Prover>();
   P->ctx = ctx;
   P->srs = srs;
@@ -679,8 +737,9 @@ Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h
   P->n = n;
   PB_CHECK(log_n >= 1 && log_n <= 26, "group order must be 2^k, 1 <= k <= 26");
   PB_CHECK(n <= srs_size(srs), "Not enough powers in setup");
-  set_custom_terms(P.get(), n_custom, h_exps);
+  set_custom_terms(P.get(), n_custom, h_exps, exp_width);
   PB_CHECK(n_custom == 0 || h_custom, "custom gate terms need their selector columns");
+  PB_CHECK(!(sharded && P->next_row), "next-row custom gate terms are not available on the sharded prover (one GPU only)");
   if (sharded) {
     Comm* cm = ctx_comm(ctx);
     P->world = comm_world(cm);
@@ -818,6 +877,9 @@ static void store_canonical(uint8_t* dst, const Fr& mont) {
 //   T1' = T1 + b10 X^n,  T2' = T2 - b10 + b11 X^n,  T3' = T3 - b11   (T1' + X^n T2' + X^2n T3' = T).
 // On H every blinded polynomial equals the unblinded one, so rounds 1-2 check the same witness; commitments, openings
 // and round 5 use the blinded polynomials, evaluations are corrected on the host.  The verifier does not change.
+// A next-row prover opens A, B, C at zeta w too, so they take a third blinder each (b12..b14):
+//   A' = A + (b12 X^2 + b1 X + b2) Z_H,  B' = B + (b13 X^2 + b3 X + b4) Z_H,  C' = C + (b14 X^2 + b5 X + b6) Z_H,
+// the permutation product reaches degree 4n + 8, deg T <= 3n + 8 and T3' has n + 9 coefficients (zk_t3_len, ZK_NR_PAD).
 
 // Fresh blinders from the OS CSPRNG: 64 bytes per scalar, reduced mod r (bias below 2^-250).  No other source: a failed
 // read fails the proof.
@@ -858,6 +920,12 @@ static void zk_random_blinders(Fr* out_mont, int count) {
 // Switch zero-knowledge mode on with zk_blinders() scalars (h_blinders: that many canonical 32-byte words, or null for
 // fresh ones per proof).  Every check comes before any change, so a refused call leaves the prover as it was.
 static void zk_enable(Prover* P, const uint8_t* h_blinders) {
+  if (P->next_row) {
+    PB_CHECK(P->n >= 16, "zero-knowledge proving with next-row terms needs n >= 16 rows: the blinded quotient has "
+                         "degree 3n + 8 < 4n");
+    PB_CHECK(srs_size(P->srs) >= P->n + 9, "Not enough powers in setup: zero-knowledge proving with next-row terms "
+                                           "needs n + 9 powers (T3' has n + 9 coefficients)");
+  }
   PB_CHECK(P->n >= 8, "zero-knowledge proving needs n >= 8 rows: the blinded quotient has degree 3n + 5 < 4n");
   PB_CHECK(srs_size(P->srs) >= P->n + 6,
            "Not enough powers in setup: zero-knowledge proving needs n + 6 powers (T3' has n + 6 coefficients)");
@@ -867,10 +935,10 @@ static void zk_enable(Prover* P, const uint8_t* h_blinders) {
     memcpy(fixed[k].v, h_blinders + 32 * k, 32);
     PB_CHECK(fp_is_canonical(fixed[k]), "zero-knowledge blinder not reduced below the field modulus");
   }
-  const size_t bytes = (P->n + Prover::ZK_PAD) * 32;
+  const size_t bytes = (P->n + P->zk_pad()) * 32;
   for (auto& b : P->zk_coeff) b.ensure(bytes);
   for (auto& b : P->zk_t) b.ensure(bytes);
-  for (auto& b : P->tmp) b.ensure(bytes);  // round 5 works on n + 8 coefficients
+  for (auto& b : P->tmp) b.ensure(bytes);  // round 5 works on n + 8 coefficients (n + 9 next-row)
   if (P->lk)
     for (auto& b : P->zk_lk) b.ensure(bytes);
   if (h_blinders) std::copy(fixed, fixed + count, P->zk_fixed_b);
@@ -914,9 +982,9 @@ static void zk_draw_blinders(Prover* P) {
   }
 }
 
-// out (n + 8, zero padded) = in (n_in coefficients) + c(X) Z_H(X) with c = c[0] + c[1] X + ... (deg < 3)
+// out (n + zk_pad(), zero padded) = in (n_in coefficients) + c(X) Z_H(X) with c = c[0] + c[1] X + ... (deg < 3)
 static void zk_blind(Prover* P, const Fr* in, uint64_t n_in, const ZkPatch& p, Fr* out) {
-  const uint64_t len = P->n + Prover::ZK_PAD;
+  const uint64_t len = P->n + P->zk_pad();
   k_zk_blind<<<PB_GRID(len, 256), 0, P->ctx->stream>>>(in, n_in, P->n, p, len, out);
   P->ctx->launches++;
 }
@@ -959,6 +1027,7 @@ void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* h_qtag, co
   const bool tagged = h_qtag != nullptr;
   const int width = tagged ? 4 : 3;
   PB_CHECK(P->world == 1, "lookups are not available on the sharded prover (one GPU only)");
+  PB_CHECK(!P->next_row, "lookups do not combine with next-row custom gate terms");
   PB_CHECK(!P->zk, "lookups do not combine with zero-knowledge mode switched on first: set the table, then "
                    "pb200_prover_set_zk_lookup");
   PB_CHECK(!P->lk, "the lookup table is already set (set it once, before the first proof)");
@@ -1226,11 +1295,10 @@ void prover_round1(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_
     k_negate<<<PB_GRID(n_public, 128), 0, st>>>(P->pi_lag.as<Fr>(), n_public);
     ctx->launches++;
   }
-  k_gate_check<<<PB_GRID(n, 128), 0, st>>>(P->lag[0].as<Fr>(), P->lag[1].as<Fr>(), P->lag[2].as<Fr>(),
-                                          P->sel_lag[Prover::QL].as<Fr>(), P->sel_lag[Prover::QR].as<Fr>(),
-                                          P->sel_lag[Prover::QM].as<Fr>(), P->sel_lag[Prover::QO].as<Fr>(),
-                                          P->sel_lag[Prover::QC].as<Fr>(), P->pi_lag.as<Fr>(), P->custom_terms(P->sel_lag),
-                                          n, P->flags.as<uint32_t>());
+  (P->next_row ? k_gate_check<true> : k_gate_check<false>)<<<PB_GRID(n, 128), 0, st>>>(
+      P->lag[0].as<Fr>(), P->lag[1].as<Fr>(), P->lag[2].as<Fr>(), P->sel_lag[Prover::QL].as<Fr>(),
+      P->sel_lag[Prover::QR].as<Fr>(), P->sel_lag[Prover::QM].as<Fr>(), P->sel_lag[Prover::QO].as<Fr>(),
+      P->sel_lag[Prover::QC].as<Fr>(), P->pi_lag.as<Fr>(), P->custom_terms(P->sel_lag), n, P->flags.as<uint32_t>());
   ctx->launches++;
   if (wires_on_device || P->world > 1) interpolate(P, abc_lag, abc_coeff, 3);
   // public inputs: few of them -> PI is a short combination of cached Lagrange-basis vectors (no transforms);
@@ -1257,6 +1325,14 @@ void prover_round1(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_
   PB_CHECK(fl[0] == 0, "AssertionError: witness does not satisfy the gate constraints (prover.py:108-116)");
   if (P->lk) lookup_index(P);
   if (P->overlap) launch_coset_ext_async(P, 0, 3, 0);
+  if (P->zk && P->next_row) {  // A' B' C': n + 3 coefficients (b12..b14 in front of the usual two)
+    const Fr* b = P->zk_b;
+    for (int k = 0; k < 3; k++)
+      zk_blind(P, P->coeff[k].as<Fr>(), n, zh_multiple({b[2 * k + 1], b[2 * k], b[11 + k]}), P->zk_coeff[k].as<Fr>());
+    const Fr* abc[3] = {P->zk_coeff[0].as<Fr>(), P->zk_coeff[1].as<Fr>(), P->zk_coeff[2].as<Fr>()};
+    P->commit_batch(abc, 3, n + 3, P->proof.pts[0]);
+    return;
+  }
   if (P->zk) {  // A' B' C': n + 2 coefficients
     const Fr* b = P->zk_b;
     for (int k = 0; k < 3; k++)
@@ -1343,15 +1419,27 @@ void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c) {
   q.n4 = ne;
   Fr* t_evals = P->world > 1 ? P->tq_loc.as<Fr>() : P->tq.as<Fr>();
   ZkCoset zk{};
-  if (P->zk) {
+  if (P->next_row && P->zk) {
+    const Fr* b = P->zk_b;
+    const Fr w = fr_root_of_unity(P->log_n), w2 = fp_sqr(w);
+    const Fr per[24] = {b[11], b[0], b[1], b[12], b[2], b[3], b[13], b[4], b[5], b[6], b[7], b[8],
+                        fp_mul(b[6], w2), fp_mul(b[7], w), b[8], fp_mul(b[11], w2), fp_mul(b[0], w), b[1],
+                        fp_mul(b[12], w2), fp_mul(b[2], w), b[3], fp_mul(b[13], w2), fp_mul(b[4], w), b[5]};
+    ZkNextCoset zn;
+    for (int k = 0; k < 4; k++)
+      for (int i = 0; i < 24; i++) zn.w[k][i] = fp_mul(per[i], P->zh[k]);
+    k_quotient<true, true><<<PB_GRID(ne, 128), 0, st>>>(q, t_evals, zn);
+  } else if (P->next_row) {
+    k_quotient<false, true><<<PB_GRID(ne, 128), 0, st>>>(q, t_evals, zk);
+  } else if (P->zk) {
     const Fr* b = P->zk_b;
     const Fr w = fr_root_of_unity(P->log_n);
     const Fr per[12] = {b[0], b[1], b[2], b[3], b[4], b[5], b[6], b[7], b[8], fp_mul(b[6], fp_sqr(w)), fp_mul(b[7], w), b[8]};
     for (int k = 0; k < 4; k++)
       for (int i = 0; i < 12; i++) zk.w[k][i] = fp_mul(per[i], P->zh[k]);
-    k_quotient<true><<<PB_GRID(ne, 128), 0, st>>>(q, t_evals, zk);
+    k_quotient<true, false><<<PB_GRID(ne, 128), 0, st>>>(q, t_evals, zk);
   } else {
-    k_quotient<false><<<PB_GRID(ne, 128), 0, st>>>(q, t_evals, zk);
+    k_quotient<false, false><<<PB_GRID(ne, 128), 0, st>>>(q, t_evals, zk);
   }
   ctx->launches++;
   if (P->lk) {  // one GPU: the slice is the whole 4n coset
@@ -1397,21 +1485,23 @@ void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c) {
   } else {
     // back to coefficients: ifft(4n) then * g^-i (poly.py:169-177 with the fixed coset)
     ntt_run(ctx, P->tq.as<Fr>(), P->tq.as<Fr>(), P->log_n + 2, true, n4, nullptr, P->ginv_pow.as<Fr>());
-    const uint64_t top = P->zk ? 3 * n + 6 : 3 * n;  // zero knowledge: deg T <= 3n + 5
+    const uint64_t top = P->zk ? P->zk_t3_len() + 2 * n : 3 * n;  // zero knowledge: deg T <= 3n + 5 (3n + 8)
     k_count_nonzero<<<PB_GRID(n4 - top, 256), 0, st>>>(P->tq.as<Fr>() + top, n4 - top, P->flags.as<uint32_t>());
     ctx->launches++;
   }
   if (P->zk) {
-    PB_CHECK(read_flag(P, 0) == 0,
-             "AssertionError: quotient has degree >= 3n + 6 (zero-knowledge mode; prover.py:205-208)");
+    PB_CHECK(read_flag(P, 0) == 0, P->next_row
+                 ? "AssertionError: quotient has degree >= 3n + 9 (zero-knowledge mode, next-row terms; prover.py:205-208)"
+                 : "AssertionError: quotient has degree >= 3n + 6 (zero-knowledge mode; prover.py:205-208)");
     // the pieces overlap in tq once blinded (T1' reaches X^n), so each gets its own buffer; one commitment pass
     const Fr* t = P->tq.as<Fr>();
     const Fr b10 = P->zk_b[9], b11 = P->zk_b[10], zero = Fr::zero();
     zk_blind(P, t, n, ZkPatch{{zero, zero, zero}, {b10, zero, zero}}, P->zk_t[0].as<Fr>());
     zk_blind(P, t + n, n, ZkPatch{{fp_neg(b10), zero, zero}, {b11, zero, zero}}, P->zk_t[1].as<Fr>());
-    zk_blind(P, t + 2 * n, n + 6, ZkPatch{{fp_neg(b11), zero, zero}, {zero, zero, zero}}, P->zk_t[2].as<Fr>());
+    const uint64_t t3 = P->zk_t3_len();
+    zk_blind(P, t + 2 * n, t3, ZkPatch{{fp_neg(b11), zero, zero}, {zero, zero, zero}}, P->zk_t[2].as<Fr>());
     const Fr* t123[3] = {P->zk_t[0].as<Fr>(), P->zk_t[1].as<Fr>(), P->zk_t[2].as<Fr>()};
-    P->commit_batch(t123, 3, n + 6, P->proof.pts[4]);
+    P->commit_batch(t123, 3, t3, P->proof.pts[4]);
     return;
   }
   PB_CHECK(read_flag(P, 0) == 0, "AssertionError: quotient has degree >= 3n (prover.py:205-208)");
@@ -1429,7 +1519,25 @@ void prover_round4(Prover* P, const Fr& zeta_c) {
   Fr xs[7] = {P->zeta, P->zeta, P->zeta, P->zeta, P->zeta, zw, P->zeta};
   Fr out[7];
   eval_polys(P, P->pi_sparse ? 6 : 7, polys, xs, out);
-  if (P->zk) {
+  if (P->next_row) {  // A, B, C at zeta w, and the third blinder of zero-knowledge mode on all six wire evaluations
+    const Fr* abc[3] = {P->coeff[0].as<Fr>(), P->coeff[1].as<Fr>(), P->coeff[2].as<Fr>()};
+    const Fr zws[3] = {zw, zw, zw};
+    eval_polys(P, 3, abc, zws, P->nr_ev);
+    if (P->zk) {
+      // A'(x) = A(x) + (b12 x^2 + b1 x + b2) Z_H(x) at x = zeta and x = zeta w, with Z_H(zeta w) = Z_H(zeta)
+      const Fr* b = P->zk_b;
+      const Fr zh = fp_sub(fp_pow_u64(P->zeta, P->n), Fr::one());
+      auto blind = [&](int k, const Fr& x) {
+        return fp_mul(fp_add(fp_mul(fp_add(fp_mul(b[11 + k], x), b[2 * k]), x), b[2 * k + 1]), zh);
+      };
+      for (int k = 0; k < 3; k++) {
+        out[k] = fp_add(out[k], blind(k, P->zeta));
+        P->nr_ev[k] = fp_add(P->nr_ev[k], blind(k, zw));
+      }
+      out[5] = fp_add(out[5], fp_mul(fp_add(fp_mul(fp_add(fp_mul(b[6], zw), b[7]), zw), b[8]), zh));
+    }
+    for (int k = 0; k < 3; k++) store_canonical(P->nr_evals[k], P->nr_ev[k]);
+  } else if (P->zk) {
     // the blinded polynomials at their points: A'(zeta) = A(zeta) + (b1 zeta + b2)(zeta^n - 1), ...,
     // Z'(zeta w) = Z(zeta w) + (b7 (zeta w)^2 + b8 zeta w + b9)(zeta^n - 1)
     const Fr* b = P->zk_b;
@@ -1563,8 +1671,10 @@ void prover_round5(Prover* P, const Fr& v_c) {
   add(P->sel_coeff[Prover::QM].as<Fr>(), fp_mul(a, b));
   add(P->sel_coeff[Prover::QO].as<Fr>(), c);
   add(P->sel_coeff[Prover::QC].as<Fr>(), one);
-  for (int t = 0; t < P->n_custom; t++)                                // m_t(a, b, c) Q_t
-    add(P->sel_coeff[Prover::CUSTOM0 + t].as<Fr>(), custom_monomial(a, b, c, P->custom_f[t]));
+  const Fr *aw = P->nr_ev, *bw = P->nr_ev + 1, *cw = P->nr_ev + 2;  // next-row provers: the wires at zeta w
+  for (int t = 0; t < P->n_custom; t++)  // m_t(a, b, c) Q_t, or m_t(a, b, c, a(zeta w), b(zeta w), c(zeta w)) Q_t
+    add(P->sel_coeff[Prover::CUSTOM0 + t].as<Fr>(),
+        P->next_row ? custom_monomial_next(a, b, c, *aw, *bw, *cw, P->custom_f[t]) : custom_monomial(a, b, c, P->custom_f[t]));
   add(zpoly, fp_add(c1, al2l0), true);                                 // Z
   add(P->sel_coeff[Prover::S3].as<Fr>(), fp_neg(fp_mul(c2, be)));
   add(tpiece[0], fp_neg(zh_ev), true);                                 // T1
@@ -1617,10 +1727,10 @@ void prover_round5(Prover* P, const Fr& v_c) {
   PB_CUDA(cudaMemsetAsync(P->flags.p, 0, 64, st));
   k_lincomb<<<PB_GRID(L.n, 128), 0, st>>>(L, wz);
   ctx->launches++;
-  const uint64_t len = zk ? n + Prover::ZK_PAD : n;  // numerator coefficients
+  const uint64_t len = zk ? n + P->zk_pad() : n;  // numerator coefficients
   if (zk) {
     tail.c0 = Fr::zero();
-    tail.n = Prover::ZK_PAD;
+    tail.n = P->zk_pad();
     tail.first = n;
     k_lincomb<<<PB_GRID(tail.n, 128), 0, st>>>(tail, wz);
     ctx->launches++;
@@ -1638,6 +1748,13 @@ void prover_round5(Prover* P, const Fr& v_c) {
     M.count = 4;
     M.c0 = fp_sub(M.c0, fp_add(fp_mul(v, P->lk_ev[2]), fp_add(fp_mul(v2, P->lk_ev[4]), fp_mul(v3, P->lk_ev[5]))));
   }
+  if (P->next_row) {  // + v (A - a(zeta w)) + v^2 (B - b(zeta w)) + v^3 (C - c(zeta w)); zero knowledge: A', B', C'
+    M.vec[1] = wire[0]; M.w[1] = v;
+    M.vec[2] = wire[1]; M.w[2] = v2;
+    M.vec[3] = wire[2]; M.w[3] = v3;
+    M.count = 4;
+    M.c0 = fp_sub(M.c0, fp_add(fp_mul(v, *aw), fp_add(fp_mul(v2, *bw), fp_mul(v3, *cw))));
+  }
   Fr* wzw = P->tmp[0].as<Fr>();  // the W_z numerator is no longer needed
   k_lincomb<<<PB_GRID(M.n, 128), 0, st>>>(M, wzw);
   ctx->launches++;
@@ -1646,25 +1763,30 @@ void prover_round5(Prover* P, const Fr& v_c) {
   PB_CHECK(read_flag(P, 0) == 0,
            "AssertionError: opening numerator is not divisible by (X - point) (prover.py:267,288,299)");
   const Fr* ws[2] = {wz_q, wzw_q};
-  // zero knowledge: W_z has n + 5 coefficients (numerator n + 6), W_zw n + 2; the rest of the buffers is zero
-  P->commit_batch(ws, 2, zk ? n + 5 : n, P->proof.pts[7]);
+  // zero knowledge: W_z has n + 5 coefficients (numerator n + 6; next-row n + 8 and n + 9), W_zw n + 2; the rest of
+  // the buffers is zero
+  P->commit_batch(ws, 2, zk ? P->zk_t3_len() - 1 : n, P->proof.pts[7]);
 }
 
 // canonical 768-byte proof: Proof.flatten() order (prover.py:18-35), G1 as x||y, every integer 32-byte
 // big-endian exactly as the transcript absorbs it (transcript.py:62-67).  A lookup proof has 1216 bytes: the 768 plain
-// bytes, then f_1 h1_1 h2_1 z2_1, then the six lookup evaluations.
+// bytes, then f_1 h1_1 h2_1 z2_1, then the six lookup evaluations.  A next-row proof has 864 bytes: the 768 plain bytes,
+// then a(zeta w), b(zeta w), c(zeta w).
 void prover_serialize(const Prover* P, uint8_t* out) {
   auto be = [](uint8_t* dst, const uint8_t* le) { for (int i = 0; i < 32; i++) dst[i] = le[31 - i]; };
   uint8_t* o = out;
   for (int k = 0; k < 7; k++) { be(o, P->proof.pts[k]); be(o + 32, P->proof.pts[k] + 32); o += 64; }
   for (int k = 0; k < 6; k++) { be(o, P->proof.evals[k]); o += 32; }
   for (int k = 7; k < 9; k++) { be(o, P->proof.pts[k]); be(o + 32, P->proof.pts[k] + 32); o += 64; }
+  if (P->next_row)
+    for (int k = 0; k < 3; k++) { be(o, P->nr_evals[k]); o += 32; }
   if (!P->lk) return;
   for (int k = 0; k < 4; k++) { be(o, P->lk_pts[k]); be(o + 32, P->lk_pts[k] + 32); o += 64; }
   for (int k = 0; k < 6; k++) { be(o, P->lk_evals[k]); o += 32; }
 }
 
-// prover.py:51-84; a prover with a lookup table runs step 1L between rounds 1 and 2 and writes the 1216-byte proof
+// prover.py:51-84; a prover with a lookup table runs step 1L between rounds 1 and 2 and writes the 1216-byte proof, a
+// next-row prover absorbs three more evaluations in round 4 and writes the 864-byte proof
 void prover_prove(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t* hC, const uint8_t* h_public,
                   uint64_t n_public, uint8_t* out, bool wires_on_device) {
   PB_CUDA(cudaSetDevice(P->ctx->device));  // the calling host thread may not be the one that created the context
@@ -1696,6 +1818,10 @@ void prover_prove(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t
   prover_round4(P, zeta);
   static const char* ev_labels[6] = {"a_eval", "b_eval", "c_eval", "s1_eval", "s2_eval", "z_shifted_eval"};
   for (int k = 0; k < 6; k++) tr.append_scalar_le(ev_labels[k], P->proof.evals[k]);
+  if (P->next_row) {  // NEXT_ROW_SCHEDULE (transcript.py)
+    static const char* nr_labels[3] = {"a_shifted_eval", "b_shifted_eval", "c_shifted_eval"};
+    for (int k = 0; k < 3; k++) tr.append_scalar_le(nr_labels[k], P->nr_evals[k]);
+  }
   if (P->lk) {
     static const char* lk_labels[6] = {"f_eval", "t_eval", "t_shifted_eval", "h2_eval", "h1_shifted_eval",
                                        "z2_shifted_eval"};

@@ -15,19 +15,33 @@ void srs_msm_batch_sharded(Context* ctx, Srs* srs, const Fr* const* d_scalars, u
 uint32_t srs_bucket_count(Srs* s);
 
 // Custom gate terms: the gate constraint gains sum_k Q_k a^i_k b^j_k c^l_k, total degree 2 or 3 (so T stays below
-// degree 3n and the proof keeps its shape).  A term is stored as the wires of its monomial: 2 or 3 of {0 a, 1 b, 2 c},
-// unused slots 3.
+// degree 3n and the proof keeps its shape).  A term is stored as the factors of its monomial: up to 3 of {0 a, 1 b,
+// 2 c, 3 a(wX), 4 b(wX), 5 c(wX)}, unused slots PB_FACTOR_ONE.  Factors 3..5 (next-row terms, degree 1 to 3) occur only
+// on a prover made by pb200_prover_create_custom_next_row (Prover::next_row).
 #define PB_MAX_CUSTOM 4
+#define PB_FACTOR_ONE 6
 struct CustomTerms {
   const Fr* Q[PB_MAX_CUSTOM];
   uint8_t f[PB_MAX_CUSTOM][3];
   int count;
 };
-// m_k(a, b, c) with degree - 1 products; the wires are selected by value so a, b, c stay in registers
+// m_k(a, b, c) of a same-row term (degree 2 or 3) with degree - 1 products; the wires are selected by value so a, b, c
+// stay in registers
 PB_HD Fr custom_monomial(const Fr& a, const Fr& b, const Fr& c, const uint8_t* f) {
   auto pick = [&](uint8_t w) -> Fr { return w == 0 ? a : (w == 1 ? b : c); };
   Fr m = fp_mul(pick(f[0]), pick(f[1]));
   if (f[2] < 3) m = fp_mul(m, pick(f[2]));
+  return m;
+}
+// m_k(a, b, c, a', b', c') of any term of a next-row prover (degree 1 to 3), a' = a(wX)
+PB_HD Fr custom_monomial_next(const Fr& a, const Fr& b, const Fr& c, const Fr& an, const Fr& bn, const Fr& cn,
+                              const uint8_t* f) {
+  auto pick = [&](uint8_t w) -> Fr {
+    return w == 0 ? a : w == 1 ? b : w == 2 ? c : w == 3 ? an : w == 4 ? bn : cn;
+  };
+  Fr m = pick(f[0]);
+  if (f[1] != PB_FACTOR_ONE) m = fp_mul(m, pick(f[1]));
+  if (f[2] != PB_FACTOR_ONE) m = fp_mul(m, pick(f[2]));
   return m;
 }
 // sum_k Q_k[i] m_k(a, b, c), unrolled over the PB_MAX_CUSTOM slots so the kernel parameters are indexed statically
@@ -44,6 +58,21 @@ __device__ __forceinline__ Fr custom_gate_sum(const CustomTerms& t, uint64_t i, 
     s.v[0] = lo.x; s.v[1] = lo.y; s.v[2] = lo.z; s.v[3] = lo.w;
     s.v[4] = hi.x; s.v[5] = hi.y; s.v[6] = hi.z; s.v[7] = hi.w;
     acc = fp_add(acc, fp_mul(custom_monomial(a, b, c, t.f[k]), s));
+  }
+  return acc;
+}
+// the same for a next-row prover: an, bn, cn are the wires of the next row (index + 1 mod n, or X -> wX on a coset)
+__device__ __forceinline__ Fr custom_gate_sum_next(const CustomTerms& t, uint64_t i, const Fr& a, const Fr& b,
+                                                   const Fr& c, const Fr& an, const Fr& bn, const Fr& cn, Fr acc) {
+#pragma unroll
+  for (int k = 0; k < PB_MAX_CUSTOM; k++) {
+    if (k >= t.count) break;
+    const uint4* q = reinterpret_cast<const uint4*>(t.Q[k] + i);
+    uint4 lo = __ldg(q), hi = __ldg(q + 1);
+    Fr s;
+    s.v[0] = lo.x; s.v[1] = lo.y; s.v[2] = lo.z; s.v[3] = lo.w;
+    s.v[4] = hi.x; s.v[5] = hi.y; s.v[6] = hi.z; s.v[7] = hi.w;
+    acc = fp_add(acc, fp_mul(custom_monomial_next(a, b, c, an, bn, cn, t.f[k]), s));
   }
   return acc;
 }
@@ -75,7 +104,12 @@ struct Prover {
   DevBuf sel_lag[8 + PB_MAX_CUSTOM];     // same, Lagrange values (QM..QC and custom for the gate check, S1..S3 for round 2)
   DevBuf sel_ext[8 + PB_MAX_CUSTOM];     // same, on this rank's slice of the fixed 4n coset
   int n_custom = 0;
-  uint8_t custom_f[PB_MAX_CUSTOM][3];    // monomial wires of each custom term (CustomTerms::f)
+  uint8_t custom_f[PB_MAX_CUSTOM][3];    // monomial factors of each custom term (CustomTerms::f)
+  // Next-row terms (pb200_prover_create_custom_next_row, one GPU): some term reads a(wX), b(wX) or c(wX).  Round 4 also
+  // evaluates A, B, C at zeta w, the zeta w opening batches them with Z, and the proof has 864 bytes.
+  bool next_row = false;
+  Fr nr_ev[3];                           // a(zeta w), b(zeta w), c(zeta w), Montgomery
+  uint8_t nr_evals[3][32];               // canonical LE
   DevBuf roots;          // w^i, i < n
   DevBuf gpow;           // (g mu^rank)^i, i < n     (coset shift on load)
   DevBuf gpow_w;         // (g mu^(rank+4))^i, i < n (only when zw_separate)
@@ -105,16 +139,20 @@ struct Prover {
   // Zero knowledge (one GPU only): the blinding of the PLONK paper with 11 scalars b1..b11 per proof.  The unblinded
   // n-coefficient vectors above stay as they are (the coset extensions read them; k_quotient adds the Z_H multiples);
   // the blinded vectors, which are longer than n, live in their own zero-padded buffers of n + 8 elements.
-  // With a lookup table (prover_set_zk_lookup) there are 21 scalars: b12..b21 blind F, H1, H2 and Z2.
-  static const int ZK_BLINDERS = 11, ZK_LK_BLINDERS = 21, ZK_PAD = 8;
+  // With a lookup table (prover_set_zk_lookup) there are 21 scalars: b12..b21 blind F, H1, H2 and Z2.  A next-row
+  // prover takes 14: b12..b14 give A, B, C a third blinder each (they are opened at zeta and at zeta w), so T3' has
+  // n + 9 coefficients and the blinded vectors get ZK_NR_PAD elements of padding.
+  static const int ZK_BLINDERS = 11, ZK_LK_BLINDERS = 21, ZK_NR_BLINDERS = 14, ZK_PAD = 8, ZK_NR_PAD = 9;
   bool zk = false;
   bool zk_fixed = false;          // the same blinders for every proof (zk_fixed_b) instead of fresh OS randomness
   Fr zk_fixed_b[ZK_LK_BLINDERS];  // canonical
-  Fr zk_b[ZK_LK_BLINDERS];        // this proof's b1..b11 (..b21 with lookups), Montgomery (drawn when round 1 starts)
-  DevBuf zk_coeff[4];             // A' B' C' (n + 2 coefficients) Z' (n + 3)
-  DevBuf zk_t[3];                 // T1' T2' (n + 1 coefficients) T3' (n + 6)
+  Fr zk_b[ZK_LK_BLINDERS];        // this proof's b1..b11 (..b14 next-row, ..b21 lookups), Montgomery (drawn in round 1)
+  DevBuf zk_coeff[4];             // A' B' C' (n + 2 coefficients, n + 3 next-row) Z' (n + 3)
+  DevBuf zk_t[3];                 // T1' T2' (n + 1 coefficients) T3' (n + 6, n + 9 next-row)
   DevBuf zk_lk[5];                // lookups: T (n, zero padded) F' H2' (n + 2) H1' Z2' (n + 3), indexed by LK_*
-  int zk_blinders() const { return lk ? ZK_LK_BLINDERS : ZK_BLINDERS; }
+  int zk_blinders() const { return lk ? ZK_LK_BLINDERS : next_row ? ZK_NR_BLINDERS : ZK_BLINDERS; }
+  uint64_t zk_pad() const { return next_row ? ZK_NR_PAD : ZK_PAD; }
+  uint64_t zk_t3_len() const { return n + (next_row ? 9 : 6); }  // coefficients of T3' (deg T <= 3n + 5, or 3n + 8)
   // Lookup argument (prover_set_lookup, one GPU): plookup over one fixed table of three columns, or over several
   // tables told apart by a tag column t4 and the selector Q_T, see "lookups" in prover.cu.  The proof gains f_1 h1_1
   // h2_1 z2_1 and six evaluations (1216 bytes).

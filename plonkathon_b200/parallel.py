@@ -23,6 +23,7 @@ import ctypes
 from typing import Optional
 
 from . import _lib
+from .custom_gates import is_next_row
 from .prover import Prover
 
 
@@ -125,6 +126,9 @@ class ShardedProver(Prover):
     def from_arrays(cls, setup, group_order, pk_arrays, group=None, ctx=None, custom=(), lookup=None, lookups=None):
         if lookup is not None or lookups is not None:
             raise ValueError("lookups are not available on the sharded prover (one GPU only)")
+        custom = list(custom)
+        if any(is_next_row(e) for e, _ in custom):
+            raise ValueError("next-row custom gate terms are not available on the sharded prover (one GPU only)")
         init_comm(ctx or setup.ctx, group)
         return super().from_arrays(setup, group_order, pk_arrays, ctx=ctx, custom=custom)
 

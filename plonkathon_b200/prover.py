@@ -16,11 +16,11 @@ import numpy as np
 
 from . import _lib
 from .curve import Scalar
-from .custom_gates import split_terms
+from .custom_gates import is_next_row, padded, split_terms
 from .lookup import PROOF_BYTES as LOOKUP_PROOF_BYTES, check_lookup, check_lookups, padded_table, to_le_rows
 from .field import CURVE_ORDER, FIELD_MODULUS, FQ
 from .poly import Basis, _log2_exact, scalars_to_bytes
-from .transcript import Message1, Message2, Message3, Message4, Message5, Transcript
+from .transcript import Message1, Message2, Message3, Message4, Message5, NextRowMessage4, Transcript
 
 PK_ORDER = ("QM", "QL", "QR", "QO", "QC", "S1", "S2", "S3")  # compiler/program.py:10-30
 PROOF_FIELDS = ("a_1", "b_1", "c_1", "z_1", "t_lo_1", "t_mid_1", "t_hi_1", "a_eval", "b_eval", "c_eval",
@@ -118,6 +118,38 @@ class LookupProof:
         return cls(plain, pt(0), pt(2), pt(4), pt(6), *[Scalar(x) for x in w[8:14]])
 
 
+NEXT_ROW_FIELDS = ("a_shifted_eval", "b_shifted_eval", "c_shifted_eval")
+NEXT_ROW_PROOF_BYTES = 864
+
+
+@dataclass
+class NextRowProof:
+    """A proof of a circuit with next-row custom gate terms (plonkathon_b200/custom_gates.py): the plain proof's 15
+    fields and the wires at zeta w.  Byte order: the plain fields in ``Proof.flatten()`` order, then a_shifted_eval,
+    b_shifted_eval, c_shifted_eval -- 864 bytes, encoded as the plain proof."""
+    plain: Proof
+    a_shifted_eval: Scalar
+    b_shifted_eval: Scalar
+    c_shifted_eval: Scalar
+
+    def flatten(self):
+        out = self.plain.flatten()
+        out.update((k, getattr(self, k)) for k in NEXT_ROW_FIELDS)
+        return out
+
+    def to_bytes(self) -> bytes:
+        return _encode(self.flatten().values())
+
+    @classmethod
+    def from_bytes(cls, raw: bytes) -> "NextRowProof":
+        """Inverse of to_bytes; ValueError for a word that is not reduced (coordinates below q, scalars below r)."""
+        if len(raw) != NEXT_ROW_PROOF_BYTES:
+            raise ValueError("a next-row proof has %d bytes, got %d" % (NEXT_ROW_PROOF_BYTES, len(raw)))
+        plain = Proof.from_bytes(raw[:768])
+        w = _decode_words(raw[768:], range(3), first=24)
+        return cls(plain, *[Scalar(x) for x in w])
+
+
 def _as_le_rows(values, n) -> np.ndarray:
     """list of ints / Scalars, or an (m,32) uint8 / (m,8) uint32 array -> contiguous (n,32) uint8, zero padded."""
     if isinstance(values, np.ndarray):
@@ -145,6 +177,7 @@ def _raise(err: _lib.PlonkB200Error):
 class Prover:
     _CREATE = "pb200_prover_create"
     _CREATE_CUSTOM = "pb200_prover_create_custom"
+    _CREATE_NEXT_ROW = "pb200_prover_create_custom_next_row"
 
     def __init__(self, setup, program):
         """prover.py:45-49."""
@@ -166,9 +199,15 @@ class Prover:
         (plonkathon_b200/lookup.py); ``prove_arrays`` then returns a 1216-byte ``LookupProof``.  ValueError for a
         malformed argument; the library refuses it on the sharded prover.
         ``lookups``: ``[(q_0, (t1, t2, t3)), (q_1, ...), ...]``, lookups over several tables told apart by a table tag
-        (table k has id k; ``check_lookups``).  The proof is a ``LookupProof`` too.  Not together with ``lookup``."""
+        (table k has id k; ``check_lookups``).  The proof is a ``LookupProof`` too.  Not together with ``lookup``.
+        A custom term with six exponents ``((i, j, l, i', j', l'), column)`` may read the next row's wires; with one
+        such term ``prove_arrays`` returns an 864-byte ``NextRowProof``.  Next-row terms do not combine with lookups
+        (ValueError)."""
         if lookup is not None and lookups is not None:
             raise ValueError("pass either lookup= (one table) or lookups= (several tables), not both")
+        custom = list(custom)
+        if (lookup is not None or lookups is not None) and any(is_next_row(e) for e, _ in custom):
+            raise ValueError("lookups do not combine with next-row custom gate terms")
         # before any device work
         lk = check_lookup(lookup, group_order) if lookup is not None else None
         lks = check_lookups(lookups, group_order) if lookups is not None else None
@@ -203,14 +242,19 @@ class Prover:
         self.ctx = ctx or setup.ctx
         self._log_n = _log2_exact(n)
         self.custom_exponents = exps
+        self.next_row = any(is_next_row(e) for e in exps)
         keep = [c if isinstance(c, bytes) else c.tobytes() for c in (cols[k] for k in PK_ORDER)]
         arr = (ctypes.c_char_p * 8)(*keep)
         h = ctypes.c_void_p()
         if exps:
             ckeep = [_as_le_rows(col, n).tobytes() for col in ccols]
             carr = (ctypes.c_char_p * len(ckeep))(*ckeep)
-            ebytes = bytes(x for e in exps for x in e)
-            create = getattr(_lib.lib(), self._CREATE_CUSTOM)
+            if self.next_row:  # six bytes per term
+                ebytes = bytes(x for e in exps for x in padded(e))
+                create = getattr(_lib.lib(), self._CREATE_NEXT_ROW)
+            else:  # three bytes per term: the same-row path
+                ebytes = bytes(x for e in exps for x in padded(e)[:3])
+                create = getattr(_lib.lib(), self._CREATE_CUSTOM)
             _lib.check(create(self.ctx.handle, setup._srs, self._log_n, ctypes.cast(arr, ctypes.c_void_p), len(exps),
                               ebytes, ctypes.cast(carr, ctypes.c_void_p), ctypes.byref(h)))
         else:
@@ -229,14 +273,19 @@ class Prover:
 
     # ------------------------------------------------------------------ array-level fast path
     def prove_arrays(self, A, B, C, public) -> bytes:
-        """One C-ABI call for the whole proof (rounds 1-5 + transcript); returns the canonical 768 bytes, or the
-        1216 bytes of a ``LookupProof`` on a prover with a lookup argument."""
+        """One C-ABI call for the whole proof (rounds 1-5 + transcript); returns the canonical 768 bytes, the
+        1216 bytes of a ``LookupProof`` on a prover with a lookup argument, or the 864 bytes of a ``NextRowProof`` on a
+        prover with next-row custom gate terms."""
         n = self.group_order
         a, b, c = (_as_le_rows(v, n) for v in (A, B, C))
         pub = _as_le_rows(public, len(public)) if len(public) else np.zeros((0, 32), dtype=np.uint8)
         lookup = getattr(self, "lookup", False)
-        out = ctypes.create_string_buffer(LOOKUP_PROOF_BYTES if lookup else 768)
-        prove = _lib.lib().pb200_prover_prove_lookup if lookup else _lib.lib().pb200_prover_prove
+        if getattr(self, "next_row", False):
+            out = ctypes.create_string_buffer(NEXT_ROW_PROOF_BYTES)
+            prove = _lib.lib().pb200_prover_prove_next_row
+        else:
+            out = ctypes.create_string_buffer(LOOKUP_PROOF_BYTES if lookup else 768)
+            prove = _lib.lib().pb200_prover_prove_lookup if lookup else _lib.lib().pb200_prover_prove
         try:
             _lib.check(prove(
                 self._h, a.ctypes.data_as(ctypes.c_void_p), b.ctypes.data_as(ctypes.c_void_p),
@@ -247,7 +296,8 @@ class Prover:
 
     # ------------------------------------------------------------------ the reference's surface
     def prove(self, witness) -> Proof:
-        """prover.py:51-84."""
+        """prover.py:51-84.  A prover with next-row custom gate terms follows NEXT_ROW_SCHEDULE and returns a
+        ``NextRowProof``."""
         transcript = Transcript(b"plonk")
         msg_1 = self.round_1(witness)  # also collects the public inputs (prover.py:57-62)
         self.beta, self.gamma = transcript.round_1(msg_1)
@@ -258,6 +308,9 @@ class Prover:
         msg_4 = self.round_4()
         self.v = transcript.round_4(msg_4)
         msg_5 = self.round_5()
+        if isinstance(msg_4, NextRowMessage4):
+            plain = Message4(*[getattr(msg_4, k) for k in PROOF_FIELDS[7:13]])
+            return NextRowProof(Proof(msg_1, msg_2, msg_3, plain, msg_5), *[getattr(msg_4, k) for k in NEXT_ROW_FIELDS])
         return Proof(msg_1, msg_2, msg_3, msg_4, msg_5)
 
     def round_1(self, witness) -> Message1:
@@ -310,7 +363,12 @@ class Prover:
         return Message3(*self._commitments(4, 3, out.raw))
 
     def round_4(self) -> Message4:
-        """prover.py:228-239."""
+        """prover.py:228-239.  A next-row prover returns a ``NextRowMessage4``: the six evaluations, then a, b, c at
+        zeta w (NEXT_ROW_SCHEDULE)."""
+        if getattr(self, "next_row", False):
+            out = ctypes.create_string_buffer(9 * 32)
+            _lib.check(_lib.lib().pb200_prover_round4_next_row(self._h, self._le(self.zeta), out))
+            return NextRowMessage4(*[Scalar(int.from_bytes(out.raw[32 * k:32 * k + 32], "little")) for k in range(9)])
         out = ctypes.create_string_buffer(192)
         _lib.check(_lib.lib().pb200_prover_round4(self._h, self._le(self.zeta), out))
         return Message4(*[Scalar(int.from_bytes(out.raw[32 * k:32 * k + 32], "little")) for k in range(6)])
@@ -344,7 +402,7 @@ class Prover:
     def _piece(self, which: int, name: str):
         if getattr(self, "zk", False):
             raise RuntimeError("%s is not available in zero-knowledge mode: the blinded quotient pieces have n + 1, "
-                               "n + 1 and n + 6 coefficients, so they have no n-value Lagrange form" % name)
+                               "n + 1 and n + 6 (or n + 9) coefficients, so they have no n-value Lagrange form" % name)
         return self._state(which, Basis.MONOMIAL).fft(ctx=self.ctx)
 
     T1 = property(lambda self: self._piece(5, "T1"))
@@ -357,12 +415,16 @@ class Prover:
         paper (eprint 2019/953), with 11 scalars b1..b11 per proof.  The proof keeps its 768 bytes and the verifier does
         not change.  ``blinders=None``: fresh scalars from the OS CSPRNG for every proof; otherwise 11 integers in
         [0, r) used for every proof (reproducible tests only: fixed blinders reveal the witness to whoever knows them).
-        Needs n >= 8 and an SRS of at least n + 6 powers; the sharded prover has no zero-knowledge mode."""
+        Needs n >= 8 and an SRS of at least n + 6 powers; the sharded prover has no zero-knowledge mode.
+        A prover with next-row custom gate terms takes 14 blinders: b12, b13, b14 give A, B, C a third one, since they
+        are opened at zeta and at zeta w (DESIGN.md section 1).  It needs n >= 16 and an SRS of n + 9 powers."""
         raw = None
         if enable and blinders is not None:
             blinders = [int(b) for b in blinders]
-            if len(blinders) != 11:
-                raise ValueError("zero knowledge takes 11 blinders b1..b11, got %d" % len(blinders))
+            count = 14 if getattr(self, "next_row", False) else 11
+            if len(blinders) != count:
+                raise ValueError("zero knowledge takes %d blinders b1..b%d%s, got %d" % (
+                    count, count, " on a prover with next-row terms" if count == 14 else "", len(blinders)))
             if any(not 0 <= b < CURVE_ORDER for b in blinders):
                 raise ValueError("zero-knowledge blinders must lie in [0, r)")
             raw = b"".join(b.to_bytes(32, "little") for b in blinders)

@@ -10,7 +10,7 @@ from typing import Optional
 from . import _lib
 from .curve import G2, Scalar, _pt_bytes, _pt_from, g2_mul
 from .field import CURVE_ORDER, FIELD_MODULUS, FQ, FQ2
-from .custom_gates import split_terms
+from .custom_gates import is_next_row, split_terms
 from .lookup import check_lookup, check_lookups, padded_table, to_le_rows
 from .poly import Basis, Polynomial, _log2_exact
 from .prover import _as_le_rows
@@ -209,12 +209,15 @@ class Setup:
         ``(q_K, (t1, t2, t3))`` as given to ``Prover.from_arrays``; the key gains [q_K], [t1], [t2], [t3] (the table
         padded to n rows), the identity for a constant-zero column.  ``lookups``: several tables as given to
         ``Prover.from_arrays``; the key gains [q_K], [t1], [t2], [t3], [Q_T], [t4] (the tables concatenated and padded).
-        Not together with ``lookup``."""
+        Not together with ``lookup``.  A custom term may have six exponents (i, j, l, i', j', l') and read the next
+        row; the key then takes ``NextRowProof`` only.  Next-row terms do not combine with lookups (ValueError)."""
         import numpy as np
         if lookup is not None and lookups is not None:
             raise ValueError("pass either lookup= (one table) or lookups= (several tables), not both")
         log_n = _log2_exact(group_order)
         exps, ccols = split_terms(custom, group_order)
+        if (lookup is not None or lookups is not None) and any(is_next_row(e) for e in exps):
+            raise ValueError("lookups do not combine with next-row custom gate terms")
         lk = check_lookup(lookup, group_order) if lookup is not None else None
         lks = check_lookups(lookups, group_order) if lookups is not None else None
 

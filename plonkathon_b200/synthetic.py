@@ -98,6 +98,11 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
 
     ``custom``: exponent triples (i, j, l) of custom gate terms; rows using them are mixed into the chain (see
     ``_custom_row``).  Without it the random draws, and so the circuit, are exactly those of a plain circuit.
+    A term with six exponents (i, j, l, i', j', l') reads the next row: its row takes three operands on its wires and
+    puts a new variable on the next row's L wire, which the next row uses as its first operand (a row whose own output
+    goes on L leaves it unused).  So such rows chain without a copy constraint between them.  QC pins the term's value,
+    computed once every row is placed; the last row of the chain reads whatever row comes next (row 0 when the chain
+    fills the circuit: rows are cyclic).  Not together with lookups.
 
     ``lookup``: a table ``(t1, t2, t3)``; lookup rows are mixed into the chain as one more kind of row (a quarter of
     the rows without custom terms): the wires take a random table row as three new variables, q_K = 1 and every gate
@@ -106,12 +111,14 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
 
     ``lookups``: a list of tables ``[(t1, t2, t3), ...]``; as ``lookup``, but each lookup row picks its table at random
     (one more draw, only with two or more tables: ``lookups=[x]`` builds the circuit of ``lookup=x``)."""
-    from .custom_gates import check_exponents
+    from .custom_gates import check_exponents, is_next_row
     from .lookup import check_lookup, check_lookups
     custom = check_exponents(custom)
     n = 1 << log_n
     if lookup is not None and lookups is not None:
         raise ValueError("pass either lookup= (one table) or lookups= (several tables), not both")
+    if (lookup is not None or lookups is not None) and any(is_next_row(e) for e in custom):
+        raise ValueError("lookups do not combine with next-row custom gate terms")
     tables = []  # (columns, rows) per table
     if lookup is not None:
         tables = [check_lookup(([0] * n, lookup), n)[1:]]
@@ -146,6 +153,8 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
     window = 64
     row = n_public
     first = True
+    carry = None     # the variable a next-row row put on this row's L wire
+    pinned = []      # (row, term) of every next-row row, whose QC is set at the end
     while row < m:
         nv = len(values)
         lo = max(0, nv - window)
@@ -154,6 +163,8 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
         if first:  # make sure the private seeds are used so every variable appears in some cell
             ia, ib = n_public, n_public + 1
             first = False
+        if carry is not None:
+            ia, carry = carry, None
         kind = rng.randrange(3 + len(custom) + bool(tables))
         out = nv
         if tables and kind == 3 + len(custom):  # (a, b, c) = a row of table t, q_t = 1
@@ -163,6 +174,15 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
             values.extend(table[w][r] for w in range(3))
             wL[row], wR[row], wO[row] = nv, nv + 1, nv + 2
             QKs[t][row] = 1
+        elif kind >= 3 and is_next_row(custom[kind - 3]):  # the term over (a, b, c) and the next row's wires
+            ic = rng.randrange(lo, nv)
+            k = rng.randrange(0, 1 << 30)
+            wL[row], wR[row], wO[row] = ia, ib, ic
+            QK[kind - 3][row] = 1
+            pinned.append((row, kind - 3))
+            if row + 1 < m:
+                values.append((values[ia] + k) % R)
+                carry = out
         elif kind >= 3:
             ic = rng.randrange(lo, nv)
             k = rng.randrange(0, 1 << 30)
@@ -188,6 +208,16 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
             if with_text:
                 text.append("%s <== %s + %d" % (name(out), name(ia), k))
         row += 1
+    if pinned:
+        from .custom_gates import padded
+        cell = lambda ids, r: values[ids[r]] if ids[r] >= 0 else 0  # noqa: E731
+        for r, t in pinned:
+            r1 = (r + 1) % n
+            ws = [cell(w, r) for w in (wL, wR, wO)] + [cell(w, r1) for w in (wL, wR, wO)]
+            mon = 1
+            for x, e in zip(ws, padded(custom[t])):
+                mon = mon * pow(x, e, R) % R
+            QC[r] = (R - mon) % R
     lk = (QKs[0], tuple(tables[0][0])) if lookup is not None else ()
     lks = tuple((q, tuple(t)) for q, (t, _) in zip(QKs, tables)) if lookups is not None else ()
     return ArrayCircuit(n, m, wL, wR, wO, QL, QR, QM, QO, QC, n_public, values, text, list(zip(custom, QK)), lk, lks)
@@ -200,7 +230,7 @@ def _custom_row(exps, Q, row, operands, k, values, wires, sel):
       * l > 0, i == 0:   a <== b^j c^l + k        (Q = -1, QL = 1, QC = -k), e.g. a = c^3 + k;
       * i, l > 0:        a^i b^j c^l == its value (Q = 1, QC = -value), e.g. the three-wire constraint a b c = k.
     A wire outside the term and the output carries an operand with a zero selector."""
-    i, j, l = exps
+    i, j, l = exps[:3]  # a six-exponent term here has no next-row exponent
     wL, wR, wO = wires
     QL, QO, QC = sel
     ia, ib, ic = operands
@@ -219,6 +249,50 @@ def _custom_row(exps, Q, row, operands, k, values, wires, sel):
         wL[row], wR[row], wO[row] = ia, ib, ic
         Q[row], QC[row] = 1, (R - prod) % R
         values.append(prod)  # keeps one new variable per row (unused by any cell)
+
+
+# the running-sum gate over the next row: bit = a(wX) - 2a and bit (bit - 1) = 0, i.e.
+# a'^2 - 4 a a' + 4 a^2 - a' + 2 a = 0  (four custom terms and QL = 2)
+RUNNING_SUM_TERMS = ((0, 0, 0, 2, 0, 0), (1, 0, 0, 1, 0, 0), (2, 0, 0, 0, 0, 0), (0, 0, 0, 1, 0, 0))
+
+
+def range_check_circuit(log_n: int, n_values: int, bits: int = 16, seed: int = 1) -> ArrayCircuit:
+    """``n_values`` random values below 2^bits, each range-checked by the running sum over the next row: bits + 1 rows
+    per value holding acc_0 = 0, acc_1, ..., acc_bits = the value on the L wire, acc_k+1 = 2 acc_k + (bit k from the
+    top), and the running-sum gate (RUNNING_SUM_TERMS) on the first ``bits`` of them.  The value's row carries it on
+    all three wires (copies), where later gates would read it.  Row 0 holds the constant 0 (QL a = 0) and every acc_0
+    is a copy of it; row 1 holds the constant 1 on all three wires (a + b + a b + c = 4), so that no selector column is
+    zero.  The rest of the circuit is unused rows."""
+    n = 1 << log_n
+    m = 2 + n_values * (bits + 1)
+    if m > n:
+        raise ValueError("%d values of %d bits need %d rows, the circuit has %d" % (n_values, bits, m, n))
+    rng = random.Random(seed)
+    wL = np.full(n, -1, dtype=np.int64)
+    wR = np.full(n, -1, dtype=np.int64)
+    wO = np.full(n, -1, dtype=np.int64)
+    QL, QR, QM, QO, QC = ([0] * n for _ in range(5))
+    Q = [[0] * n for _ in RUNNING_SUM_TERMS]
+    values = [0, 1]
+    wL[0], QL[0] = 0, 1
+    wL[1] = wR[1] = wO[1] = 1
+    QL[1], QR[1], QM[1], QO[1], QC[1] = 1, 1, 1, 1, R - 4
+    weights = (1, R - 4, 4, R - 1)  # a'^2, a a', a^2, a'
+    row = 2
+    for _ in range(n_values):
+        x = rng.randrange(1 << bits)
+        acc = 0
+        wL[row] = 0
+        for k in range(bits):
+            for q, wgt in zip(Q, weights):
+                q[row + k] = wgt
+            QL[row + k] = 2
+            acc = 2 * acc + ((x >> (bits - 1 - k)) & 1)
+            values.append(acc)
+            wL[row + k + 1] = len(values) - 1
+        wR[row + bits] = wO[row + bits] = wL[row + bits]  # the value on all three wires of its row: B, C are not zero
+        row += bits + 1
+    return ArrayCircuit(n, m, wL, wR, wO, QL, QR, QM, QO, QC, 0, values, [], list(zip(RUNNING_SUM_TERMS, Q)))
 
 
 def circuit_arrays(c: ArrayCircuit):

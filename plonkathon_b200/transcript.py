@@ -32,9 +32,16 @@ LOOKUP_SCHEDULE = {
     "5": (("W_z_1", "W_zw_1"), "point", ("u",)),
 }
 
+# The same table for a proof with next-row custom gate terms (plonkathon_b200/custom_gates.py): round 4 also absorbs the
+# wires at zeta w, after z_shifted_eval and before v is drawn.
+NEXT_ROW_SCHEDULE = dict(SCHEDULE)
+NEXT_ROW_SCHEDULE[4] = (SCHEDULE[4][0] + ("a_shifted_eval", "b_shifted_eval", "c_shifted_eval"), "scalar", ("v",))
+
 # Message1 .. Message5: plain records with exactly the reference's field names and order
 Message1, Message2, Message3, Message4, Message5 = (
     make_dataclass("Message%d" % rnd, [(name, object) for name in SCHEDULE[rnd][0]]) for rnd in sorted(SCHEDULE))
+# round 4 of a next-row prover: Message4's fields, then the three shifted wire evaluations
+NextRowMessage4 = make_dataclass("NextRowMessage4", [(name, object) for name in NEXT_ROW_SCHEDULE[4][0]])
 
 
 def _as_int(x) -> int:
@@ -82,8 +89,8 @@ class Transcript:
         return Scalar(int.from_bytes(out.raw, "little"))
 
     # ---- transcript.py:77-123
-    def _round(self, rnd: int, message):
-        fields, kind, challenges = SCHEDULE[rnd]
+    def _round(self, rnd: int, message, schedule: dict = SCHEDULE):
+        fields, kind, challenges = schedule[rnd]
         absorb = self.append_point if kind == "point" else self.append_scalar
         for name in fields:
             absorb(name.encode(), getattr(message, name))
@@ -111,7 +118,8 @@ class Transcript:
         return self._round(3, message)
 
     def round_4(self, message):
-        return self._round(4, message)
+        """a ``NextRowMessage4`` follows NEXT_ROW_SCHEDULE"""
+        return self._round(4, message, NEXT_ROW_SCHEDULE if isinstance(message, NextRowMessage4) else SCHEDULE)
 
     def round_5(self, message):
         return self._round(5, message)

@@ -14,9 +14,9 @@ from dataclasses import dataclass
 
 from .curve import G1, G2, Scalar, ec_lincomb, g1_neg, g2_add, g2_mul, pairing_product_is_one
 from . import _lib
-from .custom_gates import monomial
+from .custom_gates import is_next_row, monomial
 from .field import CURVE_ORDER, FIELD_MODULUS
-from .transcript import LOOKUP_SCHEDULE, SCHEDULE, Transcript
+from .transcript import LOOKUP_SCHEDULE, NEXT_ROW_SCHEDULE, SCHEDULE, Transcript
 
 
 def _lagrange_terms_at(group_order: int, values, x: Scalar) -> Scalar:
@@ -46,15 +46,21 @@ class VerificationKey:
     S3: object
     X_2: object
     w: Scalar
-    # custom gate terms ((i, j, l), commitment to Q_k), in the prover's order (plonkathon_b200/custom_gates.py)
+    # custom gate terms ((i, j, l) or (i, j, l, i', j', l'), commitment to Q_k), in the prover's order
+    # (plonkathon_b200/custom_gates.py); with a next-row term the key takes NextRowProof only
     custom: tuple = ()
     # lookup argument (plonkathon_b200/lookup.py): ([q_K], [t1], [t2], [t3]) for one table, ([q_K], [t1], [t2], [t3],
     # [Q_T], [t4]) for several tables told apart by a tag; the identity (None) for a zero column; () without lookups
     lookup: tuple = ()
 
-    def _custom_terms(self, a, b, c):
-        """the custom gates' part of the linearisation: sum_k m_k(a, b, c) [Q_k]"""
-        return [(pt, monomial(e, a, b, c)) for e, pt in self.custom]
+    def _custom_terms(self, a, b, c, aw=None, bw=None, cw=None):
+        """the custom gates' part of the linearisation: sum_k m_k(a, b, c, a(zeta w), b(zeta w), c(zeta w)) [Q_k]"""
+        return [(pt, monomial(e, a, b, c, aw, bw, cw)) for e, pt in self.custom]
+
+    @property
+    def next_row(self) -> bool:
+        """whether some custom term reads the next row"""
+        return any(is_next_row(e) for e, _ in self.custom)
 
     @staticmethod
     def _well_formed(pf) -> bool:
@@ -70,9 +76,9 @@ class VerificationKey:
         return True
 
     def _matches(self, pf) -> bool:
-        """a lookup key takes lookup proofs only, a plain key plain proofs only"""
-        from .prover import LookupProof
-        return bool(self.lookup) == isinstance(pf, LookupProof)
+        """a lookup key takes lookup proofs only, a next-row key next-row proofs only, a plain key plain proofs only"""
+        from .prover import LookupProof, NextRowProof
+        return bool(self.lookup) == isinstance(pf, LookupProof) and self.next_row == isinstance(pf, NextRowProof)
 
     def verify_proof(self, group_order: int, pf, public=[]) -> bool:
         """verifier.py:40-73: the batched form -- one pairing equation, the linearisation commitment never
@@ -99,13 +105,16 @@ class VerificationKey:
     def _verify(self, group_order: int, pf, public, batched: bool) -> bool:
         n = group_order
         proof = pf.flatten()
-        ch = Transcript(b"plonk").replay(LOOKUP_SCHEDULE if self.lookup else SCHEDULE, proof)
+        schedule = LOOKUP_SCHEDULE if self.lookup else NEXT_ROW_SCHEDULE if self.next_row else SCHEDULE
+        ch = Transcript(b"plonk").replay(schedule, proof)
         beta, gamma, alpha, zeta, v, u = ch["beta"], ch["gamma"], ch["alpha"], ch["zeta"], ch["v"], ch["u"]
         zh_ev = zeta ** n - 1
         l0_ev = zh_ev / ((zeta - 1) * n)
         pi_ev = _lagrange_terms_at(n, [-int(x) % CURVE_ORDER for x in public], zeta)
         a, b, c = proof["a_eval"], proof["b_eval"], proof["c_eval"]
         s1, s2, zw = proof["s1_eval"], proof["s2_eval"], proof["z_shifted_eval"]
+        # the wires at zeta w (next-row keys only)
+        aw, bw, cw = (proof.get(k) for k in ("a_shifted_eval", "b_shifted_eval", "c_shifted_eval"))
         root = Scalar.root_of_unity(n)
         zeta_n = zeta ** n
         a2 = alpha * alpha
@@ -113,7 +122,7 @@ class VerificationKey:
         sigma_bar = (a + beta * s1 + gamma) * (b + beta * s2 + gamma) * zw
         # the linearisation R without its constant, and the constant r0 (R(zeta) == 0)
         r_terms = [
-            (self.Qm, a * b), (self.Ql, a), (self.Qr, b), (self.Qo, c), (self.Qc, 1), *self._custom_terms(a, b, c),
+            (self.Qm, a * b), (self.Ql, a), (self.Qr, b), (self.Qo, c), (self.Qc, 1), *self._custom_terms(a, b, c, aw, bw, cw),
             (proof["z_1"], (a + beta * zeta + gamma) * (b + beta * 2 * zeta + gamma) * (c + beta * 3 * zeta + gamma)
              * alpha + l0_ev * a2),
             (self.S3, -sigma_bar * alpha * beta),
@@ -125,6 +134,9 @@ class VerificationKey:
         e_zeta = v * a + v2 * b + v3 * c + v4 * s1 + v5 * s2
         at_zw = [(proof["z_1"], Scalar(1))]
         e_zw = zw
+        if self.next_row:  # A, B, C join Z at zeta w: v (A - a(zeta w)) + v^2 (B - b(zeta w)) + v^3 (C - c(zeta w))
+            at_zw += [(proof["a_1"], v), (proof["b_1"], v2), (proof["c_1"], v3)]
+            e_zw = e_zw + v * aw + v2 * bw + v3 * cw
         if self.lookup:
             eta, delta, eps = ch["eta"], ch["delta"], ch["epsilon"]
             fe, te, tw = proof["f_eval"], proof["t_eval"], proof["t_shifted_eval"]
