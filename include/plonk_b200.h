@@ -229,6 +229,31 @@ int pb200_prover_prove_next_row(pb200_prover* p, const uint8_t* h_A, const uint8
                                 const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof864);
 int pb200_prover_serialize_next_row(pb200_prover* p, uint8_t* h_proof864);
 
+/* Shuffle argument: two fixed boolean selectors q_in, q_out (n x 32-byte canonical Fr, 0 or 1 on every row, as many
+ * ones in each) claim that the multiset {(a_i, b_i, c_i) : q_in[i] = 1} equals {(a_i, b_i, c_i) : q_out[i] = 1}, with
+ * no copy constraint between the two sides.  Set once, before the first proof.  Round 1 is unchanged; the transcript
+ * then draws theta and kappa after beta and gamma, round 2 commits the grand product Z3 beside Z, round 4 adds
+ * q_in(zeta) and Z3(zeta w).  A proof has 896 bytes: the 768 plain bytes, then z3_1, qin_eval, z3_shifted_eval; on a
+ * next-row prover 992 bytes, with a, b, c at zeta w before z3_1.  A witness whose two sides differ fails round 2 with
+ * "AssertionError: shuffle: the q_in rows and the q_out rows are not permutations of each other".
+ * Errors, the prover left as it was: the sharded prover, a lookup table, zero-knowledge mode, selectors already set,
+ * a selector value other than 0 / 1, unequal numbers of ones.  On a shuffle prover pb200_prover_set_lookup(_tagged)
+ * and pb200_prover_set_zk(p, 1, ...) are errors, and so are every prove / serialize / round 4 entry point of another
+ * proof size and the plain pb200_prover_round2.  Rounds 1, 3 and 5 are the plain entry points. */
+int pb200_prover_set_shuffle(pb200_prover* p, const uint8_t* h_qin, const uint8_t* h_qout);
+/* round 2 of a shuffle prover: z_1 then z3_1 */
+int pb200_prover_round2_shuffle(pb200_prover* p, const uint8_t* beta, const uint8_t* gamma, const uint8_t* theta,
+                                const uint8_t* kappa, uint8_t* h_zz3_xy /*2*64*/);
+/* round 4: the 6 plain evaluations, then qin_eval, z3_shifted_eval; the next-row form puts a, b, c at zeta w between */
+int pb200_prover_round4_shuffle(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals /*8*32*/);
+int pb200_prover_round4_next_row_shuffle(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals /*11*32*/);
+int pb200_prover_prove_shuffle(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
+                               const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof896);
+int pb200_prover_serialize_shuffle(pb200_prover* p, uint8_t* h_proof896);
+int pb200_prover_prove_next_row_shuffle(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
+                                        const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof992);
+int pb200_prover_serialize_next_row_shuffle(pb200_prover* p, uint8_t* h_proof992);
+
 /* ---- multi-GPU: one process per GPU, one communicator per context (SURVEY.md 8(e)) -------------------------
  * The library issues its data-path collectives itself, on the context's stream, through NCCL (bound at run time
  * from the libnccl.so.2 the process has loaded; the single-GPU entry points work without it).  Rendezvous stays

@@ -8,4 +8,4 @@ from .setup import Setup  # noqa: F401
 from .verifier import VerificationKey  # noqa: F401
 from ._lib import Context, PlonkB200Error, default_context  # noqa: F401
 from .transcript import Transcript, Message1, Message2, Message3, Message4, Message5  # noqa: F401
-from .prover import Prover, Proof, LookupProof, NextRowProof  # noqa: F401
+from .prover import Prover, Proof, LookupProof, NextRowProof, ShuffleProof, NextRowShuffleProof  # noqa: F401

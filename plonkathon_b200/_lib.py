@@ -95,6 +95,14 @@ def _load():
         "pb200_prover_round4_next_row": (I, [V, V, V]),
         "pb200_prover_prove_next_row": (I, [V, V, V, V, V, U64, V]),
         "pb200_prover_serialize_next_row": (I, [V, V]),
+        "pb200_prover_set_shuffle": (I, [V, V, V]),
+        "pb200_prover_round2_shuffle": (I, [V, V, V, V, V, V]),
+        "pb200_prover_round4_shuffle": (I, [V, V, V]),
+        "pb200_prover_round4_next_row_shuffle": (I, [V, V, V]),
+        "pb200_prover_prove_shuffle": (I, [V, V, V, V, V, U64, V]),
+        "pb200_prover_serialize_shuffle": (I, [V, V]),
+        "pb200_prover_prove_next_row_shuffle": (I, [V, V, V, V, V, U64, V]),
+        "pb200_prover_serialize_next_row_shuffle": (I, [V, V]),
         "pb200_g1_combine_partials_host": (I, [V, U, V, P(I)]),
         "pb200_transcript_create": (I, [V, ctypes.c_size_t, P(V)]),
         "pb200_transcript_destroy": (None, [V]),

@@ -59,6 +59,8 @@ void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* h_qtag, co
 void prover_round_lookup(Prover* P, const Fr& eta_c);
 void prover_round2_lookup(Prover* P, const Fr& beta_c, const Fr& gamma_c, const Fr& delta_c, const Fr& epsilon_c);
 void prover_round4_lookup(Prover* P, const Fr& zeta_c);
+void prover_set_shuffle(Prover* P, const uint8_t* h_qin, const uint8_t* h_qout);
+void prover_round2_shuffle(Prover* P, const Fr& beta_c, const Fr& gamma_c, const Fr& theta_c, const Fr& kappa_c);
 void g1_combine_partials_host(const G1XYZZ* parts, uint32_t count, uint8_t* out_xy, int* is_identity);
 void host_join_bucket_shards(const SR* all, uint32_t world, uint32_t sets, uint32_t nloc, G1XYZZ* out);
 void host_join_bucket_shards_strided(const SR* all, uint32_t world, uint32_t sets, G1XYZZ* out);
@@ -89,6 +91,9 @@ static Context* C(pb200_ctx* c) { return reinterpret_cast<Context*>(c); }
 // the 768-byte entry points (and the plain round 4) on a prover with next-row custom gate terms
 #define PB_NOT_NEXT_ROW(P, entry)                                                                     \
   PB_CHECK(!(P)->next_row, "this prover has next-row custom gate terms: its proofs have 864 bytes; use " entry)
+// the entry points without a shuffle (and the plain round 2 / round 4) on a prover with a shuffle
+#define PB_NOT_SHUFFLE(P, entry)                                                                      \
+  PB_CHECK(!(P)->sh, "this prover has a shuffle: its proofs have 896 bytes (992 with next-row terms); use " entry)
 
 // Every entry point that touches the GPU runs on its context's device, whatever device the calling host thread had
 // current (contexts on several GPUs in one process, provers driven from worker threads); the previous device is
@@ -464,6 +469,7 @@ int pb200_prover_prove(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, 
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   PB_NOT_LOOKUP(reinterpret_cast<Prover*>(p), "pb200_prover_prove_lookup");
   PB_NOT_NEXT_ROW(reinterpret_cast<Prover*>(p), "pb200_prover_prove_next_row");
+  PB_NOT_SHUFFLE(reinterpret_cast<Prover*>(p), "pb200_prover_prove_shuffle");
   prover_prove(reinterpret_cast<Prover*>(p), h_A, h_B, h_C, h_public, n_public, h_proof768, false);
   PB_API_END
 }
@@ -472,6 +478,7 @@ int pb200_prover_prove_device(pb200_prover* p, const void* d_A, const void* d_B,
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   PB_NOT_LOOKUP(reinterpret_cast<Prover*>(p), "pb200_prover_prove_lookup (wires in host memory)");
   PB_NOT_NEXT_ROW(reinterpret_cast<Prover*>(p), "pb200_prover_prove_next_row (wires in host memory)");
+  PB_NOT_SHUFFLE(reinterpret_cast<Prover*>(p), "pb200_prover_prove_shuffle (wires in host memory)");
   prover_prove(reinterpret_cast<Prover*>(p), (const uint8_t*)d_A, (const uint8_t*)d_B, (const uint8_t*)d_C, h_public,
                n_public, h_proof768, true);
   PB_API_END
@@ -488,6 +495,7 @@ int pb200_prover_round2(pb200_prover* p, const uint8_t* beta, const uint8_t* gam
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   Prover* P = reinterpret_cast<Prover*>(p);
   PB_NOT_LOOKUP(P, "pb200_prover_round2_lookup");
+  PB_NOT_SHUFFLE(P, "pb200_prover_round2_shuffle");
   prover_round2(P, load_fr_canonical(beta), load_fr_canonical(gamma));
   memcpy(h_z_xy, P->proof.pts[3], 64);
   PB_API_END
@@ -504,6 +512,7 @@ int pb200_prover_round4(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals) 
   Prover* P = reinterpret_cast<Prover*>(p);
   PB_NOT_LOOKUP(P, "pb200_prover_round4_lookup");
   PB_NOT_NEXT_ROW(P, "pb200_prover_round4_next_row");
+  PB_NOT_SHUFFLE(P, "pb200_prover_round4_shuffle");
   prover_round4(P, load_fr_canonical(zeta));
   memcpy(h_evals, P->proof.evals[0], 6 * 32);
   PB_API_END
@@ -548,6 +557,7 @@ int pb200_prover_serialize(pb200_prover* p, uint8_t* h_proof768) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   PB_NOT_LOOKUP(reinterpret_cast<Prover*>(p), "pb200_prover_serialize_lookup");
   PB_NOT_NEXT_ROW(reinterpret_cast<Prover*>(p), "pb200_prover_serialize_next_row");
+  PB_NOT_SHUFFLE(reinterpret_cast<Prover*>(p), "pb200_prover_serialize_shuffle");
   prover_serialize(reinterpret_cast<Prover*>(p), h_proof768);
   PB_API_END
 }
@@ -610,6 +620,7 @@ int pb200_prover_round4_next_row(pb200_prover* p, const uint8_t* zeta, uint8_t* 
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   Prover* P = reinterpret_cast<Prover*>(p);
   PB_CHECK(P->next_row, "this prover has no next-row custom gate terms: use pb200_prover_round4");
+  PB_NOT_SHUFFLE(P, "pb200_prover_round4_next_row_shuffle");
   prover_round4(P, load_fr_canonical(zeta));
   memcpy(h_evals, P->proof.evals[0], 6 * 32);
   memcpy(h_evals + 6 * 32, P->nr_evals[0], 3 * 32);
@@ -620,6 +631,7 @@ int pb200_prover_prove_next_row(pb200_prover* p, const uint8_t* h_A, const uint8
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   Prover* P = reinterpret_cast<Prover*>(p);
   PB_CHECK(P->next_row, "this prover has no next-row custom gate terms: use pb200_prover_prove (768 bytes)");
+  PB_NOT_SHUFFLE(P, "pb200_prover_prove_next_row_shuffle");
   prover_prove(P, h_A, h_B, h_C, h_public, n_public, h_proof864, false);
   PB_API_END
 }
@@ -627,7 +639,79 @@ int pb200_prover_serialize_next_row(pb200_prover* p, uint8_t* h_proof864) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   Prover* P = reinterpret_cast<Prover*>(p);
   PB_CHECK(P->next_row, "this prover has no next-row custom gate terms: use pb200_prover_serialize (768 bytes)");
+  PB_NOT_SHUFFLE(P, "pb200_prover_serialize_next_row_shuffle");
   prover_serialize(P, h_proof864);
+  PB_API_END
+}
+int pb200_prover_set_shuffle(pb200_prover* p, const uint8_t* h_qin, const uint8_t* h_qout) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  prover_set_shuffle(reinterpret_cast<Prover*>(p), h_qin, h_qout);
+  PB_API_END
+}
+int pb200_prover_round2_shuffle(pb200_prover* p, const uint8_t* beta, const uint8_t* gamma, const uint8_t* theta,
+                                const uint8_t* kappa, uint8_t* h_zz3_xy) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  prover_round2_shuffle(P, load_fr_canonical(beta), load_fr_canonical(gamma), load_fr_canonical(theta),
+                        load_fr_canonical(kappa));
+  memcpy(h_zz3_xy, P->proof.pts[3], 64);
+  memcpy(h_zz3_xy + 64, P->sh_pt, 64);
+  PB_API_END
+}
+// a shuffle prover of the kind `next_row`: its entry points of one proof size refuse the other kind
+static void shuffle_kind(const Prover* P, bool next_row, const char* other) {
+  PB_CHECK(P->sh, "this prover has no shuffle (pb200_prover_set_shuffle)");
+  PB_CHECK(P->next_row == next_row, (std::string(next_row ? "this shuffle prover has no next-row custom gate terms: use "
+                                                          : "this shuffle prover has next-row custom gate terms: use ") +
+                                     other).c_str());
+}
+int pb200_prover_round4_shuffle(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  shuffle_kind(P, false, "pb200_prover_round4_next_row_shuffle");
+  prover_round4(P, load_fr_canonical(zeta));
+  memcpy(h_evals, P->proof.evals[0], 6 * 32);
+  memcpy(h_evals + 6 * 32, P->sh_evals[0], 2 * 32);
+  PB_API_END
+}
+int pb200_prover_round4_next_row_shuffle(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  shuffle_kind(P, true, "pb200_prover_round4_shuffle");
+  prover_round4(P, load_fr_canonical(zeta));
+  memcpy(h_evals, P->proof.evals[0], 6 * 32);
+  memcpy(h_evals + 6 * 32, P->nr_evals[0], 3 * 32);
+  memcpy(h_evals + 9 * 32, P->sh_evals[0], 2 * 32);
+  PB_API_END
+}
+int pb200_prover_prove_shuffle(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
+                               const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof896) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  shuffle_kind(P, false, "pb200_prover_prove_next_row_shuffle (992 bytes)");
+  prover_prove(P, h_A, h_B, h_C, h_public, n_public, h_proof896, false);
+  PB_API_END
+}
+int pb200_prover_serialize_shuffle(pb200_prover* p, uint8_t* h_proof896) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  shuffle_kind(P, false, "pb200_prover_serialize_next_row_shuffle (992 bytes)");
+  prover_serialize(P, h_proof896);
+  PB_API_END
+}
+int pb200_prover_prove_next_row_shuffle(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
+                                        const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof992) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  shuffle_kind(P, true, "pb200_prover_prove_shuffle (896 bytes)");
+  prover_prove(P, h_A, h_B, h_C, h_public, n_public, h_proof992, false);
+  PB_API_END
+}
+int pb200_prover_serialize_next_row_shuffle(pb200_prover* p, uint8_t* h_proof992) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  shuffle_kind(P, true, "pb200_prover_serialize_shuffle (896 bytes)");
+  prover_serialize(P, h_proof992);
   PB_API_END
 }
 int pb200_g1_combine_partials_host(const uint8_t* h_xyzz, unsigned count, uint8_t* h_out_xy, int* is_identity) {

@@ -19,6 +19,8 @@
 // (prover.py:108-116), Z_n == 1 (prover.py:132), deg T < 3n (prover.py:205-208).
 // Zero-knowledge mode (prover_set_zk, one GPU) blinds A, B, C, Z and the quotient pieces as in the PLONK paper; the
 // proof keeps its 15 fields and the verifier does not change.  See "zero knowledge" below.
+// A shuffle (Prover::sh, one GPU) proves that two sets of rows hold the same multiset of (a, b, c): one more grand
+// product Z3 beside Z, see "shuffle" below; the proof gains z3_1 and two evaluations (896 bytes, 992 next-row).
 // Custom terms over the next row (Prover::next_row, one GPU) read a(wX), b(wX), c(wX): k_gate_check<true> and
 // k_quotient<ZK, true> read index + 1 (mod n) and coset index + 4, round 4 adds A, B, C at zeta w and round 5 opens them
 // there with Z; the proof gains those three evaluations (864 bytes).
@@ -460,7 +462,9 @@ __global__ void __launch_bounds__(128) k_horner_strided(EvalArgs a, Fr* H) {
 // 26 slots: round 5's largest batch is 19 plain terms (5 gate selectors, 4 custom, Z, S3, T1-T3, A, B, C, S1, S2) and
 // 7 lookup terms (q_K, Q_T with a table tag, Z2, H1, F, T, H2).
 struct LinCombArgs { const Fr* vec[26]; Fr w[26]; Fr c0; int count; uint64_t n, first; };
+// A shuffle adds 3 (Q_out, Z3, Q_in) to the 19 plain terms: 22.
 static_assert(5 + PB_MAX_CUSTOM + 10 + 7 <= 26, "round 5's largest batch must fit LinCombArgs");
+static_assert(5 + PB_MAX_CUSTOM + 10 + 3 <= 26, "round 5's batch with a shuffle must fit LinCombArgs");
 __global__ void __launch_bounds__(128) k_lincomb(LinCombArgs a, Fr* out) {
   uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= a.n) return;
@@ -650,6 +654,42 @@ __global__ void __launch_bounds__(128) k_quotient_lookup(LookupQuotientArgs q, F
                  fp_add(fp_add(q.eps_one_d, h2), fp_mul(q.delta, quad(ldg_fr(q.H1 + jw), 7))));
   acc = fp_add(acc, fp_mul(q.alpha4, fp_sub(p1, p2)));
   acc = fp_add(acc, fp_mul(q.alpha5, fp_mul(fp_sub(z2, q.one), ldg_fr(q.L0 + j))));
+  out[j] = fp_add(out[j], fp_mul(acc, q.zh_inv[j & 3]));
+}
+
+// ---- shuffle ------------------------------------------------------------------------------------------------------
+// per-row numerator / denominator of Z3: with w = a + theta b + theta^2 c, num = 1 + q_in (kappa + w - 1) and
+// den = 1 + q_out (kappa + w - 1).  The selectors are 0 or 1 on the rows, so each is 1 or kappa + w.
+struct ShuffleChallenges { Fr theta, theta2, kappa; };
+__global__ void k_shuffle_terms(const Fr* A, const Fr* B, const Fr* C, const Fr* QIN, const Fr* QOUT,
+                                ShuffleChallenges ch, uint64_t n, Fr* num, Fr* den) {
+  uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const Fr t = fp_add(ch.kappa, fp_add(ldg_fr(A + i), fp_add(fp_mul(ch.theta, ldg_fr(B + i)),
+                                                              fp_mul(ch.theta2, ldg_fr(C + i)))));
+  num[i] = ldg_fr(QIN + i).is_zero() ? Fr::one() : t;
+  den[i] = ldg_fr(QOUT + i).is_zero() ? Fr::one() : t;
+}
+
+// the two shuffle terms of the quotient, added to the plain quotient's evaluations on the 4n coset (one GPU):
+//   a3 [Z3(wX) (1 + Q_out (K + W - 1)) - Z3 (1 + Q_in (K + W - 1))] + a4 L0 (Z3 - 1),   over Z_H,
+// W = A + theta B + theta^2 C.  X -> wX is index + 4 on the coset, as for Z.
+struct ShuffleQuotientArgs {
+  const Fr *A, *B, *C, *QIN, *QOUT, *Z3, *L0;
+  Fr zh_inv[4];
+  Fr theta, theta2, kappa_m1, alpha3, alpha4, one;
+  uint64_t n4;
+};
+__global__ void __launch_bounds__(128) k_quotient_shuffle(ShuffleQuotientArgs q, Fr* out) {
+  uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= q.n4) return;
+  const uint64_t jw = j + 4 >= q.n4 ? j + 4 - q.n4 : j + 4;
+  const Fr k = fp_add(q.kappa_m1, fp_add(ldg_fr(q.A + j), fp_add(fp_mul(q.theta, ldg_fr(q.B + j)),
+                                                                   fp_mul(q.theta2, ldg_fr(q.C + j)))));
+  const Fr z3 = ldg_fr(q.Z3 + j);
+  Fr acc = fp_sub(fp_mul(ldg_fr(q.Z3 + jw), fp_add(q.one, fp_mul(ldg_fr(q.QOUT + j), k))),
+                  fp_mul(z3, fp_add(q.one, fp_mul(ldg_fr(q.QIN + j), k))));
+  acc = fp_add(fp_mul(q.alpha3, acc), fp_mul(q.alpha4, fp_mul(fp_sub(z3, q.one), ldg_fr(q.L0 + j))));
   out[j] = fp_add(out[j], fp_mul(acc, q.zh_inv[j & 3]));
 }
 
@@ -955,6 +995,7 @@ void prover_set_zk(Prover* P, bool enable, const uint8_t* h_blinders) {
     return;
   }
   PB_CHECK(P->world == 1, "zero-knowledge proving is not available on the sharded prover (one GPU only)");
+  PB_CHECK(!P->sh, "zero-knowledge mode does not combine with a shuffle");
   PB_CHECK(!P->lk, "zero-knowledge mode does not combine with lookups here: a lookup prover takes 21 blinders through "
                    "pb200_prover_set_zk_lookup");
   zk_enable(P, h_blinders);
@@ -1028,6 +1069,7 @@ void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* h_qtag, co
   const int width = tagged ? 4 : 3;
   PB_CHECK(P->world == 1, "lookups are not available on the sharded prover (one GPU only)");
   PB_CHECK(!P->next_row, "lookups do not combine with next-row custom gate terms");
+  PB_CHECK(!P->sh, "lookups do not combine with a shuffle");
   PB_CHECK(!P->zk, "lookups do not combine with zero-knowledge mode switched on first: set the table, then "
                    "pb200_prover_set_zk_lookup");
   PB_CHECK(!P->lk, "the lookup table is already set (set it once, before the first proof)");
@@ -1205,6 +1247,74 @@ static void grand_product(Prover* P, Fr* num, const Fr* den, Fr* lag, Fr* coeff,
   PB_CHECK(total == Fr::one(), not_one);
 }
 
+// ---- shuffle ------------------------------------------------------------------------------------------------------
+// Two fixed boolean selectors Q_in and Q_out claim that the multiset {(a_i, b_i, c_i) : q_in[i] = 1} equals the multiset
+// {(a_i, b_i, c_i) : q_out[i] = 1}; no copy constraint joins the two sides.  After beta and gamma the transcript draws
+// theta and kappa (no commitment in between).  With w_i = a_i + theta b_i + theta^2 c_i, Z3 is the grand product of
+// num_i / den_i = (1 + q_in[i](kappa + w_i - 1)) / (1 + q_out[i](kappa + w_i - 1)) (k_shuffle_terms), Z3_n = 1 iff
+// the two products agree.  The quotient gains k_quotient_shuffle's two terms at alpha^3, alpha^4 (degree <= 3n - 3, so T
+// keeps three pieces); round 4 evaluates Q_in at zeta and Z3 at zeta w; round 5 keeps [Q_out] and [Z3] in the
+// linearisation, opens Q_in at zeta (v^6) and Z3 at zeta w (v, or v^4 after A, B, C on a next-row prover).  A row with
+// both selectors cancels out.  Not with lookups (their alpha^3..alpha^5 terms), zero knowledge or the sharded prover.
+
+// h_qin, h_qout: n x 32 bytes canonical, 0 or 1 on every row, with as many ones in each.  Every check comes before any
+// change, so a refused call leaves the prover as it was.
+void prover_set_shuffle(Prover* P, const uint8_t* h_qin, const uint8_t* h_qout) {
+  Context* ctx = P->ctx;
+  const uint64_t n = P->n;
+  PB_CHECK(P->world == 1, "shuffles are not available on the sharded prover (one GPU only)");
+  PB_CHECK(!P->lk, "shuffles do not combine with lookups");
+  PB_CHECK(!P->zk, "shuffles do not combine with zero-knowledge mode");
+  PB_CHECK(!P->sh, "the shuffle selectors are already set (set them once, before the first proof)");
+  PB_CHECK(h_qin && h_qout, "a shuffle needs q_in and q_out");
+  uint64_t ones[2] = {0, 0};
+  const uint8_t* sel[2] = {h_qin, h_qout};
+  for (int s = 0; s < 2; s++)
+    for (uint64_t i = 0; i < n; i++) {
+      const uint8_t* e = sel[s] + 32 * i;
+      bool ok = e[0] <= 1;
+      for (int k = 1; k < 32 && ok; k++) ok = e[k] == 0;
+      PB_CHECK(ok, s ? "q_out must be 0 or 1 on every row" : "q_in must be 0 or 1 on every row");
+      ones[s] += e[0];
+    }
+  PB_CHECK(ones[0] == ones[1], ("a shuffle needs as many q_in rows as q_out rows: " + std::to_string(ones[0]) +
+                                " and " + std::to_string(ones[1])).c_str());
+  cudaStream_t st = ctx->stream;
+  for (int s = 0; s < 2; s++) {  // as q_K: Lagrange values (round 2), coefficients (rounds 4, 5), the 4n coset (round 3)
+    upload_mont(ctx, P->sh_lag[s], sel[s], n);
+    P->sh_coeff[s].alloc(n * 32);
+    ntt_run(ctx, P->sh_lag[s].as<Fr>(), P->sh_coeff[s].as<Fr>(), P->log_n, true, n, nullptr, nullptr);
+    P->sh_ext[s].alloc(P->n_ext * 32);
+    coset_extend(P, st, nullptr, P->sh_coeff[s].as<Fr>(), P->sh_ext[s].as<Fr>(), P->gpow.as<Fr>());
+  }
+  P->sh_z3_lag.alloc(n * 32);
+  P->sh_z3_coeff.alloc(n * 32);
+  P->sh_z3_ext.alloc(P->n_ext * 32);
+  PB_CUDA(cudaStreamSynchronize(st));  // the caller's host buffers may die after the call
+  P->sh = true;
+}
+
+// round 2 of a shuffle proof, after Z: the grand product Z3, then one commitment pass over Z and Z3
+static void shuffle_round2(Prover* P) {
+  Context* ctx = P->ctx;
+  const uint64_t n = P->n;
+  cudaStream_t st = ctx->stream;
+  ShuffleChallenges ch{P->theta, fp_sqr(P->theta), P->kappa};
+  Fr* num = P->tmp[2].as<Fr>();
+  Fr* den = P->tmp[3].as<Fr>();
+  k_shuffle_terms<<<PB_GRID(n, 128), 0, st>>>(P->lag[0].as<Fr>(), P->lag[1].as<Fr>(), P->lag[2].as<Fr>(),
+                                             P->sh_lag[Prover::SH_IN].as<Fr>(), P->sh_lag[Prover::SH_OUT].as<Fr>(), ch,
+                                             n, num, den);
+  ctx->launches++;
+  grand_product(P, num, den, P->sh_z3_lag.as<Fr>(), P->sh_z3_coeff.as<Fr>(),
+                "AssertionError: shuffle: the q_in rows and the q_out rows are not permutations of each other");
+  const Fr* zz[2] = {P->coeff[3].as<Fr>(), P->sh_z3_coeff.as<Fr>()};
+  uint8_t out[2][64];
+  P->commit_batch(zz, 2, n, out[0]);
+  memcpy(P->proof.pts[3], out[0], 64);
+  memcpy(P->sh_pt, out[1], 64);
+}
+
 // round 2 of a lookup proof, after Z: the grand product Z2, then one commitment pass over Z and Z2
 static void lookup_round2(Prover* P) {
   Context* ctx = P->ctx;
@@ -1368,6 +1478,10 @@ void prover_round2(Prover* P, const Fr& beta_c, const Fr& gamma_c) {
     lookup_round2(P);
     return;
   }
+  if (P->sh) {  // Z3, and Z with it in one commitment pass
+    shuffle_round2(P);
+    return;
+  }
   if (P->zk) {  // Z': n + 3 coefficients
     const Fr* b = P->zk_b;
     zk_blind(P, P->coeff[3].as<Fr>(), n, zh_multiple({b[8], b[7], b[6]}), P->zk_coeff[3].as<Fr>());
@@ -1375,6 +1489,13 @@ void prover_round2(Prover* P, const Fr& beta_c, const Fr& gamma_c) {
     return;
   }
   P->commit(P->coeff[3].as<Fr>(), n, P->proof.pts[3]);
+}
+
+void prover_round2_shuffle(Prover* P, const Fr& beta_c, const Fr& gamma_c, const Fr& theta_c, const Fr& kappa_c) {
+  PB_CHECK(P->sh, "this prover has no shuffle (pb200_prover_set_shuffle)");
+  P->theta = fp_to_mont(theta_c);
+  P->kappa = fp_to_mont(kappa_c);
+  prover_round2(P, beta_c, gamma_c);
 }
 
 void prover_round2_lookup(Prover* P, const Fr& beta_c, const Fr& gamma_c, const Fr& delta_c, const Fr& epsilon_c) {
@@ -1472,6 +1593,19 @@ void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c) {
     } else {
       k_quotient_lookup<false><<<PB_GRID(ne, 128), 0, st>>>(lq, t_evals, zl);
     }
+    ctx->launches++;
+  }
+  if (P->sh) {  // one GPU: the slice is the whole 4n coset
+    coset_extend(P, st, nullptr, P->sh_z3_coeff.as<Fr>(), P->sh_z3_ext.as<Fr>(), P->gpow.as<Fr>());
+    ShuffleQuotientArgs sq;
+    sq.A = q.A; sq.B = q.B; sq.C = q.C; sq.L0 = q.L0;
+    sq.QIN = P->sh_ext[Prover::SH_IN].as<Fr>(); sq.QOUT = P->sh_ext[Prover::SH_OUT].as<Fr>();
+    sq.Z3 = P->sh_z3_ext.as<Fr>();
+    for (int k = 0; k < 4; k++) sq.zh_inv[k] = P->zh_inv[k];
+    sq.theta = P->theta; sq.theta2 = fp_sqr(P->theta); sq.kappa_m1 = fp_sub(P->kappa, Fr::one());
+    sq.alpha3 = fp_mul(q.alpha2, P->alpha); sq.alpha4 = fp_sqr(q.alpha2); sq.one = Fr::one();
+    sq.n4 = ne;
+    k_quotient_shuffle<<<PB_GRID(ne, 128), 0, st>>>(sq, t_evals);
     ctx->launches++;
   }
   PB_CUDA(cudaMemsetAsync(P->flags.p, 0, 64, st));
@@ -1586,6 +1720,12 @@ void prover_round4(Prover* P, const Fr& zeta_c) {
       e[5] = fp_add(e[5], fp_mul(fp_add(fp_mul(fp_add(fp_mul(b[18], zw), b[19]), zw), b[20]), zh));
     }
     for (int k = 0; k < 6; k++) store_canonical(P->lk_evals[k], P->lk_ev[k]);
+  }
+  if (P->sh) {  // Q_in at zeta, Z3 at zeta w
+    const Fr* spolys[2] = {P->sh_coeff[Prover::SH_IN].as<Fr>(), P->sh_z3_coeff.as<Fr>()};
+    const Fr sxs[2] = {P->zeta, zw};
+    eval_polys(P, 2, spolys, sxs, P->sh_ev);
+    for (int k = 0; k < 2; k++) store_canonical(P->sh_evals[k], P->sh_ev[k]);
   }
 }
 
@@ -1719,6 +1859,19 @@ void prover_round5(Prover* P, const Fr& v_c) {
     lc = fp_sub(lc, fp_mul(al5, l0_ev));
     c0 = fp_add(c0, fp_sub(lc, fp_add(fp_mul(v6, fe), fp_add(fp_mul(v7, te), fp_mul(v8, h2e)))));
   }
+  // shuffle: [Q_out] and [Z3] keep their commitments in the linearisation; Q_in joins the batch at zeta
+  if (P->sh) {
+    const Fr &qin = P->sh_ev[0], &z3w = P->sh_ev[1];
+    const Fr al2 = fp_sqr(al), al3 = fp_mul(al2, al), al4 = fp_sqr(al2), v6 = fp_mul(v5, v);
+    const Fr th = P->theta;
+    const Fr km1 = fp_add(fp_sub(P->kappa, one), fp_add(a, fp_add(fp_mul(th, b), fp_mul(fp_sqr(th), c))));  // k + w - 1
+    const Fr a3z = fp_mul(al3, z3w), a4l0 = fp_mul(al4, l0_ev);
+    add(P->sh_coeff[Prover::SH_OUT].as<Fr>(), fp_mul(a3z, km1));                                    // a3 z3w (k + w - 1)
+    add(P->sh_z3_coeff.as<Fr>(), fp_sub(a4l0, fp_mul(al3, fp_add(one, fp_mul(qin, km1)))));  // -a3 (1 + q_in(..)) + a4 L0
+    add(P->sh_coeff[Prover::SH_IN].as<Fr>(), v6);
+    // a3 z3w - a4 L0(zeta) - v^6 q_in(zeta)
+    c0 = fp_add(c0, fp_sub(a3z, fp_add(a4l0, fp_mul(v6, qin))));
+  }
   L.count = k;
   L.n = n / (uint64_t)P->world;          // one proof across G ranks: every rank builds (and divides) its slab only
   L.first = L.n * (uint64_t)P->rank;
@@ -1755,6 +1908,11 @@ void prover_round5(Prover* P, const Fr& v_c) {
     M.count = 4;
     M.c0 = fp_sub(M.c0, fp_add(fp_mul(v, *aw), fp_add(fp_mul(v2, *bw), fp_mul(v3, *cw))));
   }
+  if (P->sh) {  // + v^k (Z3 - z3(zeta w)): k = 1, or 4 after A, B, C on a next-row prover
+    const Fr vk = P->next_row ? v4 : v;
+    M.vec[M.count] = P->sh_z3_coeff.as<Fr>(); M.w[M.count] = vk; M.count++;
+    M.c0 = fp_sub(M.c0, fp_mul(vk, P->sh_ev[1]));
+  }
   Fr* wzw = P->tmp[0].as<Fr>();  // the W_z numerator is no longer needed
   k_lincomb<<<PB_GRID(M.n, 128), 0, st>>>(M, wzw);
   ctx->launches++;
@@ -1771,7 +1929,7 @@ void prover_round5(Prover* P, const Fr& v_c) {
 // canonical 768-byte proof: Proof.flatten() order (prover.py:18-35), G1 as x||y, every integer 32-byte
 // big-endian exactly as the transcript absorbs it (transcript.py:62-67).  A lookup proof has 1216 bytes: the 768 plain
 // bytes, then f_1 h1_1 h2_1 z2_1, then the six lookup evaluations.  A next-row proof has 864 bytes: the 768 plain bytes,
-// then a(zeta w), b(zeta w), c(zeta w).
+// then a(zeta w), b(zeta w), c(zeta w).  A shuffle appends z3_1, q_in(zeta), Z3(zeta w): 896 bytes, 992 next-row.
 void prover_serialize(const Prover* P, uint8_t* out) {
   auto be = [](uint8_t* dst, const uint8_t* le) { for (int i = 0; i < 32; i++) dst[i] = le[31 - i]; };
   uint8_t* o = out;
@@ -1780,13 +1938,18 @@ void prover_serialize(const Prover* P, uint8_t* out) {
   for (int k = 7; k < 9; k++) { be(o, P->proof.pts[k]); be(o + 32, P->proof.pts[k] + 32); o += 64; }
   if (P->next_row)
     for (int k = 0; k < 3; k++) { be(o, P->nr_evals[k]); o += 32; }
+  if (P->sh) {
+    be(o, P->sh_pt); be(o + 32, P->sh_pt + 32); o += 64;
+    for (int k = 0; k < 2; k++) { be(o, P->sh_evals[k]); o += 32; }
+  }
   if (!P->lk) return;
   for (int k = 0; k < 4; k++) { be(o, P->lk_pts[k]); be(o + 32, P->lk_pts[k] + 32); o += 64; }
   for (int k = 0; k < 6; k++) { be(o, P->lk_evals[k]); o += 32; }
 }
 
 // prover.py:51-84; a prover with a lookup table runs step 1L between rounds 1 and 2 and writes the 1216-byte proof, a
-// next-row prover absorbs three more evaluations in round 4 and writes the 864-byte proof
+// next-row prover absorbs three more evaluations in round 4 and writes the 864-byte proof, a shuffle prover draws theta
+// and kappa after gamma, absorbs z3_1 after z_1 and two more evaluations last in round 4 (896 or 992 bytes)
 void prover_prove(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t* hC, const uint8_t* h_public,
                   uint64_t n_public, uint8_t* out, bool wires_on_device) {
   PB_CUDA(cudaSetDevice(P->ctx->device));  // the calling host thread may not be the one that created the context
@@ -1797,6 +1960,10 @@ void prover_prove(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t
   tr.append_point_le("c_1", P->proof.pts[2]);
   Fr beta = tr.get_and_append_challenge("beta");
   Fr gamma = tr.get_and_append_challenge("gamma");
+  if (P->sh) {  // SHUFFLE_SCHEDULE (transcript.py): no commitment before theta and kappa
+    P->theta = fp_to_mont(tr.get_and_append_challenge("theta"));
+    P->kappa = fp_to_mont(tr.get_and_append_challenge("kappa"));
+  }
   if (P->lk) {
     prover_round_lookup(P, tr.get_and_append_challenge("eta"));
     tr.append_point_le("f_1", P->lk_pts[0]);
@@ -1808,6 +1975,7 @@ void prover_prove(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t
   prover_round2(P, beta, gamma);
   tr.append_point_le("z_1", P->proof.pts[3]);
   if (P->lk) tr.append_point_le("z2_1", P->lk_pts[3]);
+  if (P->sh) tr.append_point_le("z3_1", P->sh_pt);
   Fr alpha = tr.get_and_append_challenge("alpha");
   Fr cof = tr.get_and_append_challenge("fft_cofactor");
   prover_round3(P, alpha, cof);
@@ -1821,6 +1989,10 @@ void prover_prove(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t
   if (P->next_row) {  // NEXT_ROW_SCHEDULE (transcript.py)
     static const char* nr_labels[3] = {"a_shifted_eval", "b_shifted_eval", "c_shifted_eval"};
     for (int k = 0; k < 3; k++) tr.append_scalar_le(nr_labels[k], P->nr_evals[k]);
+  }
+  if (P->sh) {
+    tr.append_scalar_le("qin_eval", P->sh_evals[0]);
+    tr.append_scalar_le("z3_shifted_eval", P->sh_evals[1]);
   }
   if (P->lk) {
     static const char* lk_labels[6] = {"f_eval", "t_eval", "t_shifted_eval", "h2_eval", "h1_shifted_eval",

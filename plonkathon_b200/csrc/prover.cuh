@@ -179,6 +179,19 @@ struct Prover {
   Fr lk_ev[6];                         // f, t, t(zeta w), h2, h1(zeta w), z2(zeta w) at their points (Montgomery)
   uint8_t lk_pts[4][64];               // f_1 h1_1 h2_1 z2_1 (canonical LE x||y)
   uint8_t lk_evals[6][32];             // canonical LE
+  // Shuffle argument (prover_set_shuffle, one GPU): the multiset of (a, b, c) over the rows with q_in = 1 equals the one
+  // over the rows with q_out = 1, see "shuffle" in prover.cu.  The proof gains z3_1, q_in(zeta) and Z3(zeta w) (896
+  // bytes, 992 on a next-row prover).
+  enum { SH_IN = 0, SH_OUT };
+  bool sh = false;
+  DevBuf sh_lag[2];                    // Q_in Q_out: Lagrange values (Montgomery 0 / 1) ...
+  DevBuf sh_coeff[2];                  // ... coefficients ...
+  DevBuf sh_ext[2];                    // ... on the 4n coset
+  DevBuf sh_z3_lag, sh_z3_coeff, sh_z3_ext;  // Z3: Lagrange values, coefficients, on the 4n coset
+  Fr theta, kappa;                     // Montgomery
+  Fr sh_ev[2];                         // q_in(zeta), Z3(zeta w) (Montgomery)
+  uint8_t sh_pt[64];                   // z3_1 (canonical LE x||y)
+  uint8_t sh_evals[2][32];             // canonical LE
   Proof proof;
 
   enum { QM = 0, QL, QR, QO, QC, S1, S2, S3, CUSTOM0 };

@@ -123,9 +123,12 @@ class ShardedProver(Prover):
     _CREATE_CUSTOM = "pb200_prover_create_custom_sharded"
 
     @classmethod
-    def from_arrays(cls, setup, group_order, pk_arrays, group=None, ctx=None, custom=(), lookup=None, lookups=None):
+    def from_arrays(cls, setup, group_order, pk_arrays, group=None, ctx=None, custom=(), lookup=None, lookups=None,
+                    shuffle=None):
         if lookup is not None or lookups is not None:
             raise ValueError("lookups are not available on the sharded prover (one GPU only)")
+        if shuffle is not None:
+            raise ValueError("shuffles are not available on the sharded prover (one GPU only)")
         custom = list(custom)
         if any(is_next_row(e) for e, _ in custom):
             raise ValueError("next-row custom gate terms are not available on the sharded prover (one GPU only)")

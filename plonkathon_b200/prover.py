@@ -20,7 +20,10 @@ from .custom_gates import is_next_row, padded, split_terms
 from .lookup import PROOF_BYTES as LOOKUP_PROOF_BYTES, check_lookup, check_lookups, padded_table, to_le_rows
 from .field import CURVE_ORDER, FIELD_MODULUS, FQ
 from .poly import Basis, _log2_exact, scalars_to_bytes
-from .transcript import Message1, Message2, Message3, Message4, Message5, NextRowMessage4, Transcript
+from .shuffle import NEXT_ROW_PROOF_BYTES as NEXT_ROW_SHUFFLE_PROOF_BYTES, PROOF_BYTES as SHUFFLE_PROOF_BYTES
+from .shuffle import check_shuffle
+from .transcript import (Message1, Message2, Message3, Message4, Message5, NextRowMessage4, NextRowShuffleMessage4,
+                         SHUFFLE_SCHEDULE, ShuffleMessage2, ShuffleMessage4, Transcript)
 
 PK_ORDER = ("QM", "QL", "QR", "QO", "QC", "S1", "S2", "S3")  # compiler/program.py:10-30
 PROOF_FIELDS = ("a_1", "b_1", "c_1", "z_1", "t_lo_1", "t_mid_1", "t_hi_1", "a_eval", "b_eval", "c_eval",
@@ -150,6 +153,66 @@ class NextRowProof:
         return cls(plain, *[Scalar(x) for x in w])
 
 
+SHUFFLE_FIELDS = ("z3_1", "qin_eval", "z3_shifted_eval")
+
+
+@dataclass
+class ShuffleProof:
+    """A proof of a circuit with a shuffle (plonkathon_b200/shuffle.py): the plain proof's 15 fields, then z3_1, qin_eval
+    and z3_shifted_eval -- 896 bytes, encoded as the plain proof."""
+    plain: Proof
+    z3_1: object
+    qin_eval: Scalar
+    z3_shifted_eval: Scalar
+
+    def flatten(self):
+        out = self.plain.flatten()
+        out.update((k, getattr(self, k)) for k in SHUFFLE_FIELDS)
+        return out
+
+    def to_bytes(self) -> bytes:
+        return _encode(self.flatten().values())
+
+    @classmethod
+    def from_bytes(cls, raw: bytes) -> "ShuffleProof":
+        """Inverse of to_bytes; ValueError for a word that is not reduced (coordinates below q, scalars below r)."""
+        if len(raw) != SHUFFLE_PROOF_BYTES:
+            raise ValueError("a shuffle proof has %d bytes, got %d" % (SHUFFLE_PROOF_BYTES, len(raw)))
+        plain = Proof.from_bytes(raw[:768])
+        w = _decode_words(raw[768:], range(2, 4), first=24)
+        return cls(plain, (FQ(w[0]), FQ(w[1])), Scalar(w[2]), Scalar(w[3]))
+
+
+@dataclass
+class NextRowShuffleProof:
+    """A proof of a circuit with a shuffle and next-row custom gate terms: the plain proof's 15 fields, the wires at
+    zeta w (as in ``NextRowProof``), then z3_1, qin_eval and z3_shifted_eval -- 992 bytes, encoded as the plain proof."""
+    plain: Proof
+    a_shifted_eval: Scalar
+    b_shifted_eval: Scalar
+    c_shifted_eval: Scalar
+    z3_1: object
+    qin_eval: Scalar
+    z3_shifted_eval: Scalar
+
+    def flatten(self):
+        out = self.plain.flatten()
+        out.update((k, getattr(self, k)) for k in NEXT_ROW_FIELDS + SHUFFLE_FIELDS)
+        return out
+
+    def to_bytes(self) -> bytes:
+        return _encode(self.flatten().values())
+
+    @classmethod
+    def from_bytes(cls, raw: bytes) -> "NextRowShuffleProof":
+        """Inverse of to_bytes; ValueError for a word that is not reduced (coordinates below q, scalars below r)."""
+        if len(raw) != NEXT_ROW_SHUFFLE_PROOF_BYTES:
+            raise ValueError("a next-row shuffle proof has %d bytes, got %d" % (NEXT_ROW_SHUFFLE_PROOF_BYTES, len(raw)))
+        plain = Proof.from_bytes(raw[:768])
+        w = _decode_words(raw[768:], (0, 1, 2, 5, 6), first=24)
+        return cls(plain, Scalar(w[0]), Scalar(w[1]), Scalar(w[2]), (FQ(w[3]), FQ(w[4])), Scalar(w[5]), Scalar(w[6]))
+
+
 def _as_le_rows(values, n) -> np.ndarray:
     """list of ints / Scalars, or an (m,32) uint8 / (m,8) uint32 array -> contiguous (n,32) uint8, zero padded."""
     if isinstance(values, np.ndarray):
@@ -189,7 +252,8 @@ class Prover:
         self._create(setup, self.group_order, cols)
 
     @classmethod
-    def from_arrays(cls, setup, group_order: int, pk_arrays: dict, ctx=None, custom=(), lookup=None, lookups=None):
+    def from_arrays(cls, setup, group_order: int, pk_arrays: dict, ctx=None, custom=(), lookup=None, lookups=None,
+                    shuffle=None):
         """pk_arrays: QM QL QR QO QC S1 S2 S3 -> list of ints or (n,32) uint8 little-endian arrays.
         ``ctx``: run this prover on another context (stream + scratch) of the same device than the setup's; the SRS
         is shared read-only, so several provers can be driven concurrently from different host threads.
@@ -202,15 +266,22 @@ class Prover:
         (table k has id k; ``check_lookups``).  The proof is a ``LookupProof`` too.  Not together with ``lookup``.
         A custom term with six exponents ``((i, j, l, i', j', l'), column)`` may read the next row's wires; with one
         such term ``prove_arrays`` returns an 864-byte ``NextRowProof``.  Next-row terms do not combine with lookups
-        (ValueError)."""
+        (ValueError).
+        ``shuffle``: ``(q_in, q_out)``, two boolean selectors with as many ones each: the rows with q_in = 1 hold the
+        same multiset of (a, b, c) as the rows with q_out = 1 (plonkathon_b200/shuffle.py).  ``prove_arrays`` then returns
+        an 896-byte ``ShuffleProof``, or a 992-byte ``NextRowShuffleProof`` with next-row terms.  ValueError for
+        malformed selectors and for a shuffle with lookups; the library refuses it with zero knowledge."""
         if lookup is not None and lookups is not None:
             raise ValueError("pass either lookup= (one table) or lookups= (several tables), not both")
+        if shuffle is not None and (lookup is not None or lookups is not None):
+            raise ValueError("shuffles do not combine with lookups")
         custom = list(custom)
         if (lookup is not None or lookups is not None) and any(is_next_row(e) for e, _ in custom):
             raise ValueError("lookups do not combine with next-row custom gate terms")
         # before any device work
         lk = check_lookup(lookup, group_order) if lookup is not None else None
         lks = check_lookups(lookups, group_order) if lookups is not None else None
+        sh = check_shuffle(shuffle, group_order) if shuffle is not None else None
         self = cls.__new__(cls)
         self.group_order = group_order
         self.setup = setup
@@ -222,7 +293,14 @@ class Prover:
             self._set_lookup(*lk)
         if lks is not None:
             self._set_lookup_tagged(*lks)
+        if sh is not None:
+            self._set_shuffle(*sh)
         return self
+
+    def _set_shuffle(self, q_in, q_out):
+        keep = [to_le_rows(q_in), to_le_rows(q_out)]
+        _lib.check(_lib.lib().pb200_prover_set_shuffle(self._h, *[k.ctypes.data_as(ctypes.c_void_p) for k in keep]))
+        self.shuffle = True
 
     def _set_lookup(self, qk, cols, rows):
         keep = [to_le_rows(qk)] + [to_le_rows(c) for c in cols]
@@ -274,13 +352,18 @@ class Prover:
     # ------------------------------------------------------------------ array-level fast path
     def prove_arrays(self, A, B, C, public) -> bytes:
         """One C-ABI call for the whole proof (rounds 1-5 + transcript); returns the canonical 768 bytes, the
-        1216 bytes of a ``LookupProof`` on a prover with a lookup argument, or the 864 bytes of a ``NextRowProof`` on a
-        prover with next-row custom gate terms."""
+        1216 bytes of a ``LookupProof`` on a prover with a lookup argument, the 864 bytes of a ``NextRowProof`` on a
+        prover with next-row custom gate terms, or the 896 (992) bytes of a ``ShuffleProof`` (``NextRowShuffleProof``)
+        on a prover with a shuffle."""
         n = self.group_order
         a, b, c = (_as_le_rows(v, n) for v in (A, B, C))
         pub = _as_le_rows(public, len(public)) if len(public) else np.zeros((0, 32), dtype=np.uint8)
         lookup = getattr(self, "lookup", False)
-        if getattr(self, "next_row", False):
+        if getattr(self, "shuffle", False):
+            nr = getattr(self, "next_row", False)
+            out = ctypes.create_string_buffer(NEXT_ROW_SHUFFLE_PROOF_BYTES if nr else SHUFFLE_PROOF_BYTES)
+            prove = _lib.lib().pb200_prover_prove_next_row_shuffle if nr else _lib.lib().pb200_prover_prove_shuffle
+        elif getattr(self, "next_row", False):
             out = ctypes.create_string_buffer(NEXT_ROW_PROOF_BYTES)
             prove = _lib.lib().pb200_prover_prove_next_row
         else:
@@ -297,10 +380,14 @@ class Prover:
     # ------------------------------------------------------------------ the reference's surface
     def prove(self, witness) -> Proof:
         """prover.py:51-84.  A prover with next-row custom gate terms follows NEXT_ROW_SCHEDULE and returns a
-        ``NextRowProof``."""
+        ``NextRowProof``; a prover with a shuffle follows SHUFFLE_SCHEDULE (NEXT_ROW_SHUFFLE_SCHEDULE) and returns a
+        ``ShuffleProof`` (``NextRowShuffleProof``)."""
         transcript = Transcript(b"plonk")
         msg_1 = self.round_1(witness)  # also collects the public inputs (prover.py:57-62)
-        self.beta, self.gamma = transcript.round_1(msg_1)
+        if getattr(self, "shuffle", False):
+            self.beta, self.gamma, self.theta, self.kappa = transcript.round_1(msg_1, SHUFFLE_SCHEDULE)
+        else:
+            self.beta, self.gamma = transcript.round_1(msg_1)
         msg_2 = self.round_2()
         self.alpha, self.fft_cofactor = transcript.round_2(msg_2)
         msg_3 = self.round_3()
@@ -308,6 +395,13 @@ class Prover:
         msg_4 = self.round_4()
         self.v = transcript.round_4(msg_4)
         msg_5 = self.round_5()
+        if isinstance(msg_2, ShuffleMessage2):
+            plain = Proof(msg_1, Message2(msg_2.z_1), msg_3, Message4(*[getattr(msg_4, k) for k in PROOF_FIELDS[7:13]]),
+                          msg_5)
+            tail = [msg_2.z3_1, msg_4.qin_eval, msg_4.z3_shifted_eval]
+            if isinstance(msg_4, NextRowShuffleMessage4):
+                return NextRowShuffleProof(plain, *[getattr(msg_4, k) for k in NEXT_ROW_FIELDS], *tail)
+            return ShuffleProof(plain, *tail)
         if isinstance(msg_4, NextRowMessage4):
             plain = Message4(*[getattr(msg_4, k) for k in PROOF_FIELDS[7:13]])
             return NextRowProof(Proof(msg_1, msg_2, msg_3, plain, msg_5), *[getattr(msg_4, k) for k in NEXT_ROW_FIELDS])
@@ -345,7 +439,16 @@ class Prover:
         return (int(x) % CURVE_ORDER).to_bytes(32, "little")
 
     def round_2(self) -> Message2:
-        """prover.py:121-152."""
+        """prover.py:121-152.  A shuffle prover returns a ``ShuffleMessage2`` (z_1, z3_1) and needs ``theta`` and
+        ``kappa`` set beside ``beta`` and ``gamma``."""
+        if getattr(self, "shuffle", False):
+            out = ctypes.create_string_buffer(128)
+            try:
+                _lib.check(_lib.lib().pb200_prover_round2_shuffle(self._h, self._le(self.beta), self._le(self.gamma),
+                                                                  self._le(self.theta), self._le(self.kappa), out))
+            except _lib.PlonkB200Error as e:
+                _raise(e)
+            return ShuffleMessage2(*_pts(out.raw, 2))
         out = ctypes.create_string_buffer(64)
         try:
             _lib.check(_lib.lib().pb200_prover_round2(self._h, self._le(self.beta), self._le(self.gamma), out))
@@ -364,7 +467,15 @@ class Prover:
 
     def round_4(self) -> Message4:
         """prover.py:228-239.  A next-row prover returns a ``NextRowMessage4``: the six evaluations, then a, b, c at
-        zeta w (NEXT_ROW_SCHEDULE)."""
+        zeta w (NEXT_ROW_SCHEDULE).  A shuffle prover returns a ``ShuffleMessage4`` or ``NextRowShuffleMessage4``, with
+        q_in(zeta) and Z3(zeta w) last."""
+        if getattr(self, "shuffle", False):
+            nr = getattr(self, "next_row", False)
+            count, cls = (11, NextRowShuffleMessage4) if nr else (8, ShuffleMessage4)
+            out = ctypes.create_string_buffer(count * 32)
+            fn = _lib.lib().pb200_prover_round4_next_row_shuffle if nr else _lib.lib().pb200_prover_round4_shuffle
+            _lib.check(fn(self._h, self._le(self.zeta), out))
+            return cls(*[Scalar(int.from_bytes(out.raw[32 * k:32 * k + 32], "little")) for k in range(count)])
         if getattr(self, "next_row", False):
             out = ctypes.create_string_buffer(9 * 32)
             _lib.check(_lib.lib().pb200_prover_round4_next_row(self._h, self._le(self.zeta), out))

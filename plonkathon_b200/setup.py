@@ -12,6 +12,7 @@ from .curve import G2, Scalar, _pt_bytes, _pt_from, g2_mul
 from .field import CURVE_ORDER, FIELD_MODULUS, FQ, FQ2
 from .custom_gates import is_next_row, split_terms
 from .lookup import check_lookup, check_lookups, padded_table, to_le_rows
+from .shuffle import check_shuffle
 from .poly import Basis, Polynomial, _log2_exact
 from .prover import _as_le_rows
 from .verifier import VerificationKey  # noqa: F401  (re-exported: the reference's setup.py imports it too)
@@ -202,7 +203,7 @@ class Setup:
         return h
 
     def verification_key_arrays(self, group_order: int, pk_arrays: dict, custom=(), lookup=None,
-                                lookups=None) -> VerificationKey:
+                                lookups=None, shuffle=None) -> VerificationKey:
         """``verification_key`` for circuits that exist only as arrays (``Prover.from_arrays``): QM..S3 as
         (n,32) uint8 little-endian Lagrange values in host memory.  ``custom``: the circuit's custom gate terms
         ``((i, j, l), column)`` as given to ``Prover.from_arrays``; each column is committed too.  ``lookup``:
@@ -210,16 +211,21 @@ class Setup:
         padded to n rows), the identity for a constant-zero column.  ``lookups``: several tables as given to
         ``Prover.from_arrays``; the key gains [q_K], [t1], [t2], [t3], [Q_T], [t4] (the tables concatenated and padded).
         Not together with ``lookup``.  A custom term may have six exponents (i, j, l, i', j', l') and read the next
-        row; the key then takes ``NextRowProof`` only.  Next-row terms do not combine with lookups (ValueError)."""
+        row; the key then takes ``NextRowProof`` only.  Next-row terms do not combine with lookups (ValueError).
+        ``shuffle``: ``(q_in, q_out)`` as given to ``Prover.from_arrays``; the key gains [q_in], [q_out] and takes
+        ``ShuffleProof`` only (``NextRowShuffleProof`` with a next-row term).  Not together with lookups (ValueError)."""
         import numpy as np
         if lookup is not None and lookups is not None:
             raise ValueError("pass either lookup= (one table) or lookups= (several tables), not both")
+        if shuffle is not None and (lookup is not None or lookups is not None):
+            raise ValueError("shuffles do not combine with lookups")
         log_n = _log2_exact(group_order)
         exps, ccols = split_terms(custom, group_order)
         if (lookup is not None or lookups is not None) and any(is_next_row(e) for e in exps):
             raise ValueError("lookups do not combine with next-row custom gate terms")
         lk = check_lookup(lookup, group_order) if lookup is not None else None
         lks = check_lookups(lookups, group_order) if lookups is not None else None
+        sh = check_shuffle(shuffle, group_order) if shuffle is not None else None
 
         def commit_host(col):
             col = np.ascontiguousarray(col).view(np.uint8).reshape(-1, 32)
@@ -245,7 +251,8 @@ class Setup:
             qk, qtag, cols, _rows = lks
             t1, t2, t3, t4 = padded_table(cols, group_order)
             lk_pts = tuple(commit_host(to_le_rows(c)) for c in (qk, t1, t2, t3, qtag, t4))
-        return VerificationKey(group_order, *pts, self.X2, Scalar.root_of_unity(group_order), terms, lk_pts)
+        sh_pts = tuple(commit_host(to_le_rows(q)) for q in sh) if sh is not None else ()
+        return VerificationKey(group_order, *pts, self.X2, Scalar.root_of_unity(group_order), terms, lk_pts, sh_pts)
 
     def verification_key(self, pk) -> VerificationKey:
         """setup.py:75-77."""

@@ -42,6 +42,8 @@ class ArrayCircuit:
     lookup: tuple = ()
     # lookups over several tables ((q_k per row, (t1, t2, t3)) per table, table k has id k); () without them
     lookups: tuple = ()
+    # shuffle (q_in per row, q_out per row), plonkathon_b200/shuffle.py; () without one
+    shuffle: tuple = ()
 
     def wires_values(self):
         val = self.values
@@ -91,7 +93,7 @@ def permutation_polys(wire_L, wire_R, wire_O, group_order: int, n_constraints: i
 
 
 def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: float = 1.0,
-                  with_text: bool = False, custom=(), lookup=None, lookups=None) -> ArrayCircuit:
+                  with_text: bool = False, custom=(), lookup=None, lookups=None, shuffle: bool = False) -> ArrayCircuit:
     """Deterministic synthetic circuit with 2^log_n rows: ``n_public`` public-input rows, then a chain of
     multiplication / addition / add-constant gates whose operands are drawn from recently produced
     variables (so the permutation is non-trivial and the witness values are pseudo-random field elements).
@@ -110,7 +112,13 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
     draws are unchanged.
 
     ``lookups``: a list of tables ``[(t1, t2, t3), ...]``; as ``lookup``, but each lookup row picks its table at random
-    (one more draw, only with two or more tables: ``lookups=[x]`` builds the circuit of ``lookup=x``)."""
+    (one more draw, only with two or more tables: ``lookups=[x]`` builds the circuit of ``lookup=x``).
+
+    ``shuffle``: out-rows are mixed into the chain as one more kind of row, a quarter of the rows (one more draw per row,
+    only with ``shuffle``): an out-row takes the (a, b, c) of a random earlier row not yet shuffled, as three fresh
+    variables with no copy constraint and every selector 0; that row gets q_in = 1, the out-row q_out = 1.  So a quarter
+    of the rows are in-rows, a quarter out-rows, and the out-rows hold the in-rows' tuples in a random order.  Without it
+    the random draws are unchanged.  Not together with lookups."""
     from .custom_gates import check_exponents, is_next_row
     from .lookup import check_lookup, check_lookups
     custom = check_exponents(custom)
@@ -119,6 +127,10 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
         raise ValueError("pass either lookup= (one table) or lookups= (several tables), not both")
     if (lookup is not None or lookups is not None) and any(is_next_row(e) for e in custom):
         raise ValueError("lookups do not combine with next-row custom gate terms")
+    if shuffle and (lookup is not None or lookups is not None):
+        raise ValueError("shuffles do not combine with lookups")
+    q_in, q_out = [0] * n, [0] * n
+    pool = []        # rows that may still become in-rows
     tables = []  # (columns, rows) per table
     if lookup is not None:
         tables = [check_lookup(([0] * n, lookup), n)[1:]]
@@ -165,6 +177,16 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
             first = False
         if carry is not None:
             ia, carry = carry, None
+        if shuffle and pool and rng.randrange(4) == 0:  # an out-row: an earlier row's (a, b, c) as fresh variables
+            k = rng.randrange(len(pool))
+            r = pool[k]
+            pool[k] = pool[-1]
+            pool.pop()
+            values.extend(values[w[r]] for w in (wL, wR, wO))
+            wL[row], wR[row], wO[row] = nv, nv + 1, nv + 2
+            q_in[r], q_out[row] = 1, 1
+            row += 1
+            continue
         kind = rng.randrange(3 + len(custom) + bool(tables))
         out = nv
         if tables and kind == 3 + len(custom):  # (a, b, c) = a row of table t, q_t = 1
@@ -207,6 +229,8 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
             QL[row], QC[row], QO[row] = R - 1, (R - k) % R, 1
             if with_text:
                 text.append("%s <== %s + %d" % (name(out), name(ia), k))
+        if shuffle:
+            pool.append(row)
         row += 1
     if pinned:
         from .custom_gates import padded
@@ -220,7 +244,8 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
             QC[r] = (R - mon) % R
     lk = (QKs[0], tuple(tables[0][0])) if lookup is not None else ()
     lks = tuple((q, tuple(t)) for q, (t, _) in zip(QKs, tables)) if lookups is not None else ()
-    return ArrayCircuit(n, m, wL, wR, wO, QL, QR, QM, QO, QC, n_public, values, text, list(zip(custom, QK)), lk, lks)
+    return ArrayCircuit(n, m, wL, wR, wO, QL, QR, QM, QO, QC, n_public, values, text, list(zip(custom, QK)), lk, lks,
+                        (q_in, q_out) if shuffle else ())
 
 
 def _custom_row(exps, Q, row, operands, k, values, wires, sel):
@@ -318,6 +343,12 @@ def lookup_arrays(c: ArrayCircuit):
     """-> the circuit's lookup argument ``(q_K, (t1, t2, t3))``, ready for ``Prover.from_arrays(..., lookup=)`` and
     ``Setup.verification_key_arrays(..., lookup=)``"""
     return c.lookup[0], c.lookup[1]
+
+
+def shuffle_arrays(c: ArrayCircuit):
+    """-> the circuit's shuffle ``(q_in, q_out)``, ready for ``Prover.from_arrays(..., shuffle=)`` and
+    ``Setup.verification_key_arrays(..., shuffle=)``"""
+    return c.shuffle[0], c.shuffle[1]
 
 
 def lookups_arrays(c: ArrayCircuit):

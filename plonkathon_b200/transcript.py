@@ -37,11 +37,27 @@ LOOKUP_SCHEDULE = {
 NEXT_ROW_SCHEDULE = dict(SCHEDULE)
 NEXT_ROW_SCHEDULE[4] = (SCHEDULE[4][0] + ("a_shifted_eval", "b_shifted_eval", "c_shifted_eval"), "scalar", ("v",))
 
+# The same table for a proof with a shuffle (plonkathon_b200/shuffle.py): step 1 also draws theta and kappa (no commitment
+# before them), step 2 absorbs Z3 beside Z and step 4 q_in(zeta) and Z3(zeta w) last.  NEXT_ROW_SHUFFLE_SCHEDULE is the
+# form for a circuit with next-row custom gate terms: the three shifted wire evaluations come before the shuffle's two.
+SHUFFLE_FIELDS_4 = ("qin_eval", "z3_shifted_eval")
+SHUFFLE_SCHEDULE = dict(SCHEDULE)
+SHUFFLE_SCHEDULE[1] = (SCHEDULE[1][0], "point", ("beta", "gamma", "theta", "kappa"))
+SHUFFLE_SCHEDULE[2] = (("z_1", "z3_1"), "point", SCHEDULE[2][2])
+SHUFFLE_SCHEDULE[4] = (SCHEDULE[4][0] + SHUFFLE_FIELDS_4, "scalar", ("v",))
+NEXT_ROW_SHUFFLE_SCHEDULE = dict(SHUFFLE_SCHEDULE)
+NEXT_ROW_SHUFFLE_SCHEDULE[4] = (NEXT_ROW_SCHEDULE[4][0] + SHUFFLE_FIELDS_4, "scalar", ("v",))
+
 # Message1 .. Message5: plain records with exactly the reference's field names and order
 Message1, Message2, Message3, Message4, Message5 = (
     make_dataclass("Message%d" % rnd, [(name, object) for name in SCHEDULE[rnd][0]]) for rnd in sorted(SCHEDULE))
 # round 4 of a next-row prover: Message4's fields, then the three shifted wire evaluations
 NextRowMessage4 = make_dataclass("NextRowMessage4", [(name, object) for name in NEXT_ROW_SCHEDULE[4][0]])
+# rounds 2 and 4 of a shuffle prover (round 4 with and without next-row terms)
+ShuffleMessage2 = make_dataclass("ShuffleMessage2", [(name, object) for name in SHUFFLE_SCHEDULE[2][0]])
+ShuffleMessage4 = make_dataclass("ShuffleMessage4", [(name, object) for name in SHUFFLE_SCHEDULE[4][0]])
+NextRowShuffleMessage4 = make_dataclass("NextRowShuffleMessage4",
+                                        [(name, object) for name in NEXT_ROW_SHUFFLE_SCHEDULE[4][0]])
 
 
 def _as_int(x) -> int:
@@ -108,18 +124,23 @@ class Transcript:
                 drawn[c] = self.get_and_append_challenge(c.encode())
         return drawn
 
-    def round_1(self, message):
-        return self._round(1, message)
+    def round_1(self, message, schedule: dict = SCHEDULE):
+        """``schedule=SHUFFLE_SCHEDULE`` draws theta and kappa after beta and gamma (four challenges)"""
+        return self._round(1, message, schedule)
 
     def round_2(self, message):
-        return self._round(2, message)
+        """a ``ShuffleMessage2`` follows SHUFFLE_SCHEDULE"""
+        return self._round(2, message, SHUFFLE_SCHEDULE if isinstance(message, ShuffleMessage2) else SCHEDULE)
 
     def round_3(self, message):
         return self._round(3, message)
 
     def round_4(self, message):
-        """a ``NextRowMessage4`` follows NEXT_ROW_SCHEDULE"""
-        return self._round(4, message, NEXT_ROW_SCHEDULE if isinstance(message, NextRowMessage4) else SCHEDULE)
+        """a ``NextRowMessage4`` follows NEXT_ROW_SCHEDULE, a ``ShuffleMessage4`` SHUFFLE_SCHEDULE and a
+        ``NextRowShuffleMessage4`` NEXT_ROW_SHUFFLE_SCHEDULE"""
+        schedule = {NextRowMessage4: NEXT_ROW_SCHEDULE, ShuffleMessage4: SHUFFLE_SCHEDULE,
+                    NextRowShuffleMessage4: NEXT_ROW_SHUFFLE_SCHEDULE}.get(type(message), SCHEDULE)
+        return self._round(4, message, schedule)
 
     def round_5(self, message):
         return self._round(5, message)

@@ -16,7 +16,8 @@ from .curve import G1, G2, Scalar, ec_lincomb, g1_neg, g2_add, g2_mul, pairing_p
 from . import _lib
 from .custom_gates import is_next_row, monomial
 from .field import CURVE_ORDER, FIELD_MODULUS
-from .transcript import LOOKUP_SCHEDULE, NEXT_ROW_SCHEDULE, SCHEDULE, Transcript
+from .transcript import (LOOKUP_SCHEDULE, NEXT_ROW_SCHEDULE, NEXT_ROW_SHUFFLE_SCHEDULE, SCHEDULE, SHUFFLE_SCHEDULE,
+                         Transcript)
 
 
 def _lagrange_terms_at(group_order: int, values, x: Scalar) -> Scalar:
@@ -52,6 +53,9 @@ class VerificationKey:
     # lookup argument (plonkathon_b200/lookup.py): ([q_K], [t1], [t2], [t3]) for one table, ([q_K], [t1], [t2], [t3],
     # [Q_T], [t4]) for several tables told apart by a tag; the identity (None) for a zero column; () without lookups
     lookup: tuple = ()
+    # shuffle (plonkathon_b200/shuffle.py): ([q_in], [q_out]), the identity (None) for a zero column; () without one.
+    # With a shuffle the key takes ShuffleProof only (NextRowShuffleProof with a next-row term)
+    shuffle: tuple = ()
 
     def _custom_terms(self, a, b, c, aw=None, bw=None, cw=None):
         """the custom gates' part of the linearisation: sum_k m_k(a, b, c, a(zeta w), b(zeta w), c(zeta w)) [Q_k]"""
@@ -76,9 +80,12 @@ class VerificationKey:
         return True
 
     def _matches(self, pf) -> bool:
-        """a lookup key takes lookup proofs only, a next-row key next-row proofs only, a plain key plain proofs only"""
-        from .prover import LookupProof, NextRowProof
-        return bool(self.lookup) == isinstance(pf, LookupProof) and self.next_row == isinstance(pf, NextRowProof)
+        """a lookup key takes lookup proofs only, a next-row key next-row proofs only, a shuffle key shuffle proofs only
+        (of its next-row kind), a plain key plain proofs only"""
+        from .prover import LookupProof, NextRowProof, NextRowShuffleProof, ShuffleProof
+        return (bool(self.lookup) == isinstance(pf, LookupProof)
+                and self.next_row == isinstance(pf, (NextRowProof, NextRowShuffleProof))
+                and bool(self.shuffle) == isinstance(pf, (ShuffleProof, NextRowShuffleProof)))
 
     def verify_proof(self, group_order: int, pf, public=[]) -> bool:
         """verifier.py:40-73: the batched form -- one pairing equation, the linearisation commitment never
@@ -105,7 +112,10 @@ class VerificationKey:
     def _verify(self, group_order: int, pf, public, batched: bool) -> bool:
         n = group_order
         proof = pf.flatten()
-        schedule = LOOKUP_SCHEDULE if self.lookup else NEXT_ROW_SCHEDULE if self.next_row else SCHEDULE
+        if self.shuffle:
+            schedule = NEXT_ROW_SHUFFLE_SCHEDULE if self.next_row else SHUFFLE_SCHEDULE
+        else:
+            schedule = LOOKUP_SCHEDULE if self.lookup else NEXT_ROW_SCHEDULE if self.next_row else SCHEDULE
         ch = Transcript(b"plonk").replay(schedule, proof)
         beta, gamma, alpha, zeta, v, u = ch["beta"], ch["gamma"], ch["alpha"], ch["zeta"], ch["v"], ch["u"]
         zh_ev = zeta ** n - 1
@@ -167,6 +177,24 @@ class VerificationKey:
             e_zeta = e_zeta + v6 * fe + v7 * te + v8 * h2e
             at_zw += [(proof["h1_1"], v2), (proof["z2_1"], v3)] + [(p, k * v) for p, k in t_parts]
             e_zw = e_zw + v * tw + v2 * h1w + v3 * z2w
+        if self.shuffle:
+            theta, kappa = ch["theta"], ch["kappa"]
+            qin, z3w = proof["qin_eval"], proof["z3_shifted_eval"]
+            a3, a4 = a2 * alpha, a2 * a2
+            k = kappa + a + theta * b + theta * theta * c - 1  # kappa + w - 1
+            qin_pt, qout_pt = self.shuffle
+            r_terms += [
+                # alpha^3 [z3_w (1 + Q_out k) - Z3 (1 + q_in k)] + alpha^4 L0 (Z3 - 1)
+                (qout_pt, a3 * z3w * k),
+                (proof["z3_1"], -a3 * (qin * k + 1) + a4 * l0_ev),
+            ]
+            r0 = r0 + a3 * z3w - a4 * l0_ev
+            v6 = v5 * v
+            at_zeta.append((qin_pt, v6))
+            e_zeta = e_zeta + v6 * qin
+            vk = v4 if self.next_row else v  # after A, B, C at zeta w on a next-row key
+            at_zw.append((proof["z3_1"], vk))
+            e_zw = e_zw + vk * z3w
         if batched:
             # e(W_z + u W_zw, [x]_2) == e(zeta W_z + u zeta w W_zw + F - E, [1]_2), F = [R] - r0 + both batches
             f_pt = ec_lincomb(r_terms + at_zeta + [(p, u * k) for p, k in at_zw])
