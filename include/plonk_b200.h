@@ -236,11 +236,20 @@ int pb200_prover_serialize_next_row(pb200_prover* p, uint8_t* h_proof864);
  * q_in(zeta) and Z3(zeta w).  A proof has 896 bytes: the 768 plain bytes, then z3_1, qin_eval, z3_shifted_eval; on a
  * next-row prover 992 bytes, with a, b, c at zeta w before z3_1.  A witness whose two sides differ fails round 2 with
  * "AssertionError: shuffle: the q_in rows and the q_out rows are not permutations of each other".
- * Errors, the prover left as it was: the sharded prover, a lookup table, zero-knowledge mode, selectors already set,
- * a selector value other than 0 / 1, unequal numbers of ones.  On a shuffle prover pb200_prover_set_lookup(_tagged)
- * and pb200_prover_set_zk(p, 1, ...) are errors, and so are every prove / serialize / round 4 entry point of another
- * proof size and the plain pb200_prover_round2.  Rounds 1, 3 and 5 are the plain entry points. */
+ * Errors, the prover left as it was: the sharded prover, a lookup table, zero-knowledge mode (set the shuffle first,
+ * then pb200_prover_set_zk_shuffle), selectors already set, a selector value other than 0 / 1, unequal numbers of
+ * ones.  On a shuffle prover pb200_prover_set_lookup(_tagged) and pb200_prover_set_zk(p, 1, ...) are errors, and so
+ * are every prove / serialize / round 4 entry point of another proof size and the plain pb200_prover_round2.  Rounds 1,
+ * 3 and 5 are the plain entry points. */
 int pb200_prover_set_shuffle(pb200_prover* p, const uint8_t* h_qin, const uint8_t* h_qout);
+/* Zero-knowledge shuffle proofs for every later proof of a shuffle prover: enable != 0 blinds A, B, C, Z and the
+ * quotient pieces as pb200_prover_set_zk does, and Z3 with 3 more scalars, the last three: 14 in all, 17 on a
+ * next-row prover (DESIGN.md section 1).  h_blinders == NULL: fresh scalars from the OS CSPRNG for every proof;
+ * otherwise 14 (17) x 32-byte canonical Fr used for every proof (reproducible tests).  The proofs keep their 896 (992)
+ * bytes and entry points, and the verifier does not change.  enable == 0, or pb200_prover_set_zk(p, 0, NULL), returns
+ * to plain shuffle proofs.  Errors: a prover without a shuffle, a sharded prover, n < 8 and an SRS shorter than n + 6
+ * (n < 16 and n + 9 on a next-row prover), unreduced blinders; a refused call leaves the prover as it was. */
+int pb200_prover_set_zk_shuffle(pb200_prover* p, int enable, const uint8_t* h_blinders);
 /* round 2 of a shuffle prover: z_1 then z3_1 */
 int pb200_prover_round2_shuffle(pb200_prover* p, const uint8_t* beta, const uint8_t* gamma, const uint8_t* theta,
                                 const uint8_t* kappa, uint8_t* h_zz3_xy /*2*64*/);

@@ -96,6 +96,7 @@ def _load():
         "pb200_prover_prove_next_row": (I, [V, V, V, V, V, U64, V]),
         "pb200_prover_serialize_next_row": (I, [V, V]),
         "pb200_prover_set_shuffle": (I, [V, V, V]),
+        "pb200_prover_set_zk_shuffle": (I, [V, I, V]),
         "pb200_prover_round2_shuffle": (I, [V, V, V, V, V, V]),
         "pb200_prover_round4_shuffle": (I, [V, V, V]),
         "pb200_prover_round4_next_row_shuffle": (I, [V, V, V]),

@@ -60,6 +60,7 @@ void prover_round_lookup(Prover* P, const Fr& eta_c);
 void prover_round2_lookup(Prover* P, const Fr& beta_c, const Fr& gamma_c, const Fr& delta_c, const Fr& epsilon_c);
 void prover_round4_lookup(Prover* P, const Fr& zeta_c);
 void prover_set_shuffle(Prover* P, const uint8_t* h_qin, const uint8_t* h_qout);
+void prover_set_zk_shuffle(Prover* P, bool enable, const uint8_t* h_blinders);
 void prover_round2_shuffle(Prover* P, const Fr& beta_c, const Fr& gamma_c, const Fr& theta_c, const Fr& kappa_c);
 void g1_combine_partials_host(const G1XYZZ* parts, uint32_t count, uint8_t* out_xy, int* is_identity);
 void host_join_bucket_shards(const SR* all, uint32_t world, uint32_t sets, uint32_t nloc, G1XYZZ* out);
@@ -646,6 +647,11 @@ int pb200_prover_serialize_next_row(pb200_prover* p, uint8_t* h_proof864) {
 int pb200_prover_set_shuffle(pb200_prover* p, const uint8_t* h_qin, const uint8_t* h_qout) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   prover_set_shuffle(reinterpret_cast<Prover*>(p), h_qin, h_qout);
+  PB_API_END
+}
+int pb200_prover_set_zk_shuffle(pb200_prover* p, int enable, const uint8_t* h_blinders) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  prover_set_zk_shuffle(reinterpret_cast<Prover*>(p), enable != 0, h_blinders);
   PB_API_END
 }
 int pb200_prover_round2_shuffle(pb200_prover* p, const uint8_t* beta, const uint8_t* gamma, const uint8_t* theta,

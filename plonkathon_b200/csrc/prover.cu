@@ -20,7 +20,8 @@
 // Zero-knowledge mode (prover_set_zk, one GPU) blinds A, B, C, Z and the quotient pieces as in the PLONK paper; the
 // proof keeps its 15 fields and the verifier does not change.  See "zero knowledge" below.
 // A shuffle (Prover::sh, one GPU) proves that two sets of rows hold the same multiset of (a, b, c): one more grand
-// product Z3 beside Z, see "shuffle" below; the proof gains z3_1 and two evaluations (896 bytes, 992 next-row).
+// product Z3 beside Z, see "shuffle" below; the proof gains z3_1 and two evaluations (896 bytes, 992 next-row).  In
+// zero-knowledge mode (prover_set_zk_shuffle) Z3 takes three more blinders and the proof keeps its size.
 // Custom terms over the next row (Prover::next_row, one GPU) read a(wX), b(wX), c(wX): k_gate_check<true> and
 // k_quotient<ZK, true> read index + 1 (mod n) and coset index + 4, round 4 adds A, B, C at zeta w and round 5 opens them
 // there with Z; the proof gains those three evaluations (864 bytes).
@@ -465,6 +466,8 @@ struct LinCombArgs { const Fr* vec[26]; Fr w[26]; Fr c0; int count; uint64_t n, 
 // A shuffle adds 3 (Q_out, Z3, Q_in) to the 19 plain terms: 22.
 static_assert(5 + PB_MAX_CUSTOM + 10 + 7 <= 26, "round 5's largest batch must fit LinCombArgs");
 static_assert(5 + PB_MAX_CUSTOM + 10 + 3 <= 26, "round 5's batch with a shuffle must fit LinCombArgs");
+// Zero knowledge: the tail holds the blinded vectors, Z, T1-T3, A, B, C (7), and Z3' with a shuffle: 8.
+static_assert(7 + 1 <= 26, "round 5's zero-knowledge tail with a shuffle must fit LinCombArgs");
 __global__ void __launch_bounds__(128) k_lincomb(LinCombArgs a, Fr* out) {
   uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= a.n) return;
@@ -680,14 +683,33 @@ struct ShuffleQuotientArgs {
   Fr theta, theta2, kappa_m1, alpha3, alpha4, one;
   uint64_t n4;
 };
-__global__ void __launch_bounds__(128) k_quotient_shuffle(ShuffleQuotientArgs q, Fr* out) {
+// Zero knowledge (prover_set_zk_shuffle): the kernel reads the unblinded extensions and adds the Z_H multiples, as
+// k_quotient_lookup<true> does.  Z3' = Z3 + (c2 X^2 + c1 X + c0) Z_H with Z3's blinders c2, c1, c0 (the last three), and
+// A' + theta B' + theta^2 C' = W + (e2 X^2 + e1 X + e0) Z_H with e1 = b1 + theta b3 + theta^2 b5, e0 = b2 + theta b4 +
+// theta^2 b6, e2 = b12 + theta b13 + theta^2 b14 on a next-row prover and 0 otherwise.  w[k] = Z_H class k times
+//   (e2, e1, e0,  c2, c1, c0,  c2 w^2, c1 w, c0)
+// (Z3'(wX) uses Z_H(w x) = Z_H(x)): 6 products a point.  A separate parameter after out, so the plain kernel's parameters
+// keep their offsets.
+struct ZkShuffleCoset { const Fr* X; Fr w[4][9]; };
+static_assert(sizeof(ShuffleQuotientArgs) + sizeof(Fr*) + sizeof(ZkShuffleCoset) <= 4096,
+              "k_quotient_shuffle's parameters must fit the 4 KiB parameter space");
+template <bool ZK>
+__global__ void __launch_bounds__(128) k_quotient_shuffle(ShuffleQuotientArgs q, Fr* out, ZkShuffleCoset zk) {
   uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= q.n4) return;
   const uint64_t jw = j + 4 >= q.n4 ? j + 4 - q.n4 : j + 4;
-  const Fr k = fp_add(q.kappa_m1, fp_add(ldg_fr(q.A + j), fp_add(fp_mul(q.theta, ldg_fr(q.B + j)),
-                                                                   fp_mul(q.theta2, ldg_fr(q.C + j)))));
-  const Fr z3 = ldg_fr(q.Z3 + j);
-  Fr acc = fp_sub(fp_mul(ldg_fr(q.Z3 + jw), fp_add(q.one, fp_mul(ldg_fr(q.QOUT + j), k))),
+  // zero knowledge: y + ((w_i x + w_i+1) x + w_i+2), the Z_H multiple of the blinded polynomial; in the plain instance it
+  // returns y.  Indexed in the parameter space (a pointer to the weights would copy them)
+  const uint32_t kz = (uint32_t)j & 3;
+  const Fr x = ZK ? ldg_fr(zk.X + j) : Fr::zero();
+  auto quad = [&](Fr y, int i) {
+    if constexpr (ZK) y = fp_add(y, fp_add(fp_mul(fp_add(fp_mul(zk.w[kz][i], x), zk.w[kz][i + 1]), x), zk.w[kz][i + 2]));
+    return y;
+  };
+  const Fr k = fp_add(q.kappa_m1, quad(fp_add(ldg_fr(q.A + j), fp_add(fp_mul(q.theta, ldg_fr(q.B + j)),
+                                                                        fp_mul(q.theta2, ldg_fr(q.C + j)))), 0));
+  const Fr z3 = quad(ldg_fr(q.Z3 + j), 3);
+  Fr acc = fp_sub(fp_mul(quad(ldg_fr(q.Z3 + jw), 6), fp_add(q.one, fp_mul(ldg_fr(q.QOUT + j), k))),
                   fp_mul(z3, fp_add(q.one, fp_mul(ldg_fr(q.QIN + j), k))));
   acc = fp_add(fp_mul(q.alpha3, acc), fp_mul(q.alpha4, fp_mul(fp_sub(z3, q.one), ldg_fr(q.L0 + j))));
   out[j] = fp_add(out[j], fp_mul(acc, q.zh_inv[j & 3]));
@@ -981,21 +1003,24 @@ static void zk_enable(Prover* P, const uint8_t* h_blinders) {
   for (auto& b : P->tmp) b.ensure(bytes);  // round 5 works on n + 8 coefficients (n + 9 next-row)
   if (P->lk)
     for (auto& b : P->zk_lk) b.ensure(bytes);
+  if (P->sh) P->zk_z3.ensure(bytes);
   if (h_blinders) std::copy(fixed, fixed + count, P->zk_fixed_b);
   P->zk_fixed = h_blinders != nullptr;
   P->zk = true;
 }
 
 void prover_set_zk(Prover* P, bool enable, const uint8_t* h_blinders) {
-  if (!enable) {  // also ends zero-knowledge lookup proofs (prover_set_zk_lookup)
+  if (!enable) {  // also ends zero-knowledge lookup and shuffle proofs (prover_set_zk_lookup, prover_set_zk_shuffle)
     P->zk = P->zk_fixed = false;
     for (auto& b : P->zk_coeff) b.release();
     for (auto& b : P->zk_t) b.release();
     for (auto& b : P->zk_lk) b.release();
+    P->zk_z3.release();
     return;
   }
   PB_CHECK(P->world == 1, "zero-knowledge proving is not available on the sharded prover (one GPU only)");
-  PB_CHECK(!P->sh, "zero-knowledge mode does not combine with a shuffle");
+  PB_CHECK(!P->sh, "zero-knowledge mode does not combine with a shuffle here: a shuffle prover takes 14 blinders (17 "
+                   "with next-row terms) through pb200_prover_set_zk_shuffle");
   PB_CHECK(!P->lk, "zero-knowledge mode does not combine with lookups here: a lookup prover takes 21 blinders through "
                    "pb200_prover_set_zk_lookup");
   zk_enable(P, h_blinders);
@@ -1007,6 +1032,19 @@ void prover_set_zk(Prover* P, bool enable, const uint8_t* h_blinders) {
 void prover_set_zk_lookup(Prover* P, bool enable, const uint8_t* h_blinders) {
   PB_CHECK(P->world == 1, "zero-knowledge proving is not available on the sharded prover (one GPU only)");
   PB_CHECK(P->lk, "this prover has no lookup table (pb200_prover_set_lookup): use pb200_prover_set_zk");
+  if (!enable) {
+    prover_set_zk(P, false, nullptr);
+    return;
+  }
+  zk_enable(P, h_blinders);
+}
+
+// Zero-knowledge shuffle proofs: the 11 blinders of prover_set_zk (14 on a next-row prover) and three more for Z3, the
+// last three (see "zero knowledge with a shuffle" below).  A separate entry point for the same reason as
+// prover_set_zk_lookup.
+void prover_set_zk_shuffle(Prover* P, bool enable, const uint8_t* h_blinders) {
+  PB_CHECK(P->world == 1, "zero-knowledge proving is not available on the sharded prover (one GPU only)");
+  PB_CHECK(P->sh, "this prover has no shuffle (pb200_prover_set_shuffle): use pb200_prover_set_zk");
   if (!enable) {
     prover_set_zk(P, false, nullptr);
     return;
@@ -1255,7 +1293,14 @@ static void grand_product(Prover* P, Fr* num, const Fr* den, Fr* lag, Fr* coeff,
 // the two products agree.  The quotient gains k_quotient_shuffle's two terms at alpha^3, alpha^4 (degree <= 3n - 3, so T
 // keeps three pieces); round 4 evaluates Q_in at zeta and Z3 at zeta w; round 5 keeps [Q_out] and [Z3] in the
 // linearisation, opens Q_in at zeta (v^6) and Z3 at zeta w (v, or v^4 after A, B, C on a next-row prover).  A row with
-// both selectors cancels out.  Not with lookups (their alpha^3..alpha^5 terms), zero knowledge or the sharded prover.
+// both selectors cancels out.  Not with lookups (their alpha^3..alpha^5 terms) or the sharded prover.
+// Zero knowledge with a shuffle (prover_set_zk_shuffle): everything of zero-knowledge mode (b1..b11, or b1..b14 on a
+// next-row prover), and Z3' = Z3 + (b_(m-2) X^2 + b_(m-1) X + b_m) Z_H with the last three of the m = 14 (17) blinders,
+// one scalar more than the points Z3 is revealed at (zeta w and the linearisation).  Q_in and Q_out are fixed and stay
+// as they are.  Z3 is built from the unblinded values, as the check is; k_quotient_shuffle<true> adds the Z_H multiples
+// on the coset (A', B', C' included), round 4 corrects z3(zeta w) and round 5 uses Z3'.  deg T <= 3n + 5 (3n + 8) still
+// holds (the shuffle products reach 2n + 2, 2n + 3 next-row, after the division), so T is split as in zero-knowledge
+// mode and the proof keeps its 896 (992) bytes.
 
 // h_qin, h_qout: n x 32 bytes canonical, 0 or 1 on every row, with as many ones in each.  Every check comes before any
 // change, so a refused call leaves the prover as it was.
@@ -1264,7 +1309,8 @@ void prover_set_shuffle(Prover* P, const uint8_t* h_qin, const uint8_t* h_qout) 
   const uint64_t n = P->n;
   PB_CHECK(P->world == 1, "shuffles are not available on the sharded prover (one GPU only)");
   PB_CHECK(!P->lk, "shuffles do not combine with lookups");
-  PB_CHECK(!P->zk, "shuffles do not combine with zero-knowledge mode");
+  PB_CHECK(!P->zk, "shuffles do not combine with zero-knowledge mode switched on first: set the shuffle, then "
+                   "pb200_prover_set_zk_shuffle");
   PB_CHECK(!P->sh, "the shuffle selectors are already set (set them once, before the first proof)");
   PB_CHECK(h_qin && h_qout, "a shuffle needs q_in and q_out");
   uint64_t ones[2] = {0, 0};
@@ -1308,9 +1354,14 @@ static void shuffle_round2(Prover* P) {
   ctx->launches++;
   grand_product(P, num, den, P->sh_z3_lag.as<Fr>(), P->sh_z3_coeff.as<Fr>(),
                 "AssertionError: shuffle: the q_in rows and the q_out rows are not permutations of each other");
-  const Fr* zz[2] = {P->coeff[3].as<Fr>(), P->sh_z3_coeff.as<Fr>()};
+  if (P->zk) {  // Z' and Z3': n + 3 coefficients each
+    const Fr *b = P->zk_b, *c = P->zk_z3_b();
+    zk_blind(P, P->coeff[3].as<Fr>(), n, zh_multiple({b[8], b[7], b[6]}), P->zk_coeff[3].as<Fr>());
+    zk_blind(P, P->sh_z3_coeff.as<Fr>(), n, zh_multiple({c[2], c[1], c[0]}), P->zk_z3.as<Fr>());
+  }
+  const Fr* zz[2] = {P->zk ? P->zk_coeff[3].as<Fr>() : P->coeff[3].as<Fr>(), P->sh_z3_poly()};
   uint8_t out[2][64];
-  P->commit_batch(zz, 2, n, out[0]);
+  P->commit_batch(zz, 2, P->zk ? n + 3 : n, out[0]);
   memcpy(P->proof.pts[3], out[0], 64);
   memcpy(P->sh_pt, out[1], 64);
 }
@@ -1605,7 +1656,23 @@ void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c) {
     sq.theta = P->theta; sq.theta2 = fp_sqr(P->theta); sq.kappa_m1 = fp_sub(P->kappa, Fr::one());
     sq.alpha3 = fp_mul(q.alpha2, P->alpha); sq.alpha4 = fp_sqr(q.alpha2); sq.one = Fr::one();
     sq.n4 = ne;
-    k_quotient_shuffle<<<PB_GRID(ne, 128), 0, st>>>(sq, t_evals);
+    ZkShuffleCoset zs{};
+    if (P->zk) {
+      const Fr *b = P->zk_b, *c = P->zk_z3_b();
+      const Fr w = fr_root_of_unity(P->log_n), w2 = fp_sqr(w);
+      auto wsum = [&](const Fr& x, const Fr& y, const Fr& z) {  // x + theta y + theta^2 z
+        return fp_add(x, fp_add(fp_mul(sq.theta, y), fp_mul(sq.theta2, z)));
+      };
+      const Fr e2 = P->next_row ? wsum(b[11], b[12], b[13]) : Fr::zero();
+      const Fr per[9] = {e2,   wsum(b[0], b[2], b[4]), wsum(b[1], b[3], b[5]), c[0], c[1], c[2],
+                         fp_mul(c[0], w2), fp_mul(c[1], w), c[2]};
+      zs.X = P->xs.as<Fr>();
+      for (int k = 0; k < 4; k++)
+        for (int i = 0; i < 9; i++) zs.w[k][i] = fp_mul(per[i], P->zh[k]);
+      k_quotient_shuffle<true><<<PB_GRID(ne, 128), 0, st>>>(sq, t_evals, zs);
+    } else {
+      k_quotient_shuffle<false><<<PB_GRID(ne, 128), 0, st>>>(sq, t_evals, zs);
+    }
     ctx->launches++;
   }
   PB_CUDA(cudaMemsetAsync(P->flags.p, 0, 64, st));
@@ -1725,6 +1792,11 @@ void prover_round4(Prover* P, const Fr& zeta_c) {
     const Fr* spolys[2] = {P->sh_coeff[Prover::SH_IN].as<Fr>(), P->sh_z3_coeff.as<Fr>()};
     const Fr sxs[2] = {P->zeta, zw};
     eval_polys(P, 2, spolys, sxs, P->sh_ev);
+    if (P->zk) {  // Z3'(zeta w) = Z3(zeta w) + (c2 (zeta w)^2 + c1 zeta w + c0)(zeta^n - 1); Q_in is not blinded
+      const Fr* c = P->zk_z3_b();
+      const Fr zh = fp_sub(fp_pow_u64(P->zeta, P->n), Fr::one());
+      P->sh_ev[1] = fp_add(P->sh_ev[1], fp_mul(fp_add(fp_mul(fp_add(fp_mul(c[0], zw), c[1]), zw), c[2]), zh));
+    }
     for (int k = 0; k < 2; k++) store_canonical(P->sh_evals[k], P->sh_ev[k]);
   }
 }
@@ -1859,7 +1931,8 @@ void prover_round5(Prover* P, const Fr& v_c) {
     lc = fp_sub(lc, fp_mul(al5, l0_ev));
     c0 = fp_add(c0, fp_sub(lc, fp_add(fp_mul(v6, fe), fp_add(fp_mul(v7, te), fp_mul(v8, h2e)))));
   }
-  // shuffle: [Q_out] and [Z3] keep their commitments in the linearisation; Q_in joins the batch at zeta
+  // shuffle: [Q_out] and [Z3] keep their commitments in the linearisation; Q_in joins the batch at zeta.  Zero knowledge:
+  // Z3' (n + 3 coefficients) joins the tail; Q_out and Q_in stay unblinded
   if (P->sh) {
     const Fr &qin = P->sh_ev[0], &z3w = P->sh_ev[1];
     const Fr al2 = fp_sqr(al), al3 = fp_mul(al2, al), al4 = fp_sqr(al2), v6 = fp_mul(v5, v);
@@ -1867,7 +1940,7 @@ void prover_round5(Prover* P, const Fr& v_c) {
     const Fr km1 = fp_add(fp_sub(P->kappa, one), fp_add(a, fp_add(fp_mul(th, b), fp_mul(fp_sqr(th), c))));  // k + w - 1
     const Fr a3z = fp_mul(al3, z3w), a4l0 = fp_mul(al4, l0_ev);
     add(P->sh_coeff[Prover::SH_OUT].as<Fr>(), fp_mul(a3z, km1));                                    // a3 z3w (k + w - 1)
-    add(P->sh_z3_coeff.as<Fr>(), fp_sub(a4l0, fp_mul(al3, fp_add(one, fp_mul(qin, km1)))));  // -a3 (1 + q_in(..)) + a4 L0
+    add(P->sh_z3_poly(), fp_sub(a4l0, fp_mul(al3, fp_add(one, fp_mul(qin, km1)))), true);  // -a3 (1 + q_in(..)) + a4 L0
     add(P->sh_coeff[Prover::SH_IN].as<Fr>(), v6);
     // a3 z3w - a4 L0(zeta) - v^6 q_in(zeta)
     c0 = fp_add(c0, fp_sub(a3z, fp_add(a4l0, fp_mul(v6, qin))));
@@ -1908,9 +1981,9 @@ void prover_round5(Prover* P, const Fr& v_c) {
     M.count = 4;
     M.c0 = fp_sub(M.c0, fp_add(fp_mul(v, *aw), fp_add(fp_mul(v2, *bw), fp_mul(v3, *cw))));
   }
-  if (P->sh) {  // + v^k (Z3 - z3(zeta w)): k = 1, or 4 after A, B, C on a next-row prover
+  if (P->sh) {  // + v^k (Z3 - z3(zeta w)): k = 1, or 4 after A, B, C on a next-row prover; zero knowledge: Z3', padded
     const Fr vk = P->next_row ? v4 : v;
-    M.vec[M.count] = P->sh_z3_coeff.as<Fr>(); M.w[M.count] = vk; M.count++;
+    M.vec[M.count] = P->sh_z3_poly(); M.w[M.count] = vk; M.count++;
     M.c0 = fp_sub(M.c0, fp_mul(vk, P->sh_ev[1]));
   }
   Fr* wzw = P->tmp[0].as<Fr>();  // the W_z numerator is no longer needed

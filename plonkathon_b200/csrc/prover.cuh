@@ -142,7 +142,9 @@ struct Prover {
   // With a lookup table (prover_set_zk_lookup) there are 21 scalars: b12..b21 blind F, H1, H2 and Z2.  A next-row
   // prover takes 14: b12..b14 give A, B, C a third blinder each (they are opened at zeta and at zeta w), so T3' has
   // n + 9 coefficients and the blinded vectors get ZK_NR_PAD elements of padding.
+  // With a shuffle (prover_set_zk_shuffle) Z3 takes three more, always the last three: 14 scalars, 17 next-row.
   static const int ZK_BLINDERS = 11, ZK_LK_BLINDERS = 21, ZK_NR_BLINDERS = 14, ZK_PAD = 8, ZK_NR_PAD = 9;
+  static const int ZK_SH_BLINDERS = 14, ZK_NR_SH_BLINDERS = 17;
   bool zk = false;
   bool zk_fixed = false;          // the same blinders for every proof (zk_fixed_b) instead of fresh OS randomness
   Fr zk_fixed_b[ZK_LK_BLINDERS];  // canonical
@@ -150,7 +152,13 @@ struct Prover {
   DevBuf zk_coeff[4];             // A' B' C' (n + 2 coefficients, n + 3 next-row) Z' (n + 3)
   DevBuf zk_t[3];                 // T1' T2' (n + 1 coefficients) T3' (n + 6, n + 9 next-row)
   DevBuf zk_lk[5];                // lookups: T (n, zero padded) F' H2' (n + 2) H1' Z2' (n + 3), indexed by LK_*
-  int zk_blinders() const { return lk ? ZK_LK_BLINDERS : next_row ? ZK_NR_BLINDERS : ZK_BLINDERS; }
+  DevBuf zk_z3;                   // shuffles: Z3' (n + 3, zero padded)
+  int zk_blinders() const {
+    if (lk) return ZK_LK_BLINDERS;
+    if (sh) return next_row ? ZK_NR_SH_BLINDERS : ZK_SH_BLINDERS;
+    return next_row ? ZK_NR_BLINDERS : ZK_BLINDERS;
+  }
+  const Fr* zk_z3_b() const { return zk_b + zk_blinders() - 3; }  // Z3's X^2, X and constant blinders
   uint64_t zk_pad() const { return next_row ? ZK_NR_PAD : ZK_PAD; }
   uint64_t zk_t3_len() const { return n + (next_row ? 9 : 6); }  // coefficients of T3' (deg T <= 3n + 5, or 3n + 8)
   // Lookup argument (prover_set_lookup, one GPU): plookup over one fixed table of three columns, or over several
@@ -188,6 +196,8 @@ struct Prover {
   DevBuf sh_coeff[2];                  // ... coefficients ...
   DevBuf sh_ext[2];                    // ... on the 4n coset
   DevBuf sh_z3_lag, sh_z3_coeff, sh_z3_ext;  // Z3: Lagrange values, coefficients, on the 4n coset
+  // the coefficient vector of Z3 a proof commits and opens: the unblinded sh_z3_coeff, or zk_z3 in zero-knowledge mode
+  const Fr* sh_z3_poly() const { return (zk ? zk_z3 : sh_z3_coeff).as<Fr>(); }
   Fr theta, kappa;                     // Montgomery
   Fr sh_ev[2];                         // q_in(zeta), Z3(zeta w) (Montgomery)
   uint8_t sh_pt[64];                   // z3_1 (canonical LE x||y)

@@ -149,6 +149,10 @@ class ShardedProver(Prover):
         """Zero-knowledge lookup proofs run on one GPU only (``Prover.set_zk_lookup``); so do lookups."""
         raise ValueError("zero-knowledge lookups are not available on the sharded prover (one GPU only)")
 
+    def set_zk_shuffle(self, enable: bool = True, blinders=None):
+        """Zero-knowledge shuffle proofs run on one GPU only (``Prover.set_zk_shuffle``); so do shuffles."""
+        raise ValueError("zero-knowledge shuffles are not available on the sharded prover (one GPU only)")
+
 
 # ------------------------------------------------------------------------------------------------
 # operators (BASELINE.json metric: Fr-NTT elems/s and G1-MSM pts/s at 1/2/4/8 GPUs)

@@ -270,7 +270,8 @@ class Prover:
         ``shuffle``: ``(q_in, q_out)``, two boolean selectors with as many ones each: the rows with q_in = 1 hold the
         same multiset of (a, b, c) as the rows with q_out = 1 (plonkathon_b200/shuffle.py).  ``prove_arrays`` then returns
         an 896-byte ``ShuffleProof``, or a 992-byte ``NextRowShuffleProof`` with next-row terms.  ValueError for
-        malformed selectors and for a shuffle with lookups; the library refuses it with zero knowledge."""
+        malformed selectors and for a shuffle with lookups.  Zero knowledge goes through ``set_zk_shuffle`` after the
+        prover is made; ``set_zk`` refuses a shuffle prover."""
         if lookup is not None and lookups is not None:
             raise ValueError("pass either lookup= (one table) or lookups= (several tables), not both")
         if shuffle is not None and (lookup is not None or lookups is not None):
@@ -557,6 +558,26 @@ class Prover:
                 raise ValueError("zero-knowledge blinders must lie in [0, r)")
             raw = b"".join(b.to_bytes(32, "little") for b in blinders)
         _lib.check(_lib.lib().pb200_prover_set_zk_lookup(self._h, 1 if enable else 0, raw))
+        self.zk = bool(enable)
+
+    def set_zk_shuffle(self, enable: bool = True, blinders=None):
+        """Zero-knowledge mode for the later proofs of a shuffle prover (``shuffle=``): ``set_zk``'s blinding and 3 more
+        scalars for Z3, the last three: 14 in all, 17 with next-row custom gate terms (DESIGN.md section 1).  The proofs
+        keep their 896 (992) bytes and the verifier does not change.  ``blinders=None``: fresh scalars from the OS CSPRNG
+        for every proof; otherwise 14 (17) integers in [0, r) used for every proof (reproducible tests only).
+        ``enable=False`` (or ``set_zk(False)``) returns to plain shuffle proofs.  Needs a shuffle, n >= 8 and an SRS of
+        n + 6 powers (n >= 16 and n + 9 powers with next-row terms)."""
+        raw = None
+        if enable and blinders is not None:
+            blinders = [int(b) for b in blinders]
+            count = 17 if getattr(self, "next_row", False) else 14
+            if len(blinders) != count:
+                raise ValueError("zero-knowledge shuffles take %d blinders b1..b%d%s, got %d" % (
+                    count, count, " on a prover with next-row terms" if count == 17 else "", len(blinders)))
+            if any(not 0 <= b < CURVE_ORDER for b in blinders):
+                raise ValueError("zero-knowledge blinders must lie in [0, r)")
+            raw = b"".join(b.to_bytes(32, "little") for b in blinders)
+        _lib.check(_lib.lib().pb200_prover_set_zk_shuffle(self._h, 1 if enable else 0, raw))
         self.zk = bool(enable)
 
     def _commitments(self, first_slot: int, count: int, raw: bytes):

@@ -10,11 +10,13 @@ A row with both selectors cancels out.
 The argument is one more grand product Z3 (DESIGN.md section 1): with challenges theta, kappa drawn after beta, gamma and
 w_i = a_i + theta b_i + theta^2 c_i, Z3_(i+1) = Z3_i (1 + q_in[i](kappa + w_i - 1)) / (1 + q_out[i](kappa + w_i - 1)),
 and Z3_n = 1.  A shuffle proof has 896 bytes (``ShuffleProof``), 992 with next-row custom gate terms
-(``NextRowShuffleProof``).
+(``NextRowShuffleProof``).  ``Prover.set_zk_shuffle`` makes the proofs zero-knowledge: A, B, C, Z and the quotient
+pieces are blinded as in ``Prover.set_zk``, and Z3 with three more scalars, so a guess at the in-rows or out-rows cannot
+be tested against z3_1.  The proof size and the verifier stay the same.
 
 Here: the checks on a shuffle as users give it, ``(q_in, q_out)``, shared by ``Prover.from_arrays``,
-``Setup.verification_key_arrays`` and ``synthetic.build_circuit``.  Refused: a shuffle together with lookups, with zero
-knowledge, or on the sharded prover."""
+``Setup.verification_key_arrays`` and ``synthetic.build_circuit``.  Refused: a shuffle together with lookups, or on the
+sharded prover."""
 from __future__ import annotations
 
 from .lookup import _column_ints
