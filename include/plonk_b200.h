@@ -127,6 +127,21 @@ int pb200_srs_commit_coeffs_host(pb200_ctx* ctx, pb200_srs* srs, const uint8_t* 
                                  uint8_t* h_out_xy, int* is_identity);
 
 /* ---- Prover (prover.py:39-306) ---------------------------------------------------------------- */
+/* Proof layout.  A prover's proof is the plain 15 fields, then the fields of the blocks it has (next-row custom gate
+ * terms, a shuffle, a lookup argument), in this order; a point is 64 bytes (x||y), a scalar 32, big-endian in a proof
+ * and little-endian from the round entry points.  Within each transcript step the fields are absorbed in the same
+ * order (plonkathon_b200/transcript.py holds the table).
+ *
+ *   kind                   bytes  fields after the plain 15, in byte order
+ *   plain                    768  none
+ *   next-row                 864  a_shifted_eval b_shifted_eval c_shifted_eval
+ *   shuffle                  896  z3_1 qin_eval z3_shifted_eval
+ *   next-row shuffle         992  the next-row three, then the shuffle three
+ *   lookup (one or tagged)  1216  f_1 h1_1 h2_1 z2_1 f_eval t_eval t_shifted_eval h2_eval h1_shifted_eval z2_shifted_eval
+ *
+ * Each kind has its own prove and serialize entry points, and round 2 / round 4 entry points where its fields of that
+ * step differ from the plain ones; each round entry point returns its step's fields in this order.  An entry point of
+ * another kind returns an error naming the prover's proof size and its own entry point. */
 /* prover.py:45-49  Prover(setup, program): h_pk = 8 pointers, in the order of CommonPreprocessedInput
  * (compiler/program.py:10-30): QM QL QR QO QC S1 S2 S3, each 2^log_n Lagrange values (canonical).
  * Converts them to coefficients and to a cached 4n coset extension in HBM. */
@@ -193,9 +208,9 @@ int pb200_prover_round_lookup(pb200_prover* p, const uint8_t* eta, uint8_t* h_fh
 /* round 2 with the lookup challenges: commitments z_1 z2_1 */
 int pb200_prover_round2_lookup(pb200_prover* p, const uint8_t* beta, const uint8_t* gamma, const uint8_t* delta,
                                const uint8_t* epsilon, uint8_t* h_zz2_xy /*2*64*/);
-/* round 4: the 6 plain evaluations, then f, t, t(zeta w), h2, h1(zeta w), z2(zeta w) */
+/* round 4: the 6 plain evaluations, then the six lookup evaluations (Proof layout) */
 int pb200_prover_round4_lookup(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals /*12*32*/);
-/* the whole proof: 768 plain bytes, then f_1 h1_1 h2_1 z2_1, then the six lookup evaluations (1216 bytes) */
+/* the whole proof (1216 bytes, Proof layout) */
 int pb200_prover_prove_lookup(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                               const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof1216);
 int pb200_prover_serialize_lookup(pb200_prover* p, uint8_t* h_proof1216);
@@ -224,7 +239,7 @@ int pb200_prover_create_custom_next_row(pb200_ctx* ctx, pb200_srs* srs, unsigned
                                         pb200_prover** out);
 /* round 4 of a next-row prover: the 6 plain evaluations, then a(zeta w), b(zeta w), c(zeta w) */
 int pb200_prover_round4_next_row(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals /*9*32*/);
-/* the whole proof: the 768 plain bytes, then a_shifted_eval, b_shifted_eval, c_shifted_eval (864 bytes) */
+/* the whole proof (864 bytes, Proof layout) */
 int pb200_prover_prove_next_row(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                                 const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof864);
 int pb200_prover_serialize_next_row(pb200_prover* p, uint8_t* h_proof864);
@@ -233,8 +248,8 @@ int pb200_prover_serialize_next_row(pb200_prover* p, uint8_t* h_proof864);
  * ones in each) claim that the multiset {(a_i, b_i, c_i) : q_in[i] = 1} equals {(a_i, b_i, c_i) : q_out[i] = 1}, with
  * no copy constraint between the two sides.  Set once, before the first proof.  Round 1 is unchanged; the transcript
  * then draws theta and kappa after beta and gamma, round 2 commits the grand product Z3 beside Z, round 4 adds
- * q_in(zeta) and Z3(zeta w).  A proof has 896 bytes: the 768 plain bytes, then z3_1, qin_eval, z3_shifted_eval; on a
- * next-row prover 992 bytes, with a, b, c at zeta w before z3_1.  A witness whose two sides differ fails round 2 with
+ * q_in(zeta) and Z3(zeta w).  A proof has 896 bytes, 992 on a next-row prover (Proof layout).  A witness whose two
+ * sides differ fails round 2 with
  * "AssertionError: shuffle: the q_in rows and the q_out rows are not permutations of each other".
  * Errors, the prover left as it was: the sharded prover, a lookup table, zero-knowledge mode (set the shuffle first,
  * then pb200_prover_set_zk_shuffle), selectors already set, a selector value other than 0 / 1, unequal numbers of
@@ -253,7 +268,7 @@ int pb200_prover_set_zk_shuffle(pb200_prover* p, int enable, const uint8_t* h_bl
 /* round 2 of a shuffle prover: z_1 then z3_1 */
 int pb200_prover_round2_shuffle(pb200_prover* p, const uint8_t* beta, const uint8_t* gamma, const uint8_t* theta,
                                 const uint8_t* kappa, uint8_t* h_zz3_xy /*2*64*/);
-/* round 4: the 6 plain evaluations, then qin_eval, z3_shifted_eval; the next-row form puts a, b, c at zeta w between */
+/* round 4: the plain evaluations, then the next-row (for the _next_row_shuffle form) and shuffle ones (Proof layout) */
 int pb200_prover_round4_shuffle(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals /*8*32*/);
 int pb200_prover_round4_next_row_shuffle(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals /*11*32*/);
 int pb200_prover_prove_shuffle(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,

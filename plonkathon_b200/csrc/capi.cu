@@ -47,21 +47,17 @@ void prover_prove(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t
                   uint64_t n_public, uint8_t* out, bool wires_on_device);
 void prover_round1(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t* hC, const uint8_t* h_public,
                    uint64_t n_public, bool wires_on_device);
-void prover_round2(Prover* P, const Fr& beta_c, const Fr& gamma_c);
+void prover_round2(Prover* P, const Fr* ch);
 void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c);
 void prover_round4(Prover* P, const Fr& zeta_c);
 void prover_round5(Prover* P, const Fr& v_c);
 void prover_serialize(const Prover* P, uint8_t* out);
-void prover_set_zk(Prover* P, bool enable, const uint8_t* h_blinders);
-void prover_set_zk_lookup(Prover* P, bool enable, const uint8_t* h_blinders);
+size_t copy_step(const Prover* P, int step, uint8_t* out);
+void prover_set_zk(Prover* P, unsigned block, bool enable, const uint8_t* h_blinders);
 void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* h_qtag, const uint8_t* const* h_tab,
                        uint64_t rows);
 void prover_round_lookup(Prover* P, const Fr& eta_c);
-void prover_round2_lookup(Prover* P, const Fr& beta_c, const Fr& gamma_c, const Fr& delta_c, const Fr& epsilon_c);
-void prover_round4_lookup(Prover* P, const Fr& zeta_c);
 void prover_set_shuffle(Prover* P, const uint8_t* h_qin, const uint8_t* h_qout);
-void prover_set_zk_shuffle(Prover* P, bool enable, const uint8_t* h_blinders);
-void prover_round2_shuffle(Prover* P, const Fr& beta_c, const Fr& gamma_c, const Fr& theta_c, const Fr& kappa_c);
 void g1_combine_partials_host(const G1XYZZ* parts, uint32_t count, uint8_t* out_xy, int* is_identity);
 void host_join_bucket_shards(const SR* all, uint32_t world, uint32_t sets, uint32_t nloc, G1XYZZ* out);
 void host_join_bucket_shards_strided(const SR* all, uint32_t world, uint32_t sets, G1XYZZ* out);
@@ -86,16 +82,6 @@ static thread_local std::string g_err;
 
 static Context* C(pb200_ctx* c) { return reinterpret_cast<Context*>(c); }
 
-// the 768-byte entry points (and the plain round 2 / round 4) on a prover with a lookup table
-#define PB_NOT_LOOKUP(P, entry)                                                                       \
-  PB_CHECK(!(P)->lk, "this prover has a lookup argument: its proofs have 1216 bytes; use " entry)
-// the 768-byte entry points (and the plain round 4) on a prover with next-row custom gate terms
-#define PB_NOT_NEXT_ROW(P, entry)                                                                     \
-  PB_CHECK(!(P)->next_row, "this prover has next-row custom gate terms: its proofs have 864 bytes; use " entry)
-// the entry points without a shuffle (and the plain round 2 / round 4) on a prover with a shuffle
-#define PB_NOT_SHUFFLE(P, entry)                                                                      \
-  PB_CHECK(!(P)->sh, "this prover has a shuffle: its proofs have 896 bytes (992 with next-row terms); use " entry)
-
 // Every entry point that touches the GPU runs on its context's device, whatever device the calling host thread had
 // current (contexts on several GPUs in one process, provers driven from worker threads); the previous device is
 // restored on the way out.
@@ -115,6 +101,88 @@ static Fr load_fr_canonical(const uint8_t* h) {
   memcpy(a.v, h, 32);
   PB_CHECK(fp_is_canonical(a), "Fr value not reduced below the modulus");
   return a;
+}
+
+// ---- the proof-kind entry points ------------------------------------------------------------------------------------
+// Each proof kind has its own prove, serialize and round entry points, so the size of the caller's buffer never
+// depends on the prover's state.  An entry point of kind `kind` (a set of blocks, proof_layout.cuh) serves the provers
+// that agree with it on the blocks adding fields to what it returns: one step's fields, or the whole proof.
+static std::string kind_suffix(unsigned blocks) {
+  std::string s;
+  if (blocks & BLOCK_NEXT_ROW) s += "_next_row";
+  if (blocks & BLOCK_SHUFFLE) s += "_shuffle";
+  if (blocks & BLOCK_LOOKUP) s += "_lookup";
+  return s;
+}
+
+// refuses a prover of another kind, naming its proof size and its entry point `fn`
+static void require_kind(const Prover* P, unsigned kind, const char* fn, int step = -1, const char* note = "") {
+  const unsigned blocks = P->blocks(), mask = step_blocks(step), have = blocks & mask;
+  if (have == (kind & mask)) return;
+  static const struct { unsigned block; const char *has, *lacks; } what[] = {
+      {BLOCK_LOOKUP, "a lookup argument", "no lookup table"},
+      {BLOCK_NEXT_ROW, "next-row custom gate terms", "no next-row custom gate terms"},
+      {BLOCK_SHUFFLE, "a shuffle", "no shuffle"}};
+  std::string msg = "this prover";
+  const char* join = " has ";
+  for (const auto& w : what)
+    if ((have ^ kind) & mask & w.block) {
+      msg += join;
+      msg += have & w.block ? w.has : w.lacks;
+      join = " and has ";
+    }
+  msg += ": its proofs have " + std::to_string(layout_bytes(blocks)) + " bytes";
+  if (blocks & BLOCK_NEXT_ROW)
+    msg += " (" + std::to_string(layout_bytes(blocks & ~BLOCK_NEXT_ROW)) + " without next-row terms, " +
+           std::to_string(layout_bytes(blocks)) + " with next-row terms)";
+  throw Error(msg + "; use pb200_prover_" + fn + kind_suffix(have) + note);
+}
+
+static int prove(pb200_prover* p, unsigned kind, const void* A, const void* B, const void* C, const uint8_t* h_public,
+                 uint64_t n_public, uint8_t* out, bool wires_on_device = false) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  require_kind(P, kind, "prove", -1, wires_on_device ? " (wires in host memory)" : "");
+  prover_prove(P, (const uint8_t*)A, (const uint8_t*)B, (const uint8_t*)C, h_public, n_public, out, wires_on_device);
+  PB_API_END
+}
+static int serialize(pb200_prover* p, unsigned kind, uint8_t* out) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  require_kind(P, kind, "serialize");
+  prover_serialize(P, out);
+  PB_API_END
+}
+// x, y: theta and kappa for a shuffle, delta and epsilon for lookups
+static int round2(pb200_prover* p, unsigned kind, const uint8_t* beta, const uint8_t* gamma, const uint8_t* x,
+                  const uint8_t* y, uint8_t* out) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  require_kind(P, kind, "round2", STEP_2);
+  Fr ch[PROOF_CHALLENGES] = {};
+  ch[CH_BETA] = load_fr_canonical(beta);
+  ch[CH_GAMMA] = load_fr_canonical(gamma);
+  if (kind != BLOCK_PLAIN) {
+    const bool sh = kind & BLOCK_SHUFFLE;
+    ch[sh ? CH_THETA : CH_DELTA] = load_fr_canonical(x);
+    ch[sh ? CH_KAPPA : CH_EPSILON] = load_fr_canonical(y);
+  }
+  prover_round2(P, ch);
+  copy_step(P, STEP_2, out);
+  PB_API_END
+}
+static int round4(pb200_prover* p, unsigned kind, const uint8_t* zeta, uint8_t* out) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  Prover* P = reinterpret_cast<Prover*>(p);
+  require_kind(P, kind, "round4", STEP_4);
+  prover_round4(P, load_fr_canonical(zeta));
+  copy_step(P, STEP_4, out);
+  PB_API_END
+}
+static int set_zk(pb200_prover* p, unsigned block, int enable, const uint8_t* h_blinders) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  prover_set_zk(reinterpret_cast<Prover*>(p), block, enable != 0, h_blinders);
+  PB_API_END
 }
 
 extern "C" {
@@ -467,62 +535,38 @@ void pb200_prover_destroy(pb200_prover* p) { prover_destroy(reinterpret_cast<Pro
 
 int pb200_prover_prove(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                        const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof768) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  PB_NOT_LOOKUP(reinterpret_cast<Prover*>(p), "pb200_prover_prove_lookup");
-  PB_NOT_NEXT_ROW(reinterpret_cast<Prover*>(p), "pb200_prover_prove_next_row");
-  PB_NOT_SHUFFLE(reinterpret_cast<Prover*>(p), "pb200_prover_prove_shuffle");
-  prover_prove(reinterpret_cast<Prover*>(p), h_A, h_B, h_C, h_public, n_public, h_proof768, false);
-  PB_API_END
+  return prove(p, BLOCK_PLAIN, h_A, h_B, h_C, h_public, n_public, h_proof768);
 }
 int pb200_prover_prove_device(pb200_prover* p, const void* d_A, const void* d_B, const void* d_C,
                               const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof768) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  PB_NOT_LOOKUP(reinterpret_cast<Prover*>(p), "pb200_prover_prove_lookup (wires in host memory)");
-  PB_NOT_NEXT_ROW(reinterpret_cast<Prover*>(p), "pb200_prover_prove_next_row (wires in host memory)");
-  PB_NOT_SHUFFLE(reinterpret_cast<Prover*>(p), "pb200_prover_prove_shuffle (wires in host memory)");
-  prover_prove(reinterpret_cast<Prover*>(p), (const uint8_t*)d_A, (const uint8_t*)d_B, (const uint8_t*)d_C, h_public,
-               n_public, h_proof768, true);
-  PB_API_END
+  return prove(p, BLOCK_PLAIN, d_A, d_B, d_C, h_public, n_public, h_proof768, true);
 }
 int pb200_prover_round1(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                         const uint8_t* h_public, uint64_t n_public, uint8_t* h_abc_xy) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   Prover* P = reinterpret_cast<Prover*>(p);
   prover_round1(P, h_A, h_B, h_C, h_public, n_public, false);
-  memcpy(h_abc_xy, P->proof.pts[0], 3 * 64);
+  copy_step(P, STEP_1, h_abc_xy);
   PB_API_END
 }
 int pb200_prover_round2(pb200_prover* p, const uint8_t* beta, const uint8_t* gamma, uint8_t* h_z_xy) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  Prover* P = reinterpret_cast<Prover*>(p);
-  PB_NOT_LOOKUP(P, "pb200_prover_round2_lookup");
-  PB_NOT_SHUFFLE(P, "pb200_prover_round2_shuffle");
-  prover_round2(P, load_fr_canonical(beta), load_fr_canonical(gamma));
-  memcpy(h_z_xy, P->proof.pts[3], 64);
-  PB_API_END
+  return round2(p, BLOCK_PLAIN, beta, gamma, nullptr, nullptr, h_z_xy);
 }
 int pb200_prover_round3(pb200_prover* p, const uint8_t* alpha, const uint8_t* fft_cofactor, uint8_t* h_t_xy) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   Prover* P = reinterpret_cast<Prover*>(p);
   prover_round3(P, load_fr_canonical(alpha), load_fr_canonical(fft_cofactor));
-  memcpy(h_t_xy, P->proof.pts[4], 3 * 64);
+  copy_step(P, STEP_3, h_t_xy);
   PB_API_END
 }
 int pb200_prover_round4(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  Prover* P = reinterpret_cast<Prover*>(p);
-  PB_NOT_LOOKUP(P, "pb200_prover_round4_lookup");
-  PB_NOT_NEXT_ROW(P, "pb200_prover_round4_next_row");
-  PB_NOT_SHUFFLE(P, "pb200_prover_round4_shuffle");
-  prover_round4(P, load_fr_canonical(zeta));
-  memcpy(h_evals, P->proof.evals[0], 6 * 32);
-  PB_API_END
+  return round4(p, BLOCK_PLAIN, zeta, h_evals);
 }
 int pb200_prover_round5(pb200_prover* p, const uint8_t* v, uint8_t* h_w_xy) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   Prover* P = reinterpret_cast<Prover*>(p);
   prover_round5(P, load_fr_canonical(v));
-  memcpy(h_w_xy, P->proof.pts[7], 2 * 64);
+  copy_step(P, STEP_5, h_w_xy);
   PB_API_END
 }
 
@@ -545,23 +589,15 @@ int pb200_prover_read_vector(pb200_prover* p, int which, void* d_out) {
   PB_API_END
 }
 int pb200_prover_set_zk(pb200_prover* p, int enable, const uint8_t* h_blinders) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  prover_set_zk(reinterpret_cast<Prover*>(p), enable != 0, h_blinders);
-  PB_API_END
+  return set_zk(p, BLOCK_PLAIN, enable, h_blinders);
 }
 int pb200_prover_set_zk_lookup(pb200_prover* p, int enable, const uint8_t* h_blinders) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  prover_set_zk_lookup(reinterpret_cast<Prover*>(p), enable != 0, h_blinders);
-  PB_API_END
+  return set_zk(p, BLOCK_LOOKUP, enable, h_blinders);
 }
-int pb200_prover_serialize(pb200_prover* p, uint8_t* h_proof768) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  PB_NOT_LOOKUP(reinterpret_cast<Prover*>(p), "pb200_prover_serialize_lookup");
-  PB_NOT_NEXT_ROW(reinterpret_cast<Prover*>(p), "pb200_prover_serialize_next_row");
-  PB_NOT_SHUFFLE(reinterpret_cast<Prover*>(p), "pb200_prover_serialize_shuffle");
-  prover_serialize(reinterpret_cast<Prover*>(p), h_proof768);
-  PB_API_END
+int pb200_prover_set_zk_shuffle(pb200_prover* p, int enable, const uint8_t* h_blinders) {
+  return set_zk(p, BLOCK_SHUFFLE, enable, h_blinders);
 }
+int pb200_prover_serialize(pb200_prover* p, uint8_t* h_proof768) { return serialize(p, BLOCK_PLAIN, h_proof768); }
 int pb200_prover_set_lookup(pb200_prover* p, const uint8_t* h_qk, const uint8_t* h_t1, const uint8_t* h_t2,
                             const uint8_t* h_t3, uint64_t table_rows) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
@@ -581,144 +617,61 @@ int pb200_prover_round_lookup(pb200_prover* p, const uint8_t* eta, uint8_t* h_fh
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   Prover* P = reinterpret_cast<Prover*>(p);
   prover_round_lookup(P, load_fr_canonical(eta));
-  memcpy(h_fh_xy, P->lk_pts[0], 3 * 64);
+  copy_step(P, STEP_1L, h_fh_xy);
   PB_API_END
 }
 int pb200_prover_round2_lookup(pb200_prover* p, const uint8_t* beta, const uint8_t* gamma, const uint8_t* delta,
                                const uint8_t* epsilon, uint8_t* h_zz2_xy) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  Prover* P = reinterpret_cast<Prover*>(p);
-  prover_round2_lookup(P, load_fr_canonical(beta), load_fr_canonical(gamma), load_fr_canonical(delta),
-                       load_fr_canonical(epsilon));
-  memcpy(h_zz2_xy, P->proof.pts[3], 64);
-  memcpy(h_zz2_xy + 64, P->lk_pts[3], 64);
-  PB_API_END
+  return round2(p, BLOCK_LOOKUP, beta, gamma, delta, epsilon, h_zz2_xy);
 }
 int pb200_prover_round4_lookup(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  Prover* P = reinterpret_cast<Prover*>(p);
-  prover_round4_lookup(P, load_fr_canonical(zeta));
-  memcpy(h_evals, P->proof.evals[0], 6 * 32);
-  memcpy(h_evals + 6 * 32, P->lk_evals[0], 6 * 32);
-  PB_API_END
+  return round4(p, BLOCK_LOOKUP, zeta, h_evals);
 }
 int pb200_prover_prove_lookup(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                               const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof1216) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  Prover* P = reinterpret_cast<Prover*>(p);
-  PB_CHECK(P->lk, "this prover has no lookup table (pb200_prover_set_lookup)");
-  prover_prove(P, h_A, h_B, h_C, h_public, n_public, h_proof1216, false);
-  PB_API_END
+  return prove(p, BLOCK_LOOKUP, h_A, h_B, h_C, h_public, n_public, h_proof1216);
 }
 int pb200_prover_serialize_lookup(pb200_prover* p, uint8_t* h_proof1216) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  Prover* P = reinterpret_cast<Prover*>(p);
-  PB_CHECK(P->lk, "this prover has no lookup table: use pb200_prover_serialize (768 bytes)");
-  prover_serialize(P, h_proof1216);
-  PB_API_END
+  return serialize(p, BLOCK_LOOKUP, h_proof1216);
 }
 int pb200_prover_round4_next_row(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  Prover* P = reinterpret_cast<Prover*>(p);
-  PB_CHECK(P->next_row, "this prover has no next-row custom gate terms: use pb200_prover_round4");
-  PB_NOT_SHUFFLE(P, "pb200_prover_round4_next_row_shuffle");
-  prover_round4(P, load_fr_canonical(zeta));
-  memcpy(h_evals, P->proof.evals[0], 6 * 32);
-  memcpy(h_evals + 6 * 32, P->nr_evals[0], 3 * 32);
-  PB_API_END
+  return round4(p, BLOCK_NEXT_ROW, zeta, h_evals);
 }
 int pb200_prover_prove_next_row(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                                 const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof864) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  Prover* P = reinterpret_cast<Prover*>(p);
-  PB_CHECK(P->next_row, "this prover has no next-row custom gate terms: use pb200_prover_prove (768 bytes)");
-  PB_NOT_SHUFFLE(P, "pb200_prover_prove_next_row_shuffle");
-  prover_prove(P, h_A, h_B, h_C, h_public, n_public, h_proof864, false);
-  PB_API_END
+  return prove(p, BLOCK_NEXT_ROW, h_A, h_B, h_C, h_public, n_public, h_proof864);
 }
 int pb200_prover_serialize_next_row(pb200_prover* p, uint8_t* h_proof864) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  Prover* P = reinterpret_cast<Prover*>(p);
-  PB_CHECK(P->next_row, "this prover has no next-row custom gate terms: use pb200_prover_serialize (768 bytes)");
-  PB_NOT_SHUFFLE(P, "pb200_prover_serialize_next_row_shuffle");
-  prover_serialize(P, h_proof864);
-  PB_API_END
+  return serialize(p, BLOCK_NEXT_ROW, h_proof864);
 }
 int pb200_prover_set_shuffle(pb200_prover* p, const uint8_t* h_qin, const uint8_t* h_qout) {
   PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
   prover_set_shuffle(reinterpret_cast<Prover*>(p), h_qin, h_qout);
   PB_API_END
 }
-int pb200_prover_set_zk_shuffle(pb200_prover* p, int enable, const uint8_t* h_blinders) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  prover_set_zk_shuffle(reinterpret_cast<Prover*>(p), enable != 0, h_blinders);
-  PB_API_END
-}
 int pb200_prover_round2_shuffle(pb200_prover* p, const uint8_t* beta, const uint8_t* gamma, const uint8_t* theta,
                                 const uint8_t* kappa, uint8_t* h_zz3_xy) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  Prover* P = reinterpret_cast<Prover*>(p);
-  prover_round2_shuffle(P, load_fr_canonical(beta), load_fr_canonical(gamma), load_fr_canonical(theta),
-                        load_fr_canonical(kappa));
-  memcpy(h_zz3_xy, P->proof.pts[3], 64);
-  memcpy(h_zz3_xy + 64, P->sh_pt, 64);
-  PB_API_END
-}
-// a shuffle prover of the kind `next_row`: its entry points of one proof size refuse the other kind
-static void shuffle_kind(const Prover* P, bool next_row, const char* other) {
-  PB_CHECK(P->sh, "this prover has no shuffle (pb200_prover_set_shuffle)");
-  PB_CHECK(P->next_row == next_row, (std::string(next_row ? "this shuffle prover has no next-row custom gate terms: use "
-                                                          : "this shuffle prover has next-row custom gate terms: use ") +
-                                     other).c_str());
+  return round2(p, BLOCK_SHUFFLE, beta, gamma, theta, kappa, h_zz3_xy);
 }
 int pb200_prover_round4_shuffle(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  Prover* P = reinterpret_cast<Prover*>(p);
-  shuffle_kind(P, false, "pb200_prover_round4_next_row_shuffle");
-  prover_round4(P, load_fr_canonical(zeta));
-  memcpy(h_evals, P->proof.evals[0], 6 * 32);
-  memcpy(h_evals + 6 * 32, P->sh_evals[0], 2 * 32);
-  PB_API_END
+  return round4(p, BLOCK_SHUFFLE, zeta, h_evals);
 }
 int pb200_prover_round4_next_row_shuffle(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  Prover* P = reinterpret_cast<Prover*>(p);
-  shuffle_kind(P, true, "pb200_prover_round4_shuffle");
-  prover_round4(P, load_fr_canonical(zeta));
-  memcpy(h_evals, P->proof.evals[0], 6 * 32);
-  memcpy(h_evals + 6 * 32, P->nr_evals[0], 3 * 32);
-  memcpy(h_evals + 9 * 32, P->sh_evals[0], 2 * 32);
-  PB_API_END
+  return round4(p, BLOCK_NEXT_ROW | BLOCK_SHUFFLE, zeta, h_evals);
 }
 int pb200_prover_prove_shuffle(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                                const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof896) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  Prover* P = reinterpret_cast<Prover*>(p);
-  shuffle_kind(P, false, "pb200_prover_prove_next_row_shuffle (992 bytes)");
-  prover_prove(P, h_A, h_B, h_C, h_public, n_public, h_proof896, false);
-  PB_API_END
+  return prove(p, BLOCK_SHUFFLE, h_A, h_B, h_C, h_public, n_public, h_proof896);
 }
 int pb200_prover_serialize_shuffle(pb200_prover* p, uint8_t* h_proof896) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  Prover* P = reinterpret_cast<Prover*>(p);
-  shuffle_kind(P, false, "pb200_prover_serialize_next_row_shuffle (992 bytes)");
-  prover_serialize(P, h_proof896);
-  PB_API_END
+  return serialize(p, BLOCK_SHUFFLE, h_proof896);
 }
 int pb200_prover_prove_next_row_shuffle(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                                         const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof992) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  Prover* P = reinterpret_cast<Prover*>(p);
-  shuffle_kind(P, true, "pb200_prover_prove_shuffle (896 bytes)");
-  prover_prove(P, h_A, h_B, h_C, h_public, n_public, h_proof992, false);
-  PB_API_END
+  return prove(p, BLOCK_NEXT_ROW | BLOCK_SHUFFLE, h_A, h_B, h_C, h_public, n_public, h_proof992);
 }
 int pb200_prover_serialize_next_row_shuffle(pb200_prover* p, uint8_t* h_proof992) {
-  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
-  Prover* P = reinterpret_cast<Prover*>(p);
-  shuffle_kind(P, true, "pb200_prover_serialize_shuffle (896 bytes)");
-  prover_serialize(P, h_proof992);
-  PB_API_END
+  return serialize(p, BLOCK_NEXT_ROW | BLOCK_SHUFFLE, h_proof992);
 }
 int pb200_g1_combine_partials_host(const uint8_t* h_xyzz, unsigned count, uint8_t* h_out_xy, int* is_identity) {
   PB_API_BEGIN

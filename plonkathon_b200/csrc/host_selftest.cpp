@@ -1,6 +1,7 @@
 // Host build of the limb-level arithmetic in field.cuh / curve.cuh (same code path as the device,
 // PTX carry-chain primitives replaced by their emulation).  TEST INFRASTRUCTURE: loaded only by
-// tests/test_host_arith.py through ctypes; never linked into libplonk_b200.so.
+// tests/test_host_arith.py through ctypes; never linked into libplonk_b200.so.  It also exports the proof layout
+// (proof_layout.cuh) for tests/test_proof_layout.py.
 #include "field.cuh"
 #include "curve.cuh"
 #include "msm_digits.cuh"
@@ -8,6 +9,7 @@
 #include "msm_bucket.cuh"
 #include "msm_sort.cuh"
 #include "ntt_shard.cuh"
+#include "proof_layout.cuh"
 #include <algorithm>
 #include <vector>
 #include <cstring>
@@ -523,5 +525,23 @@ int hs_msm_pipeline(const uint32_t* points, uint32_t n, const uint32_t* scalars,
     emit(r, 0);
   }
   return rounds;
+}
+}
+
+extern "C" {
+// field k of the proof layout: its label, -> is_point, step, block; null past the last field
+const char* hs_proof_field(int k, int* is_point, int* step, int* block) {
+  if (k < 0 || k >= PROOF_FIELDS) return nullptr;
+  *is_point = PROOF_LAYOUT[k].is_point;
+  *step = PROOF_LAYOUT[k].step;
+  *block = (int)PROOF_LAYOUT[k].block;
+  return PROOF_LAYOUT[k].label;
+}
+// challenge k: its label, -> step, block; null past the last challenge
+const char* hs_proof_challenge(int k, int* step, int* block) {
+  if (k < 0 || k >= PROOF_CHALLENGES) return nullptr;
+  *step = CHALLENGE_LAYOUT[k].step;
+  *block = (int)CHALLENGE_LAYOUT[k].block;
+  return CHALLENGE_LAYOUT[k].label;
 }
 }

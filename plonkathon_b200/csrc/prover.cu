@@ -21,7 +21,7 @@
 // proof keeps its 15 fields and the verifier does not change.  See "zero knowledge" below.
 // A shuffle (Prover::sh, one GPU) proves that two sets of rows hold the same multiset of (a, b, c): one more grand
 // product Z3 beside Z, see "shuffle" below; the proof gains z3_1 and two evaluations (896 bytes, 992 next-row).  In
-// zero-knowledge mode (prover_set_zk_shuffle) Z3 takes three more blinders and the proof keeps its size.
+// zero-knowledge mode (pb200_prover_set_zk_shuffle) Z3 takes three more blinders and the proof keeps its size.
 // Custom terms over the next row (Prover::next_row, one GPU) read a(wX), b(wX), c(wX): k_gate_check<true> and
 // k_quotient<ZK, true> read index + 1 (mod n) and coset index + 4, round 4 adds A, B, C at zeta w and round 5 opens them
 // there with Z; the proof gains those three evaluations (864 bytes).
@@ -618,7 +618,7 @@ struct LookupQuotientArgs {
   Fr eta, eta2, eta3, delta, eps, one_d, eps_one_d, alpha3, alpha4, alpha5, one;
   uint64_t n4;
 };
-// Zero knowledge (prover_set_zk_lookup): the kernel reads the unblinded extensions and adds the Z_H multiples, as
+// Zero knowledge (pb200_prover_set_zk_lookup): the kernel reads the unblinded extensions and adds the Z_H multiples, as
 // k_quotient<true> does.  F' = F + (b12 X + b13) Z_H, H1' = H1 + (b14 X^2 + b15 X + b16) Z_H, H2' = H2 + (b17 X + b18) Z_H,
 // Z2' = Z2 + (b19 X^2 + b20 X + b21) Z_H, and A' + eta B' + eta^2 C' = A + eta B + eta^2 C + (e1 X + e0) Z_H with
 // e1 = b1 + eta b3 + eta^2 b5, e0 = b2 + eta b4 + eta^2 b6.  w[k] = Z_H class k times
@@ -683,7 +683,7 @@ struct ShuffleQuotientArgs {
   Fr theta, theta2, kappa_m1, alpha3, alpha4, one;
   uint64_t n4;
 };
-// Zero knowledge (prover_set_zk_shuffle): the kernel reads the unblinded extensions and adds the Z_H multiples, as
+// Zero knowledge (pb200_prover_set_zk_shuffle): the kernel reads the unblinded extensions and adds the Z_H multiples, as
 // k_quotient_lookup<true> does.  Z3' = Z3 + (c2 X^2 + c1 X + c0) Z_H with Z3's blinders c2, c1, c0 (the last three), and
 // A' + theta B' + theta^2 C' = W + (e2 X^2 + e1 X + e0) Z_H with e1 = b1 + theta b3 + theta^2 b5, e0 = b2 + theta b4 +
 // theta^2 b6, e2 = b12 + theta b13 + theta^2 b14 on a next-row prover and 0 otherwise.  w[k] = Z_H class k times
@@ -1009,8 +1009,20 @@ static void zk_enable(Prover* P, const uint8_t* h_blinders) {
   P->zk = true;
 }
 
-void prover_set_zk(Prover* P, bool enable, const uint8_t* h_blinders) {
-  if (!enable) {  // also ends zero-knowledge lookup and shuffle proofs (prover_set_zk_lookup, prover_set_zk_shuffle)
+// Zero-knowledge mode through the entry point of `block`: pb200_prover_set_zk (BLOCK_PLAIN) on a prover without a
+// lookup table or shuffle; pb200_prover_set_zk_lookup (BLOCK_LOOKUP), the 11 blinders and b12..b21 for F, H1, H2 and
+// Z2 (see "zero knowledge with lookups" below); pb200_prover_set_zk_shuffle (BLOCK_SHUFFLE), the 11 blinders (14 on a
+// next-row prover) and the last three for Z3 (see "zero knowledge with a shuffle").  Separate entry points because
+// they take other numbers of blinders: the size of the caller's buffer never depends on the prover's state.
+// Switching off through any of them ends zero-knowledge mode.
+void prover_set_zk(Prover* P, unsigned block, bool enable, const uint8_t* h_blinders) {
+  if (block != BLOCK_PLAIN) {
+    PB_CHECK(P->world == 1, "zero-knowledge proving is not available on the sharded prover (one GPU only)");
+    PB_CHECK(P->blocks() & block, block == BLOCK_LOOKUP
+                                      ? "this prover has no lookup table (pb200_prover_set_lookup): use pb200_prover_set_zk"
+                                      : "this prover has no shuffle (pb200_prover_set_shuffle): use pb200_prover_set_zk");
+  }
+  if (!enable) {
     P->zk = P->zk_fixed = false;
     for (auto& b : P->zk_coeff) b.release();
     for (auto& b : P->zk_t) b.release();
@@ -1018,36 +1030,12 @@ void prover_set_zk(Prover* P, bool enable, const uint8_t* h_blinders) {
     P->zk_z3.release();
     return;
   }
-  PB_CHECK(P->world == 1, "zero-knowledge proving is not available on the sharded prover (one GPU only)");
-  PB_CHECK(!P->sh, "zero-knowledge mode does not combine with a shuffle here: a shuffle prover takes 14 blinders (17 "
-                   "with next-row terms) through pb200_prover_set_zk_shuffle");
-  PB_CHECK(!P->lk, "zero-knowledge mode does not combine with lookups here: a lookup prover takes 21 blinders through "
-                   "pb200_prover_set_zk_lookup");
-  zk_enable(P, h_blinders);
-}
-
-// Zero-knowledge lookup proofs: the 11 blinders of prover_set_zk and b12..b21 for F, H1, H2 and Z2 (see "zero knowledge
-// with lookups" below).  A separate entry point because it takes another number of blinders: the size of the caller's
-// buffer never depends on the prover's state.
-void prover_set_zk_lookup(Prover* P, bool enable, const uint8_t* h_blinders) {
-  PB_CHECK(P->world == 1, "zero-knowledge proving is not available on the sharded prover (one GPU only)");
-  PB_CHECK(P->lk, "this prover has no lookup table (pb200_prover_set_lookup): use pb200_prover_set_zk");
-  if (!enable) {
-    prover_set_zk(P, false, nullptr);
-    return;
-  }
-  zk_enable(P, h_blinders);
-}
-
-// Zero-knowledge shuffle proofs: the 11 blinders of prover_set_zk (14 on a next-row prover) and three more for Z3, the
-// last three (see "zero knowledge with a shuffle" below).  A separate entry point for the same reason as
-// prover_set_zk_lookup.
-void prover_set_zk_shuffle(Prover* P, bool enable, const uint8_t* h_blinders) {
-  PB_CHECK(P->world == 1, "zero-knowledge proving is not available on the sharded prover (one GPU only)");
-  PB_CHECK(P->sh, "this prover has no shuffle (pb200_prover_set_shuffle): use pb200_prover_set_zk");
-  if (!enable) {
-    prover_set_zk(P, false, nullptr);
-    return;
+  if (block == BLOCK_PLAIN) {
+    PB_CHECK(P->world == 1, "zero-knowledge proving is not available on the sharded prover (one GPU only)");
+    PB_CHECK(!P->sh, "zero-knowledge mode does not combine with a shuffle here: a shuffle prover takes 14 blinders (17 "
+                     "with next-row terms) through pb200_prover_set_zk_shuffle");
+    PB_CHECK(!P->lk, "zero-knowledge mode does not combine with lookups here: a lookup prover takes 21 blinders through "
+                     "pb200_prover_set_zk_lookup");
   }
   zk_enable(P, h_blinders);
 }
@@ -1086,7 +1074,7 @@ static ZkPatch zh_multiple(std::initializer_list<Fr> c) {
 // of the table each lookup row reads (0 off lookup rows).  t gains eta^3 t4, the index matches (a, b, c, Q_T), the
 // quotient's alpha^3 term gains eta^3 Q_T and round 5 one slot, alpha^3 eta^3 Q_T.  With t4 = Q_T = 0 every one of
 // these terms vanishes, so one table proves the same bytes tagged or not.
-// Zero knowledge with lookups (prover_set_zk_lookup): everything of plain zero-knowledge mode, and b12..b21 blind the
+// Zero knowledge with lookups (pb200_prover_set_zk_lookup): everything of plain zero-knowledge mode, and b12..b21 blind the
 // lookup polynomials the proof commits to, one scalar more than the points each is revealed at (PlonKup, 2022/086):
 //   F' = F + (b12 X + b13) Z_H,  H1' = H1 + (b14 X^2 + b15 X + b16) Z_H,  H2' = H2 + (b17 X + b18) Z_H,
 //   Z2' = Z2 + (b19 X^2 + b20 X + b21) Z_H.
@@ -1241,7 +1229,7 @@ void prover_round_lookup(Prover* P, const Fr& eta_c) {
     zk_blind(P, coeff[3], n, zh_multiple({b[17], b[16]}), P->zk_lk[Prover::LK_H2].as<Fr>());
   }
   const Fr* fh[3] = {P->lk_poly(Prover::LK_F), P->lk_poly(Prover::LK_H1), P->lk_poly(Prover::LK_H2)};
-  P->commit_batch(fh, 3, P->zk ? n + 3 : n, P->lk_pts[0]);
+  P->commit_batch(fh, 3, P->zk ? n + 3 : n, P->fields[F_F]);
 }
 
 // A grand product (Z of the permutation argument, Z2 of the lookup argument) from its per-row numerators and
@@ -1294,7 +1282,7 @@ static void grand_product(Prover* P, Fr* num, const Fr* den, Fr* lag, Fr* coeff,
 // keeps three pieces); round 4 evaluates Q_in at zeta and Z3 at zeta w; round 5 keeps [Q_out] and [Z3] in the
 // linearisation, opens Q_in at zeta (v^6) and Z3 at zeta w (v, or v^4 after A, B, C on a next-row prover).  A row with
 // both selectors cancels out.  Not with lookups (their alpha^3..alpha^5 terms) or the sharded prover.
-// Zero knowledge with a shuffle (prover_set_zk_shuffle): everything of zero-knowledge mode (b1..b11, or b1..b14 on a
+// Zero knowledge with a shuffle (pb200_prover_set_zk_shuffle): everything of zero-knowledge mode (b1..b11, or b1..b14 on a
 // next-row prover), and Z3' = Z3 + (b_(m-2) X^2 + b_(m-1) X + b_m) Z_H with the last three of the m = 14 (17) blinders,
 // one scalar more than the points Z3 is revealed at (zeta w and the linearisation).  Q_in and Q_out are fixed and stay
 // as they are.  Z3 is built from the unblinded values, as the check is; k_quotient_shuffle<true> adds the Z_H multiples
@@ -1362,8 +1350,8 @@ static void shuffle_round2(Prover* P) {
   const Fr* zz[2] = {P->zk ? P->zk_coeff[3].as<Fr>() : P->coeff[3].as<Fr>(), P->sh_z3_poly()};
   uint8_t out[2][64];
   P->commit_batch(zz, 2, P->zk ? n + 3 : n, out[0]);
-  memcpy(P->proof.pts[3], out[0], 64);
-  memcpy(P->sh_pt, out[1], 64);
+  memcpy(P->fields[F_Z], out[0], 64);
+  memcpy(P->fields[F_Z3], out[1], 64);
 }
 
 // round 2 of a lookup proof, after Z: the grand product Z2, then one commitment pass over Z and Z2
@@ -1393,8 +1381,8 @@ static void lookup_round2(Prover* P) {
   const Fr* zz[2] = {P->zk ? P->zk_coeff[3].as<Fr>() : P->coeff[3].as<Fr>(), P->lk_poly(Prover::LK_Z2)};
   uint8_t out[2][64];
   P->commit_batch(zz, 2, P->zk ? n + 3 : n, out[0]);
-  memcpy(P->proof.pts[3], out[0], 64);
-  memcpy(P->lk_pts[3], out[1], 64);
+  memcpy(P->fields[F_Z], out[0], 64);
+  memcpy(P->fields[F_Z2], out[1], 64);
 }
 
 // ---- round 1 (prover.py:86-119) -------------------------------------------------------------------------
@@ -1491,7 +1479,7 @@ void prover_round1(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_
     for (int k = 0; k < 3; k++)
       zk_blind(P, P->coeff[k].as<Fr>(), n, zh_multiple({b[2 * k + 1], b[2 * k], b[11 + k]}), P->zk_coeff[k].as<Fr>());
     const Fr* abc[3] = {P->zk_coeff[0].as<Fr>(), P->zk_coeff[1].as<Fr>(), P->zk_coeff[2].as<Fr>()};
-    P->commit_batch(abc, 3, n + 3, P->proof.pts[0]);
+    P->commit_batch(abc, 3, n + 3, P->fields[F_A]);
     return;
   }
   if (P->zk) {  // A' B' C': n + 2 coefficients
@@ -1499,28 +1487,34 @@ void prover_round1(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_
     for (int k = 0; k < 3; k++)
       zk_blind(P, P->coeff[k].as<Fr>(), n, zh_multiple({b[2 * k + 1], b[2 * k]}), P->zk_coeff[k].as<Fr>());
     const Fr* abc[3] = {P->zk_coeff[0].as<Fr>(), P->zk_coeff[1].as<Fr>(), P->zk_coeff[2].as<Fr>()};
-    P->commit_batch(abc, 3, n + 2, P->proof.pts[0]);
+    P->commit_batch(abc, 3, n + 2, P->fields[F_A]);
     return;
   }
   const Fr* abc[3] = {P->coeff[0].as<Fr>(), P->coeff[1].as<Fr>(), P->coeff[2].as<Fr>()};
-  P->commit_batch(abc, 3, n, P->proof.pts[0]);
+  P->commit_batch(abc, 3, n, P->fields[F_A]);
 }
 
 // ---- round 2 (prover.py:121-152) -------------------------------------------------------------------------
-void prover_round2(Prover* P, const Fr& beta_c, const Fr& gamma_c) {
+// ch: the challenges drawn before round 2, canonical, indexed by ProofChallenge -- beta and gamma, theta and kappa for a
+// shuffle, delta and epsilon for lookups (the ones of blocks the prover does not have are not read)
+void prover_round2(Prover* P, const Fr* ch) {
   Context* ctx = P->ctx;
   const uint64_t n = P->n;
   cudaStream_t st = ctx->stream;
-  P->beta = fp_to_mont(beta_c);
-  P->gamma = fp_to_mont(gamma_c);
-  PermChallenges ch{P->beta, P->gamma};
+  P->beta = fp_to_mont(ch[CH_BETA]);
+  P->gamma = fp_to_mont(ch[CH_GAMMA]);
+  P->theta = fp_to_mont(ch[CH_THETA]);
+  P->kappa = fp_to_mont(ch[CH_KAPPA]);
+  P->delta = fp_to_mont(ch[CH_DELTA]);
+  P->epsilon = fp_to_mont(ch[CH_EPSILON]);
+  PermChallenges perm{P->beta, P->gamma};
   // one proof across G ranks: rank r builds the slab [r n/G, (r+1) n/G) of the grand product (see grand_product)
   const uint64_t ns = n / (uint64_t)P->world, lo = ns * (uint64_t)P->rank;
   Fr* num = P->tmp[0].as<Fr>() + lo;
   Fr* den = P->tmp[1].as<Fr>() + lo;
   k_perm_terms<<<PB_GRID(ns, 128), 0, st>>>(P->lag[0].as<Fr>() + lo, P->lag[1].as<Fr>() + lo, P->lag[2].as<Fr>() + lo,
                                            P->sel_lag[Prover::S1].as<Fr>() + lo, P->sel_lag[Prover::S2].as<Fr>() + lo,
-                                           P->sel_lag[Prover::S3].as<Fr>() + lo, P->roots.as<Fr>() + lo, ch, ns, num, den);
+                                           P->sel_lag[Prover::S3].as<Fr>() + lo, P->roots.as<Fr>() + lo, perm, ns, num, den);
   ctx->launches++;
   grand_product(P, num, den, P->lag[3].as<Fr>(), P->coeff[3].as<Fr>(),
                 "AssertionError: permutation grand product does not close, Z_n != 1 (prover.py:132)");
@@ -1536,24 +1530,10 @@ void prover_round2(Prover* P, const Fr& beta_c, const Fr& gamma_c) {
   if (P->zk) {  // Z': n + 3 coefficients
     const Fr* b = P->zk_b;
     zk_blind(P, P->coeff[3].as<Fr>(), n, zh_multiple({b[8], b[7], b[6]}), P->zk_coeff[3].as<Fr>());
-    P->commit(P->zk_coeff[3].as<Fr>(), n + 3, P->proof.pts[3]);
+    P->commit(P->zk_coeff[3].as<Fr>(), n + 3, P->fields[F_Z]);
     return;
   }
-  P->commit(P->coeff[3].as<Fr>(), n, P->proof.pts[3]);
-}
-
-void prover_round2_shuffle(Prover* P, const Fr& beta_c, const Fr& gamma_c, const Fr& theta_c, const Fr& kappa_c) {
-  PB_CHECK(P->sh, "this prover has no shuffle (pb200_prover_set_shuffle)");
-  P->theta = fp_to_mont(theta_c);
-  P->kappa = fp_to_mont(kappa_c);
-  prover_round2(P, beta_c, gamma_c);
-}
-
-void prover_round2_lookup(Prover* P, const Fr& beta_c, const Fr& gamma_c, const Fr& delta_c, const Fr& epsilon_c) {
-  PB_CHECK(P->lk, "this prover has no lookup table (pb200_prover_set_lookup)");
-  P->delta = fp_to_mont(delta_c);
-  P->epsilon = fp_to_mont(epsilon_c);
-  prover_round2(P, beta_c, gamma_c);
+  P->commit(P->coeff[3].as<Fr>(), n, P->fields[F_Z]);
 }
 
 // ---- round 3 (prover.py:154-226) -------------------------------------------------------------------------
@@ -1702,12 +1682,12 @@ void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c) {
     const uint64_t t3 = P->zk_t3_len();
     zk_blind(P, t + 2 * n, t3, ZkPatch{{fp_neg(b11), zero, zero}, {zero, zero, zero}}, P->zk_t[2].as<Fr>());
     const Fr* t123[3] = {P->zk_t[0].as<Fr>(), P->zk_t[1].as<Fr>(), P->zk_t[2].as<Fr>()};
-    P->commit_batch(t123, 3, t3, P->proof.pts[4]);
+    P->commit_batch(t123, 3, t3, P->fields[F_T_LO]);
     return;
   }
   PB_CHECK(read_flag(P, 0) == 0, "AssertionError: quotient has degree >= 3n (prover.py:205-208)");
   const Fr* t123[3] = {P->tq.as<Fr>(), P->tq.as<Fr>() + n, P->tq.as<Fr>() + 2 * n};
-  P->commit_batch(t123, 3, n, P->proof.pts[4]);
+  P->commit_batch(t123, 3, n, P->fields[F_T_LO]);
 }
 
 // ---- round 4 (prover.py:228-239) -------------------------------------------------------------------------
@@ -1737,7 +1717,7 @@ void prover_round4(Prover* P, const Fr& zeta_c) {
       }
       out[5] = fp_add(out[5], fp_mul(fp_add(fp_mul(fp_add(fp_mul(b[6], zw), b[7]), zw), b[8]), zh));
     }
-    for (int k = 0; k < 3; k++) store_canonical(P->nr_evals[k], P->nr_ev[k]);
+    for (int k = 0; k < 3; k++) store_canonical(P->fields[F_A_SHIFTED_EVAL + k], P->nr_ev[k]);
   } else if (P->zk) {
     // the blinded polynomials at their points: A'(zeta) = A(zeta) + (b1 zeta + b2)(zeta^n - 1), ...,
     // Z'(zeta w) = Z(zeta w) + (b7 (zeta w)^2 + b8 zeta w + b9)(zeta^n - 1)
@@ -1746,7 +1726,7 @@ void prover_round4(Prover* P, const Fr& zeta_c) {
     for (int k = 0; k < 3; k++) out[k] = fp_add(out[k], fp_mul(fp_add(fp_mul(b[2 * k], P->zeta), b[2 * k + 1]), zh));
     out[5] = fp_add(out[5], fp_mul(fp_add(fp_mul(fp_add(fp_mul(b[6], zw), b[7]), zw), b[8]), zh));
   }
-  for (int k = 0; k < 6; k++) { P->ev[k] = out[k]; store_canonical(P->proof.evals[k], out[k]); }
+  for (int k = 0; k < 6; k++) { P->ev[k] = out[k]; store_canonical(P->fields[F_A_EVAL + k], out[k]); }
   if (P->pi_sparse) {
     // PI(zeta) = sum_i (-pub_i) w^i (zeta^n - 1) / (n (zeta - w^i)), one shared inversion (host arithmetic)
     const uint64_t n = P->n;
@@ -1786,7 +1766,7 @@ void prover_round4(Prover* P, const Fr& zeta_c) {
       e[4] = fp_add(e[4], fp_mul(fp_add(fp_mul(fp_add(fp_mul(b[13], zw), b[14]), zw), b[15]), zh));
       e[5] = fp_add(e[5], fp_mul(fp_add(fp_mul(fp_add(fp_mul(b[18], zw), b[19]), zw), b[20]), zh));
     }
-    for (int k = 0; k < 6; k++) store_canonical(P->lk_evals[k], P->lk_ev[k]);
+    for (int k = 0; k < 6; k++) store_canonical(P->fields[F_F_EVAL + k], P->lk_ev[k]);
   }
   if (P->sh) {  // Q_in at zeta, Z3 at zeta w
     const Fr* spolys[2] = {P->sh_coeff[Prover::SH_IN].as<Fr>(), P->sh_z3_coeff.as<Fr>()};
@@ -1797,13 +1777,8 @@ void prover_round4(Prover* P, const Fr& zeta_c) {
       const Fr zh = fp_sub(fp_pow_u64(P->zeta, P->n), Fr::one());
       P->sh_ev[1] = fp_add(P->sh_ev[1], fp_mul(fp_add(fp_mul(fp_add(fp_mul(c[0], zw), c[1]), zw), c[2]), zh));
     }
-    for (int k = 0; k < 2; k++) store_canonical(P->sh_evals[k], P->sh_ev[k]);
+    for (int k = 0; k < 2; k++) store_canonical(P->fields[F_QIN_EVAL + k], P->sh_ev[k]);
   }
-}
-
-void prover_round4_lookup(Prover* P, const Fr& zeta_c) {
-  PB_CHECK(P->lk, "this prover has no lookup table (pb200_prover_set_lookup)");
-  prover_round4(P, zeta_c);
 }
 
 // (num coefficients, n) / (X - point) -> quotient coefficients (out != num), remainder dropped.
@@ -1996,85 +1971,62 @@ void prover_round5(Prover* P, const Fr& v_c) {
   const Fr* ws[2] = {wz_q, wzw_q};
   // zero knowledge: W_z has n + 5 coefficients (numerator n + 6; next-row n + 8 and n + 9), W_zw n + 2; the rest of
   // the buffers is zero
-  P->commit_batch(ws, 2, zk ? P->zk_t3_len() - 1 : n, P->proof.pts[7]);
+  P->commit_batch(ws, 2, zk ? P->zk_t3_len() - 1 : n, P->fields[F_W_Z]);
 }
 
-// canonical 768-byte proof: Proof.flatten() order (prover.py:18-35), G1 as x||y, every integer 32-byte
-// big-endian exactly as the transcript absorbs it (transcript.py:62-67).  A lookup proof has 1216 bytes: the 768 plain
-// bytes, then f_1 h1_1 h2_1 z2_1, then the six lookup evaluations.  A next-row proof has 864 bytes: the 768 plain bytes,
-// then a(zeta w), b(zeta w), c(zeta w).  A shuffle appends z3_1, q_in(zeta), Z3(zeta w): 896 bytes, 992 next-row.
+// The canonical proof: the fields of the prover's blocks in table order (proof_layout.cuh), a G1 point as x||y, every
+// integer 32-byte big-endian exactly as the transcript absorbs it (transcript.py); layout_bytes(P->blocks()) bytes
 void prover_serialize(const Prover* P, uint8_t* out) {
-  auto be = [](uint8_t* dst, const uint8_t* le) { for (int i = 0; i < 32; i++) dst[i] = le[31 - i]; };
-  uint8_t* o = out;
-  for (int k = 0; k < 7; k++) { be(o, P->proof.pts[k]); be(o + 32, P->proof.pts[k] + 32); o += 64; }
-  for (int k = 0; k < 6; k++) { be(o, P->proof.evals[k]); o += 32; }
-  for (int k = 7; k < 9; k++) { be(o, P->proof.pts[k]); be(o + 32, P->proof.pts[k] + 32); o += 64; }
-  if (P->next_row)
-    for (int k = 0; k < 3; k++) { be(o, P->nr_evals[k]); o += 32; }
-  if (P->sh) {
-    be(o, P->sh_pt); be(o + 32, P->sh_pt + 32); o += 64;
-    for (int k = 0; k < 2; k++) { be(o, P->sh_evals[k]); o += 32; }
+  const unsigned blocks = P->blocks();
+  for (int f = 0; f < PROOF_FIELDS; f++) {
+    if (!block_present(PROOF_LAYOUT[f].block, blocks)) continue;
+    for (int w = 0; w < (PROOF_LAYOUT[f].is_point ? 2 : 1); w++, out += 32)
+      for (int i = 0; i < 32; i++) out[i] = P->fields[f][32 * w + 31 - i];
   }
-  if (!P->lk) return;
-  for (int k = 0; k < 4; k++) { be(o, P->lk_pts[k]); be(o + 32, P->lk_pts[k] + 32); o += 64; }
-  for (int k = 0; k < 6; k++) { be(o, P->lk_evals[k]); o += 32; }
 }
 
-// prover.py:51-84; a prover with a lookup table runs step 1L between rounds 1 and 2 and writes the 1216-byte proof, a
-// next-row prover absorbs three more evaluations in round 4 and writes the 864-byte proof, a shuffle prover draws theta
-// and kappa after gamma, absorbs z3_1 after z_1 and two more evaluations last in round 4 (896 or 992 bytes)
+// step's fields of the prover's blocks, little-endian, in table order (what each round entry point returns)
+size_t copy_step(const Prover* P, int step, uint8_t* out) {
+  const unsigned blocks = P->blocks();
+  size_t o = 0;
+  for (int f = 0; f < PROOF_FIELDS; f++) {
+    const ProofFieldInfo& info = PROOF_LAYOUT[f];
+    if (info.step != step || !block_present(info.block, blocks)) continue;
+    const size_t bytes = info.is_point ? 64 : 32;
+    memcpy(out + o, P->fields[f], bytes);
+    o += bytes;
+  }
+  return o;
+}
+
+// prover.py:51-84: each step runs its round, absorbs its fields of the prover's blocks in table order and draws its
+// challenges (step 1L only with lookups; u is the verifier's)
 void prover_prove(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t* hC, const uint8_t* h_public,
                   uint64_t n_public, uint8_t* out, bool wires_on_device) {
   PB_CUDA(cudaSetDevice(P->ctx->device));  // the calling host thread may not be the one that created the context
+  const unsigned blocks = P->blocks();
   Transcript tr("plonk");  // prover.py:53
-  prover_round1(P, hA, hB, hC, h_public, n_public, wires_on_device);
-  tr.append_point_le("a_1", P->proof.pts[0]);
-  tr.append_point_le("b_1", P->proof.pts[1]);
-  tr.append_point_le("c_1", P->proof.pts[2]);
-  Fr beta = tr.get_and_append_challenge("beta");
-  Fr gamma = tr.get_and_append_challenge("gamma");
-  if (P->sh) {  // SHUFFLE_SCHEDULE (transcript.py): no commitment before theta and kappa
-    P->theta = fp_to_mont(tr.get_and_append_challenge("theta"));
-    P->kappa = fp_to_mont(tr.get_and_append_challenge("kappa"));
+  Fr ch[PROOF_CHALLENGES] = {};  // canonical
+  for (int step = 0; step < PROOF_STEPS; step++) {
+    if (!layout_bytes(blocks, step)) continue;  // step 1L without lookups
+    switch (step) {
+      case STEP_1: prover_round1(P, hA, hB, hC, h_public, n_public, wires_on_device); break;
+      case STEP_1L: prover_round_lookup(P, ch[CH_ETA]); break;
+      case STEP_2: prover_round2(P, ch); break;
+      case STEP_3: prover_round3(P, ch[CH_ALPHA], ch[CH_FFT_COFACTOR]); break;
+      case STEP_4: prover_round4(P, ch[CH_ZETA]); break;
+      case STEP_5: prover_round5(P, ch[CH_V]); prover_serialize(P, out); return;
+    }
+    for (int f = 0; f < PROOF_FIELDS; f++) {
+      const ProofFieldInfo& info = PROOF_LAYOUT[f];
+      if (info.step != step || !block_present(info.block, blocks)) continue;
+      if (info.is_point) tr.append_point_le(info.label, P->fields[f]);
+      else tr.append_scalar_le(info.label, P->fields[f]);
+    }
+    for (int c = 0; c < PROOF_CHALLENGES; c++)
+      if (CHALLENGE_LAYOUT[c].step == step && block_present(CHALLENGE_LAYOUT[c].block, blocks))
+        ch[c] = tr.get_and_append_challenge(CHALLENGE_LAYOUT[c].label);
   }
-  if (P->lk) {
-    prover_round_lookup(P, tr.get_and_append_challenge("eta"));
-    tr.append_point_le("f_1", P->lk_pts[0]);
-    tr.append_point_le("h1_1", P->lk_pts[1]);
-    tr.append_point_le("h2_1", P->lk_pts[2]);
-    P->delta = fp_to_mont(tr.get_and_append_challenge("delta"));
-    P->epsilon = fp_to_mont(tr.get_and_append_challenge("epsilon"));
-  }
-  prover_round2(P, beta, gamma);
-  tr.append_point_le("z_1", P->proof.pts[3]);
-  if (P->lk) tr.append_point_le("z2_1", P->lk_pts[3]);
-  if (P->sh) tr.append_point_le("z3_1", P->sh_pt);
-  Fr alpha = tr.get_and_append_challenge("alpha");
-  Fr cof = tr.get_and_append_challenge("fft_cofactor");
-  prover_round3(P, alpha, cof);
-  tr.append_point_le("t_lo_1", P->proof.pts[4]);
-  tr.append_point_le("t_mid_1", P->proof.pts[5]);
-  tr.append_point_le("t_hi_1", P->proof.pts[6]);
-  Fr zeta = tr.get_and_append_challenge("zeta");
-  prover_round4(P, zeta);
-  static const char* ev_labels[6] = {"a_eval", "b_eval", "c_eval", "s1_eval", "s2_eval", "z_shifted_eval"};
-  for (int k = 0; k < 6; k++) tr.append_scalar_le(ev_labels[k], P->proof.evals[k]);
-  if (P->next_row) {  // NEXT_ROW_SCHEDULE (transcript.py)
-    static const char* nr_labels[3] = {"a_shifted_eval", "b_shifted_eval", "c_shifted_eval"};
-    for (int k = 0; k < 3; k++) tr.append_scalar_le(nr_labels[k], P->nr_evals[k]);
-  }
-  if (P->sh) {
-    tr.append_scalar_le("qin_eval", P->sh_evals[0]);
-    tr.append_scalar_le("z3_shifted_eval", P->sh_evals[1]);
-  }
-  if (P->lk) {
-    static const char* lk_labels[6] = {"f_eval", "t_eval", "t_shifted_eval", "h2_eval", "h1_shifted_eval",
-                                       "z2_shifted_eval"};
-    for (int k = 0; k < 6; k++) tr.append_scalar_le(lk_labels[k], P->lk_evals[k]);
-  }
-  Fr v = tr.get_and_append_challenge("v");
-  prover_round5(P, v);
-  prover_serialize(P, out);
 }
 
 }  // namespace pb200

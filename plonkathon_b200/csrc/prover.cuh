@@ -1,6 +1,7 @@
 // Prover state shared between prover.cu (the rounds) and capi.cu (the C ABI accessors).
 #pragma once
 #include "common.cuh"
+#include "proof_layout.cuh"
 
 namespace pb200 {
 
@@ -78,11 +79,6 @@ __device__ __forceinline__ Fr custom_gate_sum_next(const CustomTerms& t, uint64_
 }
 #endif
 
-struct Proof {
-  uint8_t pts[9][64];    // a_1 b_1 c_1 z_1 t_lo t_mid t_hi W_z W_zw  (canonical LE x||y)
-  uint8_t evals[6][32];  // a b c s1 s2 z_shifted (canonical LE)
-};
-
 struct Prover {
   Context* ctx;
   Srs* srs;
@@ -109,7 +105,6 @@ struct Prover {
   // evaluates A, B, C at zeta w, the zeta w opening batches them with Z, and the proof has 864 bytes.
   bool next_row = false;
   Fr nr_ev[3];                           // a(zeta w), b(zeta w), c(zeta w), Montgomery
-  uint8_t nr_evals[3][32];               // canonical LE
   DevBuf roots;          // w^i, i < n
   DevBuf gpow;           // (g mu^rank)^i, i < n     (coset shift on load)
   DevBuf gpow_w;         // (g mu^(rank+4))^i, i < n (only when zw_separate)
@@ -139,10 +134,10 @@ struct Prover {
   // Zero knowledge (one GPU only): the blinding of the PLONK paper with 11 scalars b1..b11 per proof.  The unblinded
   // n-coefficient vectors above stay as they are (the coset extensions read them; k_quotient adds the Z_H multiples);
   // the blinded vectors, which are longer than n, live in their own zero-padded buffers of n + 8 elements.
-  // With a lookup table (prover_set_zk_lookup) there are 21 scalars: b12..b21 blind F, H1, H2 and Z2.  A next-row
+  // With a lookup table (pb200_prover_set_zk_lookup) there are 21 scalars: b12..b21 blind F, H1, H2 and Z2.  A next-row
   // prover takes 14: b12..b14 give A, B, C a third blinder each (they are opened at zeta and at zeta w), so T3' has
   // n + 9 coefficients and the blinded vectors get ZK_NR_PAD elements of padding.
-  // With a shuffle (prover_set_zk_shuffle) Z3 takes three more, always the last three: 14 scalars, 17 next-row.
+  // With a shuffle (pb200_prover_set_zk_shuffle) Z3 takes three more, always the last three: 14 scalars, 17 next-row.
   static const int ZK_BLINDERS = 11, ZK_LK_BLINDERS = 21, ZK_NR_BLINDERS = 14, ZK_PAD = 8, ZK_NR_PAD = 9;
   static const int ZK_SH_BLINDERS = 14, ZK_NR_SH_BLINDERS = 17;
   bool zk = false;
@@ -185,8 +180,6 @@ struct Prover {
   DevBuf lk_ext[LK_VECS];              // ... on the 4n coset
   Fr eta, delta, epsilon;              // Montgomery
   Fr lk_ev[6];                         // f, t, t(zeta w), h2, h1(zeta w), z2(zeta w) at their points (Montgomery)
-  uint8_t lk_pts[4][64];               // f_1 h1_1 h2_1 z2_1 (canonical LE x||y)
-  uint8_t lk_evals[6][32];             // canonical LE
   // Shuffle argument (prover_set_shuffle, one GPU): the multiset of (a, b, c) over the rows with q_in = 1 equals the one
   // over the rows with q_out = 1, see "shuffle" in prover.cu.  The proof gains z3_1, q_in(zeta) and Z3(zeta w) (896
   // bytes, 992 on a next-row prover).
@@ -200,9 +193,12 @@ struct Prover {
   const Fr* sh_z3_poly() const { return (zk ? zk_z3 : sh_z3_coeff).as<Fr>(); }
   Fr theta, kappa;                     // Montgomery
   Fr sh_ev[2];                         // q_in(zeta), Z3(zeta w) (Montgomery)
-  uint8_t sh_pt[64];                   // z3_1 (canonical LE x||y)
-  uint8_t sh_evals[2][32];             // canonical LE
-  Proof proof;
+  // The proof's fields (proof_layout.cuh), canonical little-endian, indexed by ProofField: a point x||y, a scalar in
+  // the first 32 bytes.  The rounds write them; only the fields of this prover's blocks are part of its proof.
+  uint8_t fields[PROOF_FIELDS][64];
+  unsigned blocks() const {
+    return (next_row ? BLOCK_NEXT_ROW : 0) | (sh ? BLOCK_SHUFFLE : 0) | (lk ? BLOCK_LOOKUP : 0);
+  }
 
   enum { QM = 0, QL, QR, QO, QC, S1, S2, S3, CUSTOM0 };
 

@@ -20,8 +20,9 @@ from __future__ import annotations
 import numpy as np
 
 from .field import CURVE_ORDER
+from .transcript import proof_bytes
 
-PROOF_BYTES = 1216
+PROOF_BYTES = proof_bytes(lookup=True)
 
 
 def _column_ints(col) -> list:

@@ -10,24 +10,24 @@ existed as ``Program`` objects (synthetic 2^k-gate circuits) use ``Prover.from_a
 from __future__ import annotations
 
 import ctypes
-from dataclasses import dataclass
+from dataclasses import dataclass, fields, make_dataclass
+from typing import NamedTuple
 
 import numpy as np
 
 from . import _lib
 from .curve import Scalar
 from .custom_gates import is_next_row, padded, split_terms
-from .lookup import PROOF_BYTES as LOOKUP_PROOF_BYTES, check_lookup, check_lookups, padded_table, to_le_rows
+from .lookup import check_lookup, check_lookups, padded_table, to_le_rows
 from .field import CURVE_ORDER, FIELD_MODULUS, FQ
 from .poly import Basis, _log2_exact, scalars_to_bytes
-from .shuffle import NEXT_ROW_PROOF_BYTES as NEXT_ROW_SHUFFLE_PROOF_BYTES, PROOF_BYTES as SHUFFLE_PROOF_BYTES
 from .shuffle import check_shuffle
-from .transcript import (Message1, Message2, Message3, Message4, Message5, NextRowMessage4, NextRowShuffleMessage4,
-                         SHUFFLE_SCHEDULE, ShuffleMessage2, ShuffleMessage4, Transcript)
+from .transcript import (KIND, LOOKUP, NEXT_ROW, SHUFFLE, Message1, Message2, Message3, Message4, Message5,
+                         NextRowMessage4, NextRowShuffleMessage4, ShuffleMessage2, ShuffleMessage4, Transcript, blocks,
+                         proof_bytes, proof_fields, schedule)
 
 PK_ORDER = ("QM", "QL", "QR", "QO", "QC", "S1", "S2", "S3")  # compiler/program.py:10-30
-PROOF_FIELDS = ("a_1", "b_1", "c_1", "z_1", "t_lo_1", "t_mid_1", "t_hi_1", "a_eval", "b_eval", "c_eval",
-                "s1_eval", "s2_eval", "z_shifted_eval", "W_z_1", "W_zw_1")
+PROOF_FIELDS = proof_fields()
 
 
 def _encode(values) -> bytes:
@@ -41,14 +41,19 @@ def _encode(values) -> bytes:
     return bytes(out)
 
 
-def _decode_words(raw: bytes, scalar_words: range, first: int = 0) -> list:
-    """32-byte big-endian words -> ints; the words in ``scalar_words`` must be below r, the others (coordinates) below
-    q, else ValueError naming the word by its index in the proof (raw starts at word ``first``)"""
-    w = [int.from_bytes(raw[i:i + 32], "big") for i in range(0, len(raw), 32)]
-    for k, x in enumerate(w):
-        if x >= (CURVE_ORDER if k in scalar_words else FIELD_MODULUS):
-            raise ValueError("non-canonical proof encoding (word %d is not reduced)" % (first + k))
-    return w
+def _decode(raw: bytes, names) -> dict:
+    """32-byte big-endian words -> the fields ``names`` of the table (a point from two words, a scalar from one); a
+    coordinate must be below q and a scalar below r, else ValueError naming the word by its index in the proof"""
+    out, k = {}, 0
+    for name in names:
+        point = KIND[name] == "point"
+        words = [int.from_bytes(raw[32 * w:32 * w + 32], "big") for w in range(k, k + (2 if point else 1))]
+        for w, x in enumerate(words):
+            if x >= (FIELD_MODULUS if point else CURVE_ORDER):
+                raise ValueError("non-canonical proof encoding (word %d is not reduced)" % (k + w))
+        out[name] = (FQ(words[0]), FQ(words[1])) if point else Scalar(words[0])
+        k += len(words)
+    return out
 
 
 @dataclass
@@ -59,158 +64,112 @@ class Proof:
     msg_4: Message4
     msg_5: Message5
 
+    BLOCKS, FIELDS, BYTES = (), (), proof_bytes()  # no fields beyond the plain 15
+
     def flatten(self):
         """prover.py:18-35."""
-        m1, m2, m3, m4, m5 = self.msg_1, self.msg_2, self.msg_3, self.msg_4, self.msg_5
-        vals = (m1.a_1, m1.b_1, m1.c_1, m2.z_1, m3.t_lo_1, m3.t_mid_1, m3.t_hi_1, m4.a_eval, m4.b_eval,
-                m4.c_eval, m4.s1_eval, m4.s2_eval, m4.z_shifted_eval, m5.W_z_1, m5.W_zw_1)
-        return dict(zip(PROOF_FIELDS, vals))
+        out = {}
+        for m in (self.msg_1, self.msg_2, self.msg_3, self.msg_4, self.msg_5):
+            out.update((f.name, getattr(m, f.name)) for f in fields(m))
+        return out
 
     def to_bytes(self) -> bytes:
         """Canonical 768-byte form: flatten() order, G1 as x||y, 32-byte big-endian integers."""
         return _encode(self.flatten().values())
 
     @classmethod
+    def _from_values(cls, values: dict) -> "Proof":
+        """the proof of the field values ``values`` (label -> value)"""
+        return cls(*[m(*[values[f.name] for f in fields(m)]) for m in (Message1, Message2, Message3, Message4, Message5)])
+
+    @classmethod
     def from_bytes(cls, raw: bytes) -> "Proof":
         """Inverse of to_bytes.  The encoding is canonical: coordinates must be below q and evaluations below r
         (ValueError otherwise) -- a second byte string for the same proof would make proofs malleable."""
-        assert len(raw) == 768
-        w = _decode_words(raw, range(14, 20))
-        pt = lambda k: (FQ(w[k]), FQ(w[k + 1]))  # noqa: E731
-        return cls(Message1(pt(0), pt(2), pt(4)), Message2(pt(6)), Message3(pt(8), pt(10), pt(12)),
-                   Message4(*[Scalar(x) for x in w[14:20]]), Message5(pt(20), pt(22)))
+        assert len(raw) == cls.BYTES
+        return cls._from_values(_decode(raw, PROOF_FIELDS))
 
 
-LOOKUP_FIELDS = ("f_1", "h1_1", "h2_1", "z2_1", "f_eval", "t_eval", "t_shifted_eval", "h2_eval", "h1_shifted_eval",
-                 "z2_shifted_eval")
-
-
-@dataclass
-class LookupProof:
-    """A proof with a lookup argument (plonkathon_b200/lookup.py): the plain proof's 15 fields and 10 more, 13 G1 points
-    and 12 scalars.  Byte order: the plain fields in ``Proof.flatten()`` order, then f_1 h1_1 h2_1 z2_1, then the six
-    lookup evaluations in transcript order -- 1216 bytes, encoded as the plain proof."""
-    plain: Proof
-    f_1: object
-    h1_1: object
-    h2_1: object
-    z2_1: object
-    f_eval: Scalar
-    t_eval: Scalar
-    t_shifted_eval: Scalar
-    h2_eval: Scalar
-    h1_shifted_eval: Scalar
-    z2_shifted_eval: Scalar
+class _Extended:
+    """A proof with extension blocks: ``plain`` (a ``Proof``), then the blocks' fields (``FIELDS``) in byte order.
+    Encoded as the plain proof: flatten() order, G1 as x||y, 32-byte big-endian integers."""
 
     def flatten(self):
         out = self.plain.flatten()
-        out.update((k, getattr(self, k)) for k in LOOKUP_FIELDS)
+        out.update((k, getattr(self, k)) for k in self.FIELDS)
         return out
 
     def to_bytes(self) -> bytes:
         return _encode(self.flatten().values())
 
     @classmethod
-    def from_bytes(cls, raw: bytes) -> "LookupProof":
-        """Inverse of to_bytes; ValueError for a word that is not reduced (coordinates below q, scalars below r)."""
-        if len(raw) != LOOKUP_PROOF_BYTES:
-            raise ValueError("a lookup proof has %d bytes, got %d" % (LOOKUP_PROOF_BYTES, len(raw)))
-        plain = Proof.from_bytes(raw[:768])
-        w = _decode_words(raw[768:], range(8, 14), first=24)
-        pt = lambda k: (FQ(w[k]), FQ(w[k + 1]))  # noqa: E731
-        return cls(plain, pt(0), pt(2), pt(4), pt(6), *[Scalar(x) for x in w[8:14]])
-
-
-NEXT_ROW_FIELDS = ("a_shifted_eval", "b_shifted_eval", "c_shifted_eval")
-NEXT_ROW_PROOF_BYTES = 864
-
-
-@dataclass
-class NextRowProof:
-    """A proof of a circuit with next-row custom gate terms (plonkathon_b200/custom_gates.py): the plain proof's 15
-    fields and the wires at zeta w.  Byte order: the plain fields in ``Proof.flatten()`` order, then a_shifted_eval,
-    b_shifted_eval, c_shifted_eval -- 864 bytes, encoded as the plain proof."""
-    plain: Proof
-    a_shifted_eval: Scalar
-    b_shifted_eval: Scalar
-    c_shifted_eval: Scalar
-
-    def flatten(self):
-        out = self.plain.flatten()
-        out.update((k, getattr(self, k)) for k in NEXT_ROW_FIELDS)
-        return out
-
-    def to_bytes(self) -> bytes:
-        return _encode(self.flatten().values())
+    def _from_values(cls, values: dict):
+        return cls(Proof._from_values(values), *[values[k] for k in cls.FIELDS])
 
     @classmethod
-    def from_bytes(cls, raw: bytes) -> "NextRowProof":
+    def from_bytes(cls, raw: bytes):
         """Inverse of to_bytes; ValueError for a word that is not reduced (coordinates below q, scalars below r)."""
-        if len(raw) != NEXT_ROW_PROOF_BYTES:
-            raise ValueError("a next-row proof has %d bytes, got %d" % (NEXT_ROW_PROOF_BYTES, len(raw)))
-        plain = Proof.from_bytes(raw[:768])
-        w = _decode_words(raw[768:], range(3), first=24)
-        return cls(plain, *[Scalar(x) for x in w])
+        if len(raw) != cls.BYTES:
+            raise ValueError("a %s proof has %d bytes, got %d" % (cls.NAME, cls.BYTES, len(raw)))
+        return cls._from_values(_decode(raw, PROOF_FIELDS + cls.FIELDS))
 
 
-SHUFFLE_FIELDS = ("z3_1", "qin_eval", "z3_shifted_eval")
+def _proof_class(name: str, doc: str, **kind):
+    """the proof class of a kind (``next_row``, ``shuffle``, ``lookup``): ``plain``, then its fields from the table"""
+    ext = proof_fields(**kind)[len(PROOF_FIELDS):]
+    return make_dataclass(name, [("plain", Proof)] + [(k, object) for k in ext], bases=(_Extended,), namespace={
+        "__doc__": doc, "BLOCKS": blocks(**kind), "FIELDS": ext, "BYTES": proof_bytes(**kind),
+        "NAME": " ".join(b.replace("_", "-") for b in blocks(**kind))})
 
 
-@dataclass
-class ShuffleProof:
-    """A proof of a circuit with a shuffle (plonkathon_b200/shuffle.py): the plain proof's 15 fields, then z3_1, qin_eval
-    and z3_shifted_eval -- 896 bytes, encoded as the plain proof."""
-    plain: Proof
-    z3_1: object
-    qin_eval: Scalar
-    z3_shifted_eval: Scalar
-
-    def flatten(self):
-        out = self.plain.flatten()
-        out.update((k, getattr(self, k)) for k in SHUFFLE_FIELDS)
-        return out
-
-    def to_bytes(self) -> bytes:
-        return _encode(self.flatten().values())
-
-    @classmethod
-    def from_bytes(cls, raw: bytes) -> "ShuffleProof":
-        """Inverse of to_bytes; ValueError for a word that is not reduced (coordinates below q, scalars below r)."""
-        if len(raw) != SHUFFLE_PROOF_BYTES:
-            raise ValueError("a shuffle proof has %d bytes, got %d" % (SHUFFLE_PROOF_BYTES, len(raw)))
-        plain = Proof.from_bytes(raw[:768])
-        w = _decode_words(raw[768:], range(2, 4), first=24)
-        return cls(plain, (FQ(w[0]), FQ(w[1])), Scalar(w[2]), Scalar(w[3]))
+LookupProof = _proof_class("LookupProof", """A proof with a lookup argument (plonkathon_b200/lookup.py): the plain proof's
+    15 fields, then f_1 h1_1 h2_1 z2_1 and the six lookup evaluations (1216 bytes).""", lookup=True)
+NextRowProof = _proof_class("NextRowProof", """A proof of a circuit with next-row custom gate terms
+    (plonkathon_b200/custom_gates.py): the plain proof's 15 fields, then the wires at zeta w (864 bytes).""",
+                            next_row=True)
+ShuffleProof = _proof_class("ShuffleProof", """A proof of a circuit with a shuffle (plonkathon_b200/shuffle.py): the plain
+    proof's 15 fields, then z3_1, qin_eval and z3_shifted_eval (896 bytes).""", shuffle=True)
+NextRowShuffleProof = _proof_class("NextRowShuffleProof", """A proof of a circuit with a shuffle and next-row custom gate
+    terms: the plain proof's 15 fields, the wires at zeta w, then the shuffle's three fields (992 bytes).""",
+                                   next_row=True, shuffle=True)
+LOOKUP_FIELDS, NEXT_ROW_FIELDS, SHUFFLE_FIELDS = LookupProof.FIELDS, NextRowProof.FIELDS, ShuffleProof.FIELDS
+NEXT_ROW_PROOF_BYTES = NextRowProof.BYTES
 
 
-@dataclass
-class NextRowShuffleProof:
-    """A proof of a circuit with a shuffle and next-row custom gate terms: the plain proof's 15 fields, the wires at
-    zeta w (as in ``NextRowProof``), then z3_1, qin_eval and z3_shifted_eval -- 992 bytes, encoded as the plain proof."""
-    plain: Proof
-    a_shifted_eval: Scalar
-    b_shifted_eval: Scalar
-    c_shifted_eval: Scalar
-    z3_1: object
-    qin_eval: Scalar
-    z3_shifted_eval: Scalar
+class Kind(NamedTuple):
+    """How a prover of one proof kind talks to the library (the layout itself is the table in transcript.py)."""
+    proof: type       # its proof class
+    suffix: str       # its entry points: pb200_prover_prove<suffix>, pb200_prover_round4<suffix>, ...
+    round2: tuple     # (round-2 entry point, its message, the challenges it takes after beta and gamma)
+    round4: tuple     # (round-4 entry point, its message)
+    zk: str           # the zero-knowledge entry point
+    blinders: int     # ... and its number of blinders
 
-    def flatten(self):
-        out = self.plain.flatten()
-        out.update((k, getattr(self, k)) for k in NEXT_ROW_FIELDS + SHUFFLE_FIELDS)
-        return out
+    @property
+    def schedule(self) -> dict:
+        return schedule(**{b: True for b in self.proof.BLOCKS})
 
-    def to_bytes(self) -> bytes:
-        return _encode(self.flatten().values())
 
-    @classmethod
-    def from_bytes(cls, raw: bytes) -> "NextRowShuffleProof":
-        """Inverse of to_bytes; ValueError for a word that is not reduced (coordinates below q, scalars below r)."""
-        if len(raw) != NEXT_ROW_SHUFFLE_PROOF_BYTES:
-            raise ValueError("a next-row shuffle proof has %d bytes, got %d" % (NEXT_ROW_SHUFFLE_PROOF_BYTES, len(raw)))
-        plain = Proof.from_bytes(raw[:768])
-        w = _decode_words(raw[768:], (0, 1, 2, 5, 6), first=24)
-        return cls(plain, Scalar(w[0]), Scalar(w[1]), Scalar(w[2]), (FQ(w[3]), FQ(w[4])), Scalar(w[5]), Scalar(w[6]))
+_R2, _R4 = ("pb200_prover_round2", Message2, ()), ("pb200_prover_round4", Message4)
+_R2_SHUFFLE = ("pb200_prover_round2_shuffle", ShuffleMessage2, ("theta", "kappa"))
+# A lookup prover proves through prove_arrays only: its round-by-round path are the plain entry points, which the
+# library refuses on it.
+KINDS = {
+    (): Kind(Proof, "", _R2, _R4, "pb200_prover_set_zk", 11),
+    (NEXT_ROW,): Kind(NextRowProof, "_next_row", _R2, ("pb200_prover_round4_next_row", NextRowMessage4),
+                      "pb200_prover_set_zk", 14),
+    (SHUFFLE,): Kind(ShuffleProof, "_shuffle", _R2_SHUFFLE, ("pb200_prover_round4_shuffle", ShuffleMessage4),
+                     "pb200_prover_set_zk_shuffle", 14),
+    (NEXT_ROW, SHUFFLE): Kind(NextRowShuffleProof, "_next_row_shuffle", _R2_SHUFFLE,
+                              ("pb200_prover_round4_next_row_shuffle", NextRowShuffleMessage4),
+                              "pb200_prover_set_zk_shuffle", 17),
+    (LOOKUP,): Kind(LookupProof, "_lookup", _R2, _R4, "pb200_prover_set_zk_lookup", 21),
+}
+
+
+def proof_kind(next_row=False, shuffle=False, lookup=False):
+    """the kind of a prover or key with these blocks, or None for a combination without one"""
+    return KINDS.get(blocks(next_row, shuffle, lookup))
 
 
 def _as_le_rows(values, n) -> np.ndarray:
@@ -241,6 +200,7 @@ class Prover:
     _CREATE = "pb200_prover_create"
     _CREATE_CUSTOM = "pb200_prover_create_custom"
     _CREATE_NEXT_ROW = "pb200_prover_create_custom_next_row"
+    next_row, _kind = False, KINDS[()]  # a plain prover until _create or a _set_* call says otherwise
 
     def __init__(self, setup, program):
         """prover.py:45-49."""
@@ -301,20 +261,20 @@ class Prover:
     def _set_shuffle(self, q_in, q_out):
         keep = [to_le_rows(q_in), to_le_rows(q_out)]
         _lib.check(_lib.lib().pb200_prover_set_shuffle(self._h, *[k.ctypes.data_as(ctypes.c_void_p) for k in keep]))
-        self.shuffle = True
+        self._kind = proof_kind(next_row=self.next_row, shuffle=True)
 
     def _set_lookup(self, qk, cols, rows):
         keep = [to_le_rows(qk)] + [to_le_rows(c) for c in cols]
         ptr = [k.ctypes.data_as(ctypes.c_void_p) for k in keep]
         _lib.check(_lib.lib().pb200_prover_set_lookup(self._h, *ptr, rows))
-        self.lookup = True
+        self._kind = proof_kind(lookup=True)
 
     def _set_lookup_tagged(self, qk, qtag, cols, rows):
         """cols: t1, t2, t3, t4 (the table ids)"""
         keep = [to_le_rows(qk), to_le_rows(qtag)] + [to_le_rows(c) for c in cols]
         ptr = [k.ctypes.data_as(ctypes.c_void_p) for k in keep]
         _lib.check(_lib.lib().pb200_prover_set_lookup_tagged(self._h, *ptr, rows))
-        self.lookup = True
+        self._kind = proof_kind(lookup=True)
 
     def _create(self, setup, n, cols, ctx=None, custom=()):
         exps, ccols = split_terms(custom, n)  # before any device work: a malformed term is a ValueError
@@ -322,6 +282,7 @@ class Prover:
         self._log_n = _log2_exact(n)
         self.custom_exponents = exps
         self.next_row = any(is_next_row(e) for e in exps)
+        self._kind = proof_kind(next_row=self.next_row)
         keep = [c if isinstance(c, bytes) else c.tobytes() for c in (cols[k] for k in PK_ORDER)]
         arr = (ctypes.c_char_p * 8)(*keep)
         h = ctypes.c_void_p()
@@ -350,45 +311,36 @@ class Prover:
         except Exception:
             pass
 
+    def _call(self, entry: str, *args):
+        """one C-ABI call on this prover; a failed assertion of the witness becomes an AssertionError"""
+        try:
+            _lib.check(getattr(_lib.lib(), entry)(self._h, *args))
+        except _lib.PlonkB200Error as e:
+            _raise(e)
+
     # ------------------------------------------------------------------ array-level fast path
     def prove_arrays(self, A, B, C, public) -> bytes:
-        """One C-ABI call for the whole proof (rounds 1-5 + transcript); returns the canonical 768 bytes, the
-        1216 bytes of a ``LookupProof`` on a prover with a lookup argument, the 864 bytes of a ``NextRowProof`` on a
-        prover with next-row custom gate terms, or the 896 (992) bytes of a ``ShuffleProof`` (``NextRowShuffleProof``)
-        on a prover with a shuffle."""
+        """One C-ABI call for the whole proof (rounds 1-5 + transcript); returns the canonical bytes of the prover's
+        proof kind: 768 for a ``Proof``, 1216 for a ``LookupProof`` (lookup argument), 864 for a ``NextRowProof``
+        (next-row custom gate terms), 896 (992) for a ``ShuffleProof`` (``NextRowShuffleProof``)."""
         n = self.group_order
         a, b, c = (_as_le_rows(v, n) for v in (A, B, C))
         pub = _as_le_rows(public, len(public)) if len(public) else np.zeros((0, 32), dtype=np.uint8)
-        lookup = getattr(self, "lookup", False)
-        if getattr(self, "shuffle", False):
-            nr = getattr(self, "next_row", False)
-            out = ctypes.create_string_buffer(NEXT_ROW_SHUFFLE_PROOF_BYTES if nr else SHUFFLE_PROOF_BYTES)
-            prove = _lib.lib().pb200_prover_prove_next_row_shuffle if nr else _lib.lib().pb200_prover_prove_shuffle
-        elif getattr(self, "next_row", False):
-            out = ctypes.create_string_buffer(NEXT_ROW_PROOF_BYTES)
-            prove = _lib.lib().pb200_prover_prove_next_row
-        else:
-            out = ctypes.create_string_buffer(LOOKUP_PROOF_BYTES if lookup else 768)
-            prove = _lib.lib().pb200_prover_prove_lookup if lookup else _lib.lib().pb200_prover_prove
-        try:
-            _lib.check(prove(
-                self._h, a.ctypes.data_as(ctypes.c_void_p), b.ctypes.data_as(ctypes.c_void_p),
-                c.ctypes.data_as(ctypes.c_void_p), pub.ctypes.data_as(ctypes.c_void_p), pub.shape[0], out))
-        except _lib.PlonkB200Error as e:
-            _raise(e)
+        out = ctypes.create_string_buffer(self._kind.proof.BYTES)
+        self._call("pb200_prover_prove" + self._kind.suffix, *[x.ctypes.data_as(ctypes.c_void_p) for x in (a, b, c, pub)],
+                   pub.shape[0], out)
         return out.raw
 
     # ------------------------------------------------------------------ the reference's surface
     def prove(self, witness) -> Proof:
-        """prover.py:51-84.  A prover with next-row custom gate terms follows NEXT_ROW_SCHEDULE and returns a
-        ``NextRowProof``; a prover with a shuffle follows SHUFFLE_SCHEDULE (NEXT_ROW_SHUFFLE_SCHEDULE) and returns a
-        ``ShuffleProof`` (``NextRowShuffleProof``)."""
+        """prover.py:51-84, following the schedule of the prover's kind (transcript.py) and returning its proof class:
+        a ``NextRowProof`` with next-row custom gate terms, a ``ShuffleProof`` (``NextRowShuffleProof``) with a
+        shuffle."""
+        kind = self._kind
         transcript = Transcript(b"plonk")
         msg_1 = self.round_1(witness)  # also collects the public inputs (prover.py:57-62)
-        if getattr(self, "shuffle", False):
-            self.beta, self.gamma, self.theta, self.kappa = transcript.round_1(msg_1, SHUFFLE_SCHEDULE)
-        else:
-            self.beta, self.gamma = transcript.round_1(msg_1)
+        for name, value in zip(kind.schedule["1"][2], transcript.round_1(msg_1, kind.schedule)):
+            setattr(self, name, value)  # beta, gamma (and theta, kappa with a shuffle)
         msg_2 = self.round_2()
         self.alpha, self.fft_cofactor = transcript.round_2(msg_2)
         msg_3 = self.round_3()
@@ -396,17 +348,10 @@ class Prover:
         msg_4 = self.round_4()
         self.v = transcript.round_4(msg_4)
         msg_5 = self.round_5()
-        if isinstance(msg_2, ShuffleMessage2):
-            plain = Proof(msg_1, Message2(msg_2.z_1), msg_3, Message4(*[getattr(msg_4, k) for k in PROOF_FIELDS[7:13]]),
-                          msg_5)
-            tail = [msg_2.z3_1, msg_4.qin_eval, msg_4.z3_shifted_eval]
-            if isinstance(msg_4, NextRowShuffleMessage4):
-                return NextRowShuffleProof(plain, *[getattr(msg_4, k) for k in NEXT_ROW_FIELDS], *tail)
-            return ShuffleProof(plain, *tail)
-        if isinstance(msg_4, NextRowMessage4):
-            plain = Message4(*[getattr(msg_4, k) for k in PROOF_FIELDS[7:13]])
-            return NextRowProof(Proof(msg_1, msg_2, msg_3, plain, msg_5), *[getattr(msg_4, k) for k in NEXT_ROW_FIELDS])
-        return Proof(msg_1, msg_2, msg_3, msg_4, msg_5)
+        values = {}
+        for m in (msg_1, msg_2, msg_3, msg_4, msg_5):
+            values.update((f.name, getattr(m, f.name)) for f in fields(m))
+        return kind.proof._from_values(values)
 
     def round_1(self, witness) -> Message1:
         """prover.py:86-119."""
@@ -427,12 +372,7 @@ class Prover:
         a, b, c = (_as_le_rows(v, n) for v in (A, B, C))
         pub = _as_le_rows(self._public, len(self._public)) if self._public else np.zeros((0, 32), np.uint8)
         out = ctypes.create_string_buffer(192)
-        try:
-            _lib.check(_lib.lib().pb200_prover_round1(
-                self._h, a.ctypes.data_as(ctypes.c_void_p), b.ctypes.data_as(ctypes.c_void_p),
-                c.ctypes.data_as(ctypes.c_void_p), pub.ctypes.data_as(ctypes.c_void_p), pub.shape[0], out))
-        except _lib.PlonkB200Error as e:
-            _raise(e)
+        self._call("pb200_prover_round1", *[x.ctypes.data_as(ctypes.c_void_p) for x in (a, b, c, pub)], pub.shape[0], out)
         return Message1(*self._commitments(0, 3, out.raw))
 
     @staticmethod
@@ -442,56 +382,31 @@ class Prover:
     def round_2(self) -> Message2:
         """prover.py:121-152.  A shuffle prover returns a ``ShuffleMessage2`` (z_1, z3_1) and needs ``theta`` and
         ``kappa`` set beside ``beta`` and ``gamma``."""
-        if getattr(self, "shuffle", False):
-            out = ctypes.create_string_buffer(128)
-            try:
-                _lib.check(_lib.lib().pb200_prover_round2_shuffle(self._h, self._le(self.beta), self._le(self.gamma),
-                                                                  self._le(self.theta), self._le(self.kappa), out))
-            except _lib.PlonkB200Error as e:
-                _raise(e)
-            return ShuffleMessage2(*_pts(out.raw, 2))
-        out = ctypes.create_string_buffer(64)
-        try:
-            _lib.check(_lib.lib().pb200_prover_round2(self._h, self._le(self.beta), self._le(self.gamma), out))
-        except _lib.PlonkB200Error as e:
-            _raise(e)
-        return Message2(*self._commitments(3, 1, out.raw))
+        entry, message, extra = self._kind.round2
+        out = ctypes.create_string_buffer(64 * len(fields(message)))
+        self._call(entry, *[self._le(getattr(self, c)) for c in ("beta", "gamma") + extra], out)
+        return message(*self._commitments(3, len(fields(message)), out.raw))
 
     def round_3(self) -> Message3:
         """prover.py:154-226."""
         out = ctypes.create_string_buffer(192)
-        try:
-            _lib.check(_lib.lib().pb200_prover_round3(self._h, self._le(self.alpha), self._le(self.fft_cofactor), out))
-        except _lib.PlonkB200Error as e:
-            _raise(e)
+        self._call("pb200_prover_round3", self._le(self.alpha), self._le(self.fft_cofactor), out)
         return Message3(*self._commitments(4, 3, out.raw))
 
     def round_4(self) -> Message4:
         """prover.py:228-239.  A next-row prover returns a ``NextRowMessage4``: the six evaluations, then a, b, c at
         zeta w (NEXT_ROW_SCHEDULE).  A shuffle prover returns a ``ShuffleMessage4`` or ``NextRowShuffleMessage4``, with
         q_in(zeta) and Z3(zeta w) last."""
-        if getattr(self, "shuffle", False):
-            nr = getattr(self, "next_row", False)
-            count, cls = (11, NextRowShuffleMessage4) if nr else (8, ShuffleMessage4)
-            out = ctypes.create_string_buffer(count * 32)
-            fn = _lib.lib().pb200_prover_round4_next_row_shuffle if nr else _lib.lib().pb200_prover_round4_shuffle
-            _lib.check(fn(self._h, self._le(self.zeta), out))
-            return cls(*[Scalar(int.from_bytes(out.raw[32 * k:32 * k + 32], "little")) for k in range(count)])
-        if getattr(self, "next_row", False):
-            out = ctypes.create_string_buffer(9 * 32)
-            _lib.check(_lib.lib().pb200_prover_round4_next_row(self._h, self._le(self.zeta), out))
-            return NextRowMessage4(*[Scalar(int.from_bytes(out.raw[32 * k:32 * k + 32], "little")) for k in range(9)])
-        out = ctypes.create_string_buffer(192)
-        _lib.check(_lib.lib().pb200_prover_round4(self._h, self._le(self.zeta), out))
-        return Message4(*[Scalar(int.from_bytes(out.raw[32 * k:32 * k + 32], "little")) for k in range(6)])
+        entry, message = self._kind.round4
+        count = len(fields(message))
+        out = ctypes.create_string_buffer(32 * count)
+        self._call(entry, self._le(self.zeta), out)
+        return message(*[Scalar(int.from_bytes(out.raw[32 * k:32 * k + 32], "little")) for k in range(count)])
 
     def round_5(self) -> Message5:
         """prover.py:241-306."""
         out = ctypes.create_string_buffer(128)
-        try:
-            _lib.check(_lib.lib().pb200_prover_round5(self._h, self._le(self.v), out))
-        except _lib.PlonkB200Error as e:
-            _raise(e)
+        self._call("pb200_prover_round5", self._le(self.v), out)
         return Message5(*self._commitments(7, 2, out.raw))
 
     # ------------------------------------------------------------------ round state (prover.py: self.A .. self.T3)
@@ -522,6 +437,23 @@ class Prover:
     T3 = property(lambda self: self._piece(7, "T3"))
 
     # ------------------------------------------------------------------ zero knowledge
+    def _set_zk(self, block, what: str, enable: bool, blinders):
+        """the body of set_zk (block None), set_zk_lookup and set_zk_shuffle: the blinders of the kind that entry point
+        serves, checked here, then the library's own checks"""
+        kind = proof_kind(next_row=self.next_row and block != LOOKUP, shuffle=block == SHUFFLE, lookup=block == LOOKUP)
+        raw = None
+        if enable and blinders is not None:
+            blinders = [int(b) for b in blinders]
+            if len(blinders) != kind.blinders:
+                raise ValueError("%s %d blinders b1..b%d%s, got %d" % (
+                    what, kind.blinders, kind.blinders,
+                    " on a prover with next-row terms" if NEXT_ROW in kind.proof.BLOCKS else "", len(blinders)))
+            if any(not 0 <= b < CURVE_ORDER for b in blinders):
+                raise ValueError("zero-knowledge blinders must lie in [0, r)")
+            raw = b"".join(b.to_bytes(32, "little") for b in blinders)
+        _lib.check(getattr(_lib.lib(), kind.zk)(self._h, 1 if enable else 0, raw))
+        self.zk = bool(enable)
+
     def set_zk(self, enable: bool = True, blinders=None):
         """Zero-knowledge mode for every later proof: A, B, C, Z and the quotient pieces are blinded as in the PLONK
         paper (eprint 2019/953), with 11 scalars b1..b11 per proof.  The proof keeps its 768 bytes and the verifier does
@@ -530,18 +462,7 @@ class Prover:
         Needs n >= 8 and an SRS of at least n + 6 powers; the sharded prover has no zero-knowledge mode.
         A prover with next-row custom gate terms takes 14 blinders: b12, b13, b14 give A, B, C a third one, since they
         are opened at zeta and at zeta w (DESIGN.md section 1).  It needs n >= 16 and an SRS of n + 9 powers."""
-        raw = None
-        if enable and blinders is not None:
-            blinders = [int(b) for b in blinders]
-            count = 14 if getattr(self, "next_row", False) else 11
-            if len(blinders) != count:
-                raise ValueError("zero knowledge takes %d blinders b1..b%d%s, got %d" % (
-                    count, count, " on a prover with next-row terms" if count == 14 else "", len(blinders)))
-            if any(not 0 <= b < CURVE_ORDER for b in blinders):
-                raise ValueError("zero-knowledge blinders must lie in [0, r)")
-            raw = b"".join(b.to_bytes(32, "little") for b in blinders)
-        _lib.check(_lib.lib().pb200_prover_set_zk(self._h, 1 if enable else 0, raw))
-        self.zk = bool(enable)
+        self._set_zk(None, "zero knowledge takes", enable, blinders)
 
     def set_zk_lookup(self, enable: bool = True, blinders=None):
         """Zero-knowledge mode for the later proofs of a lookup prover (``lookup=`` or ``lookups=``): ``set_zk``'s
@@ -549,16 +470,7 @@ class Prover:
         bytes and the verifier does not change.  ``blinders=None``: fresh scalars from the OS CSPRNG for every proof;
         otherwise 21 integers in [0, r) used for every proof (reproducible tests only).  ``enable=False`` (or
         ``set_zk(False)``) returns to plain lookup proofs.  Needs a lookup table, n >= 8 and an SRS of n + 6 powers."""
-        raw = None
-        if enable and blinders is not None:
-            blinders = [int(b) for b in blinders]
-            if len(blinders) != 21:
-                raise ValueError("zero-knowledge lookups take 21 blinders b1..b21, got %d" % len(blinders))
-            if any(not 0 <= b < CURVE_ORDER for b in blinders):
-                raise ValueError("zero-knowledge blinders must lie in [0, r)")
-            raw = b"".join(b.to_bytes(32, "little") for b in blinders)
-        _lib.check(_lib.lib().pb200_prover_set_zk_lookup(self._h, 1 if enable else 0, raw))
-        self.zk = bool(enable)
+        self._set_zk(LOOKUP, "zero-knowledge lookups take", enable, blinders)
 
     def set_zk_shuffle(self, enable: bool = True, blinders=None):
         """Zero-knowledge mode for the later proofs of a shuffle prover (``shuffle=``): ``set_zk``'s blinding and 3 more
@@ -567,18 +479,7 @@ class Prover:
         for every proof; otherwise 14 (17) integers in [0, r) used for every proof (reproducible tests only).
         ``enable=False`` (or ``set_zk(False)``) returns to plain shuffle proofs.  Needs a shuffle, n >= 8 and an SRS of
         n + 6 powers (n >= 16 and n + 9 powers with next-row terms)."""
-        raw = None
-        if enable and blinders is not None:
-            blinders = [int(b) for b in blinders]
-            count = 17 if getattr(self, "next_row", False) else 14
-            if len(blinders) != count:
-                raise ValueError("zero-knowledge shuffles take %d blinders b1..b%d%s, got %d" % (
-                    count, count, " on a prover with next-row terms" if count == 17 else "", len(blinders)))
-            if any(not 0 <= b < CURVE_ORDER for b in blinders):
-                raise ValueError("zero-knowledge blinders must lie in [0, r)")
-            raw = b"".join(b.to_bytes(32, "little") for b in blinders)
-        _lib.check(_lib.lib().pb200_prover_set_zk_shuffle(self._h, 1 if enable else 0, raw))
-        self.zk = bool(enable)
+        self._set_zk(SHUFFLE, "zero-knowledge shuffles take", enable, blinders)
 
     def _commitments(self, first_slot: int, count: int, raw: bytes):
         """commitments a round produced"""

@@ -20,9 +20,10 @@ sharded prover."""
 from __future__ import annotations
 
 from .lookup import _column_ints
+from .transcript import proof_bytes
 
-PROOF_BYTES = 896
-NEXT_ROW_PROOF_BYTES = 992
+PROOF_BYTES = proof_bytes(shuffle=True)
+NEXT_ROW_PROOF_BYTES = proof_bytes(next_row=True, shuffle=True)
 
 
 def check_shuffle(shuffle, group_order: int):

@@ -1,8 +1,8 @@
 """Drop-in for the reference's ``transcript.py``: the five message records (transcript.py:8-55) and
 ``Transcript`` (transcript.py:58-123).  The Merlin/STROBE/Keccak machinery is host code inside
-libplonk_b200.so (csrc/transcript.cuh); this module binds it and lays the reference's per-round schedule out
-as a table: which fields of a message are absorbed (points as x then y, scalars, all 32-byte big-endian) and
-which challenges are drawn afterwards."""
+libplonk_b200.so (csrc/transcript.cuh); this module binds it and holds the proof layout as one table, from which
+every proof kind's per-round schedule follows: which fields are absorbed (points as x then y, scalars, all 32-byte
+big-endian) and which challenges are drawn afterwards."""
 from __future__ import annotations
 
 import ctypes
@@ -11,53 +11,96 @@ from dataclasses import make_dataclass
 from . import _lib
 from .curve import Scalar
 
-# round -> (message field names in absorption order, kind of those fields, challenge labels drawn afterwards)
-SCHEDULE = {
-    1: (("a_1", "b_1", "c_1"), "point", ("beta", "gamma")),
-    2: (("z_1",), "point", ("alpha", "fft_cofactor")),
-    3: (("t_lo_1", "t_mid_1", "t_hi_1"), "point", ("zeta",)),
-    4: (("a_eval", "b_eval", "c_eval", "s1_eval", "s2_eval", "z_shifted_eval"), "scalar", ("v",)),
-    5: (("W_z_1", "W_zw_1"), "point", ("u",)),
-}
+# The proof layout: every field of every proof kind as (label, kind, step, block), in byte order -- the plain proof's 15
+# fields in ``Proof.flatten()`` order, then the next-row block (plonkathon_b200/custom_gates.py), the shuffle block
+# (plonkathon_b200/shuffle.py) and the lookup block (plonkathon_b200/lookup.py).  The label is the transcript label and
+# the proof classes' attribute; a point is 64 bytes (x then y), a scalar 32.  A prover or key has a set of blocks, and
+# its proof is this table filtered to the plain block and those blocks.  One table gives both orders because
+#
+#     within each transcript step, the fields are absorbed in byte order.
+#
+# csrc/proof_layout.cuh holds the same table for the library (tests/test_proof_layout.py compares the two).
+PLAIN, NEXT_ROW, SHUFFLE, LOOKUP = "plain", "next_row", "shuffle", "lookup"
+STEPS = ("1", "1L", "2", "3", "4", "5")  # 1L: the lookup commitments, between rounds 1 and 2
+FIELDS = (
+    ("a_1", "point", "1", PLAIN), ("b_1", "point", "1", PLAIN), ("c_1", "point", "1", PLAIN),
+    ("z_1", "point", "2", PLAIN),
+    ("t_lo_1", "point", "3", PLAIN), ("t_mid_1", "point", "3", PLAIN), ("t_hi_1", "point", "3", PLAIN),
+    ("a_eval", "scalar", "4", PLAIN), ("b_eval", "scalar", "4", PLAIN), ("c_eval", "scalar", "4", PLAIN),
+    ("s1_eval", "scalar", "4", PLAIN), ("s2_eval", "scalar", "4", PLAIN), ("z_shifted_eval", "scalar", "4", PLAIN),
+    ("W_z_1", "point", "5", PLAIN), ("W_zw_1", "point", "5", PLAIN),
+    ("a_shifted_eval", "scalar", "4", NEXT_ROW), ("b_shifted_eval", "scalar", "4", NEXT_ROW),
+    ("c_shifted_eval", "scalar", "4", NEXT_ROW),
+    ("z3_1", "point", "2", SHUFFLE), ("qin_eval", "scalar", "4", SHUFFLE), ("z3_shifted_eval", "scalar", "4", SHUFFLE),
+    ("f_1", "point", "1L", LOOKUP), ("h1_1", "point", "1L", LOOKUP), ("h2_1", "point", "1L", LOOKUP),
+    ("z2_1", "point", "2", LOOKUP),
+    ("f_eval", "scalar", "4", LOOKUP), ("t_eval", "scalar", "4", LOOKUP), ("t_shifted_eval", "scalar", "4", LOOKUP),
+    ("h2_eval", "scalar", "4", LOOKUP), ("h1_shifted_eval", "scalar", "4", LOOKUP),
+    ("z2_shifted_eval", "scalar", "4", LOOKUP),
+)
+KIND = {label: kind for label, kind, _, _ in FIELDS}
+# the challenges each step draws after absorbing its fields, in drawing order, as (label, step, block)
+CHALLENGES = (
+    ("beta", "1", PLAIN), ("gamma", "1", PLAIN), ("theta", "1", SHUFFLE), ("kappa", "1", SHUFFLE), ("eta", "1", LOOKUP),
+    ("delta", "1L", LOOKUP), ("epsilon", "1L", LOOKUP), ("alpha", "2", PLAIN), ("fft_cofactor", "2", PLAIN),
+    ("zeta", "3", PLAIN), ("v", "4", PLAIN), ("u", "5", PLAIN),
+)
 
-# The same table for a proof with a lookup argument (plonkathon_b200/lookup.py): step 1 also draws eta, step 1L absorbs
-# the lookup commitments, round 2 absorbs Z2 beside Z and round 4 the six lookup evaluations after the plain ones.
-LOOKUP_SCHEDULE = {
-    "1": (("a_1", "b_1", "c_1"), "point", ("beta", "gamma", "eta")),
-    "1L": (("f_1", "h1_1", "h2_1"), "point", ("delta", "epsilon")),
-    "2": (("z_1", "z2_1"), "point", ("alpha", "fft_cofactor")),
-    "3": (("t_lo_1", "t_mid_1", "t_hi_1"), "point", ("zeta",)),
-    "4": (("a_eval", "b_eval", "c_eval", "s1_eval", "s2_eval", "z_shifted_eval", "f_eval", "t_eval", "t_shifted_eval",
-           "h2_eval", "h1_shifted_eval", "z2_shifted_eval"), "scalar", ("v",)),
-    "5": (("W_z_1", "W_zw_1"), "point", ("u",)),
-}
 
-# The same table for a proof with next-row custom gate terms (plonkathon_b200/custom_gates.py): round 4 also absorbs the
-# wires at zeta w, after z_shifted_eval and before v is drawn.
-NEXT_ROW_SCHEDULE = dict(SCHEDULE)
-NEXT_ROW_SCHEDULE[4] = (SCHEDULE[4][0] + ("a_shifted_eval", "b_shifted_eval", "c_shifted_eval"), "scalar", ("v",))
+def blocks(next_row=False, shuffle=False, lookup=False) -> tuple:
+    """the extension blocks of a proof kind, in table order"""
+    return tuple(b for b, on in ((NEXT_ROW, next_row), (SHUFFLE, shuffle), (LOOKUP, lookup)) if on)
 
-# The same table for a proof with a shuffle (plonkathon_b200/shuffle.py): step 1 also draws theta and kappa (no commitment
-# before them), step 2 absorbs Z3 beside Z and step 4 q_in(zeta) and Z3(zeta w) last.  NEXT_ROW_SHUFFLE_SCHEDULE is the
-# form for a circuit with next-row custom gate terms: the three shifted wire evaluations come before the shuffle's two.
-SHUFFLE_FIELDS_4 = ("qin_eval", "z3_shifted_eval")
-SHUFFLE_SCHEDULE = dict(SCHEDULE)
-SHUFFLE_SCHEDULE[1] = (SCHEDULE[1][0], "point", ("beta", "gamma", "theta", "kappa"))
-SHUFFLE_SCHEDULE[2] = (("z_1", "z3_1"), "point", SCHEDULE[2][2])
-SHUFFLE_SCHEDULE[4] = (SCHEDULE[4][0] + SHUFFLE_FIELDS_4, "scalar", ("v",))
-NEXT_ROW_SHUFFLE_SCHEDULE = dict(SHUFFLE_SCHEDULE)
-NEXT_ROW_SHUFFLE_SCHEDULE[4] = (NEXT_ROW_SCHEDULE[4][0] + SHUFFLE_FIELDS_4, "scalar", ("v",))
+
+def proof_fields(next_row=False, shuffle=False, lookup=False) -> tuple:
+    """the labels of a kind's proof fields in byte order"""
+    have = (PLAIN,) + blocks(next_row, shuffle, lookup)
+    return tuple(label for label, _, _, block in FIELDS if block in have)
+
+
+def proof_bytes(next_row=False, shuffle=False, lookup=False) -> int:
+    return sum(64 if KIND[f] == "point" else 32 for f in proof_fields(next_row, shuffle, lookup))
+
+
+def schedule(next_row=False, shuffle=False, lookup=False) -> dict:
+    """step -> (the step's fields in absorption order, their kind, the challenges drawn afterwards) for one proof kind;
+    a step with neither (1L without lookups) is left out"""
+    have = (PLAIN,) + blocks(next_row, shuffle, lookup)
+    out = {}
+    for step in STEPS:
+        fields = [(label, kind) for label, kind, s, block in FIELDS if s == step and block in have]
+        drawn = tuple(label for label, s, block in CHALLENGES if s == step and block in have)
+        if fields:
+            kinds = {kind for _, kind in fields}
+            assert len(kinds) == 1, "a step absorbs fields of one kind"
+            out[step] = (tuple(label for label, _ in fields), kinds.pop(), drawn)
+    return out
+
+
+SCHEDULE = schedule()
+LOOKUP_SCHEDULE = schedule(lookup=True)
+NEXT_ROW_SCHEDULE = schedule(next_row=True)
+SHUFFLE_SCHEDULE = schedule(shuffle=True)
+NEXT_ROW_SHUFFLE_SCHEDULE = schedule(next_row=True, shuffle=True)
+
+# message class -> the schedule it follows (Transcript.round_2, round_4; SCHEDULE for any other record)
+_SCHEDULE_OF = {}
+
+
+def _message(name: str, sched: dict, step: str):
+    cls = make_dataclass(name, [(label, object) for label in sched[step][0]])
+    _SCHEDULE_OF[cls] = sched
+    return cls
+
 
 # Message1 .. Message5: plain records with exactly the reference's field names and order
-Message1, Message2, Message3, Message4, Message5 = (
-    make_dataclass("Message%d" % rnd, [(name, object) for name in SCHEDULE[rnd][0]]) for rnd in sorted(SCHEDULE))
+Message1, Message2, Message3, Message4, Message5 = (_message("Message" + s, SCHEDULE, s) for s in "12345")
 # round 4 of a next-row prover: Message4's fields, then the three shifted wire evaluations
-NextRowMessage4 = make_dataclass("NextRowMessage4", [(name, object) for name in NEXT_ROW_SCHEDULE[4][0]])
+NextRowMessage4 = _message("NextRowMessage4", NEXT_ROW_SCHEDULE, "4")
 # rounds 2 and 4 of a shuffle prover (round 4 with and without next-row terms)
-ShuffleMessage2 = make_dataclass("ShuffleMessage2", [(name, object) for name in SHUFFLE_SCHEDULE[2][0]])
-ShuffleMessage4 = make_dataclass("ShuffleMessage4", [(name, object) for name in SHUFFLE_SCHEDULE[4][0]])
-NextRowShuffleMessage4 = make_dataclass("NextRowShuffleMessage4",
-                                        [(name, object) for name in NEXT_ROW_SHUFFLE_SCHEDULE[4][0]])
+ShuffleMessage2 = _message("ShuffleMessage2", SHUFFLE_SCHEDULE, "2")
+ShuffleMessage4 = _message("ShuffleMessage4", SHUFFLE_SCHEDULE, "4")
+NextRowShuffleMessage4 = _message("NextRowShuffleMessage4", NEXT_ROW_SHUFFLE_SCHEDULE, "4")
 
 
 def _as_int(x) -> int:
@@ -105,8 +148,8 @@ class Transcript:
         return Scalar(int.from_bytes(out.raw, "little"))
 
     # ---- transcript.py:77-123
-    def _round(self, rnd: int, message, schedule: dict = SCHEDULE):
-        fields, kind, challenges = schedule[rnd]
+    def _round(self, step: str, message, schedule: dict = None):
+        fields, kind, challenges = (schedule or _SCHEDULE_OF.get(type(message), SCHEDULE))[step]
         absorb = self.append_point if kind == "point" else self.append_scalar
         for name in fields:
             absorb(name.encode(), getattr(message, name))
@@ -126,21 +169,19 @@ class Transcript:
 
     def round_1(self, message, schedule: dict = SCHEDULE):
         """``schedule=SHUFFLE_SCHEDULE`` draws theta and kappa after beta and gamma (four challenges)"""
-        return self._round(1, message, schedule)
+        return self._round("1", message, schedule)
 
     def round_2(self, message):
-        """a ``ShuffleMessage2`` follows SHUFFLE_SCHEDULE"""
-        return self._round(2, message, SHUFFLE_SCHEDULE if isinstance(message, ShuffleMessage2) else SCHEDULE)
+        """the schedule of the message's type: a ``ShuffleMessage2`` follows SHUFFLE_SCHEDULE"""
+        return self._round("2", message)
 
     def round_3(self, message):
-        return self._round(3, message)
+        return self._round("3", message)
 
     def round_4(self, message):
-        """a ``NextRowMessage4`` follows NEXT_ROW_SCHEDULE, a ``ShuffleMessage4`` SHUFFLE_SCHEDULE and a
-        ``NextRowShuffleMessage4`` NEXT_ROW_SHUFFLE_SCHEDULE"""
-        schedule = {NextRowMessage4: NEXT_ROW_SCHEDULE, ShuffleMessage4: SHUFFLE_SCHEDULE,
-                    NextRowShuffleMessage4: NEXT_ROW_SHUFFLE_SCHEDULE}.get(type(message), SCHEDULE)
-        return self._round(4, message, schedule)
+        """the schedule of the message's type: a ``NextRowMessage4`` follows NEXT_ROW_SCHEDULE, a ``ShuffleMessage4``
+        SHUFFLE_SCHEDULE and a ``NextRowShuffleMessage4`` NEXT_ROW_SHUFFLE_SCHEDULE"""
+        return self._round("4", message)
 
     def round_5(self, message):
-        return self._round(5, message)
+        return self._round("5", message)

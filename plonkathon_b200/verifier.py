@@ -16,8 +16,7 @@ from .curve import G1, G2, Scalar, ec_lincomb, g1_neg, g2_add, g2_mul, pairing_p
 from . import _lib
 from .custom_gates import is_next_row, monomial
 from .field import CURVE_ORDER, FIELD_MODULUS
-from .transcript import (LOOKUP_SCHEDULE, NEXT_ROW_SCHEDULE, NEXT_ROW_SHUFFLE_SCHEDULE, SCHEDULE, SHUFFLE_SCHEDULE,
-                         Transcript)
+from .transcript import Transcript
 
 
 def _lagrange_terms_at(group_order: int, values, x: Scalar) -> Scalar:
@@ -79,13 +78,16 @@ class VerificationKey:
                 return False
         return True
 
+    @property
+    def _kind(self):
+        """the proof kind of the key's blocks (prover.KINDS), None for a combination without one"""
+        from .prover import proof_kind
+        return proof_kind(next_row=self.next_row, shuffle=bool(self.shuffle), lookup=bool(self.lookup))
+
     def _matches(self, pf) -> bool:
-        """a lookup key takes lookup proofs only, a next-row key next-row proofs only, a shuffle key shuffle proofs only
-        (of its next-row kind), a plain key plain proofs only"""
-        from .prover import LookupProof, NextRowProof, NextRowShuffleProof, ShuffleProof
-        return (bool(self.lookup) == isinstance(pf, LookupProof)
-                and self.next_row == isinstance(pf, (NextRowProof, NextRowShuffleProof))
-                and bool(self.shuffle) == isinstance(pf, (ShuffleProof, NextRowShuffleProof)))
+        """the key takes the proofs of its kind only: a plain key plain proofs, a lookup key lookup proofs, ..."""
+        kind = self._kind
+        return kind is not None and isinstance(pf, kind.proof)
 
     def verify_proof(self, group_order: int, pf, public=[]) -> bool:
         """verifier.py:40-73: the batched form -- one pairing equation, the linearisation commitment never
@@ -112,11 +114,7 @@ class VerificationKey:
     def _verify(self, group_order: int, pf, public, batched: bool) -> bool:
         n = group_order
         proof = pf.flatten()
-        if self.shuffle:
-            schedule = NEXT_ROW_SHUFFLE_SCHEDULE if self.next_row else SHUFFLE_SCHEDULE
-        else:
-            schedule = LOOKUP_SCHEDULE if self.lookup else NEXT_ROW_SCHEDULE if self.next_row else SCHEDULE
-        ch = Transcript(b"plonk").replay(schedule, proof)
+        ch = Transcript(b"plonk").replay(self._kind.schedule, proof)
         beta, gamma, alpha, zeta, v, u = ch["beta"], ch["gamma"], ch["alpha"], ch["zeta"], ch["v"], ch["u"]
         zh_ev = zeta ** n - 1
         l0_ev = zh_ev / ((zeta - 1) * n)
