@@ -155,6 +155,15 @@ int pb200_prover_create_custom(pb200_ctx* ctx, pb200_srs* srs, unsigned log_n, c
                                unsigned n_custom, const uint8_t* h_exps, const uint8_t* const* h_custom,
                                pb200_prover** out);
 void pb200_prover_destroy(pb200_prover* p);
+/* *out = 1 when the prover is sliced, else 0.  A one-GPU prover whose cache on the 4n coset (selector extensions, L0,
+ * coset points, the per-proof extensions and quotient, the 4n NTT plans) does not fit the free device memory at
+ * creation evaluates the quotient one n-point slice of the coset at a time instead: the same proofs, with the selector
+ * extensions recomputed in every proof.  PB200_SLICED=1 in the environment forces it (it cannot prevent it).  A sliced
+ * prover proves plain circuits and same-row custom terms; pb200_prover_set_zk(p, 1, ...), set_zk_lookup,
+ * set_zk_shuffle, set_lookup(_tagged) and set_shuffle return an error on it and leave it usable, and
+ * pb200_prover_create_custom_next_row fails rather than slice.  When neither layout fits, creation fails with the
+ * bytes both need and the bytes free.  The sharded prover is never sliced. */
+int pb200_prover_sliced(pb200_prover* p, int* out);
 /* prover.py:51-84  prove(witness): h_A/h_B/h_C = wire values per row (prover.py:97-103), h_public = the
  * public input values in order (prover.py:57-62; the library negates them).  Writes the canonical 768-byte
  * proof: Proof.flatten() order (prover.py:18-35), G1 as x||y, 32-byte big-endian integers.

@@ -114,6 +114,7 @@ def _load():
         "pb200_g2_mul": (I, [V, V, V, P(I)]),
         "pb200_g2_add": (I, [V, I, V, I, V, P(I)]),
         "pb200_bench_modmul": (I, [V, I, U64, U, P(ctypes.c_float)]),
+        "pb200_prover_sliced": (I, [V, P(I)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)  # AttributeError here == ABI drift: fail loudly

@@ -532,6 +532,11 @@ int pb200_prover_create_custom_sharded(pb200_ctx* ctx, pb200_srs* srs, unsigned 
   PB_API_END
 }
 void pb200_prover_destroy(pb200_prover* p) { prover_destroy(reinterpret_cast<Prover*>(p)); }
+int pb200_prover_sliced(pb200_prover* p, int* out) {
+  PB_API_BEGIN
+  *out = reinterpret_cast<Prover*>(p)->sliced ? 1 : 0;
+  PB_API_END
+}
 
 int pb200_prover_prove(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                        const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof768) {

@@ -1,7 +1,8 @@
 // Host build of the limb-level arithmetic in field.cuh / curve.cuh (same code path as the device,
 // PTX carry-chain primitives replaced by their emulation).  TEST INFRASTRUCTURE: loaded only by
 // tests/test_host_arith.py through ctypes; never linked into libplonk_b200.so.  It also exports the proof layout
-// (proof_layout.cuh) for tests/test_proof_layout.py.
+// (proof_layout.cuh) for tests/test_proof_layout.py and the prover's memory plan (memory_plan.cuh) for
+// tests/test_sliced_prover.py.
 #include "field.cuh"
 #include "curve.cuh"
 #include "msm_digits.cuh"
@@ -10,6 +11,7 @@
 #include "msm_sort.cuh"
 #include "ntt_shard.cuh"
 #include "proof_layout.cuh"
+#include "memory_plan.cuh"
 #include <algorithm>
 #include <vector>
 #include <cstring>
@@ -543,5 +545,22 @@ const char* hs_proof_challenge(int k, int* step, int* block) {
   *step = CHALLENGE_LAYOUT[k].step;
   *block = (int)CHALLENGE_LAYOUT[k].block;
   return CHALLENGE_LAYOUT[k].label;
+}
+}
+
+extern "C" {
+// the prover's device bytes by count (memory_plan.cuh): out[0..3] = full circuit, proof, ntt, msm; out[4..7] = the same
+// sliced.  Returns plan_choose for free_bytes: 0 full, 1 sliced, -1 neither fits.
+int hs_prover_memory(int log_n, int n_custom, uint32_t msm_c, uint32_t msm_batch, uint64_t msm_now, uint64_t free_bytes,
+                     int force_sliced, uint64_t* out) {
+  const ProverMemory m = prover_memory(log_n, n_custom, msm_c, msm_batch, msm_now);
+  const MemoryCount* c[2] = {&m.full, &m.sliced};
+  for (int k = 0; k < 2; k++) {
+    out[4 * k] = c[k]->circuit;
+    out[4 * k + 1] = c[k]->proof;
+    out[4 * k + 2] = c[k]->ntt;
+    out[4 * k + 3] = c[k]->msm;
+  }
+  return plan_choose(m, free_bytes, force_sliced != 0);
 }
 }

@@ -594,12 +594,12 @@ __global__ void __launch_bounds__(128) k_shard_combine(CombineArgs a) {
 
 Comm* ctx_comm(Context* ctx);
 
-static ShardTables* get_shard_tables(Context* ctx, int log_n, bool inverse) {
-  Comm* cm = ctx_comm(ctx);
-  const int key = log_n * 2 + (inverse ? 1 : 0);
+// per (log_n, inverse, G, rank): a sliced prover joins the four slices of its coset on one device
+static ShardTables* get_shard_tables(Context* ctx, int log_n, bool inverse, int log_g, int rank) {
+  PB_CHECK(log_g >= 1 && log_g <= 3 && rank >= 0 && rank < (1 << log_g), "sharded transform: 2, 4 or 8 ranks");
+  const int key = ((log_n * 2 + (inverse ? 1 : 0)) * 4 + log_g) * 8 + rank;
   auto it = ctx->shard_tables.find(key);
   if (it != ctx->shard_tables.end()) return it->second.get();
-  const int log_g = comm_log_world(cm), rank = comm_rank(cm);
   PB_CHECK(log_n > log_g, "sharded transform: fewer points than ranks");
   const uint64_t M = (uint64_t)1 << (log_n - log_g);
   auto t = std::make_unique<ShardTables>();
@@ -615,12 +615,11 @@ static ShardTables* get_shard_tables(Context* ctx, int log_n, bool inverse) {
   return raw;
 }
 
-// the join: ctx->gather holds the G sub-spectra (rank r at r * rank_stride elements, M valid entries each)
+// the join: `sub` holds the G = 2^log_g sub-spectra (rank r at r * rank_stride elements, M valid entries each);
+// `rank` only picks a cached table (the join's twiddles do not depend on it)
 void ntt_shard_combine(Context* ctx, const Fr* sub, uint64_t rank_stride, Fr* out, int log_n, bool inverse,
-                       uint64_t limit, const Fr* post_scale, uint32_t* nonzero) {
-  Comm* cm = ctx_comm(ctx);
-  const int log_g = comm_log_world(cm);
-  ShardTables* t = get_shard_tables(ctx, log_n, inverse);
+                       uint64_t limit, const Fr* post_scale, uint32_t* nonzero, int log_g, int rank) {
+  ShardTables* t = get_shard_tables(ctx, log_n, inverse, log_g, rank);
   CombineArgs a;
   a.sub = sub; a.out = out; a.M = (uint64_t)1 << (log_n - log_g); a.rank_stride = rank_stride;
   a.limit = limit; a.post_scale = post_scale; a.nonzero = nonzero; a.tw = t->dft;
@@ -638,19 +637,19 @@ void ntt_shard_combine(Context* ctx, const Fr* sub, uint64_t rank_stride, Fr* ou
 // This rank's share of `count` transforms of the same size whose inputs are spread over the G ranks by decimation
 // (logical input index i of rank r = global index G i + r; physical address in[v] + i * in_mul + in_add): local
 // M-point transforms with the join twiddle fused into the store, written to the rank's place in ctx->gather
-// ([G][count][M] layout), then ONE allgather.  ntt_shard_combine finishes each vector.
+// ([G][count][M] layout), then ONE allgather over `cm`.  ntt_shard_combine finishes each vector.  cm == nullptr: one
+// device plays every rank in turn (a sliced prover), no exchange; in[v] may then be the rank's own place in ctx->gather.
 void ntt_shard_local(Context* ctx, const Fr* const* in, int count, int log_n, bool inverse, uint64_t in_mul,
-                     uint64_t in_add) {
-  Comm* cm = ctx_comm(ctx);
-  const int log_g = comm_log_world(cm), rank = comm_rank(cm), G = 1 << log_g;
-  ShardTables* t = get_shard_tables(ctx, log_n, inverse);
+                     uint64_t in_add, int log_g, int rank, Comm* cm) {
+  const int G = 1 << log_g;
+  ShardTables* t = get_shard_tables(ctx, log_n, inverse, log_g, rank);
   const uint64_t M = (uint64_t)1 << (log_n - log_g);
   ctx->gather.ensure((size_t)G * count * M * 32);
   Fr* mine = ctx->gather.as<Fr>() + (uint64_t)rank * count * M;
   for (int v = 0; v < count; v++)
     ntt_run_fold(ctx, ctx->stream, nullptr, in[v], mine + (uint64_t)v * M, log_n - log_g, inverse, M, nullptr,
                  t->store_tw.as<Fr>(), in_mul, in_add, 1);
-  comm_allgather_inplace(cm, ctx->gather.p, (size_t)count * M * 32, ctx->stream);
+  if (cm) comm_allgather_inplace(cm, ctx->gather.p, (size_t)count * M * 32, ctx->stream);
 }
 
 // full vector in (present on every rank) -> full vector out (on every rank): poly.py:113-149 across the ranks of the
@@ -663,10 +662,10 @@ void ntt_sharded(Context* ctx, const Fr* const* in, Fr* const* out, int count, i
     return;
   }
   const uint64_t M = (uint64_t)1 << (log_n - log_g);
-  ntt_shard_local(ctx, in, count, log_n, inverse, (uint64_t)G, (uint64_t)rank);
+  ntt_shard_local(ctx, in, count, log_n, inverse, (uint64_t)G, (uint64_t)rank, log_g, rank, cm);
   for (int v = 0; v < count; v++)
     ntt_shard_combine(ctx, ctx->gather.as<Fr>() + (uint64_t)v * M, (uint64_t)count * M, out[v], log_n, inverse,
-                      (uint64_t)1 << log_n, nullptr, nullptr);
+                      (uint64_t)1 << log_n, nullptr, nullptr, log_g, rank);
 }
 
 }  // namespace pb200

@@ -33,6 +33,7 @@
 #include "comm.cuh"
 #include "transcript.cuh"
 #include "prover.cuh"
+#include "memory_plan.cuh"
 
 namespace pb200 {
 
@@ -44,9 +45,10 @@ void ntt_run_fold(Context* ctx, cudaStream_t stream, Fr* tmp, const Fr* in, Fr* 
                   uint64_t n_in, const Fr* in_scale, const Fr* out_scale, uint64_t in_mul, uint64_t in_add, uint32_t fold);
 void ntt_sharded(Context* ctx, const Fr* const* in, Fr* const* out, int count, int log_n, bool inverse);
 void ntt_shard_local(Context* ctx, const Fr* const* in, int count, int log_n, bool inverse, uint64_t in_mul,
-                     uint64_t in_add);
+                     uint64_t in_add, int log_g, int rank, Comm* cm);
 void ntt_shard_combine(Context* ctx, const Fr* sub, uint64_t rank_stride, Fr* out, int log_n, bool inverse,
-                       uint64_t limit, const Fr* post_scale, uint32_t* nonzero);
+                       uint64_t limit, const Fr* post_scale, uint32_t* nonzero, int log_g, int rank);
+uint32_t msm_default_window(uint64_t n, bool fixed_base);
 
 // Coefficients (n) -> evaluations on this rank's slice of the fixed coset (n_ext points): one forward transform of
 // size n_ext with the coset shift multiplied in on load, zero padding (n_ext > n) or wrap-around (n_ext < n).
@@ -786,6 +788,31 @@ static void set_custom_terms(Prover* P, int n_custom, const uint8_t* h_exps, int
   P->next_row = next_row;
 }
 
+// Which round-3 layout a one-GPU prover of 2^log_n rows takes (memory_plan.cuh): true for the sliced one.  Throws,
+// before anything is allocated, when neither fits the free device memory.  PB200_SLICED=1 forces the sliced layout.
+static bool plan_memory(Context* ctx, Srs* srs, int log_n, int n_custom) {
+  size_t free_b = 0, total_b = 0;
+  PB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  // the largest MSM of a proof: three commitments on the fixed-base table, or one at a time on the generic path
+  const uint32_t buckets = srs_bucket_count(srs);
+  uint32_t c = 1, batch = buckets ? 3 : 1;
+  if (buckets) while ((1u << (c - 1)) < buckets) c++;
+  else c = msm_default_window((uint64_t)1 << log_n, false);
+  uint64_t msm_now = 0;
+  for (int k = 1; k < 10; k++) msm_now += ctx->scratch[k].bytes;
+  const ProverMemory m = prover_memory(log_n, n_custom, c, batch, msm_now);
+  const char* e = getenv("PB200_SLICED");
+  const int choice = plan_choose(m, free_b, e && atoi(e) != 0);
+  if (choice < 0) {
+    char b[256];
+    const double gib = 1024.0 * 1024.0 * 1024.0;
+    snprintf(b, sizeof b, "a 2^%d prover needs %.1f GiB (%.1f GiB sliced), %.1f GiB free (%.1f GiB kept in reserve)",
+             log_n, m.full.total() / gib, m.sliced.total() / gib, free_b / gib, PB_PLAN_MARGIN / gib);
+    throw Error(b);
+  }
+  return choice == 1;
+}
+
 // h_pk: 8 vectors (QM QL QR QO QC S1 S2 S3), each n x 32 bytes canonical (compiler/program.py:10-30); h_custom:
 // n_custom more selector vectors of the same shape, with their exponents h_exps (exp_width = 3 or 6 bytes per term).
 // sharded: one proof across the ranks of the context's communicator (see Prover in prover.cuh).
@@ -808,13 +835,16 @@ Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h
     P->rank = comm_rank(cm);
     P->log_world = comm_log_world(cm);
     PB_CHECK(log_n > P->log_world, "sharded prover: fewer rows than ranks");
+  } else {
+    P->sliced = plan_memory(ctx, srs, log_n, n_custom);
+    PB_CHECK(!(P->sliced && P->next_row), PB_SLICED_WHY "next-row custom gate terms need the whole coset in round 3");
   }
   const uint32_t G = (uint32_t)P->world, R = (uint32_t)P->rank;
-  P->log_ext = log_n + 2 - P->log_world;
+  P->log_ext = P->sliced ? log_n : log_n + 2 - P->log_world;
   const uint64_t ne = P->n_ext = (uint64_t)1 << P->log_ext;
   P->fold = ne < n ? (uint32_t)(n / ne) : 1;
   P->zw_separate = (4 % G) != 0;
-  P->zw_shift = P->zw_separate ? 0 : 4 / G;
+  P->zw_shift = P->sliced ? 1 : P->zw_separate ? 0 : 4 / G;
   cudaStream_t st = ctx->stream;
   P->g = fr_from_u64(5);
   P->g_inv = fp_inv(P->g);
@@ -830,10 +860,11 @@ Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h
     P->gpow_w.alloc(n * 32);
     launch_powers(ctx, P->gpow_w.as<Fr>(), n, fp_mul(shift, fr_root_of_unity(log_n)), one);
   }
-  P->ginv_pow.alloc(n4 * 32);
-  launch_powers(ctx, P->ginv_pow.as<Fr>(), n4, P->g_inv, one);
+  const uint64_t n_ginv = P->sliced ? 3 * n : n4;  // sliced: only the join of T's 3n coefficients reads it
+  P->ginv_pow.alloc(n_ginv * 32);
+  launch_powers(ctx, P->ginv_pow.as<Fr>(), n_ginv, P->g_inv, one);
   P->xs.alloc(ne * 32);
-  launch_powers(ctx, P->xs.as<Fr>(), ne, fp_pow_u64(mu, G), shift);
+  launch_powers(ctx, P->xs.as<Fr>(), ne, fp_pow_u64(mu, P->sliced ? 4 : G), shift);  // sliced: rewritten per slice
   // Z_H on the coset takes 4 values: g^n * i^(j mod 4) - 1, i = mu^n, j the global coset index
   Fr i4 = fp_pow_u64(mu, n);
   Fr cur = fp_pow_u64(P->g, n);
@@ -842,13 +873,15 @@ Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h
     P->zh_inv[k] = fp_inv(P->zh[k]);
     cur = fp_mul(cur, i4);
   }
-  ensure_pi_basis(P.get(), 1);  // L0, for the quotient
+  if (P->sliced) P->pi_basis.emplace_back(n * 32);  // L0 of the slice round 3 is on
+  else ensure_pi_basis(P.get(), 1);                   // L0, for the quotient
   for (int k = 0; k < Prover::CUSTOM0 + n_custom; k++) {
     upload_mont(ctx, P->sel_lag[k], k < Prover::CUSTOM0 ? h_pk[k] : h_custom[k - Prover::CUSTOM0], n);
     P->sel_coeff[k].alloc(n * 32);
     ntt_run(ctx, P->sel_lag[k].as<Fr>(), P->sel_coeff[k].as<Fr>(), log_n, true, n, nullptr, nullptr);
     P->sel_ext[k].alloc(ne * 32);
-    coset_extend(P.get(), st, nullptr, P->sel_coeff[k].as<Fr>(), P->sel_ext[k].as<Fr>(), P->gpow.as<Fr>());
+    if (!P->sliced)  // sliced: recomputed for each slice in round 3
+      coset_extend(P.get(), st, nullptr, P->sel_coeff[k].as<Fr>(), P->sel_ext[k].as<Fr>(), P->gpow.as<Fr>());
   }
   for (int k = 0; k < 4; k++) P->lag[k].alloc(n * 32);
   for (int k = 0; k < 5; k++) { P->coeff[k].alloc(n * 32); P->ext[k].alloc(ne * 32); }
@@ -857,12 +890,15 @@ Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h
   if (P->world > 1) {
     P->tq.alloc(3 * n * 32);
     P->tq_loc.alloc(ne * 32);
+  } else if (P->sliced) {
+    P->tq.alloc(3 * n * 32);  // the slices' evaluations go to the four slots of the join in ctx->gather
   } else {
     P->tq.alloc(n4 * 32);
   }
   for (int k = 0; k < 5; k++) P->tmp[k].alloc(n * 32);
   P->flags.alloc(64);
   if (const char* e = getenv("PB200_OVERLAP")) P->overlap = atoi(e) != 0;
+  if (P->sliced) P->overlap = false;  // the side stream would extend onto one slice while round 3 walks all four
   PB_CUDA(cudaStreamSynchronize(st));
   PB_CUDA(cudaGetLastError());
   return P.release();
@@ -1016,6 +1052,7 @@ static void zk_enable(Prover* P, const uint8_t* h_blinders) {
 // they take other numbers of blinders: the size of the caller's buffer never depends on the prover's state.
 // Switching off through any of them ends zero-knowledge mode.
 void prover_set_zk(Prover* P, unsigned block, bool enable, const uint8_t* h_blinders) {
+  PB_CHECK(!(enable && P->sliced), PB_SLICED_WHY "zero knowledge blinds the quotient on the whole coset in round 3");
   if (block != BLOCK_PLAIN) {
     PB_CHECK(P->world == 1, "zero-knowledge proving is not available on the sharded prover (one GPU only)");
     PB_CHECK(P->blocks() & block, block == BLOCK_LOOKUP
@@ -1094,6 +1131,7 @@ void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* h_qtag, co
   const bool tagged = h_qtag != nullptr;
   const int width = tagged ? 4 : 3;
   PB_CHECK(P->world == 1, "lookups are not available on the sharded prover (one GPU only)");
+  PB_CHECK(!P->sliced, PB_SLICED_WHY "the lookup quotient needs the whole coset in round 3");
   PB_CHECK(!P->next_row, "lookups do not combine with next-row custom gate terms");
   PB_CHECK(!P->sh, "lookups do not combine with a shuffle");
   PB_CHECK(!P->zk, "lookups do not combine with zero-knowledge mode switched on first: set the table, then "
@@ -1296,6 +1334,7 @@ void prover_set_shuffle(Prover* P, const uint8_t* h_qin, const uint8_t* h_qout) 
   Context* ctx = P->ctx;
   const uint64_t n = P->n;
   PB_CHECK(P->world == 1, "shuffles are not available on the sharded prover (one GPU only)");
+  PB_CHECK(!P->sliced, PB_SLICED_WHY "the shuffle quotient needs the whole coset in round 3");
   PB_CHECK(!P->lk, "shuffles do not combine with lookups");
   PB_CHECK(!P->zk, "shuffles do not combine with zero-knowledge mode switched on first: set the shuffle, then "
                    "pb200_prover_set_zk_shuffle");
@@ -1455,7 +1494,7 @@ void prover_round1(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_
   P->n_public = n_public;
   P->pi_sparse = n_public <= 8;
   if (P->pi_sparse) {
-    ensure_pi_basis(P, (int)n_public);
+    if (!P->sliced) ensure_pi_basis(P, (int)n_public);  // sliced: made for each slice in round 3
     P->pub_neg.resize(n_public);
     for (uint64_t i = 0; i < n_public; i++) {
       Fr v;
@@ -1536,6 +1575,81 @@ void prover_round2(Prover* P, const Fr* ch) {
   P->commit(P->coeff[3].as<Fr>(), n, P->fields[F_Z]);
 }
 
+// ---- sliced round 3 -----------------------------------------------------------------------------------------
+void fr_vec_op(Context* ctx, int op, const Fr* a, const Fr* b, const Fr& scalar_canonical, Fr* out, uint64_t n,
+               uint64_t shift);
+
+// out[j] = c L_i(x_j) on slice r: Z_H is the constant zh[r] there, so L_i(x) = w^i Z_H / (n (x - w^i)) is one
+// denominator and one batched inversion (tmp[0] holds the denominators)
+static void slice_lagrange(Prover* P, int r, uint64_t i, const Fr& c, Fr* out) {
+  Context* ctx = P->ctx;
+  const uint64_t n = P->n;
+  const Fr wi = fp_pow_u64(fr_root_of_unity(P->log_n), i);
+  const Fr scale = fp_mul(fr_from_u64(n), fp_inv(fp_mul(fp_mul(wi, P->zh[r]), c)));  // 1 / den = c L_i
+  k_lagrange_den<<<PB_GRID(n, 256), 0, ctx->stream>>>(P->xs.as<Fr>(), n, wi, scale, P->tmp[0].as<Fr>());
+  const uint64_t T = (n + PB_BATCH_CH - 1) / PB_BATCH_CH;
+  k_batch_div<<<PB_GRID(T, 128), 0, ctx->stream>>>(nullptr, P->tmp[0].as<Fr>(), out, n, T);
+  ctx->launches += 2;
+}
+
+// The quotient of a sliced prover: for r = 0..3 the n points {g mu^(4j + r)} of the 4n coset (world = 4, rank = r in
+// k_quotient, so Z(w x_j) is the next point of the slice and Z_H is one constant): A, B, C, Z (PI when dense) and
+// every selector are extended onto the slice, L0 and a sparse PI come from the closed form, and the slice's inverse
+// transform goes to slot r of ctx->gather with the join's twiddle on the store (ntt_shard_local).  The join then keeps
+// T's 3n coefficients in tq and counts the non-zero top n in flags[0] (prover.py:205-208).
+static void quotient_sliced(Prover* P) {
+  Context* ctx = P->ctx;
+  const uint64_t n = P->n;
+  cudaStream_t st = ctx->stream;
+  const Fr mu = fr_root_of_unity(P->log_n + 2), w = fr_root_of_unity(P->log_n);
+  ctx->gather.ensure(4 * n * 32);
+  QuotientArgs q;
+  q.pi_cnt = 0;
+  q.A = P->ext[0].as<Fr>(); q.B = P->ext[1].as<Fr>(); q.C = P->ext[2].as<Fr>(); q.Z = P->ext[3].as<Fr>();
+  q.Zw = q.Z;
+  q.zw_shift = P->zw_shift;
+  q.world = 4;
+  q.PI = P->pi_sparse && P->n_public == 0 ? nullptr : P->ext[4].as<Fr>();
+  q.QM = P->sel_ext[Prover::QM].as<Fr>(); q.QL = P->sel_ext[Prover::QL].as<Fr>(); q.QR = P->sel_ext[Prover::QR].as<Fr>();
+  q.QO = P->sel_ext[Prover::QO].as<Fr>(); q.QC = P->sel_ext[Prover::QC].as<Fr>();
+  q.S1 = P->sel_ext[Prover::S1].as<Fr>(); q.S2 = P->sel_ext[Prover::S2].as<Fr>(); q.S3 = P->sel_ext[Prover::S3].as<Fr>();
+  q.custom = P->custom_terms(P->sel_ext);
+  q.L0 = P->pi_basis[0].as<Fr>(); q.X = P->xs.as<Fr>();
+  for (int k = 0; k < 4; k++) q.zh_inv[k] = P->zh_inv[k];
+  q.alpha = P->alpha; q.alpha2 = fp_sqr(P->alpha); q.beta = P->beta; q.gamma = P->gamma; q.one = Fr::one();
+  q.n4 = n;
+  const ZkCoset zk{};
+  for (int r = 0; r < 4; r++) {
+    const Fr shift = fp_mul(P->g, fp_pow_u64(mu, (uint64_t)r));
+    launch_powers(ctx, P->gpow.as<Fr>(), n, shift, Fr::one());
+    launch_powers(ctx, P->xs.as<Fr>(), n, w, shift);
+    for (int k = 0; k < (P->pi_sparse ? 4 : 5); k++)
+      coset_extend(P, st, nullptr, P->coeff[k].as<Fr>(), P->ext[k].as<Fr>(), P->gpow.as<Fr>());
+    for (int k = 0; k < Prover::CUSTOM0 + P->n_custom; k++)
+      coset_extend(P, st, nullptr, P->sel_coeff[k].as<Fr>(), P->sel_ext[k].as<Fr>(), P->gpow.as<Fr>());
+    slice_lagrange(P, r, 0, Fr::one(), P->pi_basis[0].as<Fr>());
+    if (P->pi_sparse) {  // PI = sum_i -public_i L_i, summed into ext[4] (tmp[1] holds a term)
+      bool first = true;
+      for (uint64_t i = 0; i < P->n_public; i++) {
+        if (P->pub_neg[i].is_zero()) continue;
+        slice_lagrange(P, r, i, P->pub_neg[i], first ? P->ext[4].as<Fr>() : P->tmp[1].as<Fr>());
+        if (!first) fr_vec_op(ctx, 0, P->ext[4].as<Fr>(), P->tmp[1].as<Fr>(), Fr::zero(), P->ext[4].as<Fr>(), n, 0);
+        first = false;
+      }
+      if (first && P->n_public) PB_CUDA(cudaMemsetAsync(P->ext[4].p, 0, n * 32, st));
+    }
+    q.rank = (uint32_t)r;
+    Fr* slot = ctx->gather.as<Fr>() + (uint64_t)r * n;
+    k_quotient<false, false><<<PB_GRID(n, 128), 0, st>>>(q, slot, zk);
+    ctx->launches++;
+    const Fr* te = slot;
+    ntt_shard_local(ctx, &te, 1, P->log_n + 2, true, 1, 0, 2, r, nullptr);
+  }
+  PB_CUDA(cudaMemsetAsync(P->flags.p, 0, 64, st));
+  ntt_shard_combine(ctx, ctx->gather.as<Fr>(), n, P->tq.as<Fr>(), P->log_n + 2, true, 3 * n, P->ginv_pow.as<Fr>(),
+                    P->flags.as<uint32_t>(), 2, 0);
+}
+
 // ---- round 3 (prover.py:154-226) -------------------------------------------------------------------------
 void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c) {
   Context* ctx = P->ctx;
@@ -1543,6 +1657,13 @@ void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c) {
   cudaStream_t st = ctx->stream;
   P->alpha = fp_to_mont(alpha_c);
   P->fft_cofactor = fp_to_mont(cofactor_c);
+  if (P->sliced) {
+    quotient_sliced(P);
+    PB_CHECK(read_flag(P, 0) == 0, "AssertionError: quotient has degree >= 3n (prover.py:205-208)");
+    const Fr* t123[3] = {P->tq.as<Fr>(), P->tq.as<Fr>() + n, P->tq.as<Fr>() + 2 * n};
+    P->commit_batch(t123, 3, n, P->fields[F_T_LO]);
+    return;
+  }
   if (P->overlap) {  // A, B, C, Z were extended on the side stream during rounds 1 and 2
     PB_CUDA(cudaStreamWaitEvent(st, ctx->aux_ev[0], 0));
     PB_CUDA(cudaStreamWaitEvent(st, ctx->aux_ev[1], 0));
@@ -1660,9 +1781,9 @@ void prover_round3(Prover* P, const Fr& alpha_c, const Fr& cofactor_c) {
     // slab-sharded inverse over the 4n coset: the local inverse transform of the slice, ONE allgather, then the
     // join multiplies g^-i in and keeps the 3n coefficients (the top n must vanish: prover.py:205-208)
     const Fr* te = t_evals;
-    ntt_shard_local(ctx, &te, 1, P->log_n + 2, true, 1, 0);
+    ntt_shard_local(ctx, &te, 1, P->log_n + 2, true, 1, 0, P->log_world, P->rank, ctx_comm(ctx));
     ntt_shard_combine(ctx, ctx->gather.as<Fr>(), ne, P->tq.as<Fr>(), P->log_n + 2, true, 3 * n,
-                      P->ginv_pow.as<Fr>(), P->flags.as<uint32_t>());
+                      P->ginv_pow.as<Fr>(), P->flags.as<uint32_t>(), P->log_world, P->rank);
   } else {
     // back to coefficients: ifft(4n) then * g^-i (poly.py:169-177 with the fixed coset)
     ntt_run(ctx, P->tq.as<Fr>(), P->tq.as<Fr>(), P->log_n + 2, true, n4, nullptr, P->ginv_pow.as<Fr>());

@@ -20,6 +20,7 @@ uint32_t srs_bucket_count(Srs* s);
 // 2 c, 3 a(wX), 4 b(wX), 5 c(wX)}, unused slots PB_FACTOR_ONE.  Factors 3..5 (next-row terms, degree 1 to 3) occur only
 // on a prover made by pb200_prover_create_custom_next_row (Prover::next_row).
 #define PB_MAX_CUSTOM 4
+#define PB_SLICED_WHY "not available on a sliced prover (its 4n-coset cache does not fit in device memory, or PB200_SLICED=1): "
 #define PB_FACTOR_ONE 6
 struct CustomTerms {
   const Fr* Q[PB_MAX_CUSTOM];
@@ -95,6 +96,12 @@ struct Prover {
   uint32_t fold = 1;     // n / n_ext when the coset slice is shorter than a coefficient vector (world = 8), else 1
   uint64_t zw_shift = 4; // Z(w x_j) = Z-extension at local index j + 4 / world ...
   bool zw_separate = false;  // ... or, when 4 % world != 0, a separately extended vector (ext[5])
+  // One GPU whose 4n-coset cache does not fit its memory (memory_plan.cuh), or PB200_SLICED=1: round 3 walks the four
+  // n-point slices {g mu^(4j + r)} in turn, as the ranks of a 4-GPU sharded prover would, and joins them on the device.
+  // sel_ext, xs, pi_basis[0] and ext[] then hold one slice (n points), recomputed for each; tq holds T's 3n
+  // coefficients.  Plain circuits and same-row custom terms only: zero knowledge, lookups, shuffles and next-row terms
+  // are refused (PB_SLICED_WHY).
+  bool sliced = false;
   // per-circuit (all Montgomery)
   DevBuf sel_coeff[8 + PB_MAX_CUSTOM];   // QM QL QR QO QC S1 S2 S3, then the custom selectors; coefficient form
   DevBuf sel_lag[8 + PB_MAX_CUSTOM];     // same, Lagrange values (QM..QC and custom for the gate check, S1..S3 for round 2)

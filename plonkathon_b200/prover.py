@@ -303,6 +303,15 @@ class Prover:
                               ctypes.byref(h)))
         self._h = h
 
+    @property
+    def sliced(self) -> bool:
+        """True when the library chose (or ``PB200_SLICED=1`` forced) the sliced round 3: the cache on the 4n coset did
+        not fit the free device memory, so the quotient is evaluated one n-point slice of the coset at a time.  Same
+        proofs; zero knowledge, lookups, shuffles and next-row terms are refused on such a prover."""
+        out = ctypes.c_int()
+        _lib.check(_lib.lib().pb200_prover_sliced(self._h, ctypes.byref(out)))
+        return bool(out.value)
+
     def __del__(self):
         try:
             if getattr(self, "_h", None):
