@@ -126,6 +126,16 @@ int pb200_srs_commit_coeffs(pb200_ctx* ctx, pb200_srs* srs, const void* d_coeffs
 int pb200_srs_commit_coeffs_host(pb200_ctx* ctx, pb200_srs* srs, const uint8_t* h_coeffs, uint64_t m,
                                  uint8_t* h_out_xy, int* is_identity);
 
+/* ---- Circuit preprocessing ------------------------------------------------------------------ */
+/* The copy-constraint permutation of a wiring (compiler/program.py:70-113): h_ids holds 3n variable ids, row-major
+ * (L, R, O of row 0, then of row 1, ...), -1 for "no variable", each in [-1, 2^32 - 2].  Every cell stores the label
+ * omega^row' (col' + 1) of the previous cell carrying its id, in cell order and cyclically; all -1 cells form one more
+ * cycle.  Writes S1, S2, S3 (n canonical 32-byte little-endian values each, one after the other) to h_S, exactly the
+ * "S1".."S3" columns of a proving key.  Runs on the context's stream and frees its device memory before returning.
+ * Refuses, before any device work, log_n outside 1..26, an id out of range (naming its cell) and more device memory
+ * than is free (naming the bytes needed: 176 n bytes + the sort's temporary storage). */
+int pb200_permutation(pb200_ctx* ctx, const int64_t* h_ids, int log_n, uint8_t* h_S);
+
 /* ---- Prover (prover.py:39-306) ---------------------------------------------------------------- */
 /* Proof layout.  A prover's proof is the plain 15 fields, then the fields of the blocks it has (next-row custom gate
  * terms, a shuffle, a lookup argument), in this order; a point is 64 bytes (x||y), a scalar 32, big-endian in a proof

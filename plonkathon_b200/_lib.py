@@ -115,6 +115,7 @@ def _load():
         "pb200_g2_add": (I, [V, I, V, I, V, P(I)]),
         "pb200_bench_modmul": (I, [V, I, U64, U, P(ctypes.c_float)]),
         "pb200_prover_sliced": (I, [V, P(I)]),
+        "pb200_permutation": (I, [V, V, I, V]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)  # AttributeError here == ABI drift: fail loudly

@@ -61,6 +61,8 @@ void prover_set_shuffle(Prover* P, const uint8_t* h_qin, const uint8_t* h_qout);
 void g1_combine_partials_host(const G1XYZZ* parts, uint32_t count, uint8_t* out_xy, int* is_identity);
 void host_join_bucket_shards(const SR* all, uint32_t world, uint32_t sets, uint32_t nloc, G1XYZZ* out);
 void host_join_bucket_shards_strided(const SR* all, uint32_t world, uint32_t sets, G1XYZZ* out);
+// permutation.cu
+void permutation_run(Context* ctx, const int64_t* h_ids, int log_n, uint8_t* h_S);
 }  // namespace pb200
 
 using namespace pb200;
@@ -531,6 +533,12 @@ int pb200_prover_create_custom_sharded(pb200_ctx* ctx, pb200_srs* srs, unsigned 
                                                        (int)n_custom, h_exps, h_custom, true, 3));
   PB_API_END
 }
+int pb200_permutation(pb200_ctx* ctx, const int64_t* h_ids, int log_n, uint8_t* h_S) {
+  PB_API_BEGIN PB_ON_CTX(C(ctx));
+  permutation_run(C(ctx), h_ids, log_n, h_S);
+  PB_API_END
+}
+
 void pb200_prover_destroy(pb200_prover* p) { prover_destroy(reinterpret_cast<Prover*>(p)); }
 int pb200_prover_sliced(pb200_prover* p, int* out) {
   PB_API_BEGIN

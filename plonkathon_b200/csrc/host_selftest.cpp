@@ -1,8 +1,8 @@
 // Host build of the limb-level arithmetic in field.cuh / curve.cuh (same code path as the device,
 // PTX carry-chain primitives replaced by their emulation).  TEST INFRASTRUCTURE: loaded only by
 // tests/test_host_arith.py through ctypes; never linked into libplonk_b200.so.  It also exports the proof layout
-// (proof_layout.cuh) for tests/test_proof_layout.py and the prover's memory plan (memory_plan.cuh) for
-// tests/test_sliced_prover.py.
+// (proof_layout.cuh) for tests/test_proof_layout.py, the prover's memory plan (memory_plan.cuh) for
+// tests/test_sliced_prover.py and the permutation's label body (permutation.cuh) for tests/test_wiring_host.py.
 #include "field.cuh"
 #include "curve.cuh"
 #include "msm_digits.cuh"
@@ -12,6 +12,7 @@
 #include "ntt_shard.cuh"
 #include "proof_layout.cuh"
 #include "memory_plan.cuh"
+#include "permutation.cuh"
 #include <algorithm>
 #include <vector>
 #include <cstring>
@@ -562,5 +563,37 @@ int hs_prover_memory(int log_n, int n_custom, uint32_t msm_c, uint32_t msm_batch
     out[4 * k + 3] = c[k]->msm;
   }
   return plan_choose(m, free_bytes, force_sliced != 0);
+}
+}
+
+extern "C" {
+// The permutation of permutation.cu on the CPU: the same id check and keys, std::sort in place of the radix sort, the
+// label body run for every sorted position.  ids: 3n ids, row-major L R O; omega: the n-th root of unity, canonical
+// (8 words); out: S1 | S2 | S3, 3n canonical values.  Returns -1, or the index of the first bad id (nothing written).
+int64_t hs_permutation(const int64_t* ids, int log_n, const uint32_t* omega, uint32_t* out) {
+  const uint64_t n = (uint64_t)1 << log_n, m = 3 * n;
+  const int cb = perm_cell_bits(log_n);
+  int64_t max_id = -1;
+  const int64_t bad = perm_check_ids(ids, m, &max_id);
+  if (bad >= 0) return bad;
+  std::vector<uint64_t> keys(m);
+  for (uint64_t k = 0; k < m; k++) keys[k] = perm_key(ids[k], k, cb);
+  std::sort(keys.begin(), keys.end());
+  if (perm_sort_bits(log_n, max_id) < 64 && keys.back() >> perm_sort_bits(log_n, max_id)) abort();  // bits unused
+  std::vector<Fr> wpow(n);
+  const Fr w = fp_to_mont(ld<Fr>(omega));
+  Fr cur = Fr::one();
+  for (uint64_t i = 0; i < n; i++) { wpow[i] = fp_from_mont(cur); cur = fp_mul(cur, w); }
+  std::vector<Fr> S(m);
+  PermArgs a;
+  a.keys = keys.data();
+  a.wpow = wpow.data();
+  a.S = S.data();
+  a.n = n;
+  a.m = m;
+  a.cb = cb;
+  for (uint64_t k = 0; k < m; k++) perm_label(a, k);
+  for (uint64_t k = 0; k < m; k++) st(out + 8 * k, S[k]);
+  return -1;
 }
 }
