@@ -11,6 +11,8 @@
  *                     (which need one modular inversion per affine addition: minutes at 2^20).
  *   oc_fr_eval_lagrange -- value at x of the polynomial given by Lagrange values (used to re-derive KZG
  *                     commitments [f(tau)]G under a structured test SRS).
+ *   oc_fr_eval_coeffs -- value at x of the polynomial given by its coefficients (Horner).  With eval_lagrange it
+ *                     checks a whole transform in O(n): one identity at one random point.
  *
  * It is cross-checked against oracle/plonk_oracle.py (itself pinned by the reference's golden vectors) in
  * tests/test_oracle_c.py.  Arithmetic: 4 x 64-bit limbs, Montgomery form R = 2^256, unsigned __int128.
@@ -157,29 +159,46 @@ int oc_fr_eval_lagrange(const uint8_t* vals, unsigned log_n, const uint8_t* x32,
   fe x; { fe t; memcpy(t.v, x32, 32); fe_to_mont(&FR, &x, &t); }
   uint64_t e[4] = {FR.p.v[0] - 1, FR.p.v[1], FR.p.v[2], FR.p.v[3]};
   for (unsigned s = 0; s < log_n; s++) { for (int i = 0; i < 4; i++) e[i] = (e[i] >> 1) | (i < 3 ? e[i + 1] << 63 : 0); }
-  fe five, w; fe_from_u64(&FR, &five, 5); fe_pow(&FR, &w, &five, e);
-  fe* d = (fe*)malloc(n * sizeof(fe)); fe* pref = (fe*)malloc(n * sizeof(fe)); fe* ws = (fe*)malloc(n * sizeof(fe));
-  if (!d || !pref || !ws) return 1;
-  fe cur = FR.r1, run = FR.r1;
+  fe five, w, w_inv; fe_from_u64(&FR, &five, 5); fe_pow(&FR, &w, &five, e); fe_inv(&FR, &w_inv, &w);
+  fe* d = (fe*)malloc(n * sizeof(fe)); fe* pref = (fe*)malloc(n * sizeof(fe));
+  if (!d || !pref) { free(d); free(pref); return 1; }
+  /* w^i / (x - w^i) = 1 / d_i with d_i = x w^-i - 1: one batch inversion of the d_i */
+  fe cur = x, run = FR.r1;
   for (size_t i = 0; i < n; i++) {
-    ws[i] = cur; fe_sub(&FR, &d[i], &x, &cur);
+    fe_sub(&FR, &d[i], &cur, &FR.r1);
     pref[i] = run; fe_mul(&FR, &run, &run, &d[i]);
-    fe_mul(&FR, &cur, &cur, &w);
+    fe_mul(&FR, &cur, &cur, &w_inv);
   }
   fe inv; fe_inv(&FR, &inv, &run);
-  fe acc = {{0, 0, 0, 0}};
+  fe acc = {{0, 0, 0, 0}};  /* canonical: a canonical value times a Montgomery-form 1/d_i is the plain quotient */
   for (size_t i = n; i-- > 0;) {
-    fe di, v, t; fe_mul(&FR, &di, &inv, &pref[i]); fe_mul(&FR, &inv, &inv, &d[i]);
+    fe di, t; fe_mul(&FR, &di, &inv, &pref[i]); fe_mul(&FR, &inv, &inv, &d[i]);
     memcpy(t.v, vals + 32 * i, 32);
     if (fe_is_zero(&t)) continue;
-    fe_to_mont(&FR, &v, &t); fe_mul(&FR, &v, &v, &ws[i]); fe_mul(&FR, &v, &v, &di); fe_add(&FR, &acc, &acc, &v);
+    fe_mul(&FR, &t, &t, &di); fe_add(&FR, &acc, &acc, &t);
   }
   /* (x^n - 1) / n */
   fe xn = x; for (unsigned s = 0; s < log_n; s++) fe_mul(&FR, &xn, &xn, &xn);
   fe num, nn, ninv; fe_sub(&FR, &num, &xn, &FR.r1); fe_from_u64(&FR, &nn, (uint64_t)n); fe_inv(&FR, &ninv, &nn);
   fe_mul(&FR, &acc, &acc, &num); fe_mul(&FR, &acc, &acc, &ninv);
-  fe o; fe_from_mont(&FR, &o, &acc); memcpy(out32, o.v, 32);
-  free(d); free(pref); free(ws);
+  memcpy(out32, acc.v, 32);
+  free(d); free(pref);
+  return 0;
+}
+
+/* value at x of sum_{i < n} c_i x^i by Horner (any n >= 0; n == 0 gives 0).  coeffs: n x 32 bytes canonical.
+ * The accumulator stays canonical: a Montgomery product with x in Montgomery form is a plain product.      */
+int oc_fr_eval_coeffs(const uint8_t* coeffs, uint64_t n, const uint8_t* x32, uint8_t* out32) {
+  ensure_init();
+  fe x; { fe t; memcpy(t.v, x32, 32); fe_to_mont(&FR, &x, &t); }
+  fe acc = {{0, 0, 0, 0}};
+  for (uint64_t i = n; i-- > 0;) {
+    fe c; memcpy(c.v, coeffs + 32 * i, 32);
+    if (fe_geq(&c, &FR.p)) return 2;  /* not canonical */
+    fe_mul(&FR, &acc, &acc, &x);
+    fe_add(&FR, &acc, &acc, &c);
+  }
+  memcpy(out32, acc.v, 32);
   return 0;
 }
 
