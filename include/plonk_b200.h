@@ -102,12 +102,14 @@ int pb200_g1_msm_host(pb200_ctx* ctx, const uint8_t* h_points, const uint8_t* h_
 int pb200_srs_create(pb200_ctx* ctx, const uint8_t* h_points, uint64_t n, int precompute, pb200_srs** out);
 /* Structured test SRS generated on the device: points [tau^i]G, i < n, for a known (toxic) tau --
  * the 2^20 / 2^22 configurations need more powers than the reference's shipped .ptau holds
- * (setup.py:27 reads 2^11).  h_tau: canonical 32-byte Fr. */
+ * (setup.py:27 reads 2^11).  h_tau: canonical 32-byte Fr.  tau == 0 is refused (an error, before any device
+ * work; the context stays usable): every point after the first would be the identity. */
 int pb200_srs_generate(pb200_ctx* ctx, const uint8_t* h_tau, uint64_t n, int precompute, pb200_srs** out);
 /* SURVEY.md 8(f) N4: the same for the Lagrange basis of the size-n domain (n a power of two): points
  * [L_i(tau)]G, i < n -- what section 12 of a snarkjs .ptau holds for the ceremony's tau.  Against such an SRS
  * Setup.commit(values) (setup.py:66-72) is ONE MSM over the values, with no inverse transform:
- * pb200_srs_commit_coeffs / _host with the LAGRANGE values in place of coefficients. */
+ * pb200_srs_commit_coeffs / _host with the LAGRANGE values in place of coefficients.  A tau with tau^n == 1 (a
+ * point of the domain) is refused like tau == 0 above: L_i(tau) would be 0 for every i but one. */
 int pb200_srs_generate_lagrange(pb200_ctx* ctx, const uint8_t* h_tau, uint64_t n, int precompute, pb200_srs** out);
 /* copy `count` points starting at `first` back to the host (canonical x||y) */
 int pb200_srs_export(pb200_ctx* ctx, pb200_srs* srs, uint8_t* h_points, uint64_t first, uint64_t count);

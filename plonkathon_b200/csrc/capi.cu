@@ -447,16 +447,24 @@ int pb200_srs_create(pb200_ctx* ctx, const uint8_t* h_points, uint64_t n, int pr
   *out = reinterpret_cast<pb200_srs*>(srs_create(C(ctx), h_points, n, precompute));
   PB_API_END
 }
+// Taus whose SRS would hold the identity are refused before any device work: tau = 0 makes [tau^i]G the identity for
+// every i > 0, and tau^n = 1 makes L_i(tau) = 0 for all i but one.  The batched affine conversion cannot represent
+// the identity (k_batch_to_affine), so such an SRS would commit to wrong points without an error.
 int pb200_srs_generate(pb200_ctx* ctx, const uint8_t* h_tau, uint64_t n, int precompute, pb200_srs** out) {
   PB_API_BEGIN PB_ON_CTX(C(ctx));
   PB_CHECK(n > 0, "empty SRS");
-  *out = reinterpret_cast<pb200_srs*>(srs_generate(C(ctx), load_fr_canonical(h_tau), n, precompute));
+  const Fr tau = load_fr_canonical(h_tau);
+  PB_CHECK(!tau.is_zero(), "tau == 0 mod r: every SRS point after the first would be the identity");
+  *out = reinterpret_cast<pb200_srs*>(srs_generate(C(ctx), tau, n, precompute));
   PB_API_END
 }
 int pb200_srs_generate_lagrange(pb200_ctx* ctx, const uint8_t* h_tau, uint64_t n, int precompute, pb200_srs** out) {
   PB_API_BEGIN PB_ON_CTX(C(ctx));
   PB_CHECK(n > 0, "empty SRS");
-  *out = reinterpret_cast<pb200_srs*>(srs_generate_lagrange(C(ctx), load_fr_canonical(h_tau), n, precompute));
+  const Fr tau = load_fr_canonical(h_tau);
+  PB_CHECK(fp_pow_u64(fp_to_mont(tau), n) != Fr::one(),
+           "tau^n == 1 mod r (tau is on the domain): every Lagrange point but one would be the identity");
+  *out = reinterpret_cast<pb200_srs*>(srs_generate_lagrange(C(ctx), tau, n, precompute));
   PB_API_END
 }
 int pb200_srs_commit_coeffs_host(pb200_ctx* ctx, pb200_srs* srs, const uint8_t* h_coeffs, uint64_t m,

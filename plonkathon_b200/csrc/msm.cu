@@ -466,7 +466,10 @@ void affine_to_mont(Context* ctx, const G1Affine* in, G1Affine* out, uint64_t n)
   PB_CUDA(cudaGetLastError());
 }
 
-// XYZZ -> affine with Montgomery's batch-inversion trick, CH points per thread (none is the identity)
+// XYZZ -> affine with Montgomery's batch-inversion trick, CH points per thread.  No input may be the identity: one
+// ZZZ == 0 zeroes the product of its chunk, and every point of that chunk comes out as (0, 0), which is neither the
+// MSM's identity encoding nor on the curve.  Every caller converts k P for a point P != O and 0 < k < r (the group
+// has prime order r); pb200_srs_generate / _lagrange refuse the taus that would make k = 0.
 __global__ void __launch_bounds__(128) k_batch_to_affine(const G1XYZZ* in, G1Affine* out, uint64_t n) {
   const int CH = 16;
   uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;

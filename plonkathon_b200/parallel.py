@@ -36,9 +36,11 @@ def shard_range(n: int, rank: int, world: int):
 
 
 def bucket_range(n_buckets: int, rank: int, world: int):
-    """Bucket magnitudes [lo, hi) of rank `rank`: the even split the library uses for sharded commitments."""
+    """Bucket magnitudes [lo, hi) of rank `rank`: n_buckets // world each, starting at rank * (n_buckets // world) as
+    the contiguous join (join_bucket_shards with nloc > 0) expects; the last rank also takes the n_buckets % world
+    left over, so the ranges cover every bucket for any world size."""
     per = n_buckets // world
-    return rank * per, (rank + 1) * per
+    return rank * per, n_buckets if rank == world - 1 else (rank + 1) * per
 
 
 def combine_partials(parts: bytes, count: int):

@@ -69,7 +69,9 @@ class Setup:
     def generate(cls, tau: int, n: int, ctx: Optional[_lib.Context] = None, precompute: bool = True):
         """Structured test SRS [tau^i]G, i < n, generated on the GPU (the shipped .ptau stops at 2^11 powers,
         setup.py:27).  ``powers_of_x`` is materialised lazily; ``X2`` = [tau]_2 comes from the library's host G2
-        arithmetic."""
+        arithmetic.  tau = 0 mod r raises ValueError: every point after the first would be the identity."""
+        if tau % CURVE_ORDER == 0:
+            raise ValueError("tau == 0 mod r: every SRS point after the first would be the identity")
         self = cls.__new__(cls)
         self._powers = None
         self._n = n
@@ -152,7 +154,8 @@ class Setup:
 
     def enable_lagrange(self, n: int):
         """Make ``commit`` of n values use the Lagrange-basis points.  From a .ptau they come from section 12; for a
-        generated SRS (known tau) they are computed on the device."""
+        generated SRS (known tau) they are computed on the device; a tau with tau^n = 1 (on the domain) raises
+        ValueError, as every Lagrange point but one would be the identity."""
         if self._lagrange.get(n):
             return True
         h = ctypes.c_void_p()
@@ -161,6 +164,9 @@ class Setup:
             _lib.check(_lib.lib().pb200_srs_create(self.ctx.handle, block, n, 1 if self._precompute else 0,
                                                    ctypes.byref(h)))
         elif getattr(self, "tau", None) is not None:
+            if pow(self.tau, n, CURVE_ORDER) == 1:
+                raise ValueError("tau^n == 1 mod r (tau is on the size-%d domain): every Lagrange point but one "
+                                 "would be the identity" % n)
             _lib.check(_lib.lib().pb200_srs_generate_lagrange(self.ctx.handle, self.tau.to_bytes(32, "little"), n,
                                                               1 if self._precompute else 0, ctypes.byref(h)))
         else:

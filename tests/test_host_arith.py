@@ -15,16 +15,28 @@ CSRC = os.path.join(ROOT, "plonkathon_b200", "csrc")
 R256 = 1 << 256
 
 
-@pytest.fixture(scope="module")
-def lib():
-    out = os.path.join(ROOT, "build", "host_selftest.so")
+def _build(name, *defines):
+    out = os.path.join(ROOT, "build", name)
     os.makedirs(os.path.dirname(out), exist_ok=True)
     src = os.path.join(CSRC, "host_selftest.cpp")
     deps = [src] + [os.path.join(CSRC, h) for h in ("field.cuh", "curve.cuh", "msm_digits.cuh", "msm_bucket.cuh", "modinv.cuh", "ntt_shard.cuh")]
     if not os.path.exists(out) or any(os.path.getmtime(d) > os.path.getmtime(out) for d in deps):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-x", "c++", src,
+        subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", *defines, "-x", "c++", src,
                                "-I", CSRC, "-o", out])
     return ctypes.CDLL(out)
+
+
+@pytest.fixture(scope="module")
+def lib():
+    return _build("host_selftest.so")
+
+
+@pytest.fixture(scope="module")
+def fast_lib():
+    """the same source built as the library builds its host code: with -DPB_HOST_FAST_MUL, fp_mul, fp_mul_lazy,
+    fp_sqr_lazy and fp_mul2_lazy run fp_mul_host64 (4 x 64-bit CIOS) on the host, the arithmetic of the pairing,
+    challenge reduction and the affine conversion of MSM results"""
+    return _build("host_selftest_fast_mul.so", "-DPB_HOST_FAST_MUL")
 
 
 def limbs(x, n=1):
@@ -272,3 +284,18 @@ def test_safegcd_inverse(lib, field, p):
     for a in vals[:400]:
         a %= p
         assert fop(lib, field, 9, a) == fop(lib, field, 4, a), a
+
+
+# ------------------------------------------------------------------ the fast host multiply (fp_mul_host64)
+def _fast_mul_checks():
+    from tests import test_group_law_host as GL
+    return {"field_ops": test_field_ops, "safegcd_inverse": test_safegcd_inverse, "sqr_matches_mul": GL.test_sqr_matches_mul,
+            "lazy_products": GL.test_lazy_products_and_differences, "sum_of_two_products": GL.test_sum_of_two_products}
+
+
+@pytest.mark.parametrize("check", sorted(_fast_mul_checks()))
+@pytest.mark.parametrize("field,p", [(0, O.R_MOD), (1, O.Q_MOD)])
+def test_fast_host_mul(fast_lib, check, field, p):
+    """the edge-value checks of the limb build, run against the -DPB_HOST_FAST_MUL build (its lazy results are
+    canonical, so the < 2p bounds hold as well)"""
+    _fast_mul_checks()[check](fast_lib, field, p)

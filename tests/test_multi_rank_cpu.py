@@ -81,6 +81,18 @@ def test_shard_range_partitions():
             assert pos == n
 
 
+def test_bucket_range_covers_every_bucket():
+    """contiguous bucket ranges for any world size: adjacent, from 0 to n_buckets, each starting at rank * (n // world)
+    (the offset the contiguous join applies)"""
+    from plonkathon_b200.parallel import bucket_range
+    for nb in (1, 8, 2048, 1 << 20):
+        for world in (1, 2, 3, 4, 5, 7, 8):
+            cuts = [bucket_range(nb, r, world) for r in range(world)]
+            assert cuts[0][0] == 0 and cuts[-1][1] == nb
+            assert all(a[1] == b[0] for a, b in zip(cuts, cuts[1:]))
+            assert all(lo == r * (nb // world) for r, (lo, _) in enumerate(cuts))
+
+
 def _ntt_cpu_worker(rank, world, port, log_n, q):
     """the slab-sharded NTT of csrc/ntt_shard.cuh (pb200_fr_ntt_sharded) with the oracle standing in for the CUDA
     kernels: local transform of x[rank::world], join twiddle on the store, ONE allgather, a G-point DFT per element"""
