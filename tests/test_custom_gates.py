@@ -1,6 +1,6 @@
 """Custom gates: selector columns Q_k for degree-2 and degree-3 wire terms a^i b^j c^l (plonkathon_b200/custom_gates.py).
 
-CPU: the oracle with custom terms (tests/custom_gate_oracle.py) proves circuits that its trapdoor verifier and the
+CPU: the oracle with custom terms (tests/extended_oracle.py) proves circuits that its trapdoor verifier and the
 product's host verifier accept, and rejects what it must; malformed terms are refused.  GPU: the prover's 768 bytes
 equal the oracle's for single terms and all four together, at several sizes and on both public-input paths; the 2^16
 golden proof is reproduced; a 2^20-gate custom circuit verifies; the sharded prover agrees with the single-GPU one."""
@@ -15,7 +15,8 @@ import pytest
 from oracle import fast as F
 from oracle import plonk_oracle as O
 from plonkathon_b200 import synthetic as syn
-from tests import custom_gate_oracle as CG
+from tests import extended_oracle as XO
+from tests.oracle_keys import host_lincomb  # noqa: F401  (a fixture)
 from tests.golden_io import GOLDEN, pt
 
 R = O.R_MOD
@@ -36,12 +37,12 @@ def _circuit(log_n, n_public, terms, seed):
 
 def _oracle_proof(c, fast=True):
     n = c.group_order
-    pk = CG.preprocessed(c)
+    pk = XO.preprocessed(c)
     A, B, C = c.wires_values()
     setup = F.Setup(TAU, n)
     if not fast:
         setup = O.Setup([setup.point(i) for i in range(n)], None)
-    return pk, setup, CG.prove(setup, pk, A, B, C, c.public_values(), fast=fast)
+    return pk, setup, XO.prove(setup, pk, A, B, C, c.public_values(), fast=fast)
 
 
 def _oracle_vk(c, pk, setup):
@@ -60,21 +61,21 @@ def test_oracle_custom_proof_verifies(terms, log_n):
     pk, setup, proof = _oracle_proof(c, fast=log_n > 4)  # 2^4: the pure-Python transforms
     vk, custom = _oracle_vk(c, pk, setup)
     public = c.public_values()
-    assert CG.verify_proof_trapdoor(c.group_order, vk, custom, proof, public, TAU)
-    assert not CG.verify_proof_trapdoor(c.group_order, vk, custom, proof, [public[0] + 1] + public[1:], TAU)
+    assert XO.verify_proof_trapdoor(c.group_order, dict(vk, custom=custom), proof, public, TAU)
+    assert not XO.verify_proof_trapdoor(c.group_order, dict(vk, custom=custom), proof, [public[0] + 1] + public[1:], TAU)
     bad = dict(proof, c_eval=(proof["c_eval"] + 1) % R)
-    assert not CG.verify_proof_trapdoor(c.group_order, vk, custom, bad, public, TAU)
+    assert not XO.verify_proof_trapdoor(c.group_order, dict(vk, custom=custom), bad, public, TAU)
 
 
 @pytest.mark.parametrize("terms", TERM_SETS, ids=TERM_IDS)
 def test_oracle_rejects_violated_custom_row(terms):
     c = _circuit(5, 2, terms, 3)
-    pk = CG.preprocessed(c)
+    pk = XO.preprocessed(c)
     A, B, C = c.wires_values()
     row = next(i for i in range(c.group_order) if any(col[i] for _, col in c.custom))
     C[row] = (C[row] + 1) % R  # every term here has c in its row's constraint (as output or as a factor)
     with pytest.raises(AssertionError, match="gate %d unsatisfied" % row):
-        CG.prove(F.Setup(TAU, c.group_order), pk, A, B, C, c.public_values(), fast=True)
+        XO.prove(F.Setup(TAU, c.group_order), pk, A, B, C, c.public_values(), fast=True)
 
 
 def test_oracle_zero_custom_columns_give_the_plain_proof():
@@ -85,7 +86,7 @@ def test_oracle_zero_custom_columns_give_the_plain_proof():
     setup = F.Setup(TAU, n)
     plain = F.prove(setup, O.Preprocessed(n, c.QM, c.QL, c.QR, c.QO, c.QC, *S), A, B, C, c.public_values())
     zero = dataclasses.replace(c, custom=[(e, [0] * n) for e in ALL_TERMS])
-    assert CG.prove(setup, CG.preprocessed(zero, S), A, B, C, c.public_values(), fast=True) == plain
+    assert XO.prove(setup, XO.preprocessed(zero, S), A, B, C, c.public_values(), fast=True) == plain
 
 
 def test_custom_keyword_off_keeps_the_plain_circuit():
@@ -96,19 +97,6 @@ def test_custom_keyword_off_keeps_the_plain_circuit():
         x, y = getattr(a, f.name), getattr(b, f.name)
         assert (np.array_equal(x, y) if isinstance(x, np.ndarray) else x == y), f.name
     assert a.custom == []
-
-
-@pytest.fixture
-def host_lincomb(monkeypatch):
-    """the verifier's G1 combinations by the oracle's double-and-add (this suite has no GPU)"""
-    import plonkathon_b200 as pb
-    from plonkathon_b200 import verifier
-
-    def lincomb(pairs, ctx=None):
-        res = O.ec_lincomb_naive([(None if p is None else (int(p[0]), int(p[1])), int(k) % R) for p, k in pairs])
-        return None if res is None else (pb.FQ(res[0]), pb.FQ(res[1]))
-    monkeypatch.setattr(verifier, "ec_lincomb", lincomb)
-    return pb
 
 
 def test_host_verifier_accepts_custom_proofs_and_rejects_wrong_keys(host_lincomb):
@@ -240,14 +228,14 @@ def test_gpu_custom_2p20_verifies():
         ("Qm", "Qm"), ("Ql", "Ql"), ("Qr", "Qr"), ("Qo", "Qo"), ("Qc", "Qc"), ("S1", "S1"), ("S2", "S2"), ("S3", "S3"))}
     ocustom = [(e, (p[0].n, p[1].n)) for e, p in vk.custom]
     proof = O.proof_from_bytes(raw)
-    assert CG.verify_proof_trapdoor(n, okey, ocustom, proof, public, TAU)
+    assert XO.verify_proof_trapdoor(n, dict(okey, custom=ocustom), proof, public, TAU)
     # one custom commitment re-derived on the CPU: [Q_k(tau)] G
     e0, col0 = c.custom[0]
     assert ocustom[0][1] == O.g1_multiply(O.G1, O.eval_lagrange_at(col0, TAU))
     k = 32 * 16  # c_eval
     bad = raw[:k] + ((int.from_bytes(raw[k:k + 32], "big") + 1) % R).to_bytes(32, "big") + raw[k + 32:]
     assert not vk.verify_proof(n, pb.Proof.from_bytes(bad), public)
-    assert not CG.verify_proof_trapdoor(n, okey, ocustom, O.proof_from_bytes(bad), public, TAU)
+    assert not XO.verify_proof_trapdoor(n, dict(okey, custom=ocustom), O.proof_from_bytes(bad), public, TAU)
 
 
 @pytest.mark.gpu

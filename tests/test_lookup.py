@@ -1,6 +1,6 @@
 """Lookups: a plookup argument over one fixed three-column table (plonkathon_b200/lookup.py).
 
-CPU: the oracle with a lookup argument (tests/lookup_oracle.py) proves circuits that its trapdoor verifier and the
+CPU: the oracle with a lookup argument (tests/extended_oracle.py) proves circuits that its trapdoor verifier and the
 product's host verifier accept, for a padded range table, a 4-bit XOR table that fills the domain and a table with
 duplicate rows, each with and without a custom term; the verifiers reject tampered proofs, wrong keys and plain proofs;
 malformed arguments are refused.  GPU: the prover's 1216 bytes equal the oracle's, the 2^16 golden lookup proof is
@@ -16,7 +16,8 @@ import pytest
 from oracle import fast as F
 from oracle import plonk_oracle as O
 from plonkathon_b200 import synthetic as syn
-from tests import lookup_oracle as LK
+from tests import extended_oracle as XO
+from tests.oracle_keys import host_lincomb  # noqa: F401  (a fixture)
 from tests.golden_io import GOLDEN
 
 R = O.R_MOD
@@ -63,10 +64,10 @@ def _commit_col(setup, col):
 
 def _oracle(c, fast=True):
     n = c.group_order
-    pk = LK.preprocessed(c)
+    pk = XO.preprocessed(c)
     A, B, C = c.wires_values()
     setup = F.Setup(TAU, n)
-    proof = LK.prove(setup, pk, A, B, C, c.public_values(), fast=fast)
+    proof = XO.prove(setup, pk, A, B, C, c.public_values(), fast=fast)
     return pk, setup, proof
 
 
@@ -76,20 +77,6 @@ def _oracle_vk(c, pk, setup):
     custom = [(e, _commit_col(setup, col)) for e, col in c.custom]
     lookup = tuple(_commit_col(setup, col) for col in [pk.qk] + pk.table)
     return vk, custom, lookup
-
-
-@pytest.fixture
-def host_lincomb(monkeypatch):
-    """the verifier's G1 combinations by the oracle's double-and-add (this suite has no GPU)"""
-    import plonkathon_b200 as pb
-    from plonkathon_b200 import verifier
-
-    def lincomb(pairs, ctx=None):
-        live = [((int(p[0]), int(p[1])), int(k) % R) for p, k in pairs if p is not None]
-        res = O.ec_lincomb_naive(live)
-        return None if res is None else (pb.FQ(res[0]), pb.FQ(res[1]))
-    monkeypatch.setattr(verifier, "ec_lincomb", lincomb)
-    return pb
 
 
 def _host_vk(pb, c, vk, custom, lookup):
@@ -113,26 +100,27 @@ def test_oracle_lookup_proof_verifies(log_n, table, custom, host_lincomb):
     pk, setup, proof = _oracle(c, fast=log_n > 4)  # 2^4: the pure-Python transforms
     vk, cpts, lpts = _oracle_vk(c, pk, setup)
     public = c.public_values()
-    assert LK.verify_proof_trapdoor(n, vk, cpts, lpts, proof, public, TAU)
+    assert XO.verify_proof_trapdoor(n, dict(vk, custom=cpts, lookup=lpts), proof, public, TAU)
     key = _host_vk(pb, c, vk, cpts, lpts)
-    pf = pb.LookupProof.from_bytes(LK.proof_bytes(proof))
+    pf = pb.LookupProof.from_bytes(XO.proof_bytes(proof))
     assert key.verify_proof(n, pf, public) and key.verify_proof_unoptimized(n, pf, public)
     if log_n == 4:
         # rejected: tampered evaluations, a wrong public input, a key whose table differs in one entry, a plain proof
         for f in ("f_eval", "h2_eval", "z2_shifted_eval"):
             bad = dict(proof, **{f: (proof[f] + 1) % R})
-            assert not LK.verify_proof_trapdoor(n, vk, cpts, lpts, bad, public, TAU), f
-            bpf = pb.LookupProof.from_bytes(LK.proof_bytes(bad))
+            assert not XO.verify_proof_trapdoor(n, dict(vk, custom=cpts, lookup=lpts), bad, public, TAU), f
+            bpf = pb.LookupProof.from_bytes(XO.proof_bytes(bad))
             assert not key.verify_proof(n, bpf, public) and not key.verify_proof_unoptimized(n, bpf, public), f
         wrong_pub = [public[0] + 1] + public[1:]
-        assert not LK.verify_proof_trapdoor(n, vk, cpts, lpts, proof, wrong_pub, TAU)
+        assert not XO.verify_proof_trapdoor(n, dict(vk, custom=cpts, lookup=lpts), proof, wrong_pub, TAU)
         assert not key.verify_proof(n, pf, wrong_pub) and not key.verify_proof_unoptimized(n, pf, wrong_pub)
         t1 = list(pk.table[0])
         t1[1] = (t1[1] + 1) % R
         bad_t1 = _commit_col(setup, t1)
         other = dataclasses.replace(key, lookup=(key.lookup[0], (pb.FQ(bad_t1[0]), pb.FQ(bad_t1[1])), *key.lookup[2:]))
         assert not other.verify_proof(n, pf, public) and not other.verify_proof_unoptimized(n, pf, public)
-        assert not LK.verify_proof_trapdoor(n, vk, cpts, (lpts[0], bad_t1) + lpts[2:], proof, public, TAU)
+        assert not XO.verify_proof_trapdoor(n, dict(vk, custom=cpts, lookup=(lpts[0], bad_t1) + lpts[2:]), proof, public,
+                                            TAU)
 
 
 def test_plain_proof_against_lookup_key_and_reverse(host_lincomb):
@@ -143,7 +131,7 @@ def test_plain_proof_against_lookup_key_and_reverse(host_lincomb):
     vk, cpts, lpts = _oracle_vk(c, pk, setup)
     key = _host_vk(pb, c, vk, cpts, lpts)
     plain_key = dataclasses.replace(key, lookup=())
-    lpf = pb.LookupProof.from_bytes(LK.proof_bytes(proof))
+    lpf = pb.LookupProof.from_bytes(XO.proof_bytes(proof))
     ppf = lpf.plain  # the plain part of a lookup proof: a 768-byte proof of the wrong kind
     public = c.public_values()
     assert not key.verify_proof(n, ppf, public) and not key.verify_proof_unoptimized(n, ppf, public)
@@ -152,19 +140,19 @@ def test_plain_proof_against_lookup_key_and_reverse(host_lincomb):
 
 def test_oracle_row_outside_the_table_raises():
     c = _circuit(5, 2, dup_table(), (), 5)
-    pk = LK.preprocessed(c)
+    pk = XO.preprocessed(c)
     A, B, C = c.wires_values()
     row = next(i for i in range(c.group_order) if c.lookup[0][i])
     C[row] = (C[row] + 1) % R
     with pytest.raises(AssertionError, match="lookup row %d is not in the table" % row):
-        LK.prove(F.Setup(TAU, c.group_order), pk, A, B, C, c.public_values(), fast=True)
+        XO.prove(F.Setup(TAU, c.group_order), pk, A, B, C, c.public_values(), fast=True)
 
 
 def test_oracle_grand_product_closes():
     c = _circuit(5, 2, range_table(32), (), 6)
-    pk = LK.preprocessed(c)
+    pk = XO.preprocessed(c)
     A, B, C = c.wires_values()
-    prover = LK.LookupProver(F.Setup(TAU, c.group_order), pk)
+    prover = XO.Prover(F.Setup(TAU, c.group_order), pk)
     with F.c_kernels():
         prover.prove(A, B, C, c.public_values())
     # Z2 starts at 1 and its last step returns to 1 (Z2_n = Z2_0)
@@ -202,11 +190,11 @@ def test_lookup_proof_bytes_round_trip():
     import plonkathon_b200 as pb
     c = _circuit(4, 2, dup_table(), (), 7)
     _, _, proof = _oracle(c, fast=False)
-    raw = LK.proof_bytes(proof)
+    raw = XO.proof_bytes(proof)
     assert len(raw) == 1216
     pf = pb.LookupProof.from_bytes(raw)
     assert pf.to_bytes() == raw
-    assert list(pf.flatten()) == list(O.PROOF_FIELDS) + list(LK.LOOKUP_FIELDS)
+    assert list(pf.flatten()) == list(XO.proof_fields(("lookup",)))
     for word, bound in ((24, pb.FIELD_MODULUS), (33, R)):  # f_1.x and t_eval
         bad = raw[:32 * word] + bound.to_bytes(32, "big") + raw[32 * word + 32:]
         with pytest.raises(ValueError, match="non-canonical"):
@@ -260,7 +248,7 @@ def test_gpu_lookup_proof_equals_oracle(log_n, n_public, table, custom):
     _, _, _, raw = _gpu_proof(pb, c)
     _, _, proof = _oracle(c)
     assert len(raw) == 1216
-    assert raw == LK.proof_bytes(proof)
+    assert raw == XO.proof_bytes(proof)
 
 
 @pytest.mark.gpu
@@ -272,7 +260,7 @@ def test_gpu_skewed_lookup_equals_oracle():
     c = dataclasses.replace(c, lookup=(c.lookup[0], table))
     _, _, _, raw = _gpu_proof(pb, c)
     _, _, proof = _oracle(c)
-    assert raw == LK.proof_bytes(proof)
+    assert raw == XO.proof_bytes(proof)
 
 
 @pytest.mark.gpu

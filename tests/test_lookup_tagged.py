@@ -1,9 +1,9 @@
 """Lookups over several tables, told apart by a table tag (plonkathon_b200/lookup.py, ``lookups=``).
 
-CPU: the oracle (tests/tagged_lookup_oracle.py, Q_T and t4 over tests/lookup_oracle.py) proves circuits with two and
+CPU: the oracle (tests/extended_oracle.py, with Q_T and t4) proves circuits with two and
 three tables that its trapdoor verifier and both host verifier routines accept; they reject a tampered evaluation, a
 key whose [Q_T] or [t4] carries another assignment of table ids and a key without the two tag commitments.  One table
-through ``lookups=`` gives the bytes of the untagged oracle (tests/lookup_oracle.py) with ``lookup=``.  A row tagged XOR whose (a, b, c) is an AND row is refused, while the same witness against the
+through ``lookups=`` gives the bytes of the untagged proof with ``lookup=``.  A row tagged XOR whose (a, b, c) is an AND row is refused, while the same witness against the
 merged untagged table proves and verifies: the tag is what makes several tables sound.  Malformed arguments are
 refused.  GPU: the prover's 1216 bytes equal the oracle's, both golden lookup proofs are reproduced, a 2^20 three-table
 circuit verifies, and the refusals of ``pb200_prover_set_lookup_tagged`` hold."""
@@ -18,10 +18,10 @@ import pytest
 from oracle import fast as F
 from oracle import plonk_oracle as O
 from plonkathon_b200 import synthetic as syn
-from tests import lookup_oracle as LK
-from tests import tagged_lookup_oracle as TL
+from tests import extended_oracle as XO
 from tests.golden_io import GOLDEN
-from tests.test_lookup import _commit_col, _host_vk, host_lincomb  # noqa: F401  (host_lincomb: a fixture)
+from tests.oracle_keys import host_lincomb  # noqa: F401  (a fixture)
+from tests.test_lookup import _commit_col, _host_vk
 
 R = O.R_MOD
 TAU = 0x1234567890ABCDEF1234567890ABCDEF1234567890ABCDEF
@@ -65,10 +65,10 @@ def _circuit(log_n, n_public, tabs, custom, seed):
 
 
 def _oracle(c, fast=True):
-    pk = TL.preprocessed(c)
+    pk = XO.preprocessed(c)
     A, B, C = c.wires_values()
     setup = F.Setup(TAU, c.group_order)
-    return pk, setup, TL.prove(setup, pk, A, B, C, c.public_values(), fast=fast)
+    return pk, setup, XO.prove(setup, pk, A, B, C, c.public_values(), fast=fast)
 
 
 def _oracle_vk(c, pk, setup):
@@ -98,26 +98,26 @@ def test_oracle_tagged_proof_verifies(log_n, count, custom, host_lincomb):
     assert any(pk.qtag) and any(pk.t4)
     vk, cpts, lpts = _oracle_vk(c, pk, setup)
     public = c.public_values()
-    assert TL.verify_proof_trapdoor(n, vk, cpts, lpts, proof, public, TAU)
+    assert XO.verify_proof_trapdoor(n, dict(vk, custom=cpts, lookup=lpts), proof, public, TAU)
     key = _host_vk(pb, c, vk, cpts, lpts)
     assert len(key.lookup) == 6
-    pf = pb.LookupProof.from_bytes(LK.proof_bytes(proof))
+    pf = pb.LookupProof.from_bytes(XO.proof_bytes(proof))
     assert key.verify_proof(n, pf, public) and key.verify_proof_unoptimized(n, pf, public)
     if log_n != 4:
         return
     # rejected: a tampered f_eval, [Q_T] or [t4] of another assignment of ids, a key without the tag commitments
     bad = dict(proof, f_eval=(proof["f_eval"] + 1) % R)
-    assert not TL.verify_proof_trapdoor(n, vk, cpts, lpts, bad, public, TAU)
-    bpf = pb.LookupProof.from_bytes(LK.proof_bytes(bad))
+    assert not XO.verify_proof_trapdoor(n, dict(vk, custom=cpts, lookup=lpts), bad, public, TAU)
+    bpf = pb.LookupProof.from_bytes(XO.proof_bytes(bad))
     assert not key.verify_proof(n, bpf, public) and not key.verify_proof_unoptimized(n, bpf, public)
     fq = lambda p: None if p is None else (pb.FQ(p[0]), pb.FQ(p[1]))  # noqa: E731
     qt2, t42 = (_commit_col(setup, col) for col in _relabelled(pk, count))
     for k, pt in ((4, qt2), (5, t42)):
         wrong = lpts[:k] + (pt,) + lpts[k + 1:]
-        assert not TL.verify_proof_trapdoor(n, vk, cpts, wrong, proof, public, TAU), k
+        assert not XO.verify_proof_trapdoor(n, dict(vk, custom=cpts, lookup=wrong), proof, public, TAU), k
         other = dataclasses.replace(key, lookup=tuple(fq(p) for p in wrong))
         assert not other.verify_proof(n, pf, public) and not other.verify_proof_unoptimized(n, pf, public), k
-    assert not TL.verify_proof_trapdoor(n, vk, cpts, lpts[:4], proof, public, TAU)
+    assert not XO.verify_proof_trapdoor(n, dict(vk, custom=cpts, lookup=lpts[:4]), proof, public, TAU)
     untagged = dataclasses.replace(key, lookup=key.lookup[:4])
     assert not untagged.verify_proof(n, pf, public) and not untagged.verify_proof_unoptimized(n, pf, public)
 
@@ -130,11 +130,11 @@ def test_one_table_through_lookups_is_the_untagged_proof(log_n):
     b = syn.build_circuit(log_n, seed=31, n_public=2, lookups=[table])
     assert a.values == b.values and b.lookups == (a.lookup,)
     assert all(np.array_equal(getattr(a, w), getattr(b, w)) for w in ("wire_L", "wire_R", "wire_O"))
-    pk_b = TL.preprocessed(b)
+    pk_b = XO.preprocessed(b)
     assert pk_b.qtag == [0] * n and pk_b.t4 == [0] * n
-    pa = LK.prove(F.Setup(TAU, n), LK.preprocessed(a), *a.wires_values(), a.public_values(), fast=log_n > 4)
+    pa = XO.prove(F.Setup(TAU, n), XO.preprocessed(a), *a.wires_values(), a.public_values(), fast=log_n > 4)
     _, _, pb_ = _oracle(b, fast=log_n > 4)
-    assert LK.proof_bytes(pa) == LK.proof_bytes(pb_)  # the untagged oracle's proof
+    assert XO.proof_bytes(pa) == XO.proof_bytes(pb_)  # the untagged oracle's proof
 
 
 def _swap_row_to(c, row, abc):
@@ -164,9 +164,9 @@ def test_tag_keeps_an_xor_row_out_of_the_and_table(host_lincomb):
     vk, cpts, lpts = _oracle_vk(merged, pk, setup)
     lpts = lpts[:4]
     public = merged.public_values()
-    assert TL.verify_proof_trapdoor(n, vk, cpts, lpts, proof, public, TAU)
+    assert XO.verify_proof_trapdoor(n, dict(vk, custom=cpts, lookup=lpts), proof, public, TAU)
     key = _host_vk(pb, merged, vk, cpts, lpts)
-    pf = pb.LookupProof.from_bytes(LK.proof_bytes(proof))
+    pf = pb.LookupProof.from_bytes(XO.proof_bytes(proof))
     assert key.verify_proof(n, pf, public) and key.verify_proof_unoptimized(n, pf, public)
 
 
@@ -242,7 +242,7 @@ def test_gpu_tagged_lookup_proof_equals_oracle(log_n, n_public, count, custom):
     _, _, _, raw = _gpu_proof(pb, c)
     _, _, proof = _oracle(c)
     assert len(raw) == 1216
-    assert raw == LK.proof_bytes(proof)
+    assert raw == XO.proof_bytes(proof)
 
 
 @pytest.mark.gpu

@@ -1,7 +1,7 @@
 """Custom gates over the next row: terms Q_k a^i b^j c^l a(wX)^i' b(wX)^j' c(wX)^l' (plonkathon_b200/custom_gates.py).
 
 CPU: exponent validation; the refusals of next-row terms with lookups and on the sharded prover; the oracle with
-next-row terms (tests/next_row_oracle.py) proves circuits at n = 16, 64 and 256 that its trapdoor verifier and both host
+next-row terms (tests/extended_oracle.py) proves circuits at n = 16, 64 and 256 that its trapdoor verifier and both host
 verifier routines accept, and both routines reject what they must; the gate check reads row 0 from row n - 1; the
 zero-knowledge oracle with random blinders verifies.  GPU: the prover's 864 bytes equal the oracle's for each kind of
 term and all four together, plain and in zero-knowledge mode, at several sizes and on both public-input paths; the
@@ -18,8 +18,8 @@ import pytest
 from oracle import fast as F
 from oracle import plonk_oracle as O
 from plonkathon_b200 import synthetic as syn
-from tests import custom_gate_oracle as CG
-from tests import next_row_oracle as NR
+from tests import extended_oracle as XO
+from tests.oracle_keys import host_lincomb  # noqa: F401  (a fixture)
 from tests.golden_io import GOLDEN, pt
 
 R = O.R_MOD
@@ -43,17 +43,17 @@ def _circuit(log_n, n_public, terms, seed):
 
 def _blinders(seed):
     rng = random.Random(seed)
-    return [rng.randrange(R) for _ in range(NR.N_BLINDERS)]
+    return [rng.randrange(R) for _ in range(14)]
 
 
 def _oracle_proof(c, blinders=None, fast=True):
     n = c.group_order
-    pk = NR.preprocessed(c)
+    pk = XO.preprocessed(c)
     A, B, C = c.wires_values()
     setup = F.Setup(TAU, n + 9)
     if not fast:
         setup = O.Setup([setup.point(i) for i in range(n + 9)], None)
-    return pk, setup, NR.prove(setup, pk, A, B, C, c.public_values(), blinders=blinders, fast=fast)
+    return pk, setup, XO.prove(setup, pk, A, B, C, c.public_values(), blinders=blinders, fast=fast)
 
 
 def _oracle_vk(c, pk):
@@ -63,19 +63,6 @@ def _oracle_vk(c, pk):
                                                   ("S1", pk.S1), ("S2", pk.S2), ("S3", pk.S3))}
         custom = [(e, setup.commit(col)) for e, col in c.custom]
     return vk, custom
-
-
-@pytest.fixture
-def host_lincomb(monkeypatch):
-    """the verifier's G1 combinations by the oracle's double-and-add (this suite has no GPU)"""
-    import plonkathon_b200 as pb
-    from plonkathon_b200 import verifier
-
-    def lincomb(pairs, ctx=None):
-        res = O.ec_lincomb_naive([(None if p is None else (int(p[0]), int(p[1])), int(k) % R) for p, k in pairs])
-        return None if res is None else (pb.FQ(res[0]), pb.FQ(res[1]))
-    monkeypatch.setattr(verifier, "ec_lincomb", lincomb)
-    return pb
 
 
 def _host_vk(pb, n, vk, custom):
@@ -97,9 +84,9 @@ def test_three_exponent_terms_equal_their_padded_form(host_lincomb):
     # a plain custom-gate proof verifies under a key whose terms are written with six exponents
     c = syn.build_circuit(4, seed=21, n_public=2, custom=[(2, 0, 0), (1, 1, 1)])
     n = c.group_order
-    pk = CG.preprocessed(c)
+    pk = XO.preprocessed(c)
     A, B, C = c.wires_values()
-    proof = CG.prove(F.Setup(TAU, n), pk, A, B, C, c.public_values(), fast=True)
+    proof = XO.prove(F.Setup(TAU, n), pk, A, B, C, c.public_values(), fast=True)
     vk, custom = _oracle_vk(c, pk)
     base, x2, w, terms = _host_vk(pb, n, vk, custom)
     key = pb.VerificationKey(n, *base, x2, w, tuple((e + (0, 0, 0), p) for e, p in terms))
@@ -174,11 +161,11 @@ def test_oracle_next_row_proof_verifies(terms, log_n, host_lincomb):
     pk, _, proof = _oracle_proof(c, fast=log_n > 4)  # 2^4: the pure-Python transforms
     vk, custom = _oracle_vk(c, pk)
     public = c.public_values()
-    assert NR.verify_proof_trapdoor(n, vk, custom, proof, public, TAU)
-    assert not NR.verify_proof_trapdoor(n, vk, custom, proof, [public[0] + 1] + public[1:], TAU)
+    assert XO.verify_proof_trapdoor(n, dict(vk, custom=custom), proof, public, TAU)
+    assert not XO.verify_proof_trapdoor(n, dict(vk, custom=custom), proof, [public[0] + 1] + public[1:], TAU)
     base, x2, w, terms_pt = _host_vk(pb, n, vk, custom)
     key = pb.VerificationKey(n, *base, x2, w, terms_pt)
-    raw = NR.proof_bytes(proof)
+    raw = XO.proof_bytes(proof)
     pf = pb.NextRowProof.from_bytes(raw)
     assert pf.to_bytes() == raw and key.next_row
     assert key.verify_proof(n, pf, public) and key.verify_proof_unoptimized(n, pf, public)
@@ -190,16 +177,16 @@ def test_oracle_running_sum_range_check_verifies(host_lincomb):
     n = c.group_order
     pk, _, proof = _oracle_proof(c)
     vk, custom = _oracle_vk(c, pk)
-    assert NR.verify_proof_trapdoor(n, vk, custom, proof, [], TAU)
+    assert XO.verify_proof_trapdoor(n, dict(vk, custom=custom), proof, [], TAU)
     base, x2, w, terms = _host_vk(pb, n, vk, custom)
     key = pb.VerificationKey(n, *base, x2, w, terms)
-    pf = pb.NextRowProof.from_bytes(NR.proof_bytes(proof))
+    pf = pb.NextRowProof.from_bytes(XO.proof_bytes(proof))
     assert key.verify_proof(n, pf, []) and key.verify_proof_unoptimized(n, pf, [])
     # a value that is not a running sum of bits: acc_1 = 2 breaks the first row of the first value
     A, B, C = c.wires_values()
     A[3] = 2
     with pytest.raises(AssertionError, match="gate 2 unsatisfied"):
-        NR.prove(F.Setup(TAU, n), pk, A, B, C, [], fast=True)
+        XO.prove(F.Setup(TAU, n), pk, A, B, C, [], fast=True)
 
 
 def test_both_routines_reject_tampered_proofs_and_wrong_keys(host_lincomb):
@@ -211,14 +198,14 @@ def test_both_routines_reject_tampered_proofs_and_wrong_keys(host_lincomb):
     base, x2, w, terms = _host_vk(pb, n, vk, custom)
     good = pb.VerificationKey(n, *base, x2, w, terms)
     public = c.public_values()
-    raw = NR.proof_bytes(proof)
+    raw = XO.proof_bytes(proof)
     pf = pb.NextRowProof.from_bytes(raw)
     assert good.verify_proof(n, pf, public) and good.verify_proof_unoptimized(n, pf, public)
     bad = {}
-    for k in NR.NEXT_ROW_FIELDS:
-        bad["tampered " + k] = pb.NextRowProof.from_bytes(NR.proof_bytes(dict(proof, **{k: (proof[k] + 1) % R})))
+    for k in XO.FIELDS["next_row"]["4"]:
+        bad["tampered " + k] = pb.NextRowProof.from_bytes(XO.proof_bytes(dict(proof, **{k: (proof[k] + 1) % R})))
     bad["swapped openings"] = pb.NextRowProof.from_bytes(
-        NR.proof_bytes(dict(proof, W_z_1=proof["W_zw_1"], W_zw_1=proof["W_z_1"])))
+        XO.proof_bytes(dict(proof, W_z_1=proof["W_zw_1"], W_zw_1=proof["W_z_1"])))
     bad["a plain proof"] = pb.Proof.from_bytes(raw[:768])
     for why, p in bad.items():
         assert not good.verify_proof(n, p, public), why
@@ -240,7 +227,7 @@ def test_non_canonical_next_row_encoding_is_rejected():
     import plonkathon_b200 as pb
     c = _circuit(4, 2, ALL_TERMS, 21)
     _, _, proof = _oracle_proof(c)
-    raw = NR.proof_bytes(proof)
+    raw = XO.proof_bytes(proof)
     for word in (24, 25, 26):
         x = int.from_bytes(raw[32 * word:32 * word + 32], "big") + R
         with pytest.raises(ValueError, match="word %d" % word):
@@ -262,43 +249,43 @@ def _wrapping_circuit(log_n, seed):
 def test_oracle_rejects_a_broken_wrap_around_row():
     c = _wrapping_circuit(5, 1)
     n = c.group_order
-    pk = NR.preprocessed(c)
+    pk = XO.preprocessed(c)
     A, B, C = c.wires_values()
     public = c.public_values()
-    NR.prove(F.Setup(TAU, n), pk, A, B, C, public, fast=True)  # the witness as built proves
+    XO.prove(F.Setup(TAU, n), pk, A, B, C, public, fast=True)  # the witness as built proves
     # row 0 is a public row: moving its value and the public input together keeps row 0 and breaks row n - 1
     A[0], public = (A[0] + 1) % R, [(public[0] + 1) % R] + public[1:]
     with pytest.raises(AssertionError, match="gate %d unsatisfied" % (n - 1)):
-        NR.prove(F.Setup(TAU, n), pk, A, B, C, public, fast=True)
+        XO.prove(F.Setup(TAU, n), pk, A, B, C, public, fast=True)
 
 
-def test_zk_oracle_verifies_and_blinded_wires_agree_on_h(host_lincomb):
+def test_oracle_zk_proof_verifies_and_blinded_wires_agree_on_h(host_lincomb):
     pb = host_lincomb
     c = _circuit(5, 2, ALL_TERMS, 40)
     n = c.group_order
-    pk = NR.preprocessed(c)
+    pk = XO.preprocessed(c)
     A, B, C = c.wires_values()
     setup = F.Setup(TAU, n + 9)
     with F.c_kernels():
-        prover = NR.ZkNextRowProver(setup, pk, _blinders(5))
+        prover = XO.Prover(setup, pk, _blinders(5))
         proof = prover.prove(A, B, C, c.public_values())
-        plain = NR.prove(setup, pk, A, B, C, c.public_values())
+        plain = XO.prove(setup, pk, A, B, C, c.public_values())
     roots = O.roots_of_unity(n)
     for blinded, vals in ((prover.Ab, A), (prover.Bb, B), (prover.Cb, C)):
         assert len(blinded) == n + 3 and any(blinded[n:])
-        assert [NR.ZO.poly_eval(blinded, x) for x in roots] == [v % R for v in vals]
+        assert [XO.poly_eval(blinded, x) for x in roots] == [v % R for v in vals]
     vk, custom = _oracle_vk(c, pk)
     public = c.public_values()
-    assert NR.verify_proof_trapdoor(n, vk, custom, proof, public, TAU)
+    assert XO.verify_proof_trapdoor(n, dict(vk, custom=custom), proof, public, TAU)
     base, x2, w, terms = _host_vk(pb, n, vk, custom)
     key = pb.VerificationKey(n, *base, x2, w, terms)
-    pf = pb.NextRowProof.from_bytes(NR.proof_bytes(proof))
+    pf = pb.NextRowProof.from_bytes(XO.proof_bytes(proof))
     assert key.verify_proof(n, pf, public) and key.verify_proof_unoptimized(n, pf, public)
     assert proof["a_1"] != plain["a_1"] and proof["a_shifted_eval"] != plain["a_shifted_eval"]
     # zero blinders give the plain next-row proof
     with F.c_kernels():
-        zero = NR.ZkNextRowProver(setup, pk, [0] * NR.N_BLINDERS).prove(A, B, C, public)
-    assert NR.proof_bytes(zero) == NR.proof_bytes(plain)
+        zero = XO.Prover(setup, pk, [0] * 14).prove(A, B, C, public)
+    assert XO.proof_bytes(zero) == XO.proof_bytes(plain)
 
 
 # ---- GPU -----------------------------------------------------------------------------------------------------------
@@ -324,7 +311,7 @@ def test_gpu_next_row_proof_equals_oracle(terms, log_n, n_public):
     raw = prover.prove_arrays(*wires)
     assert len(raw) == 864 and prover.next_row
     _, _, proof = _oracle_proof(c)
-    assert raw == NR.proof_bytes(proof)
+    assert raw == XO.proof_bytes(proof)
 
 
 @pytest.mark.gpu
@@ -338,7 +325,7 @@ def test_gpu_zk_next_row_proof_equals_oracle(terms, log_n, n_public):
     prover.set_zk(True, blinders)
     raw = prover.prove_arrays(*wires)
     _, _, proof = _oracle_proof(c, blinders=blinders)
-    assert raw == NR.proof_bytes(proof)
+    assert raw == XO.proof_bytes(proof)
 
 
 @pytest.mark.gpu
@@ -501,5 +488,5 @@ def test_gpu_same_row_six_exponent_terms_take_the_plain_path():
     assert not six.next_row
     raw = six.prove_arrays(A, B, C, public)
     assert len(raw) == 768 and raw == three.prove_arrays(A, B, C, public)
-    proof = CG.prove(F.Setup(TAU, n), CG.preprocessed(c), *c.wires_values(), public, fast=True)
+    proof = XO.prove(F.Setup(TAU, n), XO.preprocessed(c), *c.wires_values(), public, fast=True)
     assert raw == O.proof_bytes(proof)

@@ -1,6 +1,6 @@
 """CPU: the proof layout is one table in C++ (csrc/proof_layout.cuh, exported by csrc/host_selftest.cpp) and one in
 Python (plonkathon_b200/transcript.py).  The two must agree field by field, and each proof kind's filtered table must
-give the field order and byte count the oracles state independently."""
+give the field order and byte count stated here and by the oracle (tests/extended_oracle.py) independently."""
 import ctypes
 import os
 import subprocess
@@ -9,9 +9,7 @@ import pytest
 
 from oracle import plonk_oracle as O
 from plonkathon_b200 import transcript as T
-from tests import lookup_oracle as LK
-from tests import next_row_oracle as NR
-from tests import shuffle_oracle as SO
+from tests import extended_oracle as XO
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "plonkathon_b200", "csrc")
@@ -47,13 +45,20 @@ def test_cpp_table_is_python_table(lib):
     assert tuple(challenges) == T.CHALLENGES
 
 
+NEXT_ROW = ("a_shifted_eval", "b_shifted_eval", "c_shifted_eval")
+SHUFFLE = ("z3_1", "qin_eval", "z3_shifted_eval")
+LOOKUP = ("f_1", "h1_1", "h2_1", "z2_1", "f_eval", "t_eval", "t_shifted_eval", "h2_eval", "h1_shifted_eval",
+          "z2_shifted_eval")
+
+
 @pytest.mark.parametrize("kind, extension, size", [
     ({}, (), 768),
-    ({"next_row": True}, NR.NEXT_ROW_FIELDS, 864),
-    ({"shuffle": True}, SO.SHUFFLE_FIELDS, 896),
-    ({"next_row": True, "shuffle": True}, NR.NEXT_ROW_FIELDS + SO.SHUFFLE_FIELDS, 992),
-    ({"lookup": True}, LK.LOOKUP_FIELDS, 1216),
+    ({"next_row": True}, NEXT_ROW, 864),
+    ({"shuffle": True}, SHUFFLE, 896),
+    ({"next_row": True, "shuffle": True}, NEXT_ROW + SHUFFLE, 992),
+    ({"lookup": True}, LOOKUP, 1216),
 ])
 def test_kinds_match_the_oracles(kind, extension, size):
     assert T.proof_fields(**kind) == tuple(O.PROOF_FIELDS) + tuple(extension)
     assert T.proof_bytes(**kind) == size
+    assert XO.proof_fields(tuple(kind)) == T.proof_fields(**kind)

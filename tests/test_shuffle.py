@@ -1,9 +1,9 @@
 """Shuffles: the rows with q_in = 1 hold the same multiset of (a, b, c) as the rows with q_out = 1
 (plonkathon_b200/shuffle.py).
 
-CPU: the oracle with a shuffle (tests/shuffle_oracle.py) proves circuits at n = 16, 64 and 256, plain and with same-row
+CPU: the oracle with a shuffle (tests/extended_oracle.py) proves circuits at n = 16, 64 and 256, plain and with same-row
 or next-row terms, that its trapdoor verifier and both host verifier routines accept; both routines reject tampered
-proofs, swapped openings, wrong keys and proofs of the wrong kind; a_1 b_1 c_1 z_1 equal the custom-gate oracle's and
+proofs, swapped openings, wrong keys and proofs of the wrong kind; a_1 b_1 c_1 z_1 equal the pinned plain oracle's and
 with no shuffled rows z3_1 is the generator; out-rows that are not a permutation raise; the selector checks and the
 canonical decoding.  GPU: the prover's 896 and 992 bytes equal the oracle's at several sizes, on both public-input paths
 and for a skewed shuffle; the round-by-round ABI gives the same bytes; the 2^16 golden proof is reproduced; a 2^20 proof
@@ -18,8 +18,8 @@ import pytest
 from oracle import fast as F
 from oracle import plonk_oracle as O
 from plonkathon_b200 import synthetic as syn
-from tests import custom_gate_oracle as CG
-from tests import shuffle_oracle as SO
+from tests import extended_oracle as XO
+from tests.oracle_keys import host_lincomb  # noqa: F401  (a fixture)
 from tests.golden_io import GOLDEN
 
 R = O.R_MOD
@@ -41,12 +41,12 @@ def _circuit(log_n, n_public, terms, seed):
 
 def _oracle_proof(c, fast=True):
     n = c.group_order
-    pk = SO.preprocessed(c)
+    pk = XO.preprocessed(c)
     A, B, C = c.wires_values()
     setup = F.Setup(TAU, n)
     if not fast:
         setup = O.Setup([setup.point(i) for i in range(n)], None)
-    return pk, SO.prove(setup, pk, A, B, C, c.public_values(), fast=fast)
+    return pk, XO.prove(setup, pk, A, B, C, c.public_values(), fast=fast)
 
 
 def _oracle_vk(c, pk):
@@ -57,19 +57,6 @@ def _oracle_vk(c, pk):
         custom = [(e, setup.commit(col)) for e, col in c.custom]
         shuffle = tuple(setup.commit(q) if any(q) else None for q in c.shuffle)
     return vk, custom, shuffle
-
-
-@pytest.fixture
-def host_lincomb(monkeypatch):
-    """the verifier's G1 combinations by the oracle's double-and-add (this suite has no GPU)"""
-    import plonkathon_b200 as pb
-    from plonkathon_b200 import verifier
-
-    def lincomb(pairs, ctx=None):
-        res = O.ec_lincomb_naive([(None if p is None else (int(p[0]), int(p[1])), int(k) % R) for p, k in pairs])
-        return None if res is None else (pb.FQ(res[0]), pb.FQ(res[1]))
-    monkeypatch.setattr(verifier, "ec_lincomb", lincomb)
-    return pb
 
 
 def _host_key(pb, n, vk, custom, shuffle):
@@ -146,10 +133,10 @@ def test_oracle_shuffle_proof_verifies(terms, log_n, host_lincomb):
     pk, proof = _oracle_proof(c, fast=log_n > 4)  # 2^4: the pure-Python transforms
     vk, custom, shuffle = _oracle_vk(c, pk)
     public = c.public_values()
-    assert SO.verify_proof_trapdoor(n, vk, custom, shuffle, proof, public, TAU)
-    assert not SO.verify_proof_trapdoor(n, vk, custom, shuffle, proof, [public[0] + 1] + public[1:], TAU)
+    assert XO.verify_proof_trapdoor(n, dict(vk, custom=custom, shuffle=shuffle), proof, public, TAU)
+    assert not XO.verify_proof_trapdoor(n, dict(vk, custom=custom, shuffle=shuffle), proof, [public[0] + 1] + public[1:], TAU)
     key = _host_key(pb, n, vk, custom, shuffle)
-    raw = SO.proof_bytes(proof)
+    raw = XO.proof_bytes(proof)
     assert len(raw) == (992 if terms == NEXT_TERMS else 896)
     pf = _host_proof(pb, raw)
     assert pf.to_bytes() == raw
@@ -165,14 +152,14 @@ def test_both_routines_reject_tampered_proofs_and_wrong_keys(terms, host_lincomb
     vk, custom, shuffle = _oracle_vk(c, pk)
     good = _host_key(pb, n, vk, custom, shuffle)
     public = c.public_values()
-    raw = SO.proof_bytes(proof)
+    raw = XO.proof_bytes(proof)
     pf = _host_proof(pb, raw)
     assert good.verify_proof(n, pf, public) and good.verify_proof_unoptimized(n, pf, public)
     bad = {}
     for k in ("qin_eval", "z3_shifted_eval"):
-        bad["tampered " + k] = _host_proof(pb, SO.proof_bytes(dict(proof, **{k: (proof[k] + 1) % R})))
-    bad["swapped openings"] = _host_proof(pb, SO.proof_bytes(dict(proof, W_z_1=proof["W_zw_1"], W_zw_1=proof["W_z_1"])))
-    bad["z3_1 replaced by z_1"] = _host_proof(pb, SO.proof_bytes(dict(proof, z3_1=proof["z_1"])))
+        bad["tampered " + k] = _host_proof(pb, XO.proof_bytes(dict(proof, **{k: (proof[k] + 1) % R})))
+    bad["swapped openings"] = _host_proof(pb, XO.proof_bytes(dict(proof, W_z_1=proof["W_zw_1"], W_zw_1=proof["W_z_1"])))
+    bad["z3_1 replaced by z_1"] = _host_proof(pb, XO.proof_bytes(dict(proof, z3_1=proof["z_1"])))
     bad["a plain proof"] = pb.Proof.from_bytes(raw[:768])
     if terms == NEXT_TERMS:
         bad["a next-row proof"] = pb.NextRowProof.from_bytes(raw[:864])
@@ -194,20 +181,26 @@ def test_proof_of_the_other_kind_is_refused(host_lincomb):
     for c in (c_plain, c_next):
         pk, proof = _oracle_proof(c)
         keys.append((_host_key(pb, c.group_order, *_oracle_vk(c, pk)), c.public_values()))
-        proofs.append(_host_proof(pb, SO.proof_bytes(proof)))
+        proofs.append(_host_proof(pb, XO.proof_bytes(proof)))
     for (key, public), pf in ((keys[0], proofs[1]), (keys[1], proofs[0])):
         assert not key.verify_proof(16, pf, public) and not key.verify_proof_unoptimized(16, pf, public)
 
 
-def test_cross_pins_with_the_custom_gate_oracle():
-    """round 1 is the custom-gate oracle's, and beta, gamma are drawn before theta, kappa: a_1 b_1 c_1 z_1 agree.
-    With no shuffled rows Z3 is the constant 1, so z3_1 is the generator."""
+def test_cross_pins_with_the_pinned_oracle():
+    """rounds 1 and 2 are the pinned oracle's (oracle/plonk_oracle.py), and beta, gamma are drawn before theta, kappa:
+    a_1 b_1 c_1 z_1 agree.  With no shuffled rows Z3 is the constant 1, so z3_1 is the generator."""
     c = _circuit(6, 2, [(2, 0, 0), (1, 1, 1)], 7)
     n = c.group_order
     pk, proof = _oracle_proof(c)
-    plain = CG.prove(F.Setup(TAU, n), CG.preprocessed(c), *c.wires_values(), c.public_values(), fast=True)
-    for k in ("a_1", "b_1", "c_1", "z_1"):
-        assert proof[k] == plain[k], k
+    plain = O.Prover(F.Setup(TAU, n), pk, check=False)  # its gate check does not know the custom terms
+    plain.PI = [(-v) % R for v in c.public_values()] + [0] * (n - len(c.public_values()))
+    tr = O.Transcript(b"plonk")
+    with F.c_kernels():
+        a_1, b_1, c_1 = plain.round_1(*c.wires_values())
+        plain.beta, plain.gamma = tr.round_1(a_1, b_1, c_1)
+        z_1 = plain.round_2()
+    for k, x in (("a_1", a_1), ("b_1", b_1), ("c_1", c_1), ("z_1", z_1)):
+        assert proof[k] == x, k
     empty = syn.ArrayCircuit(**{**c.__dict__, "shuffle": ([0] * n, [0] * n)})
     _, proof0 = _oracle_proof(empty)
     assert proof0["z3_1"] == O.G1 and proof0["z3_shifted_eval"] == 1 and proof0["qin_eval"] == 0
@@ -216,12 +209,12 @@ def test_cross_pins_with_the_custom_gate_oracle():
 def test_out_rows_that_are_not_a_permutation_raise():
     c = _circuit(5, 2, [], 9)
     n = c.group_order
-    pk = SO.preprocessed(c)
+    pk = XO.preprocessed(c)
     A, B, C = c.wires_values()
     r = pk.q_out.index(1)
     A[r] = (A[r] + 1) % R  # an out-row whose a is not the a of its in-row (the row's selectors are all zero)
     with pytest.raises(AssertionError, match="not permutations of each other"):
-        SO.prove(F.Setup(TAU, n), pk, A, B, C, c.public_values(), fast=True)
+        XO.prove(F.Setup(TAU, n), pk, A, B, C, c.public_values(), fast=True)
 
 
 def test_non_canonical_encodings_are_rejected():
@@ -229,7 +222,7 @@ def test_non_canonical_encodings_are_rejected():
     for terms, cls, scalars, points in (([], pb.ShuffleProof, (26, 27), (24, 25)),
                                         (NEXT_TERMS, pb.NextRowShuffleProof, (24, 25, 26, 29, 30), (27, 28))):
         _, proof = _oracle_proof(_circuit(4, 2, terms, 21))
-        raw = SO.proof_bytes(proof)
+        raw = XO.proof_bytes(proof)
         assert cls.from_bytes(raw).to_bytes() == raw
         for word in scalars + points:
             x = int.from_bytes(raw[32 * word:32 * word + 32], "big") + (R if word in scalars else O.Q_MOD)
@@ -266,7 +259,7 @@ def test_gpu_shuffle_proof_equals_oracle(terms, log_n, n_public):
     raw = prover.prove_arrays(*wires)
     _, proof = _oracle_proof(c)
     assert len(raw) == (896 if terms in ([], [(2, 0, 0), (1, 1, 1)]) else 992)
-    assert raw == SO.proof_bytes(proof)
+    assert raw == XO.proof_bytes(proof)
 
 
 def _skewed_circuit(log_n):
@@ -297,7 +290,7 @@ def test_gpu_skewed_shuffle_equals_oracle(log_n):
     _, _, prover, wires = _gpu_prover(pb, c)
     raw = prover.prove_arrays(*wires)
     _, proof = _oracle_proof(c)
-    assert len(raw) == 896 and raw == SO.proof_bytes(proof)
+    assert len(raw) == 896 and raw == XO.proof_bytes(proof)
 
 
 @pytest.mark.gpu

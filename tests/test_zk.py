@@ -1,4 +1,4 @@
-"""Zero-knowledge proving: A, B, C, Z and the quotient pieces blinded as in the PLONK paper (tests/zk_oracle.py has the
+"""Zero-knowledge proving: A, B, C, Z and the quotient pieces blinded as in the PLONK paper (tests/extended_oracle.py has the
 construction), with the proof format, the transcript and the verifier unchanged.
 
 CPU: the zero-knowledge oracle's proofs verify (trapdoor check and the product's host verifier) and tampered ones do not;
@@ -16,8 +16,8 @@ import pytest
 from oracle import fast as F
 from oracle import plonk_oracle as O
 from plonkathon_b200 import synthetic as syn
-from tests import custom_gate_oracle as CG
-from tests import zk_oracle as ZK
+from tests import extended_oracle as XO
+from tests.oracle_keys import host_lincomb  # noqa: F401  (a fixture)
 from tests.golden_io import GOLDEN, PTAU_HEAD, ints, load_circuit, pt
 
 R = O.R_MOD
@@ -31,7 +31,7 @@ EVALUATIONS = ("a_eval", "b_eval", "c_eval", "s1_eval", "s2_eval", "z_shifted_ev
 
 def _blinders(seed):
     rng = random.Random(seed)
-    return [rng.randrange(1, R) for _ in range(ZK.N_BLINDERS)]
+    return [rng.randrange(1, R) for _ in range(11)]
 
 
 def _custom_circuit(log_n, n_public, seed):
@@ -46,12 +46,11 @@ def _custom_circuit(log_n, n_public, seed):
 def _oracle(c, blinders, fast=True):
     """(pk, fast setup of n + 6 powers, oracle zero-knowledge proof, prover object) of a synthetic circuit"""
     n = c.group_order
-    pk = CG.preprocessed(c) if c.custom else O.Preprocessed(
-        n, c.QM, c.QL, c.QR, c.QO, c.QC, *syn.permutation_polys(c.wire_L, c.wire_R, c.wire_O, n, c.n_constraints))
+    pk = XO.preprocessed(c)
     A, B, C = c.wires_values()
     fsetup = F.Setup(TAU, n + 6)
     setup = fsetup if fast else O.Setup([fsetup.point(i) for i in range(n + 6)], None)
-    prover = ZK.make_prover(setup, pk, blinders)
+    prover = XO.Prover(setup, pk, blinders)
     if fast:
         with F.c_kernels():
             proof = prover.prove(A, B, C, c.public_values())
@@ -65,19 +64,6 @@ def _oracle_vk(pk, fsetup):
         vk = {k: fsetup.commit(getattr(pk, a)) for k, a in VK_KEYS}
         custom = [(e, fsetup.commit(col)) for e, col in getattr(pk, "custom", ())]
     return vk, custom
-
-
-@pytest.fixture
-def host_lincomb(monkeypatch):
-    """the verifier's G1 combinations by the oracle's double-and-add (this part of the suite has no GPU)"""
-    import plonkathon_b200 as pb
-    from plonkathon_b200 import verifier
-
-    def lincomb(pairs, ctx=None):
-        res = O.ec_lincomb_naive([(None if p is None else (int(p[0]), int(p[1])), int(k) % R) for p, k in pairs])
-        return None if res is None else (pb.FQ(res[0]), pb.FQ(res[1]))
-    monkeypatch.setattr(verifier, "ec_lincomb", lincomb)
-    return pb
 
 
 # ---- CPU ---------------------------------------------------------------------------------------------------------
@@ -107,15 +93,15 @@ def test_oracle_zero_blinders_give_the_plain_proof():
     """the reference's test/proof.pickle circuit on the shipped .ptau, and a synthetic circuit"""
     entry, arr = load_circuit("prover_test")
     osetup = O.Setup.from_file(PTAU_HEAD)
-    opk = O.Preprocessed(entry["n"], *[arr[k] for k in PK_KEYS])
+    opk = XO.Preprocessed(entry["n"], *[arr[k] for k in PK_KEYS])
     public = ints(entry["public"])
-    zk = ZK.prove(osetup, opk, arr["A"], arr["B"], arr["C"], public, [0] * ZK.N_BLINDERS)
+    zk = XO.prove(osetup, opk, arr["A"], arr["B"], arr["C"], public, [0] * 11)
     plain = O.Prover(osetup, opk).prove(arr["A"], arr["B"], arr["C"], public)
     assert O.proof_bytes(zk) == O.proof_bytes(plain)
     assert all(((pt(v) if isinstance(v, list) else int(v)) == zk[k]) for k, v in entry["proof"].items())
     c = syn.build_circuit(6, seed=9, n_public=3)
     n = c.group_order
-    pk, fsetup, zk, _ = _oracle(c, [0] * ZK.N_BLINDERS)
+    pk, fsetup, zk, _ = _oracle(c, [0] * 11)
     A, B, C = c.wires_values()
     assert zk == F.prove(fsetup, pk, A, B, C, c.public_values())
 
@@ -139,8 +125,8 @@ def test_oracle_blinded_pieces_recombine_to_the_quotient():
     assert any(prover.T[3 * n:])  # the blinded quotient reaches past 3n
     x = random.Random(7).randrange(R)
     xn = pow(x, n, R)
-    got = (ZK.poly_eval(prover.T1b, x) + xn * ZK.poly_eval(prover.T2b, x) + xn * xn * ZK.poly_eval(prover.T3b, x)) % R
-    assert got == ZK.poly_eval(prover.T, x)
+    got = (XO.poly_eval(prover.T1b, x) + xn * XO.poly_eval(prover.T2b, x) + xn * xn * XO.poly_eval(prover.T3b, x)) % R
+    assert got == XO.poly_eval(prover.T, x)
 
 
 def test_oracle_custom_gates_with_zero_knowledge():
@@ -149,8 +135,8 @@ def test_oracle_custom_gates_with_zero_knowledge():
     pk, fsetup, proof, _ = _oracle(c, _blinders(6))
     vk, custom = _oracle_vk(pk, fsetup)
     public = c.public_values()
-    assert CG.verify_proof_trapdoor(n, vk, custom, proof, public, TAU)
-    assert not CG.verify_proof_trapdoor(n, vk, custom, dict(proof, a_eval=(proof["a_eval"] + 1) % R), public, TAU)
+    assert XO.verify_proof_trapdoor(n, dict(vk, custom=custom), proof, public, TAU)
+    assert not XO.verify_proof_trapdoor(n, dict(vk, custom=custom), dict(proof, a_eval=(proof["a_eval"] + 1) % R), public, TAU)
 
 
 def test_set_zk_argument_checks():
@@ -200,7 +186,7 @@ def test_gpu_zero_blinders_reproduce_golden_proofs(name):
     entry, arr = load_circuit(name)
     setup = pb.Setup.from_file(PTAU_HEAD)
     prover = pb.Prover.from_arrays(setup, entry["n"], {k: arr[k] for k in PK_KEYS})
-    prover.set_zk(True, [0] * ZK.N_BLINDERS)
+    prover.set_zk(True, [0] * 11)
     raw = prover.prove_arrays(arr["A"], arr["B"], arr["C"], ints(entry["public"]))
     assert hashlib.sha256(raw).hexdigest() == entry["proof_sha256"]
 
@@ -213,7 +199,7 @@ def test_gpu_zk_2p20_zero_blinders_golden_and_fresh_blinders_verify():
     rec = json.load(open(os.path.join(GOLDEN, "proof_2p20.json")))
     c = syn.build_circuit(20, seed=rec["seed"], n_public=2)
     n = c.group_order
-    setup, pk, prover, (A, B, C, public) = _gpu_prover(pb, c, blinders=[0] * ZK.N_BLINDERS)
+    setup, pk, prover, (A, B, C, public) = _gpu_prover(pb, c, blinders=[0] * 11)
     raw = prover.prove_arrays(A, B, C, public)
     assert raw.hex() == rec["proof_hex"], "zero-blinder proof differs from the golden 2^20 proof"
     prover.set_zk(True)
@@ -323,7 +309,7 @@ def test_gpu_refusals_and_unchanged_round_state():
     setup = pb.Setup.generate(TAU, n + 6)
     raw_checked = pb.Prover.from_arrays(setup, n, pk)
     with pytest.raises(_lib.PlonkB200Error, match="not reduced"):  # the library checks the raw blinders itself
-        _lib.check(_lib.lib().pb200_prover_set_zk(raw_checked._h, 1, b"\xff" * 32 * ZK.N_BLINDERS))
+        _lib.check(_lib.lib().pb200_prover_set_zk(raw_checked._h, 1, b"\xff" * 32 * 11))
     plain = pb.Prover.from_arrays(setup, n, pk)
     plain.prove_arrays(A, B, C, public)
     zk = pb.Prover.from_arrays(setup, n, pk)
@@ -344,7 +330,7 @@ def test_gpu_refusals_and_unchanged_round_state():
     oz.setup = type("NoCommit", (), {"commit": lambda self, v: None})()
     oz.round_2()
     assert [x.n for x in zk.Z.values] == oz.Z
-    zk.set_zk(True, [0] * ZK.N_BLINDERS)
+    zk.set_zk(True, [0] * 11)
     zk.prove_arrays(A, B, C, public)
     assert [x.n for x in zk.Z.values] == [x.n for x in plain.Z.values]
     with pytest.raises(RuntimeError, match="T1"):

@@ -1,8 +1,8 @@
-"""Zero-knowledge lookup proofs: the blinding of plain zero-knowledge mode plus F, H1, H2 and Z2 (tests/zk_lookup_oracle.py
+"""Zero-knowledge lookup proofs: the blinding of plain zero-knowledge mode plus F, H1, H2 and Z2 (tests/extended_oracle.py
 has the construction), with the 1216-byte proof, the transcript and the verifier unchanged.
 
-CPU: with zero blinders the oracle gives the bytes of the lookup oracles (one table: tests/lookup_oracle.py, two and
-three: tests/tagged_lookup_oracle.py); with random blinders its proofs pass the trapdoor check and both host verifier
+CPU: with zero blinders the oracle gives the bytes of the lookup proofs tests/golden/oracle_kinds.json pins (one
+table untagged, two and three tagged); with random blinders its proofs pass the trapdoor check and both host verifier
 routines, and tampered ones do not; the blinded polynomials agree with the unblinded ones on H and the blinded quotient
 pieces recombine to T; the lookup commitments a witness guess recomputes from the transcript's eta match a plain lookup
 proof and none of a zero-knowledge one.  GPU: the prover's 1216 bytes equal the oracle's with fixed blinders, zero
@@ -10,6 +10,7 @@ blinders reproduce the lookup goldens, the 2^16 zero-knowledge lookup golden is 
 commitment and verify, the round-by-round path gives the whole proof, the mode switches off through either entry point,
 the refusals leave the prover usable, and a 2^20 proof verifies."""
 import ctypes
+import hashlib
 import json
 import os
 import random
@@ -20,13 +21,12 @@ import pytest
 from oracle import fast as F
 from oracle import plonk_oracle as O
 from plonkathon_b200 import synthetic as syn
-from tests import lookup_oracle as LK
-from tests import tagged_lookup_oracle as TL
+from tests import extended_oracle as XO
 from tests import test_lookup as TLK
-from tests import zk_lookup_oracle as ZL
-from tests import zk_oracle as ZK
+from tests.golden.make_oracle_kinds import circuit, pinned
 from tests.golden_io import GOLDEN
-from tests.test_lookup import _commit_col, _host_vk, host_lincomb  # noqa: F401  (host_lincomb: a fixture)
+from tests.oracle_keys import host_lincomb  # noqa: F401  (a fixture)
+from tests.test_lookup import _commit_col, _host_vk
 from tests.test_lookup_tagged import _circuit as _tagged_circuit
 from tests.test_lookup_tagged import and_table, range_table, tables, xor_table
 
@@ -38,7 +38,7 @@ POINTS = ("a_1", "b_1", "c_1", "z_1", "t_lo_1", "t_mid_1", "t_hi_1", "W_z_1", "W
 
 def _blinders(seed):
     rng = random.Random(seed)
-    return [rng.randrange(1, R) for _ in range(ZL.N_BLINDERS)]
+    return [rng.randrange(1, R) for _ in range(21)]
 
 
 def _circuit(log_n, n_public, count, custom, seed):
@@ -52,10 +52,10 @@ def _circuit(log_n, n_public, count, custom, seed):
 def _oracle(c, blinders, fast=True):
     """(pk, setup of n + 6 powers, proof, prover object)"""
     n = c.group_order
-    pk = TL.preprocessed(c)
+    pk = XO.preprocessed(c)
     A, B, C = c.wires_values()
     setup = F.Setup(TAU, n + 6)
-    prover = ZL.make_prover(setup, pk, blinders)
+    prover = XO.Prover(setup, pk, blinders)
     if fast:
         with F.c_kernels():
             proof = prover.prove(A, B, C, c.public_values())
@@ -69,8 +69,8 @@ def _plain_oracle(c, fast=True):
     n = c.group_order
     A, B, C = c.wires_values()
     if c.lookups:
-        return TL.prove(F.Setup(TAU, n), TL.preprocessed(c), A, B, C, c.public_values(), fast=fast)
-    return LK.prove(F.Setup(TAU, n), LK.preprocessed(c), A, B, C, c.public_values(), fast=fast)
+        return XO.prove(F.Setup(TAU, n), XO.preprocessed(c), A, B, C, c.public_values(), fast=fast)
+    return XO.prove(F.Setup(TAU, n), XO.preprocessed(c), A, B, C, c.public_values(), fast=fast)
 
 
 def _oracle_vk(c, pk, setup):
@@ -85,9 +85,10 @@ def _oracle_vk(c, pk, setup):
 @pytest.mark.parametrize("count", [1, 2, 3])
 @pytest.mark.parametrize("log_n", [4, 6, 8])
 def test_oracle_zero_blinders_give_the_lookup_proof(log_n, count):
-    c = _circuit(log_n, 2, count, (), 100 + log_n + count)
-    _, _, proof, _ = _oracle(c, [0] * ZL.N_BLINDERS, fast=log_n > 4)
-    assert LK.proof_bytes(proof) == LK.proof_bytes(_plain_oracle(c, fast=log_n > 4))
+    """against the lookup proofs, one table untagged, that tests/golden/oracle_kinds.json pins"""
+    rec = pinned("lookup", log_n, (), count)
+    _, _, proof, _ = _oracle(circuit(rec), [0] * 21, fast=log_n > 4)
+    assert hashlib.sha256(XO.proof_bytes(proof)).hexdigest() == rec["sha256"]
 
 
 @pytest.mark.parametrize("custom", [(), TERM], ids=["plain", "x2"])
@@ -104,10 +105,10 @@ def test_oracle_zk_lookup_proof_verifies(log_n, count, custom, host_lincomb):
     bad = [dict(proof, **{k: (proof[k] + 1) % R}) for k in ("f_eval", "h1_shifted_eval", "z2_shifted_eval")]
     bad.append(dict(proof, W_z_1=proof["W_zw_1"], W_zw_1=proof["W_z_1"]))
     for p, ok in [(proof, True)] + [(b, False) for b in bad]:
-        assert TL.verify_proof_trapdoor(n, vk, cpts, lpts, p, public, TAU) is ok
+        assert XO.verify_proof_trapdoor(n, dict(vk, custom=cpts, lookup=lpts), p, public, TAU) is ok
         if log_n == 8 and not ok:
             continue  # the host routines' rejections once per table count and term, at the smaller sizes
-        pf = pb.LookupProof.from_bytes(LK.proof_bytes(p))
+        pf = pb.LookupProof.from_bytes(XO.proof_bytes(p))
         assert key.verify_proof(n, pf, public) is ok and key.verify_proof_unoptimized(n, pf, public) is ok
 
 
@@ -119,24 +120,24 @@ def test_oracle_blinded_polynomials_agree_on_h_and_pieces_recombine():
     for name, blinded, length in (("F", prover.Fb, n + 2), ("H1", prover.H1b, n + 3), ("H2", prover.H2b, n + 2),
                                   ("Z2", prover.Z2b, n + 3)):
         assert len(blinded) == length and blinded[n:] != [0] * (length - n), name
-        assert [ZK.poly_eval(blinded, pow(w, i, R)) for i in range(n)] == getattr(prover, name), name
+        assert [XO.poly_eval(blinded, pow(w, i, R)) for i in range(n)] == getattr(prover, name), name
     assert any(prover.T[3 * n:])  # the blinded quotient reaches past 3n
     x = random.Random(7).randrange(R)
     xn = pow(x, n, R)
-    got = (ZK.poly_eval(prover.T1b, x) + xn * ZK.poly_eval(prover.T2b, x) + xn * xn * ZK.poly_eval(prover.T3b, x)) % R
-    assert got == ZK.poly_eval(prover.T, x)
+    got = (XO.poly_eval(prover.T1b, x) + xn * XO.poly_eval(prover.T2b, x) + xn * xn * XO.poly_eval(prover.T3b, x)) % R
+    assert got == XO.poly_eval(prover.T, x)
 
 
 def _guess_commitments(c, proof):
     """f_1, h1_1, h2_1 recomputed from the witness and the eta of the proof's own transcript"""
     n = c.group_order
     setup = F.Setup(TAU, n)
-    guess = TL.TaggedProver(setup, TL.preprocessed(c))
+    guess = XO.Prover(setup, XO.preprocessed(c))
     guess.PI = [(-int(v)) % R for v in c.public_values()] + [0] * (n - len(c.public_values()))
     with F.c_kernels():
         guess.round_1(*c.wires_values())
-        guess.eta = LK.challenges(proof)["eta"]
-        return guess.round_lookup()
+        guess.eta = XO.challenges(proof)["eta"]
+        return tuple(guess.round_1L().values())
 
 
 @pytest.mark.parametrize("count", [1, 3])
@@ -196,7 +197,7 @@ def test_gpu_zk_lookup_proof_equals_oracle(log_n, n_public, count, custom):
     raw = prover.prove_arrays(A, B, C, public)
     _, _, proof, _ = _oracle(c, bl)
     assert len(raw) == 1216
-    assert raw == LK.proof_bytes(proof)
+    assert raw == XO.proof_bytes(proof)
     assert prover.prove_arrays(A, B, C, public) == raw  # fixed blinders: the same proof again
 
 
@@ -216,7 +217,7 @@ def test_gpu_zero_blinders_reproduce_lookup_goldens(name, tagged):
     rec = json.load(open(os.path.join(GOLDEN, name)))
     c = _golden_circuit(rec, tagged)
     setup = pb.Setup.generate(TAU, c.group_order + 6)
-    _, _, prover, (A, B, C, public) = _gpu_prover(pb, c, setup, [0] * ZL.N_BLINDERS)
+    _, _, prover, (A, B, C, public) = _gpu_prover(pb, c, setup, [0] * 21)
     assert prover.prove_arrays(A, B, C, public).hex() == rec["proof_hex"]
 
 
@@ -250,7 +251,7 @@ def test_gpu_fresh_blinders_differ_and_verify():
     setup, pk, prover, (A, B, C, public) = _gpu_prover(pb, c)
     p1 = prover.prove_arrays(A, B, C, public)
     p2 = prover.prove_arrays(A, B, C, public)
-    f1, f2 = LK.proof_from_bytes(p1), LK.proof_from_bytes(p2)
+    f1, f2 = XO.proof_from_bytes(p1), XO.proof_from_bytes(p2)
     assert all(f1[k] != f2[k] for k in POINTS)
     vk = _vk(setup, c, pk)
     for raw in (p1, p2):
@@ -269,7 +270,7 @@ def test_gpu_round_by_round_equals_whole_proof(count):
     c = _circuit(8, 2, count, TERM, 21)
     _, _, prover, (A, B, C, public) = _gpu_prover(pb, c, blinders=_blinders(21))
     raw = prover.prove_arrays(A, B, C, public)
-    ch = LK.challenges(LK.proof_from_bytes(raw))
+    ch = XO.challenges(XO.proof_from_bytes(raw))
     le = lambda k: (ch[k] % R).to_bytes(32, "little")  # noqa: E731
     ptr = lambda a: a.ctypes.data_as(ctypes.c_void_p)  # noqa: E731
     pub = np.ascontiguousarray(np.frombuffer(b"".join(int(x).to_bytes(32, "little") for x in public), np.uint8))
@@ -307,14 +308,14 @@ def test_gpu_switching_and_refusals():
         assert not prover.zk and golden()
     # refusals, each leaving the prover as it was
     L = _lib.lib()
-    assert L.pb200_prover_set_zk_lookup(prover._h, 1, b"\xff" * 32 * ZL.N_BLINDERS) != 0
+    assert L.pb200_prover_set_zk_lookup(prover._h, 1, b"\xff" * 32 * 21) != 0
     assert "not reduced" in L.pb200_last_error().decode()
     with pytest.raises(_lib.PlonkB200Error, match="zero-knowledge mode does not combine with lookups"):
         prover.set_zk(True)
     assert golden()
-    prover.set_zk_lookup(True, [0] * ZL.N_BLINDERS)
+    prover.set_zk_lookup(True, [0] * 21)
     with pytest.raises(_lib.PlonkB200Error, match="zero-knowledge mode does not combine with lookups"):
-        prover.set_zk(True, [0] * ZK.N_BLINDERS)
+        prover.set_zk(True, [0] * 11)
     assert golden()  # still in zero-knowledge lookup mode, with zero blinders
     prover.set_zk_lookup(False)
     plain = pb.Prover.from_arrays(setup, n, pk)

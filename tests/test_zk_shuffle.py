@@ -1,7 +1,7 @@
-"""Zero-knowledge shuffle proofs: the blinding of zero-knowledge mode plus Z3 (tests/zk_shuffle_oracle.py has the
+"""Zero-knowledge shuffle proofs: the blinding of zero-knowledge mode plus Z3 (tests/extended_oracle.py has the
 construction), with the 896- and 992-byte proofs, the transcript and the verifier unchanged.
 
-CPU: with zero blinders the oracle gives the bytes of the shuffle oracle (tests/shuffle_oracle.py) for plain, same-row
+CPU: with zero blinders the oracle gives the bytes of the shuffle proofs tests/golden/oracle_kinds.json pins for plain, same-row
 and next-row circuits; with random blinders its proofs pass the trapdoor check and both host verifier routines, and
 tampered ones do not; Z3' agrees with Z3 on H and the blinded quotient pieces recombine to T; the z3_1 a witness guess
 recomputes from the transcript's theta and kappa matches a plain shuffle proof and no zero-knowledge one; the Python
@@ -10,6 +10,7 @@ reproduce the shuffle golden, the 2^16 zero-knowledge shuffle golden is reproduc
 commitment and every blinded evaluation and verify, the round-by-round path gives the whole proof, the mode switches off
 through either entry point, the refusals leave the prover usable, and a 2^20 proof verifies."""
 import ctypes
+import hashlib
 import json
 import os
 import random
@@ -20,9 +21,9 @@ import pytest
 from oracle import fast as F
 from oracle import plonk_oracle as O
 from plonkathon_b200 import synthetic as syn
-from tests import shuffle_oracle as SO
-from tests import zk_oracle as ZO
-from tests import zk_shuffle_oracle as ZS
+from tests import extended_oracle as XO
+from tests.golden.make_oracle_kinds import circuit, pinned
+from tests.oracle_keys import host_lincomb  # noqa: F401  (a fixture)
 from tests.golden_io import GOLDEN
 from tests.test_shuffle import (GPU_SIZES, GPU_TERM_IDS, GPU_TERMS, NEXT_TERMS, TERM_IDS, TERM_SETS, _circuit, _host_key,
                                 _host_proof, _oracle_vk, _skewed_circuit)
@@ -40,12 +41,12 @@ def _blinders(count, seed):
 def _oracle(c, blinders, fast=True):
     """(pk, proof, prover object) of the zero-knowledge oracle on an SRS of n + 9 powers"""
     n = c.group_order
-    pk = SO.preprocessed(c)
+    pk = XO.preprocessed(c)
     A, B, C = c.wires_values()
     setup = F.Setup(TAU, n + 9)
     if not fast:
         setup = O.Setup([setup.point(i) for i in range(n + 9)], None)
-    prover = ZS.ZkShuffleProver(setup, pk, blinders)
+    prover = XO.Prover(setup, pk, blinders)
     if fast:
         with F.c_kernels():
             proof = prover.prove(A, B, C, c.public_values())
@@ -54,29 +55,15 @@ def _oracle(c, blinders, fast=True):
     return pk, proof, prover
 
 
-@pytest.fixture
-def host_lincomb(monkeypatch):
-    """the verifier's G1 combinations by the oracle's double-and-add (this suite has no GPU)"""
-    import plonkathon_b200 as pb
-    from plonkathon_b200 import verifier
-
-    def lincomb(pairs, ctx=None):
-        res = O.ec_lincomb_naive([(None if p is None else (int(p[0]), int(p[1])), int(k) % R) for p, k in pairs])
-        return None if res is None else (pb.FQ(res[0]), pb.FQ(res[1]))
-    monkeypatch.setattr(verifier, "ec_lincomb", lincomb)
-    return pb
-
-
 # ---- CPU ---------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("terms", TERM_SETS, ids=TERM_IDS)
 @pytest.mark.parametrize("log_n", [4, 6, 8])
 def test_oracle_zero_blinders_give_the_shuffle_proof(terms, log_n):
-    c = _circuit(log_n, 2, terms, 100 + log_n)
-    n = c.group_order
-    pk = SO.preprocessed(c)
-    _, proof, _ = _oracle(c, [0] * ZS.blinder_count(pk), fast=log_n > 4)
-    plain = SO.prove(F.Setup(TAU, n), pk, *c.wires_values(), c.public_values(), fast=True)
-    assert SO.proof_bytes(proof) == SO.proof_bytes(plain)
+    """against the shuffle proofs that tests/golden/oracle_kinds.json pins"""
+    rec = pinned("shuffle", log_n, terms)
+    c = circuit(rec)
+    _, proof, _ = _oracle(c, [0] * XO.blinder_count(XO.preprocessed(c)), fast=log_n > 4)
+    assert hashlib.sha256(XO.proof_bytes(proof)).hexdigest() == rec["sha256"]
 
 
 @pytest.mark.parametrize("terms", TERM_SETS, ids=TERM_IDS)
@@ -85,18 +72,18 @@ def test_oracle_zk_shuffle_proof_verifies(terms, log_n, host_lincomb):
     pb = host_lincomb
     c = _circuit(log_n, 2, terms, 200 + log_n)
     n = c.group_order
-    pk = SO.preprocessed(c)
-    _, proof, _ = _oracle(c, _blinders(ZS.blinder_count(pk), log_n), fast=log_n > 4)
+    pk = XO.preprocessed(c)
+    _, proof, _ = _oracle(c, _blinders(XO.blinder_count(pk), log_n), fast=log_n > 4)
     vk, custom, shuffle = _oracle_vk(c, pk)
     public = c.public_values()
     key = _host_key(pb, n, vk, custom, shuffle)
     bad = [dict(proof, **{k: (proof[k] + 1) % R}) for k in ("z3_shifted_eval", "a_eval")]
     bad.append(dict(proof, W_z_1=proof["W_zw_1"], W_zw_1=proof["W_z_1"]))
     for p, ok in [(proof, True)] + [(b, False) for b in bad]:
-        assert SO.verify_proof_trapdoor(n, vk, custom, shuffle, p, public, TAU) is ok
+        assert XO.verify_proof_trapdoor(n, dict(vk, custom=custom, shuffle=shuffle), p, public, TAU) is ok
         if log_n == 8 and not ok:
             continue  # the host routines' rejections once per term set, at the smaller sizes
-        raw = SO.proof_bytes(p)
+        raw = XO.proof_bytes(p)
         assert len(raw) == (992 if terms == NEXT_TERMS else 896)
         pf = _host_proof(pb, raw)
         assert key.verify_proof(n, pf, public) is ok and key.verify_proof_unoptimized(n, pf, public) is ok
@@ -106,24 +93,24 @@ def test_oracle_zk_shuffle_proof_verifies(terms, log_n, host_lincomb):
 def test_oracle_blinded_z3_agrees_on_h_and_pieces_recombine(terms):
     c = _circuit(6, 2, terms, 17)
     n = c.group_order
-    pk = SO.preprocessed(c)
-    _, _, prover = _oracle(c, _blinders(ZS.blinder_count(pk), 5))
+    pk = XO.preprocessed(c)
+    _, _, prover = _oracle(c, _blinders(XO.blinder_count(pk), 5))
     w = O.root_of_unity(n)
     assert len(prover.Z3c) == n + 3 and prover.Z3c[n:] != [0, 0, 0]
-    assert [ZO.poly_eval(prover.Z3c, pow(w, i, R)) for i in range(n)] == prover.Z3
+    assert [XO.poly_eval(prover.Z3c, pow(w, i, R)) for i in range(n)] == prover.Z3
     T = prover.T
     assert any(T[3 * n:])  # the blinded quotient reaches past 3n
     assert not any(T[3 * n + (9 if terms else 6):])  # deg T <= 3n + 5 (3n + 8 with next-row terms)
     x = random.Random(7).randrange(R)
     xn = pow(x, n, R)
-    got = (ZO.poly_eval(prover.T1b, x) + xn * ZO.poly_eval(prover.T2b, x) + xn * xn * ZO.poly_eval(prover.T3b, x)) % R
-    assert got == ZO.poly_eval(T, x)
+    got = (XO.poly_eval(prover.T1b, x) + xn * XO.poly_eval(prover.T2b, x) + xn * xn * XO.poly_eval(prover.T3b, x)) % R
+    assert got == XO.poly_eval(T, x)
 
 
-def _guess_z3_1(c, proof, next_row):
+def _guess_z3_1(c, proof):
     """z3_1 recomputed from the witness and the theta, kappa of the proof's own transcript"""
     n = c.group_order
-    ch = SO.challenges(proof, next_row)
+    ch = XO.challenges(proof)
     th, ka = ch["theta"], ch["kappa"]
     A, B, C = ([int(v) % R for v in X] for X in c.wires_values())
     q_in, q_out = c.shuffle
@@ -141,12 +128,12 @@ def test_witness_guess_matches_plain_shuffle_proofs_only(terms):
     proof's z3_1 (the test can see the leak), different from every zero-knowledge shuffle proof's"""
     c = _circuit(6, 2, terms, 300)
     n = c.group_order
-    pk = SO.preprocessed(c)
-    plain = SO.prove(F.Setup(TAU, n), pk, *c.wires_values(), c.public_values(), fast=True)
-    assert _guess_z3_1(c, plain, bool(terms)) == plain["z3_1"]
+    pk = XO.preprocessed(c)
+    plain = XO.prove(F.Setup(TAU, n), pk, *c.wires_values(), c.public_values(), fast=True)
+    assert _guess_z3_1(c, plain) == plain["z3_1"]
     for seed in (1, 2):
-        _, zk, _ = _oracle(c, _blinders(ZS.blinder_count(pk), seed))
-        assert _guess_z3_1(c, zk, bool(terms)) != zk["z3_1"]
+        _, zk, _ = _oracle(c, _blinders(XO.blinder_count(pk), seed))
+        assert _guess_z3_1(c, zk) != zk["z3_1"]
 
 
 def test_set_zk_shuffle_argument_checks():
@@ -182,7 +169,7 @@ def _vk(setup, c, pk):
 
 
 def _count(c):
-    return ZS.blinder_count(SO.preprocessed(c))
+    return XO.blinder_count(XO.preprocessed(c))
 
 
 @pytest.mark.gpu
@@ -198,7 +185,7 @@ def test_gpu_zk_shuffle_proof_equals_oracle(terms, log_n, n_public):
     raw = prover.prove_arrays(*wires)
     _, proof, _ = _oracle(c, bl)
     assert len(raw) == (896 if terms in ([], [(2, 0, 0), (1, 1, 1)]) else 992)
-    assert raw == SO.proof_bytes(proof)
+    assert raw == XO.proof_bytes(proof)
     assert prover.prove_arrays(*wires) == raw  # fixed blinders: the same proof again
 
 
@@ -207,11 +194,11 @@ def test_gpu_zk_shuffle_proof_equals_oracle(terms, log_n, n_public):
 def test_gpu_skewed_zk_shuffle_equals_oracle(log_n):
     import plonkathon_b200 as pb
     c = _skewed_circuit(log_n)
-    bl = _blinders(ZS.N_BLINDERS, log_n)
+    bl = _blinders(14, log_n)
     _, _, prover, wires = _gpu_prover(pb, c, blinders=bl)
     raw = prover.prove_arrays(*wires)
     _, proof, _ = _oracle(c, bl)
-    assert len(raw) == 896 and raw == SO.proof_bytes(proof)
+    assert len(raw) == 896 and raw == XO.proof_bytes(proof)
 
 
 def _golden_circuit(rec):
@@ -225,7 +212,7 @@ def test_gpu_zero_blinders_reproduce_the_shuffle_golden():
     rec = json.load(open(os.path.join(GOLDEN, "proof_shuffle_2p16.json")))
     c = _golden_circuit(rec)
     setup = pb.Setup.generate(TAU, c.group_order + 9)
-    _, _, prover, wires = _gpu_prover(pb, c, setup, [0] * ZS.N_NEXT_ROW_BLINDERS)
+    _, _, prover, wires = _gpu_prover(pb, c, setup, [0] * 17)
     assert prover.prove_arrays(*wires).hex() == rec["proof_hex"]
 
 
@@ -274,10 +261,10 @@ def test_gpu_fresh_blinders_differ_and_verify(terms):
     assert all(f1[k] != f2[k] for k in POINTS + tuple(blinded))
     # zeta differs between the two proofs, so no evaluation repeats; the fixed polynomials S1, S2 and Q_in are not
     # blinded, so their evaluations are those of the columns at each proof's own zeta, and the wires' are not
-    spk = SO.preprocessed(c)
+    spk = XO.preprocessed(c)
     A_ = [int(v) % R for v in c.wires_values()[0]]
     for f in (f1, f2):
-        zeta = SO.challenges(f, bool(terms))["zeta"]
+        zeta = XO.challenges(f)["zeta"]
         for k, col in (("s1_eval", spk.S1), ("s2_eval", spk.S2), ("qin_eval", spk.q_in)):
             assert f[k] == O.barycentric_eval(col, zeta), k
         assert f["a_eval"] != O.barycentric_eval(A_, zeta)
@@ -296,7 +283,7 @@ def test_gpu_round_by_round_abi_gives_the_whole_proof(terms):
     c = _circuit(8, 2, terms, 55)
     _, _, prover, (A, B, C, public) = _gpu_prover(pb, c, blinders=_blinders(_count(c), 55))
     raw = prover.prove_arrays(A, B, C, public)
-    ch = SO.challenges(_proof_dict(pb, raw), bool(terms))
+    ch = XO.challenges(_proof_dict(pb, raw))
     le = lambda k: (int(ch[k]) % R).to_bytes(32, "little")  # noqa: E731
     ptr = lambda a: a.ctypes.data_as(ctypes.c_void_p)  # noqa: E731
     pub = np.ascontiguousarray(np.frombuffer(b"".join(int(x).to_bytes(32, "little") for x in public), np.uint8))
@@ -334,12 +321,12 @@ def test_gpu_switching_and_refusals():
         assert not prover.zk and golden()
     # refusals, each leaving the prover as it was
     L = _lib.lib()
-    assert L.pb200_prover_set_zk_shuffle(prover._h, 1, b"\xff" * 32 * ZS.N_NEXT_ROW_BLINDERS) != 0
+    assert L.pb200_prover_set_zk_shuffle(prover._h, 1, b"\xff" * 32 * 17) != 0
     assert "not reduced" in L.pb200_last_error().decode()
     with pytest.raises(_lib.PlonkB200Error, match="does not combine with a shuffle"):
         prover.set_zk(True)
     assert golden()
-    prover.set_zk_shuffle(True, [0] * ZS.N_NEXT_ROW_BLINDERS)
+    prover.set_zk_shuffle(True, [0] * 17)
     with pytest.raises(_lib.PlonkB200Error, match="does not combine with a shuffle"):
         prover.set_zk(True, [0] * 14)
     assert golden()  # still in zero-knowledge shuffle mode, with zero blinders
