@@ -100,6 +100,26 @@ int pb200_g1_msm_host(pb200_ctx* ctx, const uint8_t* h_points, const uint8_t* h_
 /* setup.py:16-22  Setup.powers_of_x.  h_points: n affine points (canonical).  precompute != 0 builds the
  * fixed-base window table in HBM (size ceil(256/c) * n * 64 bytes). */
 int pb200_srs_create(pb200_ctx* ctx, const uint8_t* h_points, uint64_t n, int precompute, pb200_srs** out);
+/* Ceremony SRS from a snarkjs .ptau, checked.  h_g1: `count` points exactly as section 2 (tauG1) stores them: x || y,
+ * 32-byte little-endian Montgomery values (R = 2^256), 64 bytes per point -- the library's own device form, so the
+ * bytes go to the device unconverted, in chunks through pinned staging.  h_tau_g2: [tau]_2 as section 3 stores its
+ * second point (x.c0 x.c1 y.c0 y.c1, Montgomery, 128 bytes).  precompute as for pb200_srs_create.  Refused (an error;
+ * nothing is kept and the context stays usable) unless every coordinate is below q (the error names the lowest bad
+ * point), every point is on y^2 = x^3 + 3 and none is the identity (ditto), point 0 is the generator (1, 2), [tau]_2
+ * is on the twist and r [tau]_2 = O, and e(sum r_i G_(i+1), G2) = e(sum r_i G_i, [tau]_2) for fresh 128-bit r_i from
+ * getrandom(2) -- one two-vector MSM over the loaded points and one pairing product, which with the generator check
+ * makes G_i = [tau^i]G for the tau of [tau]_2 except with probability about 2^-128.  Messages start "ptau: ". */
+int pb200_srs_create_ptau(pb200_ctx* ctx, const uint8_t* h_g1, uint64_t count, const uint8_t* h_tau_g2, int precompute,
+                          pb200_srs** out);
+/* The Lagrange block of the size-n domain (n a power of two) as section 12 stores it (points n - 1 .. 2n - 2 of the
+ * section, same encoding), checked like the points above and against srs_monomial (at least n powers): for random
+ * values v, sum_i v_i [L_i] must equal the commitment of iNTT(v) to the monomial powers. */
+int pb200_srs_create_ptau_lagrange(pb200_ctx* ctx, const uint8_t* h_block, uint64_t n, pb200_srs* srs_monomial,
+                                   int precompute, pb200_srs** out);
+/* Stage times (ms) of the calling thread's last pb200_srs_create_ptau / _lagrange, in this order: host-to-device copy,
+ * check kernel (CUDA events), window table, random scalars, consistency MSM, pairing, [tau]_2 checks.  Stages a call
+ * did not reach read 0. */
+void pb200_srs_ptau_stages(double* ms, int count);
 /* Structured test SRS generated on the device: points [tau^i]G, i < n, for a known (toxic) tau --
  * the 2^20 / 2^22 configurations need more powers than the reference's shipped .ptau holds
  * (setup.py:27 reads 2^11).  h_tau: canonical 32-byte Fr.  tau == 0 is refused (an error, before any device

@@ -61,6 +61,9 @@ def _load():
         "pb200_g1_msm": (I, [V, V, V, U64, V, P(I)]),
         "pb200_g1_msm_host": (I, [V, V, V, U64, V, P(I)]),
         "pb200_srs_create": (I, [V, V, U64, I, P(V)]),
+        "pb200_srs_create_ptau": (I, [V, V, U64, V, I, P(V)]),
+        "pb200_srs_create_ptau_lagrange": (I, [V, V, U64, V, I, P(V)]),
+        "pb200_srs_ptau_stages": (None, [P(ctypes.c_double), I]),
         "pb200_srs_generate": (I, [V, V, U64, I, P(V)]),
         "pb200_srs_generate_lagrange": (I, [V, V, U64, I, P(V)]),
         "pb200_srs_export": (I, [V, V, V, U64, U64]),

@@ -63,6 +63,15 @@ void host_join_bucket_shards(const SR* all, uint32_t world, uint32_t sets, uint3
 void host_join_bucket_shards_strided(const SR* all, uint32_t world, uint32_t sets, G1XYZZ* out);
 // permutation.cu
 void permutation_run(Context* ctx, const int64_t* h_ids, int log_n, uint8_t* h_S);
+// ptau.cu
+Srs* srs_create_ptau(Context* ctx, const uint8_t* h_g1, uint64_t count, const uint8_t* h_tau_g2, int precompute);
+Srs* srs_create_ptau_lagrange(Context* ctx, const uint8_t* h_block, uint64_t n, Srs* monomial, int precompute);
+void ptau_stages(double* out_ms, int count);
+
+const Bn254Pairing& pairing_engine() {
+  static const Bn254Pairing engine;  // constants derived once (thread-safe static initialisation)
+  return engine;
+}
 }  // namespace pb200
 
 using namespace pb200;
@@ -447,6 +456,20 @@ int pb200_srs_create(pb200_ctx* ctx, const uint8_t* h_points, uint64_t n, int pr
   *out = reinterpret_cast<pb200_srs*>(srs_create(C(ctx), h_points, n, precompute));
   PB_API_END
 }
+int pb200_srs_create_ptau(pb200_ctx* ctx, const uint8_t* h_g1, uint64_t count, const uint8_t* h_tau_g2, int precompute,
+                          pb200_srs** out) {
+  PB_API_BEGIN PB_ON_CTX(C(ctx));
+  *out = reinterpret_cast<pb200_srs*>(srs_create_ptau(C(ctx), h_g1, count, h_tau_g2, precompute));
+  PB_API_END
+}
+int pb200_srs_create_ptau_lagrange(pb200_ctx* ctx, const uint8_t* h_block, uint64_t n, pb200_srs* srs_monomial,
+                                   int precompute, pb200_srs** out) {
+  PB_API_BEGIN PB_ON_CTX(C(ctx));
+  *out = reinterpret_cast<pb200_srs*>(
+      srs_create_ptau_lagrange(C(ctx), h_block, n, reinterpret_cast<Srs*>(srs_monomial), precompute));
+  PB_API_END
+}
+void pb200_srs_ptau_stages(double* ms, int count) { ptau_stages(ms, count); }
 // Taus whose SRS would hold the identity are refused before any device work: tau = 0 makes [tau^i]G the identity for
 // every i > 0, and tau^n = 1 makes L_i(tau) = 0 for all i but one.  The batched affine conversion cannot represent
 // the identity (k_batch_to_affine), so such an SRS would commit to wrong points without an error.
@@ -784,11 +807,6 @@ static void store_g2(const G2Affine& q, uint8_t* out, int* is_identity) {
   const Fq c[4] = {fp_from_mont(q.x.a), fp_from_mont(q.x.b), fp_from_mont(q.y.a), fp_from_mont(q.y.b)};
   for (int k = 0; k < 4; k++) memcpy(out + 32 * k, c[k].v, 32);
 }
-static const Bn254Pairing& pairing_engine() {
-  static const Bn254Pairing engine;  // constants derived once (thread-safe static initialisation)
-  return engine;
-}
-
 int pb200_pairing_check(const uint8_t* h_g1, const uint8_t* h_g1_identity, const uint8_t* h_g2,
                         const uint8_t* h_g2_identity, unsigned count, int* ok) {
   PB_API_BEGIN

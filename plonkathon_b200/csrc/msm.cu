@@ -928,6 +928,15 @@ Srs* srs_create(Context* ctx, const uint8_t* h_points, uint64_t n, int precomput
   return srs.release();
 }
 
+// base: n affine points already in HBM in Montgomery form (a checked .ptau section, ptau.cu), moved into the SRS
+Srs* srs_adopt(Context* ctx, DevBuf&& base, uint64_t n, int precompute) {
+  auto srs = std::make_unique<Srs>();
+  srs->n = n;
+  srs->base = std::move(base);
+  srs_finish(ctx, srs.get(), precompute);
+  return srs.release();
+}
+
 // builds the fixed-base window table 2^(c*w) * P_i, w < W, in HBM
 static void srs_finish(Context* ctx, Srs* srs, int precompute) {
   const uint64_t n = srs->n;

@@ -49,6 +49,55 @@ def ptau_sections(contents: bytes) -> dict:
     return out
 
 
+PTAU_SECTION_HEADER, PTAU_SECTION_TAU_G1, PTAU_SECTION_TAU_G2 = 1, 2, 3
+
+
+def ptau_layout(f) -> dict:
+    """Section table of an open snarkjs binfile, read by seeking: {section id: (data offset, declared size, bytes
+    present)}.  Follows ``ptau_sections``' layout, but keeps a section the file cuts off, with the bytes it has.  Raises
+    ValueError for a wrong magic or a section header cut off."""
+    f.seek(0, 2)
+    file_size = f.tell()
+    f.seek(0)
+    head = f.read(12)
+    if len(head) < 12 or head[:4] != b"ptau":
+        raise ValueError("ptau: not a .ptau file (the magic 'ptau' is missing)")
+    count = int.from_bytes(head[8:12], "little")
+    out, pos = {}, 12
+    for _ in range(count):
+        if pos >= file_size:
+            break
+        f.seek(pos)
+        sh = f.read(12)
+        if len(sh) < 12:
+            raise ValueError("ptau: the header of section %d is cut off at byte %d" % (len(out) + 1, pos))
+        sid, size = int.from_bytes(sh[:4], "little"), int.from_bytes(sh[4:12], "little")
+        out[sid] = (pos + 12, size, max(0, min(size, file_size - pos - 12)))
+        pos += 12 + size
+    return out
+
+
+def _ptau_header(f, sections) -> int:
+    """section 1: n8 = 32, q = BN254's q; returns the power p"""
+    if PTAU_SECTION_HEADER not in sections:
+        raise ValueError("ptau: section 1 (header) is missing")
+    off, size, have = sections[PTAU_SECTION_HEADER]
+    if have < 40 or have < size:
+        raise ValueError("ptau: section 1 (header) is truncated")
+    f.seek(off)
+    h = f.read(40)
+    n8 = int.from_bytes(h[:4], "little")
+    if n8 != 32:
+        raise ValueError("ptau: section 1 says n8 = %d, BN254 has 32-byte coordinates" % n8)
+    if int.from_bytes(h[4:36], "little") != FIELD_MODULUS:
+        raise ValueError("ptau: section 1 names a field modulus that is not BN254's q")
+    return int.from_bytes(h[36:40], "little")
+
+
+def _mont_to_int(raw: bytes) -> int:
+    return int.from_bytes(raw, "little") * pow(2, -256, FIELD_MODULUS) % FIELD_MODULUS
+
+
 class Setup:
     def __init__(self, powers_of_x, X2, ctx: Optional[_lib.Context] = None, precompute: bool = True):
         self._powers = list(powers_of_x)
@@ -57,6 +106,7 @@ class Setup:
         self.tau = None
         self._lagrange = {}        # domain size -> SRS handle holding [L_i(tau)]_1
         self._lagrange_raw = None  # canonical x||y bytes of the .ptau Lagrange section (blocks of 2^p points)
+        self._ptau_lagrange = None  # (file name, offset, bytes) of the .ptau Lagrange section (from_ptau)
         self._precompute = precompute
         self.ctx = ctx or _lib.default_context()
         raw = b"".join(_pt_bytes(p) for p in self._powers)
@@ -77,6 +127,7 @@ class Setup:
         self._n = n
         self._lagrange = {}
         self._lagrange_raw = None
+        self._ptau_lagrange = None
         self._precompute = precompute
         self.tau = tau % CURVE_ORDER
         self.X2 = g2_mul(G2, self.tau)
@@ -145,6 +196,66 @@ class Setup:
             self.load_lagrange_section(contents[sec[0]:sec[0] + sec[1]], factor)
         return self
 
+    @classmethod
+    def from_ptau(cls, filename, powers: Optional[int] = None, ctx=None, precompute: bool = True):
+        """Ceremony SRS from a snarkjs .ptau, checked by the library (``pb200_srs_create_ptau``): every point reduced,
+        on the curve and not the identity, point 0 the generator, [tau]_2 in G2, and the points successive powers of
+        the tau behind [tau]_2.  Only the header, the section table and the needed byte ranges are read; the tauG1
+        bytes go to the device as stored (Montgomery form), so no point becomes a Python object.
+
+        ``powers``: how many tauG1 points to load; None takes 2^p (section 1's power, the count ``from_file`` takes),
+        any count up to what section 2 holds (2^(p+1) - 1 in a ceremony file) is allowed.  A missing section, a wrong
+        magic, a wrong q, or a truncated section 2 raises ValueError before any library call.  Section 3 (tauG2) may
+        end after its second point, [tau]_2.  Section 12 (Lagrange blocks), if present, is read block by block in
+        ``enable_lagrange``."""
+        import numpy as np
+        with open(filename, "rb") as f:
+            sections = ptau_layout(f)
+            p = _ptau_header(f, sections)
+            if PTAU_SECTION_TAU_G1 not in sections:
+                raise ValueError("ptau: section 2 (tauG1) is missing")
+            g1_off, g1_size, g1_have = sections[PTAU_SECTION_TAU_G1]
+            if g1_have < g1_size:
+                raise ValueError("ptau: section 2 (tauG1) is truncated: %d of its %d bytes are in the file"
+                                 % (g1_have, g1_size))
+            if g1_size % 64:
+                raise ValueError("ptau: section 2 (tauG1) is %d bytes, not a whole number of 64-byte points" % g1_size)
+            held = g1_size // 64
+            count = 2 ** p if powers is None else int(powers)
+            if count < 1:
+                raise ValueError("ptau: powers must be at least 1")
+            if count > held:
+                raise ValueError("Not enough powers in setup: %d asked for, the file's tauG1 section holds %d (power %d)"
+                                 % (count, held, p))
+            if PTAU_SECTION_TAU_G2 not in sections:
+                raise ValueError("ptau: section 3 (tauG2) is missing")
+            g2_off, _, g2_have = sections[PTAU_SECTION_TAU_G2]
+            if g2_have < 256:
+                raise ValueError("ptau: section 3 (tauG2) ends before its second point, [tau]_2")
+            f.seek(g2_off + 128)
+            tau_g2 = f.read(128)
+        g1 = np.memmap(filename, dtype=np.uint8, mode="r", offset=g1_off, shape=(64 * count,))
+        self = cls.__new__(cls)
+        self._powers = None
+        self._n = count
+        self._lagrange = {}
+        self._lagrange_raw = None
+        self._ptau_lagrange = None
+        self._precompute = precompute
+        self.tau = None
+        self.ctx = ctx or _lib.default_context()
+        h = ctypes.c_void_p()
+        _lib.check(_lib.lib().pb200_srs_create_ptau(self.ctx.handle, g1.ctypes.data_as(ctypes.c_void_p), count,
+                                                    tau_g2, 1 if precompute else 0, ctypes.byref(h)))
+        self._srs = h
+        del g1
+        c = [_mont_to_int(tau_g2[i:i + 32]) for i in range(0, 128, 32)]
+        self.X2 = (FQ2(c[0:2]), FQ2(c[2:4]))
+        sec = sections.get(PTAU_SECTION_LAGRANGE_G1)
+        if sec is not None:
+            self._ptau_lagrange = (filename, sec[0], sec[2])
+        return self
+
     # ---- Lagrange-basis SRS (SURVEY 8(f) N4): commit = one MSM over the values, no inverse transform
     def load_lagrange_section(self, raw: bytes, factor: int = pow(2, 256, FIELD_MODULUS)):
         """``raw``: the data of .ptau section 12 (or a prefix of it): for p = 0, 1, 2, ... a block of 2^p points
@@ -159,7 +270,17 @@ class Setup:
         if self._lagrange.get(n):
             return True
         h = ctypes.c_void_p()
-        if self._lagrange_raw is not None and 64 * (2 * n - 1) <= len(self._lagrange_raw):
+        lag = getattr(self, "_ptau_lagrange", None)
+        if lag is not None and 64 * (2 * n - 1) <= lag[2]:
+            # block log2(n) of the .ptau's section 12, as stored, checked against the monomial points
+            import numpy as np
+            _log2_exact(n)
+            block = np.memmap(lag[0], dtype=np.uint8, mode="r", offset=lag[1] + 64 * (n - 1), shape=(64 * n,))
+            _lib.check(_lib.lib().pb200_srs_create_ptau_lagrange(
+                self.ctx.handle, block.ctypes.data_as(ctypes.c_void_p), n, self._srs, 1 if self._precompute else 0,
+                ctypes.byref(h)))
+            del block
+        elif self._lagrange_raw is not None and 64 * (2 * n - 1) <= len(self._lagrange_raw):
             block = self._lagrange_raw[64 * (n - 1):64 * (2 * n - 1)]
             _lib.check(_lib.lib().pb200_srs_create(self.ctx.handle, block, n, 1 if self._precompute else 0,
                                                    ctypes.byref(h)))
@@ -204,7 +325,8 @@ class Setup:
         """SRS of the size-n Lagrange basis if there is one: .ptau blocks are picked up on first use, device-generated
         ones only after ``enable_lagrange(n)`` (they cost as much HBM as the monomial SRS)."""
         h = self._lagrange.get(n)
-        if h is None and self._lagrange_raw is not None and self.enable_lagrange(n):
+        if h is None and (self._lagrange_raw is not None or getattr(self, "_ptau_lagrange", None) is not None) \
+                and self.enable_lagrange(n):
             h = self._lagrange[n]
         return h
 
