@@ -319,6 +319,33 @@ int pb200_prover_prove_next_row_shuffle(pb200_prover* p, const uint8_t* h_A, con
                                         const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof992);
 int pb200_prover_serialize_next_row_shuffle(pb200_prover* p, uint8_t* h_proof992);
 
+/* ---- Witness check: every failing constraint, without proving -------------------------------------------------------
+ * Checks a witness (A, B, C per row, canonical, and the public inputs as for pb200_prover_prove) against the prover's
+ * own key and reports five categories, each as an exact count and its lowest `limit` locations in ascending order:
+ *   gate     rows whose gate constraint (custom and next-row terms included, PI_i = -public_i) is not 0;
+ *   copy     cells c = 3 row + col whose value differs from that of sigma(c), the cell whose label omega^row' (col' + 1)
+ *            is S_col[row] -- the previous cell of its cycle;
+ *   key      cells whose S entry is no cell label, or repeats the label of a lower cell: S is not a permutation and no
+ *            witness can prove;
+ *   lookup   lookup provers: rows with q_K = 1 whose (a, b, c), or (a, b, c, Q_T) tagged, is not a row of the table;
+ *   shuffle  shuffle provers: rows with q_in = 1 or q_out = 1 whose (a, b, c) occurs a different number of times among
+ *            the q_in rows than among the q_out rows (a row with both selectors counts on both sides).
+ * counts[5]: gate, copy, key, lookup, shuffle.  lists: gate rows (limit), copy pairs (2*limit: c, sigma(c)),
+ * key cells (limit), lookup rows (limit), shuffle rows (limit) -- 6*limit uint32, ascending, unused entries 0xffffffff.
+ * Equality is decided on full field elements, so for a key that is a permutation all counts are 0 iff rounds 1 and 2 of
+ * a proof pass their checks (up to the proof's own soundness error).  Draws no blinders and leaves the round state and
+ * every later proof unchanged.  The first call builds sigma on the device and keeps it with the prover (12n bytes);
+ * every other buffer is freed before the call returns.  Refused, with the prover and the context usable afterwards: the
+ * sharded prover, a null h_public with n_public > 0, more public inputs than rows, limit > 3n, values not reduced below
+ * r (the prove messages), and more device memory than is free, or than PB200_CHECK_MAX_BYTES if set (naming the bytes). */
+int pb200_prover_check(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
+                       const uint8_t* h_public, uint64_t n_public, uint32_t limit, uint64_t* h_counts, uint32_t* h_lists);
+/* same, with the wire values already resident in HBM (canonical form, n x 32 bytes each), read on the context's stream:
+ * writes to them on another stream must be finished or ordered before the call */
+int pb200_prover_check_device(pb200_prover* p, const void* d_A, const void* d_B, const void* d_C,
+                              const uint8_t* h_public, uint64_t n_public, uint32_t limit, uint64_t* h_counts,
+                              uint32_t* h_lists);
+
 /* ---- multi-GPU: one process per GPU, one communicator per context (SURVEY.md 8(e)) -------------------------
  * The library issues its data-path collectives itself, on the context's stream, through NCCL (bound at run time
  * from the libnccl.so.2 the process has loaded; the single-GPU entry points work without it).  Rendezvous stays

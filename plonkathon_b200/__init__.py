@@ -10,3 +10,4 @@ from ._lib import Context, PlonkB200Error, default_context  # noqa: F401
 from .transcript import Transcript, Message1, Message2, Message3, Message4, Message5  # noqa: F401
 from .prover import Prover, Proof, LookupProof, NextRowProof, ShuffleProof, NextRowShuffleProof  # noqa: F401
 from .wiring import permutation_arrays  # noqa: F401
+from .witness import WitnessReport  # noqa: F401

@@ -119,6 +119,8 @@ def _load():
         "pb200_bench_modmul": (I, [V, I, U64, U, P(ctypes.c_float)]),
         "pb200_prover_sliced": (I, [V, P(I)]),
         "pb200_permutation": (I, [V, V, I, V]),
+        "pb200_prover_check": (I, [V, V, V, V, V, U64, ctypes.c_uint32, V, V]),
+        "pb200_prover_check_device": (I, [V, V, V, V, V, U64, ctypes.c_uint32, V, V]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)  # AttributeError here == ABI drift: fail loudly

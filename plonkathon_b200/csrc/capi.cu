@@ -61,6 +61,9 @@ void prover_set_shuffle(Prover* P, const uint8_t* h_qin, const uint8_t* h_qout);
 void g1_combine_partials_host(const G1XYZZ* parts, uint32_t count, uint8_t* out_xy, int* is_identity);
 void host_join_bucket_shards(const SR* all, uint32_t world, uint32_t sets, uint32_t nloc, G1XYZZ* out);
 void host_join_bucket_shards_strided(const SR* all, uint32_t world, uint32_t sets, G1XYZZ* out);
+// check.cu
+void prover_check(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t* hC, const uint8_t* h_public,
+                  uint64_t n_public, uint32_t limit, uint64_t* h_counts, uint32_t* h_lists, bool wires_on_device);
 // permutation.cu
 void permutation_run(Context* ctx, const int64_t* h_ids, int log_n, uint8_t* h_S);
 // ptau.cu
@@ -716,6 +719,20 @@ int pb200_prover_prove_next_row_shuffle(pb200_prover* p, const uint8_t* h_A, con
 }
 int pb200_prover_serialize_next_row_shuffle(pb200_prover* p, uint8_t* h_proof992) {
   return serialize(p, BLOCK_NEXT_ROW | BLOCK_SHUFFLE, h_proof992);
+}
+int pb200_prover_check(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
+                       const uint8_t* h_public, uint64_t n_public, uint32_t limit, uint64_t* h_counts, uint32_t* h_lists) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  prover_check(reinterpret_cast<Prover*>(p), h_A, h_B, h_C, h_public, n_public, limit, h_counts, h_lists, false);
+  PB_API_END
+}
+int pb200_prover_check_device(pb200_prover* p, const void* d_A, const void* d_B, const void* d_C,
+                              const uint8_t* h_public, uint64_t n_public, uint32_t limit, uint64_t* h_counts,
+                              uint32_t* h_lists) {
+  PB_API_BEGIN PB_ON_CTX(reinterpret_cast<Prover*>(p)->ctx);
+  prover_check(reinterpret_cast<Prover*>(p), (const uint8_t*)d_A, (const uint8_t*)d_B, (const uint8_t*)d_C, h_public,
+               n_public, limit, h_counts, h_lists, true);
+  PB_API_END
 }
 int pb200_g1_combine_partials_host(const uint8_t* h_xyzz, unsigned count, uint8_t* h_out_xy, int* is_identity) {
   PB_API_BEGIN

@@ -515,19 +515,6 @@ __global__ void k_scan_tile_sums(const uint32_t* counts, uint32_t nb, uint32_t p
 __global__ void k_scan_tiles(uint32_t* tile_sums, uint32_t n_tiles, uint32_t* total_out);
 __global__ void k_scan_apply(uint32_t* counts, uint32_t nb, uint32_t pad, const uint32_t* tile_sums, uint32_t* offsets);
 
-// the order of the sorted table copy: (t1, t2, t3[, t4]) lexicographically, each by Montgomery limbs from the top.
-// width 3 for one untagged table, 4 with the table tag t4 (y[3] is read only then).  Unrolled, so y stays in registers.
-PB_HD int lookup_cmp(const Fr* x, const Fr (&y)[4], int width) {
-#pragma unroll
-  for (int w = 0; w < 4; w++) {
-    if (w == width) break;
-#pragma unroll
-    for (int l = 7; l >= 0; l--)
-      if (x[w].v[l] != y[w].v[l]) return x[w].v[l] < y[w].v[l] ? -1 : 1;
-  }
-  return 0;
-}
-
 // j_i: for a lookup row (q_K = 1) the lowest table index of a row equal to (a_i, b_i, c_i[, Q_T[i]]) -- the first of
 // the equal rows in the sorted copy, which keeps table order among them --, else 0.  QT == nullptr: one untagged table,
 // keys of three columns.  A row not in the table: the lowest such i goes to *missing.
@@ -824,6 +811,7 @@ Prover* prover_create(Context* ctx, Srs* srs, int log_n, const uint8_t* const* h
   P->log_n = log_n;
   const uint64_t n = (uint64_t)1 << log_n, n4 = 4 * n;
   P->n = n;
+  P->sharded = sharded;
   PB_CHECK(log_n >= 1 && log_n <= 26, "group order must be 2^k, 1 <= k <= 26");
   PB_CHECK(n <= srs_size(srs), "Not enough powers in setup");
   set_custom_terms(P.get(), n_custom, h_exps, exp_width);

@@ -80,6 +80,20 @@ __device__ __forceinline__ Fr custom_gate_sum_next(const CustomTerms& t, uint64_
 }
 #endif
 
+// the order of the sorted table copy: (t1, t2, t3[, t4]) lexicographically, each by Montgomery limbs from the top.
+// width 3 for one untagged table, 4 with the table tag t4 (y[3] is read only then).  Unrolled, so y stays in registers.
+// The prover's table index (k_lookup_index) and the witness check (k_check_lookup) both search with it.
+PB_HD int lookup_cmp(const Fr* x, const Fr (&y)[4], int width) {
+#pragma unroll
+  for (int w = 0; w < 4; w++) {
+    if (w == width) break;
+#pragma unroll
+    for (int l = 7; l >= 0; l--)
+      if (x[w].v[l] != y[w].v[l]) return x[w].v[l] < y[w].v[l] ? -1 : 1;
+  }
+  return 0;
+}
+
 struct Prover {
   Context* ctx;
   Srs* srs;
@@ -203,6 +217,10 @@ struct Prover {
   // The proof's fields (proof_layout.cuh), canonical little-endian, indexed by ProofField: a point x||y, a scalar in
   // the first 32 bytes.  The rounds write them; only the fields of this prover's blocks are part of its proof.
   uint8_t fields[PROOF_FIELDS][64];
+  // The witness check (check.cu): the copy permutation sigma as 3n uint32 cell indices, built on the first check and
+  // kept (12n bytes).  No round reads it.
+  DevBuf chk_sigma;
+  bool sharded = false;  // made by a _sharded entry point (the witness check refuses it, whatever the world size)
   unsigned blocks() const {
     return (next_row ? BLOCK_NEXT_ROW : 0) | (sh ? BLOCK_SHUFFLE : 0) | (lk ? BLOCK_LOOKUP : 0);
   }

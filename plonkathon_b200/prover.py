@@ -22,6 +22,7 @@ from .lookup import check_lookup, check_lookups, padded_table, to_le_rows
 from .field import CURVE_ORDER, FIELD_MODULUS, FQ
 from .poly import Basis, _log2_exact, scalars_to_bytes
 from .shuffle import check_shuffle
+from .witness import WitnessReport
 from .transcript import (KIND, LOOKUP, NEXT_ROW, SHUFFLE, Message1, Message2, Message3, Message4, Message5,
                          NextRowMessage4, NextRowShuffleMessage4, ShuffleMessage2, ShuffleMessage4, Transcript, blocks,
                          proof_bytes, proof_fields, schedule)
@@ -185,6 +186,28 @@ def _as_le_rows(values, n) -> np.ndarray:
     return np.ascontiguousarray(arr)
 
 
+def _is_cuda_tensor(x) -> bool:
+    return type(x).__module__.startswith("torch") and getattr(x, "is_cuda", False)
+
+
+def _wire_rows(name, values, n) -> np.ndarray:
+    """a wire column as check_arrays takes it -> contiguous (n,32) uint8, zero padded; ValueError when malformed"""
+    if isinstance(values, np.ndarray):
+        if not ((values.dtype == np.uint8 and values.ndim == 2 and values.shape[1] == 32)
+                or (values.dtype == np.uint32 and values.ndim == 2 and values.shape[1] == 8)):
+            raise ValueError("%s must be an (m,32) uint8 or (m,8) uint32 array, got %s %s"
+                             % (name, values.dtype, values.shape))
+        m = values.shape[0]
+    else:
+        try:
+            m = len(values)
+        except TypeError:
+            raise ValueError("%s must be a sequence of field elements or an array" % name) from None
+    if m > n:
+        raise ValueError("%s has %d rows, the circuit %d" % (name, m, n))
+    return _as_le_rows(values, n)
+
+
 def _pts(raw: bytes, count: int):
     return [(FQ(int.from_bytes(raw[64 * k:64 * k + 32], "little")),
              FQ(int.from_bytes(raw[64 * k + 32:64 * k + 64], "little"))) for k in range(count)]
@@ -262,6 +285,7 @@ class Prover:
         keep = [to_le_rows(q_in), to_le_rows(q_out)]
         _lib.check(_lib.lib().pb200_prover_set_shuffle(self._h, *[k.ctypes.data_as(ctypes.c_void_p) for k in keep]))
         self._kind = proof_kind(next_row=self.next_row, shuffle=True)
+        self._shuffle = tuple(k[:, 0] != 0 for k in keep)  # for WitnessReport's counts of a tuple on each side
 
     def _set_lookup(self, qk, cols, rows):
         keep = [to_le_rows(qk)] + [to_le_rows(c) for c in cols]
@@ -340,6 +364,66 @@ class Prover:
                    pub.shape[0], out)
         return out.raw
 
+    # ------------------------------------------------------------------ witness check
+    def check_arrays(self, A, B, C, public, limit: int = 16) -> WitnessReport:
+        """Check a witness against this prover's key without proving: every failing gate, copy constraint, lookup row
+        and shuffle row, each category as an exact count and its lowest ``limit`` locations (``WitnessReport``).  The
+        report is empty iff rounds 1 and 2 of ``prove_arrays`` pass their checks.  Draws no blinders and changes no
+        later proof.  A, B, C as for ``prove_arrays`` (lists of ints, or (m,32) uint8 / (m,8) uint32 arrays, m <= n,
+        zero padded), or (n,32) uint8 CUDA tensors on the prover's device, which stay there.  The first check of a
+        prover builds the copy permutation on the device and keeps it (12 bytes a row).  ValueError for malformed
+        inputs, before the library is called; the library refuses values not reduced below r and the sharded
+        prover."""
+        return self._check(A, B, C, public, limit)
+
+    def _check(self, A, B, C, public, limit, names=None) -> WitnessReport:
+        """check_arrays; names(row, col) -> the variable of a cell, for this report only"""
+        n = self.group_order
+        if isinstance(limit, bool) or not isinstance(limit, (int, np.integer)) or not 0 <= limit <= 3 * n:
+            raise ValueError("limit must be an integer in [0, 3n = %d], got %r" % (3 * n, limit))
+        limit = int(limit)
+        if len(public) > n:
+            raise ValueError("%d public inputs for %d rows" % (len(public), n))
+        on_device = [_is_cuda_tensor(X) for X in (A, B, C)]
+        if any(on_device) and not all(on_device):
+            raise ValueError("A, B and C must all be CUDA tensors or all be host values")
+        if all(on_device):
+            for name, X in zip("ABC", (A, B, C)):
+                if tuple(X.shape) != (n, 32) or str(X.dtype) != "torch.uint8" or not X.is_contiguous():
+                    raise ValueError("%s must be a contiguous (%d, 32) uint8 tensor, got %s %s"
+                                     % (name, n, tuple(X.shape), X.dtype))
+                if X.device.index != self.ctx.device:
+                    raise ValueError("%s is on cuda:%s, the prover on cuda:%d" % (name, X.device.index, self.ctx.device))
+            import torch
+            for X in (A, B, C):
+                torch.cuda.current_stream(X.device).synchronize()  # the library runs on its own stream
+            ptrs = [ctypes.c_void_p(X.data_ptr()) for X in (A, B, C)]
+            entry, wires = "pb200_prover_check_device", None
+        else:
+            wires = tuple(_wire_rows(name, X, n) for name, X in zip("ABC", (A, B, C)))
+            ptrs = [w.ctypes.data_as(ctypes.c_void_p) for w in wires]
+            entry = "pb200_prover_check"
+        pub = _as_le_rows([int(x) % CURVE_ORDER for x in public], len(public)) if len(public) else \
+            np.zeros((0, 32), np.uint8)
+        counts = (ctypes.c_uint64 * 5)()
+        lists = (ctypes.c_uint32 * max(1, 6 * limit))()
+        _lib.check(getattr(_lib.lib(), entry)(self._h, *ptrs, pub.ctypes.data_as(ctypes.c_void_p), pub.shape[0], limit,
+                                               counts, lists))
+        if wires is None and any(counts):  # the values the report prints
+            wires = tuple(X.cpu().numpy() for X in (A, B, C))
+        return WitnessReport._from_library(counts, lists[:6 * limit], limit, wires, getattr(self, "_shuffle", None),
+                                           names)
+
+    def check(self, witness, limit: int = 16) -> WitnessReport:
+        """``check_arrays`` for a prover made from a reference ``Program``, with the witness dict ``prove`` takes; the
+        report names each copy-constraint cell by its variable (``program.wires()``)."""
+        if self.program is None:
+            raise ValueError("check(witness) needs a prover made from a Program; use check_arrays")
+        A, B, C, public = self._witness_columns(witness)
+        wires = self.program.wires()
+        return self._check(A, B, C, public, limit,
+                           lambda row, col: getattr(wires[row], "LRO"[col]) if row < len(wires) else None)
+
     # ------------------------------------------------------------------ the reference's surface
     def prove(self, witness) -> Proof:
         """prover.py:51-84, following the schedule of the prover's kind (transcript.py) and returning its proof class:
@@ -362,16 +446,19 @@ class Prover:
             values.update((f.name, getattr(m, f.name)) for f in fields(m))
         return kind.proof._from_values(values)
 
-    def round_1(self, witness) -> Message1:
-        """prover.py:86-119."""
+    def _witness_columns(self, witness):
+        """prover.py:86-103: a witness dict (variable -> value) -> the wire columns A, B, C and the public inputs"""
         if None not in witness:
             witness[None] = 0
         wires = self.program.wires()
-        n = self.group_order
         A = [int(witness[w.L]) % CURVE_ORDER for w in wires]
         B = [int(witness[w.R]) % CURVE_ORDER for w in wires]
         C = [int(witness[w.O]) % CURVE_ORDER for w in wires]
-        self._public = [int(witness[v]) % CURVE_ORDER for v in self.program.get_public_assignments()]
+        return A, B, C, [int(witness[v]) % CURVE_ORDER for v in self.program.get_public_assignments()]
+
+    def round_1(self, witness) -> Message1:
+        """prover.py:86-119."""
+        A, B, C, self._public = self._witness_columns(witness)
         return self.round_1_arrays(A, B, C, self._public)
 
     def round_1_arrays(self, A, B, C, public) -> Message1:
