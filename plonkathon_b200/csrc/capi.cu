@@ -36,6 +36,7 @@ void srs_export(Context* ctx, Srs* srs, uint8_t* h_points, uint64_t first, uint6
 void srs_msm(Context* ctx, Srs* srs, const Fr* d_scalars, uint64_t m, bool scalars_mont, uint8_t* out_xy, int* is_identity);
 uint64_t srs_size(Srs* s);
 uint32_t msm_default_window(uint64_t n, bool fixed_base);
+void msm_init_device();
 void msm_run(Context* ctx, const G1Affine* points, uint64_t n, const Fr* scalars, bool scalars_mont, uint32_t c,
              bool fixed_base, uint64_t point_stride, uint8_t* out_xy, int* is_identity);
 void affine_to_mont(Context* ctx, const G1Affine* in, G1Affine* out, uint64_t n);
@@ -222,6 +223,11 @@ int pb200_ctx_create(int device, void* cuda_stream, pb200_ctx** out) {
     PB_CUDA(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
     ctx->own_stream = true;
   }
+  int prio_least = 0, prio_greatest = 0;
+  PB_CUDA(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
+  PB_CUDA(cudaStreamCreateWithPriority(&ctx->prio_stream, cudaStreamNonBlocking, prio_greatest));
+  PB_CUDA(cudaEventCreateWithFlags(&ctx->join_ev, cudaEventDisableTiming));
+  msm_init_device();
   *out = reinterpret_cast<pb200_ctx*>(ctx.release());
   PB_API_END
 }

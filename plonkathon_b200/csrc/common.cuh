@@ -76,6 +76,10 @@ struct Context {
   cudaEvent_t aux_ev[4] = {nullptr, nullptr, nullptr, nullptr};
   cudaStream_t copy_stream = nullptr;   // host->device staging that overlaps compute on `stream`
   cudaEvent_t copy_done[4] = {nullptr, nullptr, nullptr, nullptr};
+  // the device's highest stream priority: the MSM phases that hardly use the integer multiplier (sort, stitch, upper
+  // reduction levels), so that their blocks are dispatched ahead of another context's bucket accumulation (msm.cu)
+  cudaStream_t prio_stream = nullptr;
+  cudaEvent_t join_ev = nullptr;        // orders `stream` and `prio_stream` (stream_join)
   int sm_count = 132;
   std::map<int, std::unique_ptr<NttPlan>> plans;  // key: log_n * 2 + inverse
   DevBuf scratch[10];                              // reusable temporaries
@@ -84,25 +88,32 @@ struct Context {
   DevBuf gather;                                   // receive buffer of the sharded transforms' allgather
   std::map<int, std::unique_ptr<ShardTables>> shard_tables;  // per (log_n, inverse): twiddles of the sharded NTT join
   uint64_t launches = 0;                           // kernels launched through this context
-  // optional per-kernel timing (bench.py roofline): CUDA event pairs on the launching stream
+  // optional per-kernel timing (bench.py roofline): CUDA event pairs on the stream the phase runs on (default:
+  // `stream`)
   bool timing = false;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> timed[4];  // 0: MSM bucket accumulate, 1: NTT passes
-  void time_begin(int cat) {
+  void time_begin(int cat, cudaStream_t on = nullptr) {
     if (!timing) return;
     cudaEvent_t a, b;
     cudaEventCreate(&a);
     cudaEventCreate(&b);
-    cudaEventRecord(a, stream);
+    cudaEventRecord(a, on ? on : stream);
     timed[cat].push_back({a, b});
   }
-  void time_end(int cat) {
+  void time_end(int cat, cudaStream_t on = nullptr) {
     if (!timing) return;
-    cudaEventRecord(timed[cat].back().second, stream);
+    cudaEventRecord(timed[cat].back().second, on ? on : stream);
   }
   Context();
   ~Context();
 };
 
 NttPlan* get_plan(Context* ctx, int log_n, bool inverse);
+
+// `waiter` runs nothing enqueued after this call before everything enqueued on `producer` so far has finished
+inline void stream_join(Context* ctx, cudaStream_t waiter, cudaStream_t producer) {
+  PB_CUDA(cudaEventRecord(ctx->join_ev, producer));
+  PB_CUDA(cudaStreamWaitEvent(waiter, ctx->join_ev, 0));
+}
 
 }  // namespace pb200

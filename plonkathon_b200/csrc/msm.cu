@@ -20,6 +20,15 @@
 //   6. the few remaining group operations (last <= 8 reduction pairs, bucket-range offset or the join of the ranks'
 //      shares, window Horner, one inversion to affine) on the host, which has to read the point anyway to feed the
 //      Fiat-Shamir transcript.
+// Streams: steps 1-3, the stitch of step 4 and the upper levels of step 5 run on the context's high-priority stream,
+// the accumulation and reduction level 0 on its main stream, joined by events, so the order of work is unchanged.
+// With two contexts proving at once, the blocks of these short phases then take the SM slots that the other
+// context's retiring accumulation blocks free, instead of waiting for its whole grid to drain (traces before and
+// after, and what they gained: DESIGN.md section 5, profiles/h100_inflight_trace.md).  A retiring accumulation block
+// frees 128 x 128 = 16,384 registers and no shared memory.  The bin kernels are held to 32 registers at 512 threads
+// and the stitch kernels to 128 at 128 threads so that one block fits there.  k_reduce_block (168 registers at 128
+// threads) needs the slots of two: capped at 128 registers it spills 224 bytes per thread in its chains of dependent
+// additions, so it is left as it is.
 // Multi-GPU: a call may own a sub-range of the buckets of every bucket set -- contiguous [bucket_lo, bucket_hi), or,
 // with a communicator, every G-th bucket -- it walks all digits but sorts, accumulates and reduces only its own
 // buckets, so the whole MSM (not just the accumulation) divides by the number of ranks; and/or a POINT RANGE (a
@@ -77,7 +86,7 @@ __device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t v, uint32_t* s
 }
 
 // ---- two-level counting sort of the bucket entries (msm_sort.cuh holds the thread bodies) -----------------------
-__global__ void __launch_bounds__(PB_SORT_BIN_THREADS) k_msm_bin_count(SortArgs a) {
+__global__ void __launch_bounds__(PB_SORT_BIN_THREADS, 4) k_msm_bin_count(SortArgs a) {
   __shared__ uint32_t sh_cnt[PB_SORT_MAX_BINS];
   const uint32_t t = threadIdx.x, nt = blockDim.x;
   sort_zero(sh_cnt, a.nbins, t, nt);
@@ -88,7 +97,7 @@ __global__ void __launch_bounds__(PB_SORT_BIN_THREADS) k_msm_bin_count(SortArgs 
 }
 
 // dynamic shared memory: the stage, PB_SORT_BIN_STAGE entries
-__global__ void __launch_bounds__(PB_SORT_BIN_THREADS) k_msm_bin_scatter(SortArgs a) {
+__global__ void __launch_bounds__(PB_SORT_BIN_THREADS, 4) k_msm_bin_scatter(SortArgs a) {
   __shared__ uint32_t sh_cnt[PB_SORT_MAX_BINS], sh_loc[PB_SORT_MAX_BINS], sh_base[PB_SORT_MAX_BINS], sh_scan[32];
   extern __shared__ SortEntry stage[];
   const uint32_t t = threadIdx.x, nt = blockDim.x;
@@ -300,7 +309,7 @@ struct HeavyPiece { uint32_t item, index; };
 
 // one thread per segment: if it owns a boundary-crossing bucket, stitch it (or queue it as heavy; a bucket that
 // spans more than PB_STITCH_PIECE segments is also cut into pieces that k_msm_stitch_pieces sums block by block)
-__global__ void __launch_bounds__(128) k_msm_stitch(const uint32_t* offsets, uint32_t nb, uint32_t L,
+__global__ void __launch_bounds__(128, 4) k_msm_stitch(const uint32_t* offsets, uint32_t nb, uint32_t L,
                                                     uint32_t n_segments, const G1XYZZ* slots,
                                                     const uint32_t* slot_bucket, const uint32_t* own_slot,
                                                     G1XYZZ* buckets, HeavyItem* heavy, uint32_t* heavy_count,
@@ -346,7 +355,7 @@ __device__ __forceinline__ void block_sum_xyzz(G1XYZZ* sh, const G1XYZZ& mine) {
 
 // pieces of very heavy buckets: one block each (grid-stride over the piece list): partial[p] = sum of the first-run
 // slots of the piece's segments
-__global__ void __launch_bounds__(128) k_msm_stitch_pieces(const G1XYZZ* slots, const HeavyItem* heavy,
+__global__ void __launch_bounds__(128, 4) k_msm_stitch_pieces(const G1XYZZ* slots, const HeavyItem* heavy,
                                                            const uint32_t* heavy_count, const HeavyPiece* pieces,
                                                            G1XYZZ* partial) {
   __shared__ G1XYZZ sh[128];
@@ -368,7 +377,7 @@ __global__ void __launch_bounds__(128) k_msm_stitch_pieces(const G1XYZZ* slots, 
 }
 
 // heavy buckets: one block each (grid-stride over the queue), strided partial sums + shared-memory tree
-__global__ void __launch_bounds__(128) k_msm_stitch_heavy(const G1XYZZ* slots, const HeavyItem* heavy,
+__global__ void __launch_bounds__(128, 4) k_msm_stitch_heavy(const G1XYZZ* slots, const HeavyItem* heavy,
                                                           const uint32_t* heavy_count, const G1XYZZ* partial,
                                                           G1XYZZ* buckets) {
   __shared__ G1XYZZ sh[128];
@@ -506,6 +515,14 @@ struct Srs {
 };
 
 static uint32_t windows_for(uint32_t c) { return (256 + c - 1) / c; }
+
+// Kernel attributes of the current device, set when a context (which is tied to one device) is created: the sort's
+// shared-memory stages
+void msm_init_device() {
+  PB_CUDA(cudaFuncSetAttribute(k_msm_bin_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)(PB_SORT_BIN_STAGE * sizeof(SortEntry))));
+  PB_CUDA(cudaFuncSetAttribute(k_msm_chunk_place, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(PB_SORT_CHUNK * 4)));
+}
 
 uint32_t msm_default_window(uint64_t n, bool fixed_base) {
   int lg = 0;
@@ -706,27 +723,29 @@ void msm_run_batch(Context* ctx, const G1Affine* points, uint64_t n, const Fr* c
   const uint32_t count_grid = (uint32_t)std::min<uint64_t>((uint64_t)ctx->sm_count * 4, chunk_bound);
   const uint32_t place_grid = (uint32_t)std::min<uint64_t>((uint64_t)ctx->sm_count * 2, chunk_bound);
   const size_t bin_stage_bytes = PB_SORT_BIN_STAGE * sizeof(SortEntry), chunk_stage_bytes = PB_SORT_CHUNK * 4;
-  // (a per-device setting: set on every call, as contexts of several devices may share the process)
-  PB_CUDA(cudaFuncSetAttribute(k_msm_bin_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bin_stage_bytes));
-  PB_CUDA(cudaFuncSetAttribute(k_msm_chunk_place, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)chunk_stage_bytes));
 
-  cudaStream_t st = ctx->stream;
-  ctx->time_begin(2);
-  PB_CUDA(cudaMemsetAsync(counts.p, 0, (size_t)g.nb * 4 + 16, st));
-  PB_CUDA(cudaMemsetAsync(bin_cnt, 0, (size_t)sa.nbins * 4, st));
-  if (pad) PB_CUDA(cudaMemsetAsync(sorted.p, 0xff, positions * 4, st));
-  k_msm_bin_count<<<bin_grid, PB_SORT_BIN_THREADS, 0, st>>>(sa);
-  k_scan_tile_sums<<<1, 256, 0, st>>>(bin_cnt, sa.nbins, 0, tile_sums, nullptr);
-  k_scan_tiles<<<1, 256, 0, st>>>(tile_sums, 1, bin_off + sa.nbins);
-  k_scan_apply<<<1, 256, 0, st>>>(bin_cnt, sa.nbins, 0, tile_sums, bin_off);
-  k_msm_bin_scatter<<<bin_grid, PB_SORT_BIN_THREADS, bin_stage_bytes, st>>>(sa);
-  k_msm_chunk_map<<<1, 256, 0, st>>>(sa);
-  k_msm_chunk_count<<<count_grid, PB_SORT_CHUNK_THREADS, 0, st>>>(sa);
-  k_scan_tile_sums<<<n_tiles, 256, 0, st>>>(counts.as<uint32_t>(), g.nb, pad, tile_sums, max_cnt);
-  k_scan_tiles<<<1, 256, 0, st>>>(tile_sums, n_tiles, offsets.as<uint32_t>() + g.nb);
-  k_scan_apply<<<n_tiles, 256, 0, st>>>(counts.as<uint32_t>(), g.nb, pad, tile_sums, offsets.as<uint32_t>());
-  k_msm_chunk_place<<<place_grid, PB_SORT_CHUNK_THREADS, chunk_stage_bytes, st>>>(sa);
-  ctx->time_end(2);
+  // The sort, the stitch and the upper reduction levels run on the context's high-priority stream, the accumulation
+  // and reduction level 0 (bound by field products) on its main stream; every phase still waits for the one before.
+  // Another context's accumulation fills the SMs with thousands of blocks: on the priority stream, these short
+  // phases get each SM slot that one of its blocks frees instead of waiting for that whole grid to drain.
+  cudaStream_t st = ctx->stream, ps = ctx->prio_stream;
+  stream_join(ctx, ps, st);  // the scalars, and the previous call's last readers of this scratch
+  ctx->time_begin(2, ps);
+  PB_CUDA(cudaMemsetAsync(counts.p, 0, (size_t)g.nb * 4 + 16, ps));
+  PB_CUDA(cudaMemsetAsync(bin_cnt, 0, (size_t)sa.nbins * 4, ps));
+  if (pad) PB_CUDA(cudaMemsetAsync(sorted.p, 0xff, positions * 4, ps));
+  k_msm_bin_count<<<bin_grid, PB_SORT_BIN_THREADS, 0, ps>>>(sa);
+  k_scan_tile_sums<<<1, 256, 0, ps>>>(bin_cnt, sa.nbins, 0, tile_sums, nullptr);
+  k_scan_tiles<<<1, 256, 0, ps>>>(tile_sums, 1, bin_off + sa.nbins);
+  k_scan_apply<<<1, 256, 0, ps>>>(bin_cnt, sa.nbins, 0, tile_sums, bin_off);
+  k_msm_bin_scatter<<<bin_grid, PB_SORT_BIN_THREADS, bin_stage_bytes, ps>>>(sa);
+  k_msm_chunk_map<<<1, 256, 0, ps>>>(sa);
+  k_msm_chunk_count<<<count_grid, PB_SORT_CHUNK_THREADS, 0, ps>>>(sa);
+  k_scan_tile_sums<<<n_tiles, 256, 0, ps>>>(counts.as<uint32_t>(), g.nb, pad, tile_sums, max_cnt);
+  k_scan_tiles<<<1, 256, 0, ps>>>(tile_sums, n_tiles, offsets.as<uint32_t>() + g.nb);
+  k_scan_apply<<<n_tiles, 256, 0, ps>>>(counts.as<uint32_t>(), g.nb, pad, tile_sums, offsets.as<uint32_t>());
+  k_msm_chunk_place<<<place_grid, PB_SORT_CHUNK_THREADS, chunk_stage_bytes, ps>>>(sa);
+  ctx->time_end(2, ps);
   ctx->launches += 11;
 
   ReduceArgs ra;
@@ -748,6 +767,7 @@ void msm_run_batch(Context* ctx, const G1Affine* points, uint64_t n, const Fr* c
     uint64_t cap = fixed_base ? n * g.W : n;
     uint32_t max_rounds = 1;
     while (max_rounds < 32 && (1ull << max_rounds) < cap) max_rounds++;
+    stream_join(ctx, st, ps);
     ctx->time_begin(0);
     for (uint32_t r = 0; r < std::min<uint32_t>(max_rounds, PB_AFF_GRID_ROUNDS); r++) {
       a.r = r;
@@ -795,20 +815,23 @@ void msm_run_batch(Context* ctx, const G1Affine* points, uint64_t n, const Fr* c
     uint32_t* heavy_count = own_slot + n_seg;  // [0] heavy items, [1] pieces
     HeavyItem* heavy = reinterpret_cast<HeavyItem*>(heavy_count + 4);
     HeavyPiece* pieces = reinterpret_cast<HeavyPiece*>(heavy + n_seg);
-    PB_CUDA(cudaMemsetAsync(buckets.p, 0, (size_t)g.nb * sizeof(G1XYZZ), st));
-    PB_CUDA(cudaMemsetAsync(own_slot, 0xff, (size_t)n_seg * 4, st));
-    PB_CUDA(cudaMemsetAsync(heavy_count, 0, 16, st));
+    PB_CUDA(cudaMemsetAsync(buckets.p, 0, (size_t)g.nb * sizeof(G1XYZZ), ps));
+    PB_CUDA(cudaMemsetAsync(own_slot, 0xff, (size_t)n_seg * 4, ps));
+    PB_CUDA(cudaMemsetAsync(heavy_count, 0, 16, ps));
+    stream_join(ctx, st, ps);
     ctx->time_begin(0);
     k_msm_seg_accumulate<<<(n_seg + 127) / 128, 128, 0, st>>>(points, offsets.as<uint32_t>(), sorted.as<uint32_t>(),
                                                              g.nb, L, buckets.as<G1XYZZ>(), slots, slot_bucket, own_slot);
     ctx->time_end(0);
-    k_msm_stitch<<<(n_seg + 127) / 128, 128, 0, st>>>(offsets.as<uint32_t>(), g.nb, L, n_seg, slots, slot_bucket,
+    stream_join(ctx, ps, st);
+    k_msm_stitch<<<(n_seg + 127) / 128, 128, 0, ps>>>(offsets.as<uint32_t>(), g.nb, L, n_seg, slots, slot_bucket,
                                                      own_slot, buckets.as<G1XYZZ>(), heavy, heavy_count, pieces, 16);
-    k_msm_stitch_pieces<<<std::min<uint32_t>(max_pieces, 592), 128, 0, st>>>(slots, heavy, heavy_count, pieces, piece_partial);
-    k_msm_stitch_heavy<<<296, 128, 0, st>>>(slots, heavy, heavy_count, piece_partial, buckets.as<G1XYZZ>());
+    k_msm_stitch_pieces<<<std::min<uint32_t>(max_pieces, 592), 128, 0, ps>>>(slots, heavy, heavy_count, pieces, piece_partial);
+    k_msm_stitch_heavy<<<296, 128, 0, ps>>>(slots, heavy, heavy_count, piece_partial, buckets.as<G1XYZZ>());
     ctx->launches += 4;
     ra.xb = buckets.as<G1XYZZ>();
   }
+  stream_join(ctx, st, ps);
 
   // bucket reduction: levels of grouped running sums until one (S, R) pair per set is left
   // level-0 group size: 16 buckets per thread when that still fills the machine, down to 4 for small bucket counts
@@ -833,6 +856,7 @@ void msm_run_batch(Context* ctx, const G1Affine* points, uint64_t n, const Fr* c
     k_reduce_level0<<<(unsigned)((groups + 127) / 128), 128, 0, st>>>(ra);
     ctx->launches++;
   }
+  stream_join(ctx, ps, st);
   uint32_t m = reduce_groups(ra.m, ra.g), log_G = log_g0;
   SR* cur = lvl_a.as<SR>();
   SR* nxt = lvl_b.as<SR>();
@@ -842,13 +866,14 @@ void msm_run_batch(Context* ctx, const G1Affine* points, uint64_t n, const Fr* c
   while (m > m_stop) {
     BlockLevelArgs ba;
     ba.in = cur; ba.out = nxt; ba.sets = g.sets; ba.m = m; ba.log_G = log_G;
-    k_reduce_block<<<dim3(reduce_chunks(m), g.sets), PB_REDUCE_THREADS, 0, st>>>(ba);
+    k_reduce_block<<<dim3(reduce_chunks(m), g.sets), PB_REDUCE_THREADS, 0, ps>>>(ba);
     ctx->launches++;
     m = reduce_chunks(m);
     log_G += 9;  // log2(PB_REDUCE_CHUNK)
     std::swap(cur, nxt);
   }
-  ctx->time_end(3);
+  ctx->time_end(3, ps);
+  stream_join(ctx, st, ps);  // the host reads the result on `st`
   PB_CUDA(cudaGetLastError());
   // the remaining m (<= 8) elements per set are folded on the host (reduce_fold_final)
   std::vector<G1XYZZ> ws(g.sets);

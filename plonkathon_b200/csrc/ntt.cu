@@ -490,6 +490,8 @@ Context::~Context() {
   for (auto& e : aux_ev) if (e) cudaEventDestroy(e);
   if (aux_stream) cudaStreamDestroy(aux_stream);
   if (copy_stream) cudaStreamDestroy(copy_stream);
+  if (join_ev) cudaEventDestroy(join_ev);
+  if (prio_stream) cudaStreamDestroy(prio_stream);
   if (own_stream && stream) cudaStreamDestroy(stream);
 }
 
