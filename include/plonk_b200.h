@@ -158,6 +158,30 @@ int pb200_srs_commit_coeffs_host(pb200_ctx* ctx, pb200_srs* srs, const uint8_t* 
  * than is free (naming the bytes needed: 176 n bytes + the sort's temporary storage). */
 int pb200_permutation(pb200_ctx* ctx, const int64_t* h_ids, int log_n, uint8_t* h_S);
 
+/* The wire values A, B, C of a circuit from the values of its input variables, the way the reference runs a program
+ * (compiler/program.py:161-192).  h_ids: 3n variable ids as pb200_permutation takes them; rows from n_constraints on
+ * are unused (their ids are not read).  h_sel: QL, QR, QM, QO, QC (n canonical 32-byte little-endian values each);
+ * n_custom custom gate terms as six exponents each (i, j, l, i', j', l') in h_exps, their selectors in h_custom.
+ * n_inputs variables with given values: ids in h_input_ids, canonical values in h_input_values (32 bytes each).
+ * A row r < n_constraints defines its O variable v when v is not -1, QO[r] != 0, no term whose selector is non-zero at
+ * r reads c or the next row, v is no input and no earlier row defines v; it sets
+ * c = -(QL a + QR b + QM a b + QC + sum_k Q_k a^i b^j) / QO.  Unused cells get 0.
+ * h_counts[2]: the exact number of
+ *   unset  cells whose variable is neither an input nor defined by a row,
+ *   order  L or R cells of a defining row whose variable that row or a later row defines;
+ * h_lists (3 limit uint32): the lowest `limit` unset cells (3 row + col), then `limit` (cell, defining row) pairs of
+ * order cells, ascending, unused entries 0xffffffff.  With either count non-zero nothing is written to `out`;
+ * otherwise out[0..2] get A, B, C (n canonical values each): device buffers when out_on_device, else host buffers.
+ * Runs on the context's stream and frees its device memory before returning.  Refuses, before any device work, log_n
+ * outside 1..26, an id out of range (naming its cell), an input id out of range, two inputs naming one variable, an
+ * input value not reduced below r and more device memory than is free or than PB200_SOLVE_MAX_BYTES allows (naming the
+ * bytes needed); afterwards, a selector value not reduced below r. */
+int pb200_solve_wires(pb200_ctx* ctx, const int64_t* h_ids, int log_n, uint64_t n_constraints,
+                      const uint8_t* const* h_sel, unsigned n_custom, const uint8_t* h_exps,
+                      const uint8_t* const* h_custom, uint64_t n_inputs, const int64_t* h_input_ids,
+                      const uint8_t* h_input_values, uint32_t limit, uint64_t* h_counts, uint32_t* h_lists,
+                      void* const* out, int out_on_device);
+
 /* ---- Prover (prover.py:39-306) ---------------------------------------------------------------- */
 /* Proof layout.  A prover's proof is the plain 15 fields, then the fields of the blocks it has (next-row custom gate
  * terms, a shuffle, a lookup argument), in this order; a point is 64 bytes (x||y), a scalar 32, big-endian in a proof
@@ -254,6 +278,9 @@ int pb200_prover_round4_lookup(pb200_prover* p, const uint8_t* zeta, uint8_t* h_
 /* the whole proof (1216 bytes, Proof layout) */
 int pb200_prover_prove_lookup(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                               const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof1216);
+/* same, with the wire values already resident in HBM (canonical form, n x 32 bytes each) */
+int pb200_prover_prove_device_lookup(pb200_prover* p, const void* d_A, const void* d_B, const void* d_C,
+                                     const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof1216);
 int pb200_prover_serialize_lookup(pb200_prover* p, uint8_t* h_proof1216);
 /* Zero-knowledge lookup proofs for every later proof of a lookup prover (one table or several): enable != 0 blinds A,
  * B, C, Z and the quotient pieces as pb200_prover_set_zk does, and F, H1, H2, Z2 with 10 more scalars (21 in all,
@@ -283,6 +310,9 @@ int pb200_prover_round4_next_row(pb200_prover* p, const uint8_t* zeta, uint8_t* 
 /* the whole proof (864 bytes, Proof layout) */
 int pb200_prover_prove_next_row(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                                 const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof864);
+/* same, with the wire values already resident in HBM (canonical form, n x 32 bytes each) */
+int pb200_prover_prove_device_next_row(pb200_prover* p, const void* d_A, const void* d_B, const void* d_C,
+                                       const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof864);
 int pb200_prover_serialize_next_row(pb200_prover* p, uint8_t* h_proof864);
 
 /* Shuffle argument: two fixed boolean selectors q_in, q_out (n x 32-byte canonical Fr, 0 or 1 on every row, as many
@@ -314,9 +344,15 @@ int pb200_prover_round4_shuffle(pb200_prover* p, const uint8_t* zeta, uint8_t* h
 int pb200_prover_round4_next_row_shuffle(pb200_prover* p, const uint8_t* zeta, uint8_t* h_evals /*11*32*/);
 int pb200_prover_prove_shuffle(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                                const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof896);
+/* same, with the wire values already resident in HBM (canonical form, n x 32 bytes each) */
+int pb200_prover_prove_device_shuffle(pb200_prover* p, const void* d_A, const void* d_B, const void* d_C,
+                                      const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof896);
 int pb200_prover_serialize_shuffle(pb200_prover* p, uint8_t* h_proof896);
 int pb200_prover_prove_next_row_shuffle(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                                         const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof992);
+/* same, with the wire values already resident in HBM (canonical form, n x 32 bytes each) */
+int pb200_prover_prove_device_next_row_shuffle(pb200_prover* p, const void* d_A, const void* d_B, const void* d_C,
+                                               const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof992);
 int pb200_prover_serialize_next_row_shuffle(pb200_prover* p, uint8_t* h_proof992);
 
 /* ---- Witness check: every failing constraint, without proving -------------------------------------------------------

@@ -11,3 +11,4 @@ from .transcript import Transcript, Message1, Message2, Message3, Message4, Mess
 from .prover import Prover, Proof, LookupProof, NextRowProof, ShuffleProof, NextRowShuffleProof  # noqa: F401
 from .wiring import permutation_arrays  # noqa: F401
 from .witness import WitnessReport  # noqa: F401
+from .solve import WireSolution, solve_wires  # noqa: F401

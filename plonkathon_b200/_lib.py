@@ -121,6 +121,11 @@ def _load():
         "pb200_permutation": (I, [V, V, I, V]),
         "pb200_prover_check": (I, [V, V, V, V, V, U64, ctypes.c_uint32, V, V]),
         "pb200_prover_check_device": (I, [V, V, V, V, V, U64, ctypes.c_uint32, V, V]),
+        "pb200_solve_wires": (I, [V, V, I, U64, V, U, V, V, U64, V, V, ctypes.c_uint32, V, V, V, I]),
+        "pb200_prover_prove_device_lookup": (I, [V, V, V, V, V, U64, V]),
+        "pb200_prover_prove_device_next_row": (I, [V, V, V, V, V, U64, V]),
+        "pb200_prover_prove_device_shuffle": (I, [V, V, V, V, V, U64, V]),
+        "pb200_prover_prove_device_next_row_shuffle": (I, [V, V, V, V, V, U64, V]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)  # AttributeError here == ABI drift: fail loudly

@@ -67,6 +67,11 @@ void prover_check(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t
                   uint64_t n_public, uint32_t limit, uint64_t* h_counts, uint32_t* h_lists, bool wires_on_device);
 // permutation.cu
 void permutation_run(Context* ctx, const int64_t* h_ids, int log_n, uint8_t* h_S);
+// solve.cu
+void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constraints, const uint8_t* const* h_sel,
+               int n_custom, const uint8_t* h_exps, const uint8_t* const* h_custom, uint64_t n_inputs,
+               const int64_t* h_in_ids, const uint8_t* h_in_vals, uint32_t limit, uint64_t* h_counts,
+               uint32_t* h_lists, void* const* out, bool out_on_device);
 // ptau.cu
 Srs* srs_create_ptau(Context* ctx, const uint8_t* h_g1, uint64_t count, const uint8_t* h_tau_g2, int precompute);
 Srs* srs_create_ptau_lagrange(Context* ctx, const uint8_t* h_block, uint64_t n, Srs* monomial, int precompute);
@@ -578,6 +583,16 @@ int pb200_permutation(pb200_ctx* ctx, const int64_t* h_ids, int log_n, uint8_t* 
   permutation_run(C(ctx), h_ids, log_n, h_S);
   PB_API_END
 }
+int pb200_solve_wires(pb200_ctx* ctx, const int64_t* h_ids, int log_n, uint64_t n_constraints,
+                      const uint8_t* const* h_sel, unsigned n_custom, const uint8_t* h_exps,
+                      const uint8_t* const* h_custom, uint64_t n_inputs, const int64_t* h_input_ids,
+                      const uint8_t* h_input_values, uint32_t limit, uint64_t* h_counts, uint32_t* h_lists,
+                      void* const* out, int out_on_device) {
+  PB_API_BEGIN PB_ON_CTX(C(ctx));
+  solve_run(C(ctx), h_ids, log_n, n_constraints, h_sel, (int)n_custom, h_exps, h_custom, n_inputs, h_input_ids,
+            h_input_values, limit, h_counts, h_lists, out, out_on_device != 0);
+  PB_API_END
+}
 
 void pb200_prover_destroy(pb200_prover* p) { prover_destroy(reinterpret_cast<Prover*>(p)); }
 int pb200_prover_sliced(pb200_prover* p, int* out) {
@@ -684,6 +699,10 @@ int pb200_prover_prove_lookup(pb200_prover* p, const uint8_t* h_A, const uint8_t
                               const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof1216) {
   return prove(p, BLOCK_LOOKUP, h_A, h_B, h_C, h_public, n_public, h_proof1216);
 }
+int pb200_prover_prove_device_lookup(pb200_prover* p, const void* d_A, const void* d_B, const void* d_C,
+                                     const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof1216) {
+  return prove(p, BLOCK_LOOKUP, d_A, d_B, d_C, h_public, n_public, h_proof1216, true);
+}
 int pb200_prover_serialize_lookup(pb200_prover* p, uint8_t* h_proof1216) {
   return serialize(p, BLOCK_LOOKUP, h_proof1216);
 }
@@ -693,6 +712,10 @@ int pb200_prover_round4_next_row(pb200_prover* p, const uint8_t* zeta, uint8_t* 
 int pb200_prover_prove_next_row(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                                 const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof864) {
   return prove(p, BLOCK_NEXT_ROW, h_A, h_B, h_C, h_public, n_public, h_proof864);
+}
+int pb200_prover_prove_device_next_row(pb200_prover* p, const void* d_A, const void* d_B, const void* d_C,
+                                       const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof864) {
+  return prove(p, BLOCK_NEXT_ROW, d_A, d_B, d_C, h_public, n_public, h_proof864, true);
 }
 int pb200_prover_serialize_next_row(pb200_prover* p, uint8_t* h_proof864) {
   return serialize(p, BLOCK_NEXT_ROW, h_proof864);
@@ -716,12 +739,20 @@ int pb200_prover_prove_shuffle(pb200_prover* p, const uint8_t* h_A, const uint8_
                                const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof896) {
   return prove(p, BLOCK_SHUFFLE, h_A, h_B, h_C, h_public, n_public, h_proof896);
 }
+int pb200_prover_prove_device_shuffle(pb200_prover* p, const void* d_A, const void* d_B, const void* d_C,
+                                      const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof896) {
+  return prove(p, BLOCK_SHUFFLE, d_A, d_B, d_C, h_public, n_public, h_proof896, true);
+}
 int pb200_prover_serialize_shuffle(pb200_prover* p, uint8_t* h_proof896) {
   return serialize(p, BLOCK_SHUFFLE, h_proof896);
 }
 int pb200_prover_prove_next_row_shuffle(pb200_prover* p, const uint8_t* h_A, const uint8_t* h_B, const uint8_t* h_C,
                                         const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof992) {
   return prove(p, BLOCK_NEXT_ROW | BLOCK_SHUFFLE, h_A, h_B, h_C, h_public, n_public, h_proof992);
+}
+int pb200_prover_prove_device_next_row_shuffle(pb200_prover* p, const void* d_A, const void* d_B, const void* d_C,
+                                               const uint8_t* h_public, uint64_t n_public, uint8_t* h_proof992) {
+  return prove(p, BLOCK_NEXT_ROW | BLOCK_SHUFFLE, d_A, d_B, d_C, h_public, n_public, h_proof992, true);
 }
 int pb200_prover_serialize_next_row_shuffle(pb200_prover* p, uint8_t* h_proof992) {
   return serialize(p, BLOCK_NEXT_ROW | BLOCK_SHUFFLE, h_proof992);

@@ -13,6 +13,8 @@
 #include "proof_layout.cuh"
 #include "memory_plan.cuh"
 #include "permutation.cuh"
+#include "solve.cuh"
+#include <unordered_map>
 #include <algorithm>
 #include <vector>
 #include <cstring>
@@ -595,5 +597,59 @@ int64_t hs_permutation(const int64_t* ids, int log_n, const uint32_t* omega, uin
   for (uint64_t k = 0; k < m; k++) perm_label(a, k);
   for (uint64_t k = 0; k < m; k++) st(out + 8 * k, S[k]);
   return -1;
+}
+}
+
+extern "C" {
+// The wire solver of solve.cu on the CPU: the rows in row order, each defining row through the same solve_gate body.
+// ids: 3n ids, row-major L R O, rows from m on unused; sel: QL QR QM QO QC (n canonical values each, 8 words a value);
+// exps: six exponents per custom term, custom: their selectors; inputs: n_in ids and canonical values.  out: A | B | C.
+// Returns 0, or 1 when a cell has no value (unset, or read by a defining row before its variable is defined).
+int hs_solve(const int64_t* ids, int log_n, uint64_t m, const uint32_t* sel, int n_custom, const uint8_t* exps,
+             const uint32_t* custom, uint64_t n_in, const int64_t* in_ids, const uint32_t* in_vals, uint32_t* out) {
+  const uint64_t n = (uint64_t)1 << log_n;
+  uint8_t f[PB_MAX_CUSTOM][3];
+  for (int k = 0; k < n_custom; k++) {
+    int s = 0;
+    for (int w = 0; w < 6; w++)
+      for (int t = 0; t < exps[6 * k + w]; t++) f[k][s++] = (uint8_t)w;
+    while (s < 3) f[k][s++] = PB_FACTOR_ONE;
+  }
+  auto col = [&](const uint32_t* base, uint64_t c, uint64_t r) { return fp_to_mont(ld<Fr>(base + 8 * (c * n + r))); };
+  std::unordered_map<int64_t, Fr> val;
+  for (uint64_t k = 0; k < n_in; k++) val[in_ids[k]] = fp_to_mont(ld<Fr>(in_vals + 8 * k));
+  auto get = [&](int64_t id, Fr* x) {
+    if (id < 0) { *x = Fr::zero(); return true; }
+    auto it = val.find(id);
+    if (it == val.end()) return false;
+    *x = it->second;
+    return true;
+  };
+  for (uint64_t r = 0; r < m; r++) {
+    const int64_t v = ids[3 * r + 2];
+    SolveRow row;
+    const Fr qo = col(sel, 3, r);
+    bool defines = v >= 0 && !qo.is_zero() && !val.count(v);
+    for (int k = 0; k < n_custom; k++) {
+      row.q[k] = col(custom, k, r);
+      if (solve_term_reads_c(f[k]) && !row.q[k].is_zero()) defines = false;
+    }
+    if (!defines) continue;
+    Fr a, b;
+    if (!get(ids[3 * r], &a) || !get(ids[3 * r + 1], &b)) return 1;
+    row.ql = col(sel, 0, r);
+    row.qr = col(sel, 1, r);
+    row.qm = col(sel, 2, r);
+    row.qc = col(sel, 4, r);
+    row.neg_inv_qo = fp_neg(fp_inv_gcd(qo));
+    val[v] = solve_gate(row, f, n_custom, a, b);
+  }
+  for (uint64_t c = 0; c < 3 * n; c++) {
+    const uint64_t r = c / 3, w = c - 3 * r;
+    Fr x = Fr::zero();
+    if (r < m && !get(ids[c], &x)) return 1;
+    st(out + 8 * (w * n + r), fp_from_mont(x));
+  }
+  return 0;
 }
 }

@@ -1,0 +1,440 @@
+// Wire values A, B, C of a circuit from the values of its input variables (pb200_solve_wires), the way the reference
+// runs a program (compiler/program.py:161-192), on the GPU.  solve.cuh has the gate body; DESIGN.md section 3 the rule.
+//
+//   1. group:    the 3n cells' keys (id + 1) << cb | cell are sorted as permutation.cu sorts them (perm_sort_keys); each
+//                run of one id is one variable, numbered densely by an inclusive sum of the run heads.
+//   2. source:   a variable is the constant 0 (id -1), an input (binary search of the sorted input ids), or defined by
+//                the lowest row whose O cell carries it and that may define (k_solve_qualify): runs are in cell order,
+//                so an atomicMin over the run's qualifying O cells finds it.  Errors, per cell in cell order:
+//                  unset  the variable is neither an input nor defined by any row;
+//                  order  an L or R cell of a defining row whose variable that row or a later one defines.
+//                Each kind is an exact count and its lowest `limit` cells (cub::DeviceSelect::Flagged, as check.cu).
+//   3. divisor:  1 / QO of every row by one batched inversion (k_batch_div); the body negates it.
+//   4. evaluate: k_solve_eval, persistent: each warp takes the next 32 defining rows in row order through one global
+//                ticket; a lane computes its row once the ready flags of its L and R variables are set (acquire), then
+//                stores c and sets its O variable's flag (release).  A lane whose operand a lower lane of its warp
+//                defines sees it on a later pass of the warp's loop.  Every wait is bounded: a warp that makes no
+//                progress for PB_SOLVE_STALL_NS sets the stall flag, and every warp leaves on it.
+//   5. write:    every cell gets its variable's value, canonical, in A | B | C.
+// Device memory: about 430 bytes a row plus the outputs (DESIGN.md section 2), all freed before the call returns.
+#include <algorithm>
+#include <cuda/atomic>
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
+#include <cub/device/device_select.cuh>
+#include <thrust/iterator/counting_iterator.h>
+
+#include "common.cuh"
+#include "permutation.cuh"
+#include "solve.cuh"
+
+namespace pb200 {
+// poly_ops.cu
+void fr_to_mont(Context* ctx, const Fr* in, Fr* out, uint64_t n);
+void fr_from_mont(Context* ctx, const Fr* in, Fr* out, uint64_t n);
+// prover.cu
+__global__ void k_batch_div(const Fr* num, const Fr* den, Fr* out, uint64_t n, uint64_t T);
+__global__ void k_count_noncanonical(const Fr* v, uint64_t n, uint32_t* bad);
+// permutation.cu
+void perm_require_ids(const int64_t* h_ids, uint64_t m, int64_t* max_id);
+uint64_t* perm_sort_keys(Context* ctx, const int64_t* h_ids, uint64_t m, int cb, int end_bit, DevBuf& keys, DevBuf& alt,
+                         DevBuf& temp, size_t temp_bytes, uint64_t m_ids);
+
+#define PB_SOLVE_GRID(n, t) (unsigned)(((n) + (t)-1) / (t)), (t)
+#define PB_SOLVE_BATCH_CH 16              // k_batch_div's chain length (PB_BATCH_CH)
+#define PB_SOLVE_STALL_NS 10000000000ull  // 10 s without progress of a warp: the evaluation has stalled
+
+__device__ __forceinline__ Fr sv_ld(const Fr* p) {
+  const uint4* q = reinterpret_cast<const uint4*>(p);
+  uint4 a = __ldg(q), b = __ldg(q + 1);
+  Fr r;
+  r.v[0] = a.x; r.v[1] = a.y; r.v[2] = a.z; r.v[3] = a.w;
+  r.v[4] = b.x; r.v[5] = b.y; r.v[6] = b.z; r.v[7] = b.w;
+  return r;
+}
+
+struct SolveSel {
+  const Fr *ql, *qr, *qm, *qo, *qc, *inv_qo;  // Montgomery, n each
+  const Fr* q[PB_MAX_CUSTOM];
+  uint8_t f[PB_MAX_CUSTOM][3];
+  int n_custom;
+};
+
+// one flag per row: r < n_rows, QO != 0 and no term whose selector is non-zero at r reads c or the next row
+__global__ void k_solve_qualify(SolveSel s, uint64_t n_rows, uint8_t* qual) {
+  const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_rows) return;
+  bool ok = !sv_ld(s.qo + r).is_zero();
+#pragma unroll
+  for (int k = 0; k < PB_MAX_CUSTOM; k++)
+    if (k < s.n_custom && solve_term_reads_c(s.f[k]) && !sv_ld(s.q[k] + r).is_zero()) ok = false;
+  qual[r] = ok ? 1 : 0;
+}
+
+__global__ void k_solve_heads(const uint64_t* keys, uint64_t m, int cb, uint32_t* head) {
+  const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < m) head[k] = (k == 0 || (keys[k] >> cb) != (keys[k - 1] >> cb)) ? 1 : 0;
+}
+
+// sorted position k: its cell's variable; at a run head the variable's input (binary search of the sorted input ids,
+// PB_SOLVE_NONE without one, PB_SOLVE_ZERO for id -1); at a qualifying O cell of a variable without input, a candidate
+// defining row
+#define PB_SOLVE_ZERO 0xfffffffeu
+__global__ void k_solve_vars(const uint64_t* keys, const uint32_t* run, uint64_t m, int cb, const uint64_t* in_ids,
+                             uint64_t n_in, const uint8_t* qual, uint32_t* var_of_cell, uint32_t* inp,
+                             uint32_t* def_row) {
+  const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= m) return;
+  const uint64_t key = keys[k], g = key >> cb;
+  const uint32_t cell = (uint32_t)(key & (((uint64_t)1 << cb) - 1)), var = run[k] - 1;
+  var_of_cell[cell] = var;
+  uint32_t src = PB_SOLVE_ZERO;
+  if (g != 0) {
+    uint64_t lo = 0, hi = n_in;  // in_ids: id + 1, ascending
+    while (lo < hi) {
+      const uint64_t mid = (lo + hi) / 2;
+      if (in_ids[mid] < g) lo = mid + 1;
+      else hi = mid;
+    }
+    src = (lo < n_in && in_ids[lo] == g) ? (uint32_t)lo : PB_SOLVE_NONE;
+  }
+  if (k == 0 || (keys[k - 1] >> cb) != g) inp[var] = src;
+  const uint32_t row = cell / 3;
+  if (src == PB_SOLVE_NONE && cell - 3 * row == 2 && qual[row]) atomicMin(def_row + var, row);
+}
+
+// per cell: unset (a variable with no source) and order (an operand of a defining row that it or a later row defines);
+// per row: whether it defines its O variable
+__global__ void k_solve_flags(const uint32_t* var_of_cell, const uint32_t* inp, const uint32_t* def_row, uint64_t n,
+                              uint8_t* unset, uint8_t* order, uint8_t* defines) {
+  const uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= 3 * n) return;
+  const uint32_t row = (uint32_t)(c / 3), col = (uint32_t)(c - 3 * (uint64_t)row), v = var_of_cell[c];
+  const uint32_t d = def_row[v];
+  unset[c] = (inp[v] == PB_SOLVE_NONE && d == PB_SOLVE_NONE) ? 1 : 0;
+  const bool row_defines = def_row[var_of_cell[3 * (uint64_t)row + 2]] == row;
+  order[c] = (col < 2 && row_defines && d != PB_SOLVE_NONE && d >= row) ? 1 : 0;
+  if (col == 2) defines[row] = row_defines ? 1 : 0;
+}
+
+// the variables' starting values: 0 for id -1, the inputs (canonical -> Montgomery); ready flag set for both
+__global__ void k_solve_init(const uint32_t* inp, const Fr* in_vals, uint64_t n_vars, Fr* val, uint32_t* ready) {
+  const uint64_t v = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= n_vars) return;
+  const uint32_t s = inp[v];
+  if (s == PB_SOLVE_ZERO) val[v] = Fr::zero();
+  else if (s != PB_SOLVE_NONE) val[v] = fp_to_mont(sv_ld(in_vals + s));
+  ready[v] = s != PB_SOLVE_NONE ? 1 : 0;
+}
+
+__device__ __forceinline__ uint64_t sv_now() {
+  uint64_t t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+
+// the defining rows rows[0, n_def), ascending, in dependency order (see the file comment).  status[0]: the ticket,
+// status[1]: set when a warp stalled.
+__global__ void __launch_bounds__(128) k_solve_eval(SolveSel s, const uint32_t* rows, uint64_t n_def,
+                                                    const uint32_t* var_of_cell, Fr* val, uint32_t* ready,
+                                                    uint32_t* status) {
+  const uint32_t lane = threadIdx.x & 31;
+  cuda::atomic_ref<uint32_t, cuda::thread_scope_device> stalled(status[1]);
+  for (;;) {
+    uint32_t t = 0;
+    if (lane == 0) t = atomicAdd(status, 1u);
+    t = __shfl_sync(0xffffffffu, t, 0);
+    const uint64_t i = (uint64_t)t * 32 + lane;
+    if ((uint64_t)t * 32 >= n_def) return;
+    bool done = i >= n_def;
+    uint32_t vl = 0, vr = 0, vo = 0;
+    SolveRow sr;
+    if (!done) {
+      const uint64_t r = rows[i];
+      vl = var_of_cell[3 * r];
+      vr = var_of_cell[3 * r + 1];
+      vo = var_of_cell[3 * r + 2];
+      sr.ql = sv_ld(s.ql + r);
+      sr.qr = sv_ld(s.qr + r);
+      sr.qm = sv_ld(s.qm + r);
+      sr.qc = sv_ld(s.qc + r);
+      sr.neg_inv_qo = fp_neg(sv_ld(s.inv_qo + r));
+#pragma unroll
+      for (int k = 0; k < PB_MAX_CUSTOM; k++) sr.q[k] = k < s.n_custom ? sv_ld(s.q[k] + r) : Fr::zero();
+    }
+    uint64_t since = sv_now();
+    while (!__all_sync(0xffffffffu, done)) {
+      bool moved = false;
+      if (!done) {
+        cuda::atomic_ref<uint32_t, cuda::thread_scope_device> rl(ready[vl]), rr(ready[vr]);
+        if (rl.load(cuda::memory_order_acquire) && rr.load(cuda::memory_order_acquire)) {
+          const Fr a = val[vl], b = val[vr];
+          val[vo] = solve_gate(sr, s.f, s.n_custom, a, b);
+          cuda::atomic_ref<uint32_t, cuda::thread_scope_device>(ready[vo]).store(1, cuda::memory_order_release);
+          done = moved = true;
+        }
+      }
+      if (__any_sync(0xffffffffu, moved)) {
+        since = sv_now();
+        continue;
+      }
+      // leave together: the decisions are the warp's, so no lane is left in a later __all_sync alone
+      if (__any_sync(0xffffffffu, lane == 0 && stalled.load(cuda::memory_order_relaxed))) return;
+      if (__any_sync(0xffffffffu, lane == 0 && sv_now() - since > PB_SOLVE_STALL_NS)) {
+        if (lane == 0) stalled.store(1, cuda::memory_order_relaxed);
+        return;
+      }
+      __nanosleep(64);
+    }
+  }
+}
+
+// every cell's value, canonical: W = A | B | C, column-major
+__global__ void k_solve_write(const uint32_t* var_of_cell, const Fr* val, uint64_t n, Fr* A, Fr* B, Fr* C) {
+  const uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= 3 * n) return;
+  const uint64_t row = c / 3, col = c - 3 * row;
+  const Fr x = fp_from_mont(val[var_of_cell[c]]);
+  (col == 0 ? A : col == 1 ? B : C)[row] = x;
+}
+
+// the order list's second entry: the row defining the variable of each listed cell
+__global__ void k_solve_order_rows(const uint32_t* cells, uint32_t count, const uint32_t* var_of_cell,
+                                   const uint32_t* def_row, uint32_t* out) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < count) out[k] = def_row[var_of_cell[cells[k]]];
+}
+
+// flags[0, m) -> *count and the lowest min(count, limit) flagged indices at h_out
+static uint64_t solve_compact(Context* ctx, const uint8_t* flags, uint64_t m, DevBuf& temp, uint32_t* d_idx,
+                              uint32_t* d_num, uint32_t limit, uint32_t* h_out) {
+  cudaStream_t st = ctx->stream;
+  size_t tb = temp.bytes;
+  PB_CUDA(cub::DeviceSelect::Flagged(temp.p, tb, thrust::counting_iterator<uint32_t>(0), flags, d_idx, d_num, (int)m,
+                                     st));
+  ctx->launches++;
+  uint32_t num = 0;
+  PB_CUDA(cudaMemcpyAsync(&num, d_num, 4, cudaMemcpyDeviceToHost, st));
+  PB_CUDA(cudaStreamSynchronize(st));
+  const uint32_t take = num < limit ? num : limit;
+  if (take && h_out) {
+    PB_CUDA(cudaMemcpyAsync(h_out, d_idx, (size_t)take * 4, cudaMemcpyDeviceToHost, st));
+    PB_CUDA(cudaStreamSynchronize(st));
+  }
+  return num;
+}
+
+static void solve_launched(Context* ctx) {
+  ctx->launches++;
+  PB_CUDA(cudaGetLastError());
+}
+
+// see plonk_b200.h (pb200_solve_wires)
+void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constraints, const uint8_t* const* h_sel,
+               int n_custom, const uint8_t* h_exps, const uint8_t* const* h_custom, uint64_t n_inputs,
+               const int64_t* h_in_ids, const uint8_t* h_in_vals, uint32_t limit, uint64_t* h_counts,
+               uint32_t* h_lists, void* const* out, bool out_on_device) {
+  PB_CHECK(log_n >= 1 && log_n <= 26, "group order must be 2^k, 1 <= k <= 26 (the prover's range)");
+  const uint64_t n = (uint64_t)1 << log_n, m = 3 * n;
+  PB_CHECK(n_constraints <= n, "n_constraints above the group order");
+  PB_CHECK(h_ids && h_sel && h_counts && (h_lists || limit == 0) && out && (h_in_ids || n_inputs == 0) &&
+               (h_in_vals || n_inputs == 0),
+           "solving the wires needs the ids, the selectors, the inputs and the outputs");
+  for (int k = 0; k < 5; k++) PB_CHECK(h_sel[k], "solving the wires needs QL, QR, QM, QO and QC");
+  for (int k = 0; k < 3; k++) PB_CHECK(out[k], "solving the wires needs three output buffers");
+  PB_CHECK(limit <= m, "limit above 3n, the most entries a list can have");
+  PB_CHECK(n_custom >= 0 && n_custom <= PB_MAX_CUSTOM, "at most 4 custom gate terms");
+  PB_CHECK(n_custom == 0 || (h_exps && h_custom), "custom gate terms need their exponents and selectors");
+  SolveSel s = {};
+  s.n_custom = n_custom;
+  for (int k = 0; k < n_custom; k++) {
+    const uint8_t* e = h_exps + 6 * k;
+    const int deg = e[0] + e[1] + e[2] + e[3] + e[4] + e[5];
+    PB_CHECK(deg >= 1 && deg <= 3, "custom gate term must have total degree 1, 2 or 3");
+    PB_CHECK(h_custom[k], "custom gate term without its selector");
+    int f = 0;
+    for (int w = 0; w < 6; w++)
+      for (int t = 0; t < e[w]; t++) s.f[k][f++] = (uint8_t)w;
+    while (f < 3) s.f[k][f++] = PB_FACTOR_ONE;
+  }
+  // ids (only rows below n_constraints are read), inputs and their values, before any device work
+  int64_t max_id = -1;
+  perm_require_ids(h_ids, 3 * n_constraints, &max_id);
+  std::vector<uint64_t> order(n_inputs);
+  for (uint64_t k = 0; k < n_inputs; k++) {
+    const int64_t id = h_in_ids[k];
+    if (id < 0 || id > PB_PERM_MAX_ID) {
+      char b[256];
+      snprintf(b, sizeof b, "input %llu: variable id %lld is outside [0, 2^32 - 2]", (unsigned long long)k,
+               (long long)id);
+      throw Error(b);
+    }
+    Fr x;
+    memcpy(x.v, h_in_vals + 32 * k, 32);
+    if (!fp_is_canonical(x)) {
+      char b[256];
+      snprintf(b, sizeof b, "input %llu (variable %lld): value not reduced below the field modulus",
+               (unsigned long long)k, (long long)id);
+      throw Error(b);
+    }
+    order[k] = k;
+  }
+  std::sort(order.begin(), order.end(), [&](uint64_t a, uint64_t b) {
+    return h_in_ids[a] != h_in_ids[b] ? h_in_ids[a] < h_in_ids[b] : a < b;
+  });
+  std::vector<uint64_t> in_keys(n_inputs);
+  std::vector<uint8_t> in_vals(n_inputs * 32);
+  for (uint64_t k = 0; k < n_inputs; k++) {
+    if (k > 0 && h_in_ids[order[k]] == h_in_ids[order[k - 1]]) {
+      char b[256];
+      snprintf(b, sizeof b, "inputs %llu and %llu both name variable %lld", (unsigned long long)order[k - 1],
+               (unsigned long long)order[k], (long long)h_in_ids[order[k]]);
+      throw Error(b);
+    }
+    in_keys[k] = (uint64_t)(h_in_ids[order[k]] + 1);
+    memcpy(&in_vals[32 * k], h_in_vals + 32 * order[k], 32);
+  }
+
+  const int cb = perm_cell_bits(log_n);
+  const int end_bit = perm_sort_bits(log_n, max_id);
+  cudaStream_t st = ctx->stream;
+  size_t t_sort = 0, t_scan = 0, t_sel = 0;
+  {
+    cub::DoubleBuffer<uint64_t> d(nullptr, nullptr);
+    PB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, t_sort, d, (int)m, 0, end_bit, st));
+    PB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, t_scan, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)m, st));
+    PB_CUDA(cub::DeviceSelect::Flagged(nullptr, t_sel, thrust::counting_iterator<uint32_t>(0), (const uint8_t*)nullptr,
+                                       (uint32_t*)nullptr, (uint32_t*)nullptr, (int)m, st));
+  }
+  const uint64_t temp_bytes = std::max(t_sort, std::max(t_scan, t_sel));
+  // keys and alt (8 each), heads / run (4 each), var_of_cell, inp, def_row, ready (4 each), the values (32), the index
+  // list (4), three flag bytes: per cell.  Selectors, 1 / QO and the custom selectors (32 each), the qualify and
+  // defines flags: per row.  The inputs, the host outputs' staging and the sort's storage.
+  const uint64_t need = m * (8 + 8 + 4 + 4 + 4 * 4 + 32 + 4 + 3) + n * (32 * (6 + (uint64_t)n_custom) + 2) +
+                        n_inputs * 40 + (out_on_device ? 0 : m * 32) + temp_bytes + 256;
+  size_t free_b = 0, total_b = 0;
+  PB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  // PB200_SOLVE_MAX_BYTES: the most device memory a solve may take (read per call), so it leaves room for other work
+  if (const char* e = getenv("PB200_SOLVE_MAX_BYTES")) free_b = std::min<size_t>(free_b, strtoull(e, nullptr, 10));
+  if (need > free_b) {
+    char b[256];
+    snprintf(b, sizeof b, "solving the wires of 2^%d rows needs %llu bytes of device memory, %llu are free", log_n,
+             (unsigned long long)need, (unsigned long long)free_b);
+    throw Error(b);
+  }
+
+  DevBuf temp(temp_bytes), keys(m * 8), alt(m * 8), head(m * 4), run(m * 4), voc(m * 4), inp(m * 4), defr(m * 4),
+      ready(m * 4), val(m * 32), idx(m * 4), flags(3 * m), small(64), inids(n_inputs * 8 + 8), invals(n_inputs * 32 + 32),
+      sel((6 + (uint64_t)n_custom) * n * 32), qual(n), defines(n);
+  Fr* selp = sel.as<Fr>();
+  const Fr* sel_col[5];
+  for (int k = 0; k < 5 + n_custom; k++) {
+    Fr* col = selp + (uint64_t)k * n;
+    PB_CUDA(cudaMemcpyAsync(col, k < 5 ? h_sel[k] : h_custom[k - 5], n * 32, cudaMemcpyHostToDevice, st));
+    if (k < 5) sel_col[k] = col;
+    else s.q[k - 5] = col;
+  }
+  uint32_t* small_u = small.as<uint32_t>();
+  PB_CUDA(cudaMemsetAsync(small.p, 0, 64, st));
+  k_count_noncanonical<<<PB_SOLVE_GRID((5 + (uint64_t)n_custom) * n, 256), 0, st>>>(selp, (5 + (uint64_t)n_custom) * n,
+                                                                                   small_u + 2);
+  solve_launched(ctx);
+  fr_to_mont(ctx, selp, selp, (5 + (uint64_t)n_custom) * n);
+  s.ql = sel_col[0];
+  s.qr = sel_col[1];
+  s.qm = sel_col[2];
+  s.qo = sel_col[3];
+  s.qc = sel_col[4];
+  Fr* inv = selp + (5 + (uint64_t)n_custom) * n;
+  s.inv_qo = inv;
+  const uint64_t T = (n + PB_SOLVE_BATCH_CH - 1) / PB_SOLVE_BATCH_CH;
+  k_batch_div<<<PB_SOLVE_GRID(T, 128), 0, st>>>(nullptr, s.qo, inv, n, T);
+  solve_launched(ctx);
+  uint32_t bad_sel = 0;
+  PB_CUDA(cudaMemcpyAsync(&bad_sel, small_u + 2, 4, cudaMemcpyDeviceToHost, st));
+  PB_CUDA(cudaStreamSynchronize(st));
+  PB_CHECK(bad_sel == 0, "selector value not reduced below the field modulus");
+  if (n_inputs) {
+    PB_CUDA(cudaMemcpyAsync(inids.p, in_keys.data(), n_inputs * 8, cudaMemcpyHostToDevice, st));
+    PB_CUDA(cudaMemcpyAsync(invals.p, in_vals.data(), n_inputs * 32, cudaMemcpyHostToDevice, st));
+  }
+
+  // 1. group
+  const uint64_t* sorted = perm_sort_keys(ctx, h_ids, m, cb, end_bit, keys, alt, temp, temp_bytes, 3 * n_constraints);
+  k_solve_heads<<<PB_SOLVE_GRID(m, 256), 0, st>>>(sorted, m, cb, head.as<uint32_t>());
+  solve_launched(ctx);
+  size_t tb = temp.bytes;
+  PB_CUDA(cub::DeviceScan::InclusiveSum(temp.p, tb, head.as<uint32_t>(), run.as<uint32_t>(), (int)m, st));
+  ctx->launches++;
+  // 2. sources and errors
+  k_solve_qualify<<<PB_SOLVE_GRID(n, 256), 0, st>>>(s, n_constraints, qual.as<uint8_t>());
+  solve_launched(ctx);
+  PB_CUDA(cudaMemsetAsync(defr.p, 0xff, m * 4, st));
+  PB_CUDA(cudaMemsetAsync(inp.p, 0xff, m * 4, st));  // variables past the last run: no source
+  k_solve_vars<<<PB_SOLVE_GRID(m, 256), 0, st>>>(sorted, run.as<uint32_t>(), m, cb, inids.as<uint64_t>(), n_inputs,
+                                                qual.as<uint8_t>(), voc.as<uint32_t>(), inp.as<uint32_t>(),
+                                                defr.as<uint32_t>());
+  solve_launched(ctx);
+  uint8_t* f_unset = flags.as<uint8_t>();
+  uint8_t* f_order = f_unset + m;
+  k_solve_flags<<<PB_SOLVE_GRID(m, 256), 0, st>>>(voc.as<uint32_t>(), inp.as<uint32_t>(), defr.as<uint32_t>(), n,
+                                                 f_unset, f_order, defines.as<uint8_t>());
+  solve_launched(ctx);
+  for (uint64_t k = 0; k < 3 * (uint64_t)limit; k++) h_lists[k] = 0xffffffffu;
+  uint32_t* num = small_u + 1;
+  h_counts[0] = solve_compact(ctx, f_unset, m, temp, idx.as<uint32_t>(), num, limit, h_lists);
+  std::vector<uint32_t> cells(limit);
+  h_counts[1] = solve_compact(ctx, f_order, m, temp, idx.as<uint32_t>(), num, limit, cells.data());
+  const uint32_t listed = (uint32_t)std::min<uint64_t>(h_counts[1], limit);
+  if (listed) {  // (cell, the row defining its variable)
+    DevBuf pairs((size_t)listed * 8);
+    PB_CUDA(cudaMemcpyAsync(pairs.p, cells.data(), (size_t)listed * 4, cudaMemcpyHostToDevice, st));
+    k_solve_order_rows<<<PB_SOLVE_GRID(listed, 128), 0, st>>>(pairs.as<uint32_t>(), listed, voc.as<uint32_t>(),
+                                                              defr.as<uint32_t>(), pairs.as<uint32_t>() + listed);
+    solve_launched(ctx);
+    std::vector<uint32_t> rows(listed);
+    PB_CUDA(cudaMemcpyAsync(rows.data(), pairs.as<uint32_t>() + listed, (size_t)listed * 4, cudaMemcpyDeviceToHost,
+                            st));
+    PB_CUDA(cudaStreamSynchronize(st));
+    for (uint32_t k = 0; k < listed; k++) {
+      h_lists[limit + 2 * (uint64_t)k] = cells[k];
+      h_lists[limit + 2 * (uint64_t)k + 1] = rows[k];
+    }
+  }
+  if (h_counts[0] || h_counts[1]) {
+    PB_CUDA(cudaStreamSynchronize(st));  // the call's buffers die here
+    return;
+  }
+
+  // 3.-4. the defining rows in row order, evaluated
+  k_solve_init<<<PB_SOLVE_GRID(m, 256), 0, st>>>(inp.as<uint32_t>(), invals.as<Fr>(), m, val.as<Fr>(),
+                                                ready.as<uint32_t>());
+  solve_launched(ctx);
+  const uint64_t n_def = solve_compact(ctx, defines.as<uint8_t>(), n, temp, idx.as<uint32_t>(), num, 0, nullptr);
+  if (n_def) {
+    int per_sm = 0;
+    PB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_solve_eval, 128, 0));
+    const uint64_t warps = (n_def + 31) / 32;
+    const uint64_t blocks = std::min<uint64_t>((uint64_t)std::max(per_sm, 1) * ctx->sm_count, (warps + 3) / 4);
+    k_solve_eval<<<(unsigned)blocks, 128, 0, st>>>(s, idx.as<uint32_t>(), n_def, voc.as<uint32_t>(), val.as<Fr>(),
+                                                   ready.as<uint32_t>(), small_u + 4);
+    solve_launched(ctx);
+    uint32_t stalled = 0;
+    PB_CUDA(cudaMemcpyAsync(&stalled, small_u + 5, 4, cudaMemcpyDeviceToHost, st));
+    PB_CUDA(cudaStreamSynchronize(st));
+    PB_CHECK(stalled == 0, "solving the wires stalled: a defining row waited too long for its operands");
+  }
+  // 5. write
+  DevBuf staging(out_on_device ? 0 : m * 32);
+  Fr* W[3];
+  for (int k = 0; k < 3; k++)
+    W[k] = out_on_device ? reinterpret_cast<Fr*>(out[k]) : staging.as<Fr>() + (uint64_t)k * n;
+  k_solve_write<<<PB_SOLVE_GRID(m, 256), 0, st>>>(voc.as<uint32_t>(), val.as<Fr>(), n, W[0], W[1], W[2]);
+  solve_launched(ctx);
+  if (!out_on_device)
+    for (int k = 0; k < 3; k++)
+      PB_CUDA(cudaMemcpyAsync(out[k], W[k], n * 32, cudaMemcpyDeviceToHost, st));
+  PB_CUDA(cudaStreamSynchronize(st));
+}
+
+}  // namespace pb200

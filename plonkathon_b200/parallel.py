@@ -122,6 +122,7 @@ class ShardedProver(Prover):
     same bytes.  Every rank must make the same calls with the same inputs (the collectives inside are matched
     pairwise); the context needs a communicator (``init_comm``)."""
     _CREATE = "pb200_prover_create_sharded"
+    sharded = True
     _CREATE_CUSTOM = "pb200_prover_create_custom_sharded"
 
     @classmethod

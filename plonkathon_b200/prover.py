@@ -150,6 +150,11 @@ class Kind(NamedTuple):
     def schedule(self) -> dict:
         return schedule(**{b: True for b in self.proof.BLOCKS})
 
+    @property
+    def device(self) -> str:
+        """its whole-proof entry point for wire values already in device memory"""
+        return "pb200_prover_prove_device" + self.suffix
+
 
 _R2, _R4 = ("pb200_prover_round2", Message2, ()), ("pb200_prover_round4", Message4)
 _R2_SHUFFLE = ("pb200_prover_round2_shuffle", ShuffleMessage2, ("theta", "kappa"))
@@ -224,6 +229,7 @@ class Prover:
     _CREATE_CUSTOM = "pb200_prover_create_custom"
     _CREATE_NEXT_ROW = "pb200_prover_create_custom_next_row"
     next_row, _kind = False, KINDS[()]  # a plain prover until _create or a _set_* call says otherwise
+    sharded = False  # one proof across several GPUs (parallel.ShardedProver)
 
     def __init__(self, setup, program):
         """prover.py:45-49."""
@@ -355,14 +361,42 @@ class Prover:
     def prove_arrays(self, A, B, C, public) -> bytes:
         """One C-ABI call for the whole proof (rounds 1-5 + transcript); returns the canonical bytes of the prover's
         proof kind: 768 for a ``Proof``, 1216 for a ``LookupProof`` (lookup argument), 864 for a ``NextRowProof``
-        (next-row custom gate terms), 896 (992) for a ``ShuffleProof`` (``NextRowShuffleProof``)."""
+        (next-row custom gate terms), 896 (992) for a ``ShuffleProof`` (``NextRowShuffleProof``).
+        A, B, C may also be contiguous (n, 32) uint8 CUDA tensors on the prover's device (``solve_wires(device=True)``),
+        which are read where they are; ValueError for malformed tensors and on the sharded prover."""
         n = self.group_order
-        a, b, c = (_as_le_rows(v, n) for v in (A, B, C))
         pub = _as_le_rows(public, len(public)) if len(public) else np.zeros((0, 32), dtype=np.uint8)
         out = ctypes.create_string_buffer(self._kind.proof.BYTES)
+        ptrs = self._device_wires(A, B, C)
+        if ptrs is not None:
+            if self.sharded:
+                raise ValueError("the sharded prover takes wire values in host memory, not CUDA tensors")
+            self._call(self._kind.device, *ptrs, pub.ctypes.data_as(ctypes.c_void_p), pub.shape[0], out)
+            return out.raw
+        a, b, c = (_as_le_rows(v, n) for v in (A, B, C))
         self._call("pb200_prover_prove" + self._kind.suffix, *[x.ctypes.data_as(ctypes.c_void_p) for x in (a, b, c, pub)],
                    pub.shape[0], out)
         return out.raw
+
+    def _device_wires(self, A, B, C):
+        """pointers to A, B, C when they are CUDA tensors, checked and with their stream synchronised (the library
+        runs on its own stream); None for host values; ValueError for a mix or a malformed tensor"""
+        n = self.group_order
+        on_device = [_is_cuda_tensor(X) for X in (A, B, C)]
+        if any(on_device) and not all(on_device):
+            raise ValueError("A, B and C must all be CUDA tensors or all be host values")
+        if not all(on_device):
+            return None
+        for name, X in zip("ABC", (A, B, C)):
+            if tuple(X.shape) != (n, 32) or str(X.dtype) != "torch.uint8" or not X.is_contiguous():
+                raise ValueError("%s must be a contiguous (%d, 32) uint8 tensor, got %s %s"
+                                 % (name, n, tuple(X.shape), X.dtype))
+            if X.device.index != self.ctx.device:
+                raise ValueError("%s is on cuda:%s, the prover on cuda:%d" % (name, X.device.index, self.ctx.device))
+        import torch
+        for X in (A, B, C):
+            torch.cuda.current_stream(X.device).synchronize()
+        return [ctypes.c_void_p(X.data_ptr()) for X in (A, B, C)]
 
     # ------------------------------------------------------------------ witness check
     def check_arrays(self, A, B, C, public, limit: int = 16) -> WitnessReport:
@@ -384,20 +418,8 @@ class Prover:
         limit = int(limit)
         if len(public) > n:
             raise ValueError("%d public inputs for %d rows" % (len(public), n))
-        on_device = [_is_cuda_tensor(X) for X in (A, B, C)]
-        if any(on_device) and not all(on_device):
-            raise ValueError("A, B and C must all be CUDA tensors or all be host values")
-        if all(on_device):
-            for name, X in zip("ABC", (A, B, C)):
-                if tuple(X.shape) != (n, 32) or str(X.dtype) != "torch.uint8" or not X.is_contiguous():
-                    raise ValueError("%s must be a contiguous (%d, 32) uint8 tensor, got %s %s"
-                                     % (name, n, tuple(X.shape), X.dtype))
-                if X.device.index != self.ctx.device:
-                    raise ValueError("%s is on cuda:%s, the prover on cuda:%d" % (name, X.device.index, self.ctx.device))
-            import torch
-            for X in (A, B, C):
-                torch.cuda.current_stream(X.device).synchronize()  # the library runs on its own stream
-            ptrs = [ctypes.c_void_p(X.data_ptr()) for X in (A, B, C)]
+        ptrs = self._device_wires(A, B, C)
+        if ptrs is not None:
             entry, wires = "pb200_prover_check_device", None
         else:
             wires = tuple(_wire_rows(name, X, n) for name, X in zip("ABC", (A, B, C)))

@@ -1,0 +1,187 @@
+"""A circuit's wire values from the values of its input variables, computed on the GPU (csrc/solve.cu).
+
+``solve_wires`` runs a circuit given as arrays -- the wiring ``permutation_arrays`` takes, the gate selectors, the
+custom terms -- the way the reference runs a program (compiler/program.py:161-192): a row r < n_constraints defines
+its O variable v when v is not -1, QO[r] != 0, no custom term whose selector is non-zero at r reads c or the next
+row, v is not an input and no earlier row defines v; it sets c = -(QL a + QR b + QM a b + QC + sum_k Q_k a^i b^j) / QO.
+Every other variable (lookup and shuffle rows, public inputs, rows whose terms involve c or the next row, hints)
+must come as an input.  The wires stay on the device if asked, for ``Prover.check_arrays`` and ``prove_arrays``."""
+from __future__ import annotations
+
+import ctypes
+from dataclasses import dataclass, field
+
+import numpy as np
+
+from ._lib import check, default_context, lib
+from .custom_gates import padded, split_terms
+from .field import CURVE_ORDER
+from .wiring import MAX_ID, MAX_LOG_N, _wire
+
+WIRE = "LRO"
+SEL = ("QL", "QR", "QM", "QO", "QC")
+
+
+@dataclass
+class WireSolution:
+    """What ``solve_wires`` found: the wires A, B, C when ``ok``, else the errors, each an exact count and its lowest
+    ``limit`` locations:
+
+    * ``unset``: cells whose variable is neither an input nor defined by a row (``unset_cells``: cell = 3 row + col);
+    * ``order``: L or R cells of a defining row whose variable that row or a later row defines (``order_cells``:
+      (cell, the defining row))."""
+    A: object
+    B: object
+    C: object
+    unset: int
+    order: int
+    unset_cells: list
+    order_cells: list
+    limit: int
+    _ids: np.ndarray = field(default=None, repr=False, compare=False)
+
+    @property
+    def ok(self) -> bool:
+        return not (self.unset or self.order)
+
+    def lines(self) -> list:
+        out = []
+        for c in self.unset_cells:
+            row, col = divmod(c, 3)
+            out.append("unset: cell (row %d, %s) variable %d is neither an input nor defined by a row"
+                       % (row, WIRE[col], int(self._ids[c])))
+        for c, d in self.order_cells:
+            row, col = divmod(c, 3)
+            out.append("order: row %d reads variable %d (cell (%d, %s)), which row %d defines"
+                       % (row, int(self._ids[c]), row, WIRE[col], d))
+        for k, listed in (("unset", self.unset_cells), ("order", self.order_cells)):
+            if getattr(self, k) > len(listed):
+                out.append("%s: %d more" % (k, getattr(self, k) - len(listed)))
+        return out
+
+    def __str__(self) -> str:
+        if self.ok:
+            return "wires solved"
+        head = "wires unsolved: " + ", ".join("%d %s" % (getattr(self, k), k) for k in ("unset", "order")
+                                              if getattr(self, k))
+        return "\n".join([head] + ["  " + s for s in self.lines()])
+
+
+def _column(name, col, n) -> np.ndarray:
+    """a selector column: n ints or an (n, 32) uint8 array of canonical little-endian values"""
+    if isinstance(col, np.ndarray) and col.dtype == np.uint8:
+        if col.shape != (n, 32):
+            raise ValueError("%s must be an (%d, 32) uint8 array, got %s" % (name, n, col.shape))
+        return np.ascontiguousarray(col)
+    vals = list(col)
+    if len(vals) != n:
+        raise ValueError("%s must have group_order = %d values, got %d" % (name, n, len(vals)))
+    vals = [int(v.n if hasattr(v, "n") else v) for v in vals]
+    if any(not 0 <= v < CURVE_ORDER for v in vals):
+        raise ValueError("%s holds a value not reduced below r" % name)
+    return np.frombuffer(b"".join(v.to_bytes(32, "little") for v in vals), dtype=np.uint8).reshape(n, 32).copy()
+
+
+def _inputs(inputs):
+    """a dict id -> value, or (ids, (k, 32) uint8 values) -> (int64 ids, (k, 32) uint8 values); ValueError for
+    duplicate or out-of-range ids and values not reduced below r"""
+    if isinstance(inputs, dict):
+        ids = np.fromiter((int(k) for k in inputs), dtype=np.int64, count=len(inputs)) if inputs else \
+            np.zeros(0, np.int64)
+        vals = [int(v.n if hasattr(v, "n") else v) for v in inputs.values()]
+        if any(not 0 <= v < CURVE_ORDER for v in vals):
+            bad = next(k for k, v in zip(inputs, vals) if not 0 <= v < CURVE_ORDER)
+            raise ValueError("input %d: value not reduced below r" % int(bad))
+        raw = np.frombuffer(b"".join(v.to_bytes(32, "little") for v in vals), dtype=np.uint8).reshape(-1, 32)
+    else:
+        try:
+            ids, raw = inputs
+        except (TypeError, ValueError):
+            raise ValueError("inputs must be a dict id -> value or a pair (ids, (k, 32) uint8 values)") from None
+        ids = np.asarray(ids)
+        if ids.ndim != 1 or not np.issubdtype(ids.dtype, np.integer):
+            raise ValueError("input ids must be a 1-D integer array, got %s %s" % (ids.dtype, ids.shape))
+        raw = np.asarray(raw)
+        if raw.dtype != np.uint8 or raw.shape != (len(ids), 32):
+            raise ValueError("input values must be a (%d, 32) uint8 array, got %s %s" % (len(ids), raw.dtype, raw.shape))
+        if len(ids):
+            words = np.ascontiguousarray(raw).view("<u8")  # (k, 4) little-endian 64-bit words
+            r = [(CURVE_ORDER >> (64 * w)) & (2**64 - 1) for w in range(4)]
+            lt = np.zeros(len(ids), bool)
+            eq = np.ones(len(ids), bool)
+            for w in (3, 2, 1, 0):
+                lt |= eq & (words[:, w] < np.uint64(r[w]))
+                eq &= words[:, w] == np.uint64(r[w])
+            if not lt.all():
+                k = int(np.flatnonzero(~lt)[0])
+                raise ValueError("input %d (variable %d): value not reduced below r" % (k, int(ids[k])))
+    ids = ids.astype(np.int64)
+    if len(ids) and (ids.min() < 0 or ids.max() > MAX_ID):
+        k = int(np.flatnonzero((ids < 0) | (ids > MAX_ID))[0])
+        raise ValueError("input %d: variable id %d is outside [0, 2^32 - 2]" % (k, int(ids[k])))
+    s = np.sort(ids)
+    dup = np.flatnonzero(s[1:] == s[:-1])
+    if len(dup):
+        raise ValueError("two inputs name variable %d" % int(s[dup[0]]))
+    return np.ascontiguousarray(ids), np.ascontiguousarray(raw, dtype=np.uint8)
+
+
+def solve_wires(wire_L, wire_R, wire_O, pk: dict, inputs, group_order: int, n_constraints: int | None = None,
+                custom=(), device: bool = False, limit: int = 16, ctx=None) -> WireSolution:
+    """-> ``WireSolution``: the wire values A, B, C of the circuit, each (n, 32) canonical little-endian, or its
+    errors.
+
+    ``wire_L``, ``wire_R``, ``wire_O``: variable ids as ``permutation_arrays`` takes them.  ``pk``: a dict with at least
+    QL QR QM QO QC (n ints or (n, 32) uint8 arrays).  ``inputs``: a dict variable id -> value, or a pair (ids,
+    (k, 32) uint8 values).  ``custom``: the custom terms as ``Prover.from_arrays(custom=)`` takes them.  ``device``:
+    A, B, C as (n, 32) uint8 CUDA tensors on the context's device (no copy to the host), else numpy arrays.
+    ``limit``: how many locations of each error kind to list.  Malformed arguments are a ValueError before the library
+    is called; the solve runs on the GPU of ``ctx`` (default: the default context)."""
+    n = group_order
+    if isinstance(n, bool) or not isinstance(n, (int, np.integer)) or n < 2 or n & (n - 1) or n > 1 << MAX_LOG_N:
+        raise ValueError("group_order must be a power of two in [2, 2^%d], got %r" % (MAX_LOG_N, n))
+    n = int(n)
+    m = n if n_constraints is None else n_constraints
+    if isinstance(m, bool) or not isinstance(m, (int, np.integer)) or not 0 <= m <= n:
+        raise ValueError("n_constraints must be an integer in [0, group_order = %d], got %r" % (n, m))
+    m = int(m)
+    if isinstance(limit, bool) or not isinstance(limit, (int, np.integer)) or not 0 <= limit <= 3 * n:
+        raise ValueError("limit must be an integer in [0, 3n = %d], got %r" % (3 * n, limit))
+    limit = int(limit)
+    ids = np.full((n, 3), -1, dtype=np.int64)
+    for col, (name, w) in enumerate((("wire_L", wire_L), ("wire_R", wire_R), ("wire_O", wire_O))):
+        ids[:m, col] = _wire(name, w, n, m)
+    missing = [k for k in SEL if k not in pk]
+    if missing:
+        raise ValueError("pk lacks %s" % ", ".join(missing))
+    sel = [_column(k, pk[k], n) for k in SEL]
+    exps, ccols = split_terms(custom, n)
+    cust = [_column("custom selector %r" % (e,), c, n) for e, c in zip(exps, ccols)]
+    in_ids, in_vals = _inputs(inputs)
+    ctx = ctx or default_context()
+
+    vp = ctypes.c_void_p
+    sel_arr = (vp * 5)(*[s.ctypes.data for s in sel])
+    cust_arr = (vp * max(1, len(cust)))(*[c.ctypes.data for c in cust])
+    ebytes = bytes(x for e in exps for x in padded(e)) or b"\0"
+    counts = (ctypes.c_uint64 * 2)()
+    lists = (ctypes.c_uint32 * max(1, 3 * limit))()
+    if device:
+        import torch
+        dev = torch.device("cuda", ctx.device)
+        torch.cuda.current_stream(dev).synchronize()  # the blocks may have served work still queued on torch's stream
+        out = [torch.empty((n, 32), dtype=torch.uint8, device=dev) for _ in range(3)]
+        ptrs = [t.data_ptr() for t in out]
+    else:
+        out = [np.empty((n, 32), dtype=np.uint8) for _ in range(3)]
+        ptrs = [a.ctypes.data for a in out]
+    check(lib().pb200_solve_wires(ctx.handle, ids.ctypes.data_as(vp), n.bit_length() - 1, m, sel_arr, len(exps),
+                                  ebytes, cust_arr, len(in_ids), in_ids.ctypes.data_as(vp), in_vals.ctypes.data_as(vp),
+                                  limit, counts, lists, (vp * 3)(*ptrs), 1 if device else 0))
+    raw = [int(x) for x in lists[:3 * limit]]
+    unset = [x for x in raw[:limit] if x != 0xffffffff]
+    pairs = raw[limit:3 * limit]
+    order = [(pairs[2 * k], pairs[2 * k + 1]) for k in range(limit) if pairs[2 * k] != 0xffffffff]
+    ok = not (counts[0] or counts[1])
+    A, B, C = out if ok else (None, None, None)
+    return WireSolution(A, B, C, int(counts[0]), int(counts[1]), unset, order, limit, ids.reshape(-1))
