@@ -181,6 +181,31 @@ int pb200_solve_wires(pb200_ctx* ctx, const int64_t* h_ids, int log_n, uint64_t 
                       const uint8_t* const* h_custom, uint64_t n_inputs, const int64_t* h_input_ids,
                       const uint8_t* h_input_values, uint32_t limit, uint64_t* h_counts, uint32_t* h_lists,
                       void* const* out, int out_on_device);
+/* pb200_solve_wires for a circuit with lookups: rows that read a table also define their O variable from it.
+ * h_qk (n x 32 bytes, 0 or 1), and the table h_t1..h_t3 (table_rows x 32 bytes each, canonical) as
+ * pb200_prover_set_lookup takes them; for several tables h_qtag (Q_T) and h_t4 as pb200_prover_set_lookup_tagged takes
+ * them, else both NULL.  The gate rule is unchanged.  In addition a row r < n_constraints defines its O variable v from
+ * its table when q_K[r] != 0, QO[r] = 0, v is not -1, no input and not defined by an earlier row (of either kind): it
+ * sets c = t3 of the table rows whose (t1, t2[, t4]) equal (a, b[, Q_T[r]]).  h_counts[4]: unset and order as
+ * pb200_solve_wires counts them, then
+ *   miss       rows that define from their table and whose key matches no table row,
+ *   ambiguous  rows that define from their table and whose key matches table rows with different t3;
+ * these two are found while the rows are evaluated, so they are counted only when unset and order are both 0.
+ * h_lists (5 limit uint32): pb200_solve_wires' 3 limit entries, then the lowest `limit` miss rows and the lowest
+ * `limit` ambiguous rows, unused entries 0xffffffff.  h_operands (4 limit x 32 bytes, or NULL): a and b (canonical)
+ * of each listed miss row, then of each listed ambiguous row, at 64 limit bytes.  With any count non-zero nothing is
+ * written to `out`.  Refuses what pb200_solve_wires refuses and, before any device work, what
+ * pb200_prover_set_lookup(_tagged) refuses: q_K not 0/1, Q_T not canonical or not 0 where q_K = 0, a table value not
+ * reduced below r, an empty table, more table rows than n.  The table index (about 174 bytes a table row, plus 66 bytes
+ * a row for q_K, Q_T and the error flags) is counted against free memory and PB200_SOLVE_MAX_BYTES and freed before
+ * the call returns. */
+int pb200_solve_wires_lookup(pb200_ctx* ctx, const int64_t* h_ids, int log_n, uint64_t n_constraints,
+                             const uint8_t* const* h_sel, unsigned n_custom, const uint8_t* h_exps,
+                             const uint8_t* const* h_custom, uint64_t n_inputs, const int64_t* h_input_ids,
+                             const uint8_t* h_input_values, const uint8_t* h_qk, const uint8_t* h_qtag,
+                             const uint8_t* h_t1, const uint8_t* h_t2, const uint8_t* h_t3, const uint8_t* h_t4,
+                             uint64_t table_rows, uint32_t limit, uint64_t* h_counts, uint32_t* h_lists,
+                             uint8_t* h_operands, void* const* out, int out_on_device);
 
 /* ---- Prover (prover.py:39-306) ---------------------------------------------------------------- */
 /* Proof layout.  A prover's proof is the plain 15 fields, then the fields of the blocks it has (next-row custom gate

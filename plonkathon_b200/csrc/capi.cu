@@ -71,7 +71,8 @@ void permutation_run(Context* ctx, const int64_t* h_ids, int log_n, uint8_t* h_S
 void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constraints, const uint8_t* const* h_sel,
                int n_custom, const uint8_t* h_exps, const uint8_t* const* h_custom, uint64_t n_inputs,
                const int64_t* h_in_ids, const uint8_t* h_in_vals, uint32_t limit, uint64_t* h_counts,
-               uint32_t* h_lists, void* const* out, bool out_on_device);
+               uint32_t* h_lists, void* const* out, bool out_on_device, const uint8_t* h_qk, const uint8_t* h_qtag,
+               const uint8_t* const* h_tab, uint64_t tab_rows, uint8_t* h_operands);
 // ptau.cu
 Srs* srs_create_ptau(Context* ctx, const uint8_t* h_g1, uint64_t count, const uint8_t* h_tau_g2, int precompute);
 Srs* srs_create_ptau_lagrange(Context* ctx, const uint8_t* h_block, uint64_t n, Srs* monomial, int precompute);
@@ -590,7 +591,22 @@ int pb200_solve_wires(pb200_ctx* ctx, const int64_t* h_ids, int log_n, uint64_t 
                       void* const* out, int out_on_device) {
   PB_API_BEGIN PB_ON_CTX(C(ctx));
   solve_run(C(ctx), h_ids, log_n, n_constraints, h_sel, (int)n_custom, h_exps, h_custom, n_inputs, h_input_ids,
-            h_input_values, limit, h_counts, h_lists, out, out_on_device != 0);
+            h_input_values, limit, h_counts, h_lists, out, out_on_device != 0, nullptr, nullptr, nullptr, 0, nullptr);
+  PB_API_END
+}
+int pb200_solve_wires_lookup(pb200_ctx* ctx, const int64_t* h_ids, int log_n, uint64_t n_constraints,
+                             const uint8_t* const* h_sel, unsigned n_custom, const uint8_t* h_exps,
+                             const uint8_t* const* h_custom, uint64_t n_inputs, const int64_t* h_input_ids,
+                             const uint8_t* h_input_values, const uint8_t* h_qk, const uint8_t* h_qtag,
+                             const uint8_t* h_t1, const uint8_t* h_t2, const uint8_t* h_t3, const uint8_t* h_t4,
+                             uint64_t table_rows, uint32_t limit, uint64_t* h_counts, uint32_t* h_lists,
+                             uint8_t* h_operands, void* const* out, int out_on_device) {
+  PB_API_BEGIN PB_ON_CTX(C(ctx));
+  PB_CHECK(!h_qtag == !h_t4, "tagged lookups need both Q_T and the table tag column t4");
+  const uint8_t* tab[4] = {h_t1, h_t2, h_t3, h_t4};
+  solve_run(C(ctx), h_ids, log_n, n_constraints, h_sel, (int)n_custom, h_exps, h_custom, n_inputs, h_input_ids,
+            h_input_values, limit, h_counts, h_lists, out, out_on_device != 0, h_qk, h_qtag, tab, table_rows,
+            h_operands);
   PB_API_END
 }
 

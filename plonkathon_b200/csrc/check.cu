@@ -238,8 +238,9 @@ __global__ void k_check_pairs(const uint32_t* cells, uint32_t count, const uint3
 }
 
 // ---- host ----------------------------------------------------------------------------------------------------------
-// a field element from getrandom(2), canonical and not zero, in Montgomery form
-static Fr check_random_fr() {
+// a field element from getrandom(2), canonical and not zero, in Montgomery form (the wire solver's table index draws
+// its theta here too)
+Fr check_random_fr() {
   for (;;) {
     Fr x;
     size_t got = 0;

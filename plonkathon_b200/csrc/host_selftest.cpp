@@ -652,4 +652,107 @@ int hs_solve(const int64_t* ids, int log_n, uint64_t m, const uint32_t* sel, int
   }
   return 0;
 }
+
+// hs_solve with rows that define from their table, through the same table index and solve_probe as solve.cu: qk and
+// qt (NULL untagged) n canonical values each, tab the table columns t1 t2 t3 (t4) one after the other, rows values
+// each.  The index is built here with std::sort and a fixed theta (stepped on a collision of words).  errs[0], errs[1]:
+// the miss and ambiguous rows.  Returns 0, 1 as hs_solve, or 2 when errs is not zero.
+int hs_solve_lookup(const int64_t* ids, int log_n, uint64_t m, const uint32_t* sel, int n_custom, const uint8_t* exps,
+                    const uint32_t* custom, uint64_t n_in, const int64_t* in_ids, const uint32_t* in_vals,
+                    const uint32_t* qk, const uint32_t* qt, const uint32_t* tab, uint64_t rows, uint32_t* out,
+                    uint64_t* errs) {
+  const uint64_t n = (uint64_t)1 << log_n;
+  const int width = qt ? 4 : 3;
+  uint8_t f[PB_MAX_CUSTOM][3];
+  for (int k = 0; k < n_custom; k++) {
+    int s = 0;
+    for (int w = 0; w < 6; w++)
+      for (int t = 0; t < exps[6 * k + w]; t++) f[k][s++] = (uint8_t)w;
+    while (s < 3) f[k][s++] = PB_FACTOR_ONE;
+  }
+  // the index: distinct keys in ascending word order, none sharing a word
+  std::vector<Fr> tm(width * rows);
+  for (uint64_t k = 0; k < width * rows; k++) tm[k] = fp_to_mont(ld<Fr>(tab + 8 * k));
+  SolveTable T = {};
+  for (int w = 0; w < width; w++) T.t[w] = tm.data() + w * rows;
+  auto tag_of = [&](uint64_t r) { return qt ? T.t[3][r] : Fr::zero(); };
+  std::vector<std::pair<uint64_t, uint32_t>> kv(rows);
+  std::vector<uint64_t> words;
+  std::vector<uint32_t> keyrow;
+  std::vector<uint8_t> amb;
+  Fr seed = Fr::zero();
+  seed.v[0] = 0x9e3779b9u;
+  for (bool clean = false; !clean;) {
+    seed.v[1]++;
+    T.theta = fp_to_mont(seed);
+    T.theta2 = fp_mul(T.theta, T.theta);
+    for (uint64_t r = 0; r < rows; r++)
+      kv[r] = {solve_table_word(tag_of(r), T.t[0][r], T.t[1][r], T.theta, T.theta2), (uint32_t)r};
+    std::sort(kv.begin(), kv.end());
+    words.clear(), keyrow.clear(), amb.clear();
+    clean = true;
+    for (uint64_t k = 0; k < rows && clean; k++) {
+      const uint32_t r = kv[k].second;
+      if (k == 0 || kv[k].first != kv[k - 1].first) {
+        words.push_back(kv[k].first), keyrow.push_back(r), amb.push_back(0);
+        continue;
+      }
+      const uint32_t p = kv[k - 1].second;
+      if (T.t[0][r] != T.t[0][p] || T.t[1][r] != T.t[1][p] || tag_of(r) != tag_of(p)) clean = false;
+      if (T.t[2][r] != T.t[2][p]) amb.back() = 1;
+    }
+  }
+  T.word = words.data();
+  T.row = keyrow.data();
+  T.amb = amb.data();
+  T.n_keys = words.size();
+
+  auto col = [&](const uint32_t* base, uint64_t c, uint64_t r) { return fp_to_mont(ld<Fr>(base + 8 * (c * n + r))); };
+  std::unordered_map<int64_t, Fr> val;
+  for (uint64_t k = 0; k < n_in; k++) val[in_ids[k]] = fp_to_mont(ld<Fr>(in_vals + 8 * k));
+  auto get = [&](int64_t id, Fr* x) {
+    if (id < 0) { *x = Fr::zero(); return true; }
+    auto it = val.find(id);
+    if (it == val.end()) return false;
+    *x = it->second;
+    return true;
+  };
+  errs[0] = errs[1] = 0;
+  for (uint64_t r = 0; r < m; r++) {
+    const int64_t v = ids[3 * r + 2];
+    if (v < 0 || val.count(v)) continue;
+    SolveRow row;
+    const Fr qo = col(sel, 3, r);
+    bool gate = !qo.is_zero();
+    for (int k = 0; k < n_custom; k++) {
+      row.q[k] = col(custom, k, r);
+      if (solve_term_reads_c(f[k]) && !row.q[k].is_zero()) gate = false;
+    }
+    const bool table = qo.is_zero() && !ld<Fr>(qk + 8 * r).is_zero();
+    if (!gate && !table) continue;
+    Fr a, b;
+    if (!get(ids[3 * r], &a) || !get(ids[3 * r + 1], &b)) return 1;
+    if (table) {
+      Fr c;
+      const Fr tag = qt ? fp_to_mont(ld<Fr>(qt + 8 * r)) : Fr::zero();
+      const int e = solve_probe(T, tag, a, b, &c);
+      if (e != PB_SOLVE_HIT) errs[e - 1]++;
+      val[v] = c;
+      continue;
+    }
+    row.ql = col(sel, 0, r);
+    row.qr = col(sel, 1, r);
+    row.qm = col(sel, 2, r);
+    row.qc = col(sel, 4, r);
+    row.neg_inv_qo = fp_neg(fp_inv_gcd(qo));
+    val[v] = solve_gate(row, f, n_custom, a, b);
+  }
+  for (uint64_t c = 0; c < 3 * n; c++) {
+    const uint64_t r = c / 3, w = c - 3 * r;
+    Fr x = Fr::zero();
+    if (r < m && !get(ids[c], &x)) return 1;
+    st(out + 8 * (w * n + r), fp_from_mont(x));
+  }
+  return errs[0] || errs[1] ? 2 : 0;
+}
 }

@@ -17,6 +17,12 @@
 //                progress for PB_SOLVE_STALL_NS sets the stall flag, and every warp leaves on it.
 //   5. write:    every cell gets its variable's value, canonical, in A | B | C.
 // Device memory: about 430 bytes a row plus the outputs (DESIGN.md section 2), all freed before the call returns.
+//
+// With a table (pb200_solve_wires_lookup) a row with q_K != 0 and QO = 0 may also define its O variable, as t3 of the
+// table row matching its (tag, a, b).  k_solve_qualify_lookup flags it 2 beside the gate rows' 1, so both kinds go
+// through steps 2 and 4 as one ascending list.  Before step 4 the table index is built (solve_table_index: words of
+// the keys sorted, checked on full values, one entry per distinct key); k_solve_eval_lookup probes it (solve.cuh,
+// solve_probe) and flags miss and ambiguous rows, which still store 0 and release their flag.
 #include <algorithm>
 #include <cuda/atomic>
 #include <cub/device/device_radix_sort.cuh>
@@ -35,6 +41,8 @@ void fr_from_mont(Context* ctx, const Fr* in, Fr* out, uint64_t n);
 // prover.cu
 __global__ void k_batch_div(const Fr* num, const Fr* den, Fr* out, uint64_t n, uint64_t T);
 __global__ void k_count_noncanonical(const Fr* v, uint64_t n, uint32_t* bad);
+// check.cu
+Fr check_random_fr();
 // permutation.cu
 void perm_require_ids(const int64_t* h_ids, uint64_t m, int64_t* max_id);
 uint64_t* perm_sort_keys(Context* ctx, const int64_t* h_ids, uint64_t m, int cb, int end_bit, DevBuf& keys, DevBuf& alt,
@@ -69,6 +77,62 @@ __global__ void k_solve_qualify(SolveSel s, uint64_t n_rows, uint8_t* qual) {
   for (int k = 0; k < PB_MAX_CUSTOM; k++)
     if (k < s.n_custom && solve_term_reads_c(s.f[k]) && !sv_ld(s.q[k] + r).is_zero()) ok = false;
   qual[r] = ok ? 1 : 0;
+}
+
+// with a table: 1 where a row defines by the gate rule (as k_solve_qualify), else 2 where it defines from its table:
+// q_K != 0 and QO = 0 (qk canonical)
+#define PB_SOLVE_BY_TABLE 2
+__global__ void k_solve_qualify_lookup(SolveSel s, const Fr* qk, uint64_t n_rows, uint8_t* qual) {
+  const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_rows) return;
+  const bool qo = !sv_ld(s.qo + r).is_zero();
+  bool ok = qo;
+#pragma unroll
+  for (int k = 0; k < PB_MAX_CUSTOM; k++)
+    if (k < s.n_custom && solve_term_reads_c(s.f[k]) && !sv_ld(s.q[k] + r).is_zero()) ok = false;
+  qual[r] = ok ? 1 : (!qo && !sv_ld(qk + r).is_zero()) ? PB_SOLVE_BY_TABLE : 0;
+}
+
+// ---- the table index (solve.cuh, SolveTable) -----------------------------------------------------------------------
+// table row k: the word of its key (t4, t1, t2) and k
+__global__ void k_solve_tab_keys(SolveTable T, uint64_t rows, uint64_t* keys, uint32_t* idx) {
+  const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= rows) return;
+  const Fr tag = T.t[3] ? sv_ld(T.t[3] + k) : Fr::zero();
+  keys[k] = solve_table_word(tag, sv_ld(T.t[0] + k), sv_ld(T.t[1] + k), T.theta, T.theta2);
+  idx[k] = (uint32_t)k;
+}
+// sorted position k: head[k] = 1 where a run of equal words starts; *impure counts neighbours with equal words and
+// different keys (then theta is drawn again); split[k] = 1 where k's t3 differs from its neighbour's in the same run
+__global__ void k_solve_tab_heads(SolveTable T, const uint64_t* keys, const uint32_t* idx, uint64_t rows,
+                                  uint32_t* head, uint8_t* split, uint32_t* impure) {
+  const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= rows) return;
+  const bool start = k == 0 || keys[k] != keys[k - 1];
+  head[k] = start ? 1 : 0;
+  bool differs = false;
+  if (!start) {
+    const uint32_t r = idx[k], p = idx[k - 1];
+    if (sv_ld(T.t[0] + r) != sv_ld(T.t[0] + p) || sv_ld(T.t[1] + r) != sv_ld(T.t[1] + p) ||
+        (T.t[3] && sv_ld(T.t[3] + r) != sv_ld(T.t[3] + p)))
+      atomicAdd(impure, 1u);
+    differs = sv_ld(T.t[2] + r) != sv_ld(T.t[2] + p);
+  }
+  split[k] = differs ? 1 : 0;
+}
+// per run u (run[k]: 1-based run of sorted position k): its word, its first table row, and amb[u] = 1 when two of its
+// rows give different t3 (amb zeroed before)
+__global__ void k_solve_tab_unique(const uint64_t* keys, const uint32_t* idx, const uint32_t* head,
+                                   const uint32_t* run, const uint8_t* split, uint64_t rows, uint64_t* word,
+                                   uint32_t* row, uint8_t* amb) {
+  const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= rows) return;
+  const uint32_t u = run[k] - 1;
+  if (head[k]) {
+    word[u] = keys[k];
+    row[u] = idx[k];
+  }
+  if (split[k]) amb[u] = 1;
 }
 
 __global__ void k_solve_heads(const uint64_t* keys, uint64_t m, int cb, uint32_t* head) {
@@ -133,6 +197,15 @@ __device__ __forceinline__ uint64_t sv_now() {
   return t;
 }
 
+// what the evaluation of table-defining rows reads and writes: the qualify flags (PB_SOLVE_BY_TABLE), Q_T (Montgomery,
+// null for one untagged table), the index, and per row a miss and an ambiguous flag
+struct SolveLk {
+  const uint8_t* qual;
+  const Fr* qt;
+  SolveTable T;
+  uint8_t *miss, *amb;
+};
+
 // the defining rows rows[0, n_def), ascending, in dependency order (see the file comment).  status[0]: the ticket,
 // status[1]: set when a warp stalled.
 __global__ void __launch_bounds__(128) k_solve_eval(SolveSel s, const uint32_t* rows, uint64_t n_def,
@@ -189,6 +262,90 @@ __global__ void __launch_bounds__(128) k_solve_eval(SolveSel s, const uint32_t* 
   }
 }
 
+// k_solve_eval with rows that define from their table: a row flagged PB_SOLVE_BY_TABLE probes the index (solve_probe)
+// instead of running the gate body.  A miss or an ambiguous key sets the row's flag and still stores c = 0 and the
+// ready flag, so the rows that depend on it finish.  (A kernel of its own, so that k_solve_eval stays as it was.)
+__global__ void __launch_bounds__(128) k_solve_eval_lookup(SolveSel s, SolveLk lk, const uint32_t* rows,
+                                                           uint64_t n_def, const uint32_t* var_of_cell, Fr* val,
+                                                           uint32_t* ready, uint32_t* status) {
+  const uint32_t lane = threadIdx.x & 31;
+  cuda::atomic_ref<uint32_t, cuda::thread_scope_device> stalled(status[1]);
+  for (;;) {
+    uint32_t t = 0;
+    if (lane == 0) t = atomicAdd(status, 1u);
+    t = __shfl_sync(0xffffffffu, t, 0);
+    const uint64_t i = (uint64_t)t * 32 + lane;
+    if ((uint64_t)t * 32 >= n_def) return;
+    bool done = i >= n_def;
+    uint32_t vl = 0, vr = 0, vo = 0;
+    SolveRow sr;
+    uint64_t row = 0;
+    bool table = false;
+    Fr tag;
+    if (!done) {
+      const uint64_t r = rows[i];
+      vl = var_of_cell[3 * r];
+      vr = var_of_cell[3 * r + 1];
+      vo = var_of_cell[3 * r + 2];
+      row = r;
+      table = lk.qual[r] == PB_SOLVE_BY_TABLE;
+      if (table) {
+        tag = lk.qt ? sv_ld(lk.qt + r) : Fr::zero();
+      } else {
+        sr.ql = sv_ld(s.ql + r);
+        sr.qr = sv_ld(s.qr + r);
+        sr.qm = sv_ld(s.qm + r);
+        sr.qc = sv_ld(s.qc + r);
+        sr.neg_inv_qo = fp_neg(sv_ld(s.inv_qo + r));
+#pragma unroll
+        for (int k = 0; k < PB_MAX_CUSTOM; k++) sr.q[k] = k < s.n_custom ? sv_ld(s.q[k] + r) : Fr::zero();
+      }
+    }
+    uint64_t since = sv_now();
+    while (!__all_sync(0xffffffffu, done)) {
+      bool moved = false;
+      if (!done) {
+        cuda::atomic_ref<uint32_t, cuda::thread_scope_device> rl(ready[vl]), rr(ready[vr]);
+        if (rl.load(cuda::memory_order_acquire) && rr.load(cuda::memory_order_acquire)) {
+          const Fr a = val[vl], b = val[vr];
+          if (table) {
+            Fr c;
+            const int e = solve_probe(lk.T, tag, a, b, &c);
+            if (e == PB_SOLVE_MISS) lk.miss[row] = 1;
+            if (e == PB_SOLVE_AMBIGUOUS) lk.amb[row] = 1;
+            val[vo] = c;
+          } else {
+            val[vo] = solve_gate(sr, s.f, s.n_custom, a, b);
+          }
+          cuda::atomic_ref<uint32_t, cuda::thread_scope_device>(ready[vo]).store(1, cuda::memory_order_release);
+          done = moved = true;
+        }
+      }
+      if (__any_sync(0xffffffffu, moved)) {
+        since = sv_now();
+        continue;
+      }
+      // leave together: the decisions are the warp's, so no lane is left in a later __all_sync alone
+      if (__any_sync(0xffffffffu, lane == 0 && stalled.load(cuda::memory_order_relaxed))) return;
+      if (__any_sync(0xffffffffu, lane == 0 && sv_now() - since > PB_SOLVE_STALL_NS)) {
+        if (lane == 0) stalled.store(1, cuda::memory_order_relaxed);
+        return;
+      }
+      __nanosleep(64);
+    }
+  }
+}
+
+// a and b of each listed row, canonical, for the miss and ambiguous messages
+__global__ void k_solve_operands(const uint32_t* rows, uint32_t count, const uint32_t* var_of_cell, const Fr* val,
+                                 Fr* out) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= count) return;
+  const uint64_t r = rows[k];
+  out[2 * k] = fp_from_mont(val[var_of_cell[3 * r]]);
+  out[2 * k + 1] = fp_from_mont(val[var_of_cell[3 * r + 1]]);
+}
+
 // every cell's value, canonical: W = A | B | C, column-major
 __global__ void k_solve_write(const uint32_t* var_of_cell, const Fr* val, uint64_t n, Fr* A, Fr* B, Fr* C) {
   const uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -229,13 +386,89 @@ static void solve_launched(Context* ctx) {
   PB_CUDA(cudaGetLastError());
 }
 
-// see plonk_b200.h (pb200_solve_wires)
+// the table index of T's columns (rows table rows) into T.word / T.row / T.amb; sets T.theta, T.theta2 and T.n_keys.
+// The (word, row) pairs are sorted; neighbours with equal words must have equal keys, else theta is drawn again.  The
+// runs of equal words are then the distinct keys, in ascending word order.  temp: at least SortPairs' storage over rows
+// items and InclusiveSum's; impure: one device word.
+static void solve_table_index(Context* ctx, SolveTable& T, uint64_t rows, DevBuf& temp, uint32_t* impure) {
+  cudaStream_t st = ctx->stream;
+  DevBuf k1(rows * 8), k2(rows * 8), r1(rows * 4), r2(rows * 4), head(rows * 4), run(rows * 4), split(rows);
+  cub::DoubleBuffer<uint64_t> keys(k1.as<uint64_t>(), k2.as<uint64_t>());
+  cub::DoubleBuffer<uint32_t> idx(r1.as<uint32_t>(), r2.as<uint32_t>());
+  for (int draw = 0;; draw++) {
+    PB_CHECK(draw < 8, "solving the wires: eight table words in a row had colliding keys");
+    T.theta = check_random_fr();
+    T.theta2 = fp_sqr(T.theta);
+    k_solve_tab_keys<<<PB_SOLVE_GRID(rows, 128), 0, st>>>(T, rows, k1.as<uint64_t>(), r1.as<uint32_t>());
+    solve_launched(ctx);
+    keys = cub::DoubleBuffer<uint64_t>(k1.as<uint64_t>(), k2.as<uint64_t>());
+    idx = cub::DoubleBuffer<uint32_t>(r1.as<uint32_t>(), r2.as<uint32_t>());
+    size_t tb = temp.bytes;
+    PB_CUDA(cub::DeviceRadixSort::SortPairs(temp.p, tb, keys, idx, (int)rows, 0, 64, st));
+    ctx->launches++;
+    PB_CUDA(cudaMemsetAsync(impure, 0, 4, st));
+    k_solve_tab_heads<<<PB_SOLVE_GRID(rows, 256), 0, st>>>(T, keys.Current(), idx.Current(), rows, head.as<uint32_t>(),
+                                                           split.as<uint8_t>(), impure);
+    solve_launched(ctx);
+    uint32_t imp = 0;
+    PB_CUDA(cudaMemcpyAsync(&imp, impure, 4, cudaMemcpyDeviceToHost, st));
+    PB_CUDA(cudaStreamSynchronize(st));
+    if (imp == 0) break;
+  }
+  size_t tb = temp.bytes;
+  PB_CUDA(cub::DeviceScan::InclusiveSum(temp.p, tb, head.as<uint32_t>(), run.as<uint32_t>(), (int)rows, st));
+  ctx->launches++;
+  PB_CUDA(cudaMemsetAsync(const_cast<uint8_t*>(T.amb), 0, rows, st));
+  k_solve_tab_unique<<<PB_SOLVE_GRID(rows, 256), 0, st>>>(keys.Current(), idx.Current(), head.as<uint32_t>(),
+                                                          run.as<uint32_t>(), split.as<uint8_t>(), rows,
+                                                          const_cast<uint64_t*>(T.word), const_cast<uint32_t*>(T.row),
+                                                          const_cast<uint8_t*>(T.amb));
+  solve_launched(ctx);
+  uint32_t keys_n = 0;
+  PB_CUDA(cudaMemcpyAsync(&keys_n, run.as<uint32_t>() + rows - 1, 4, cudaMemcpyDeviceToHost, st));
+  PB_CUDA(cudaStreamSynchronize(st));  // the index's temporaries die here
+  T.n_keys = keys_n;
+}
+
+// q_K, Q_T and the table as pb200_prover_set_lookup(_tagged) takes them, with its refusals (prover.cu,
+// prover_set_lookup)
+static void solve_require_lookup(uint64_t n, const uint8_t* h_qk, const uint8_t* h_qtag, const uint8_t* const* h_tab,
+                                 uint64_t rows) {
+  const bool tagged = h_qtag != nullptr;
+  PB_CHECK(h_qk && h_tab[0] && h_tab[1] && h_tab[2], "lookups need q_K and three table columns");
+  PB_CHECK(!tagged || h_tab[3], "tagged lookups need the table tag column t4");
+  PB_CHECK(rows >= 1, "the lookup table is empty");
+  PB_CHECK(rows <= n, "the lookup table has more rows than the circuit");
+  for (uint64_t i = 0; i < n; i++) {
+    const uint8_t* e = h_qk + 32 * i;
+    bool ok = e[0] <= 1;
+    for (int k = 1; k < 32 && ok; k++) ok = e[k] == 0;
+    PB_CHECK(ok, "q_K must be 0 or 1 on every row");
+    if (!tagged) continue;
+    Fr x;
+    memcpy(x.v, h_qtag + 32 * i, 32);
+    PB_CHECK(fp_is_canonical(x), ("Q_T on row " + std::to_string(i) + " not reduced below the field modulus").c_str());
+    PB_CHECK(e[0] == 1 || x.is_zero(), ("Q_T must be 0 where q_K = 0: row " + std::to_string(i)).c_str());
+  }
+  for (int w = 0; w < (tagged ? 4 : 3); w++)
+    for (uint64_t r = 0; r < rows; r++) {
+      Fr x;
+      memcpy(x.v, h_tab[w] + 32 * r, 32);
+      PB_CHECK(fp_is_canonical(x), "lookup table value not reduced below the field modulus");
+    }
+}
+
+// see plonk_b200.h (pb200_solve_wires, and pb200_solve_wires_lookup when h_tab is not null: then h_counts has four
+// entries and h_lists 5 limit)
 void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constraints, const uint8_t* const* h_sel,
                int n_custom, const uint8_t* h_exps, const uint8_t* const* h_custom, uint64_t n_inputs,
                const int64_t* h_in_ids, const uint8_t* h_in_vals, uint32_t limit, uint64_t* h_counts,
-               uint32_t* h_lists, void* const* out, bool out_on_device) {
+               uint32_t* h_lists, void* const* out, bool out_on_device, const uint8_t* h_qk, const uint8_t* h_qtag,
+               const uint8_t* const* h_tab, uint64_t tab_rows, uint8_t* h_operands) {
   PB_CHECK(log_n >= 1 && log_n <= 26, "group order must be 2^k, 1 <= k <= 26 (the prover's range)");
   const uint64_t n = (uint64_t)1 << log_n, m = 3 * n;
+  const bool lookup = h_tab != nullptr;
+  const bool tagged = lookup && h_qtag != nullptr;
   PB_CHECK(n_constraints <= n, "n_constraints above the group order");
   PB_CHECK(h_ids && h_sel && h_counts && (h_lists || limit == 0) && out && (h_in_ids || n_inputs == 0) &&
                (h_in_vals || n_inputs == 0),
@@ -294,24 +527,33 @@ void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constra
     in_keys[k] = (uint64_t)(h_in_ids[order[k]] + 1);
     memcpy(&in_vals[32 * k], h_in_vals + 32 * order[k], 32);
   }
+  if (lookup) solve_require_lookup(n, h_qk, h_qtag, h_tab, tab_rows);
 
   const int cb = perm_cell_bits(log_n);
   const int end_bit = perm_sort_bits(log_n, max_id);
   cudaStream_t st = ctx->stream;
-  size_t t_sort = 0, t_scan = 0, t_sel = 0;
+  size_t t_sort = 0, t_scan = 0, t_sel = 0, t_tab = 0;
   {
     cub::DoubleBuffer<uint64_t> d(nullptr, nullptr);
     PB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, t_sort, d, (int)m, 0, end_bit, st));
     PB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, t_scan, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)m, st));
     PB_CUDA(cub::DeviceSelect::Flagged(nullptr, t_sel, thrust::counting_iterator<uint32_t>(0), (const uint8_t*)nullptr,
                                        (uint32_t*)nullptr, (uint32_t*)nullptr, (int)m, st));
+    if (lookup) {
+      cub::DoubleBuffer<uint32_t> v(nullptr, nullptr);
+      PB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t_tab, d, v, (int)tab_rows, 0, 64, st));
+    }
   }
-  const uint64_t temp_bytes = std::max(t_sort, std::max(t_scan, t_sel));
+  const uint64_t temp_bytes = std::max(std::max(t_sort, t_tab), std::max(t_scan, t_sel));
   // keys and alt (8 each), heads / run (4 each), var_of_cell, inp, def_row, ready (4 each), the values (32), the index
   // list (4), three flag bytes: per cell.  Selectors, 1 / QO and the custom selectors (32 each), the qualify and
   // defines flags: per row.  The inputs, the host outputs' staging and the sort's storage.
-  const uint64_t need = m * (8 + 8 + 4 + 4 + 4 * 4 + 32 + 4 + 3) + n * (32 * (6 + (uint64_t)n_custom) + 2) +
-                        n_inputs * 40 + (out_on_device ? 0 : m * 32) + temp_bytes + 256;
+  uint64_t need = m * (8 + 8 + 4 + 4 + 4 * 4 + 32 + 4 + 3) + n * (32 * (6 + (uint64_t)n_custom) + 2) +
+                  n_inputs * 40 + (out_on_device ? 0 : m * 32) + temp_bytes + 256;
+  // with a table: q_K and Q_T (32 each) and the miss and ambiguous flags (1 each) per row; per table row its columns
+  // (4 x 32), the sort's words and rows (2 x 8, 2 x 4), heads and runs (4 each), the split flag, the index (8 + 4 + 1);
+  // the listed rows' operands
+  if (lookup) need += n * (32 + 32 + 2) + tab_rows * (4 * 32 + 16 + 8 + 8 + 1 + 13) + (uint64_t)limit * 2 * 64 + 256;
   size_t free_b = 0, total_b = 0;
   PB_CUDA(cudaMemGetInfo(&free_b, &total_b));
   // PB200_SOLVE_MAX_BYTES: the most device memory a solve may take (read per call), so it leaves room for other work
@@ -358,6 +600,30 @@ void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constra
     PB_CUDA(cudaMemcpyAsync(inids.p, in_keys.data(), n_inputs * 8, cudaMemcpyHostToDevice, st));
     PB_CUDA(cudaMemcpyAsync(invals.p, in_vals.data(), n_inputs * 32, cudaMemcpyHostToDevice, st));
   }
+  // the table: q_K (canonical), Q_T and the table columns (Montgomery), the per-row error flags
+  const int width = tagged ? 4 : 3;
+  DevBuf qkb(lookup ? n * 32 : 0), qtb(tagged ? n * 32 : 0), tabb(lookup ? width * tab_rows * 32 : 0),
+      errf(lookup ? 2 * n : 0);
+  SolveLk lk = {};
+  if (lookup) {
+    PB_CUDA(cudaMemcpyAsync(qkb.p, h_qk, n * 32, cudaMemcpyHostToDevice, st));
+    if (tagged) {
+      PB_CUDA(cudaMemcpyAsync(qtb.p, h_qtag, n * 32, cudaMemcpyHostToDevice, st));
+      fr_to_mont(ctx, qtb.as<Fr>(), qtb.as<Fr>(), n);
+    }
+    for (int w = 0; w < width; w++) {
+      lk.T.t[w] = tabb.as<Fr>() + (uint64_t)w * tab_rows;
+      PB_CUDA(cudaMemcpyAsync(tabb.as<Fr>() + (uint64_t)w * tab_rows, h_tab[w], tab_rows * 32, cudaMemcpyHostToDevice,
+                              st));
+    }
+    fr_to_mont(ctx, tabb.as<Fr>(), tabb.as<Fr>(), width * tab_rows);
+    PB_CUDA(cudaMemsetAsync(errf.p, 0, 2 * n, st));
+    lk.qual = qual.as<uint8_t>();
+    lk.qt = tagged ? qtb.as<Fr>() : nullptr;
+    lk.miss = errf.as<uint8_t>();
+    lk.amb = lk.miss + n;
+    h_counts[2] = h_counts[3] = 0;
+  }
 
   // 1. group
   const uint64_t* sorted = perm_sort_keys(ctx, h_ids, m, cb, end_bit, keys, alt, temp, temp_bytes, 3 * n_constraints);
@@ -367,7 +633,8 @@ void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constra
   PB_CUDA(cub::DeviceScan::InclusiveSum(temp.p, tb, head.as<uint32_t>(), run.as<uint32_t>(), (int)m, st));
   ctx->launches++;
   // 2. sources and errors
-  k_solve_qualify<<<PB_SOLVE_GRID(n, 256), 0, st>>>(s, n_constraints, qual.as<uint8_t>());
+  if (lookup) k_solve_qualify_lookup<<<PB_SOLVE_GRID(n, 256), 0, st>>>(s, qkb.as<Fr>(), n_constraints, qual.as<uint8_t>());
+  else k_solve_qualify<<<PB_SOLVE_GRID(n, 256), 0, st>>>(s, n_constraints, qual.as<uint8_t>());
   solve_launched(ctx);
   PB_CUDA(cudaMemsetAsync(defr.p, 0xff, m * 4, st));
   PB_CUDA(cudaMemsetAsync(inp.p, 0xff, m * 4, st));  // variables past the last run: no source
@@ -380,7 +647,7 @@ void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constra
   k_solve_flags<<<PB_SOLVE_GRID(m, 256), 0, st>>>(voc.as<uint32_t>(), inp.as<uint32_t>(), defr.as<uint32_t>(), n,
                                                  f_unset, f_order, defines.as<uint8_t>());
   solve_launched(ctx);
-  for (uint64_t k = 0; k < 3 * (uint64_t)limit; k++) h_lists[k] = 0xffffffffu;
+  for (uint64_t k = 0; k < (lookup ? 5 : 3) * (uint64_t)limit; k++) h_lists[k] = 0xffffffffu;
   uint32_t* num = small_u + 1;
   h_counts[0] = solve_compact(ctx, f_unset, m, temp, idx.as<uint32_t>(), num, limit, h_lists);
   std::vector<uint32_t> cells(limit);
@@ -410,19 +677,55 @@ void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constra
   k_solve_init<<<PB_SOLVE_GRID(m, 256), 0, st>>>(inp.as<uint32_t>(), invals.as<Fr>(), m, val.as<Fr>(),
                                                 ready.as<uint32_t>());
   solve_launched(ctx);
+  DevBuf ix_word(lookup ? tab_rows * 8 : 0), ix_row(lookup ? tab_rows * 4 : 0), ix_amb(lookup ? tab_rows : 0);
+  if (lookup) {
+    lk.T.word = ix_word.as<uint64_t>();
+    lk.T.row = ix_row.as<uint32_t>();
+    lk.T.amb = ix_amb.as<uint8_t>();
+    solve_table_index(ctx, lk.T, tab_rows, temp, small_u + 6);
+  }
   const uint64_t n_def = solve_compact(ctx, defines.as<uint8_t>(), n, temp, idx.as<uint32_t>(), num, 0, nullptr);
   if (n_def) {
     int per_sm = 0;
-    PB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_solve_eval, 128, 0));
+    if (lookup) PB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_solve_eval_lookup, 128, 0));
+    else PB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_solve_eval, 128, 0));
     const uint64_t warps = (n_def + 31) / 32;
     const uint64_t blocks = std::min<uint64_t>((uint64_t)std::max(per_sm, 1) * ctx->sm_count, (warps + 3) / 4);
-    k_solve_eval<<<(unsigned)blocks, 128, 0, st>>>(s, idx.as<uint32_t>(), n_def, voc.as<uint32_t>(), val.as<Fr>(),
-                                                   ready.as<uint32_t>(), small_u + 4);
+    if (lookup)
+      k_solve_eval_lookup<<<(unsigned)blocks, 128, 0, st>>>(s, lk, idx.as<uint32_t>(), n_def, voc.as<uint32_t>(),
+                                                            val.as<Fr>(), ready.as<uint32_t>(), small_u + 4);
+    else
+      k_solve_eval<<<(unsigned)blocks, 128, 0, st>>>(s, idx.as<uint32_t>(), n_def, voc.as<uint32_t>(), val.as<Fr>(),
+                                                     ready.as<uint32_t>(), small_u + 4);
     solve_launched(ctx);
     uint32_t stalled = 0;
     PB_CUDA(cudaMemcpyAsync(&stalled, small_u + 5, 4, cudaMemcpyDeviceToHost, st));
     PB_CUDA(cudaStreamSynchronize(st));
     PB_CHECK(stalled == 0, "solving the wires stalled: a defining row waited too long for its operands");
+  }
+  if (lookup) {  // miss and ambiguous: rows, and the operands a, b of the listed ones
+    uint32_t* l_miss = h_lists + 3 * (uint64_t)limit;
+    uint32_t* l_amb = l_miss + limit;
+    h_counts[2] = solve_compact(ctx, lk.miss, n, temp, idx.as<uint32_t>(), num, limit, l_miss);
+    h_counts[3] = solve_compact(ctx, lk.amb, n, temp, idx.as<uint32_t>(), num, limit, l_amb);
+    const uint32_t take[2] = {(uint32_t)std::min<uint64_t>(h_counts[2], limit),
+                              (uint32_t)std::min<uint64_t>(h_counts[3], limit)};
+    if (h_operands && take[0] + take[1]) {
+      DevBuf lrows((size_t)(take[0] + take[1]) * 4), ops((size_t)(take[0] + take[1]) * 64);
+      PB_CUDA(cudaMemcpyAsync(lrows.p, l_miss, (size_t)take[0] * 4, cudaMemcpyHostToDevice, st));
+      PB_CUDA(cudaMemcpyAsync(lrows.as<uint32_t>() + take[0], l_amb, (size_t)take[1] * 4, cudaMemcpyHostToDevice, st));
+      k_solve_operands<<<PB_SOLVE_GRID(take[0] + take[1], 128), 0, st>>>(lrows.as<uint32_t>(), take[0] + take[1],
+                                                                          voc.as<uint32_t>(), val.as<Fr>(), ops.as<Fr>());
+      solve_launched(ctx);
+      PB_CUDA(cudaMemcpyAsync(h_operands, ops.p, (size_t)take[0] * 64, cudaMemcpyDeviceToHost, st));
+      PB_CUDA(cudaMemcpyAsync(h_operands + (uint64_t)limit * 64, ops.as<uint8_t>() + (size_t)take[0] * 64,
+                              (size_t)take[1] * 64, cudaMemcpyDeviceToHost, st));
+      PB_CUDA(cudaStreamSynchronize(st));
+    }
+    if (h_counts[2] || h_counts[3]) {
+      PB_CUDA(cudaStreamSynchronize(st));  // the call's buffers die here
+      return;
+    }
   }
   // 5. write
   DevBuf staging(out_on_device ? 0 : m * 32);

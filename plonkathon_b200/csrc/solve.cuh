@@ -1,5 +1,6 @@
-// Wire values of a circuit from its inputs (solve.cu): the gate body of a defining row, shared by the GPU solver and
-// csrc/host_selftest.cpp, which runs it on the CPU in row order.
+// Wire values of a circuit from its inputs (solve.cu): the gate body of a defining row and the table probe of a row
+// that defines from its table, shared by the GPU solver and csrc/host_selftest.cpp, which runs them on the CPU in row
+// order.
 //
 // A defining row r sets its O variable to c = -(QL a + QR b + QM a b + QC + sum_k Q_k m_k(a, b, 0)) / QO.  A row
 // defines only when no custom term whose selector is non-zero there reads c or the next row, so m_k is evaluated
@@ -36,6 +37,50 @@ PB_HD Fr solve_gate(const SolveRow& s, const uint8_t (*f)[3], int n_custom, cons
     acc = fp_add(acc, fp_mul(custom_monomial_next(a, b, z, z, z, z, f[k]), s.q[k]));
   }
   return fp_mul(acc, s.neg_inv_qo);
+}
+
+// ---- rows that define from their table (pb200_solve_wires_lookup) ----------------------------------------------------
+// A row r with q_K != 0 and QO = 0 sets c = t3 of the table rows whose (t4, t1, t2) equal (Q_T[r], a, b) (t4 = Q_T = 0
+// for one untagged table).  The table index holds the distinct keys (tag, t1, t2) of the table in ascending order of
+// their word (solve_table_word), with no two keys sharing a word (theta is drawn again until none do); for each key
+// one table row that carries it, and whether the table rows with that key give two different t3.
+struct SolveTable {
+  const uint64_t* word;  // n_keys words, ascending and distinct
+  const uint32_t* row;   // a table row with each key
+  const uint8_t* amb;    // 1 where the rows with the key disagree on t3
+  const Fr* t[4];        // t1 t2 t3 t4, Montgomery; t[3] null for one untagged table
+  uint64_t n_keys;
+  Fr theta, theta2;  // Montgomery
+};
+
+#define PB_SOLVE_HIT 0
+#define PB_SOLVE_MISS 1
+#define PB_SOLVE_AMBIGUOUS 2
+
+// the 64-bit word of a key: the low word of t1 + theta t2 + theta^2 tag (Montgomery)
+PB_HD uint64_t solve_table_word(const Fr& tag, const Fr& x, const Fr& y, const Fr& theta, const Fr& theta2) {
+  const Fr h = fp_add(x, fp_add(fp_mul(theta, y), fp_mul(theta2, tag)));
+  return (uint64_t)h.v[0] | ((uint64_t)h.v[1] << 32);
+}
+
+// c of a row that reads (a, b) from table `tag` (zero untagged), Montgomery.  The word only finds the one key that can
+// match; whether it does is decided on full values.  PB_SOLVE_MISS: no table row has the key; PB_SOLVE_AMBIGUOUS: its
+// rows give two different t3.  Both leave c = 0.
+PB_HD int solve_probe(const SolveTable& T, const Fr& tag, const Fr& a, const Fr& b, Fr* c) {
+  *c = Fr::zero();
+  const uint64_t w = solve_table_word(tag, a, b, T.theta, T.theta2);
+  uint64_t lo = 0, hi = T.n_keys;
+  while (lo < hi) {
+    const uint64_t mid = (lo + hi) / 2;
+    if (T.word[mid] < w) lo = mid + 1;
+    else hi = mid;
+  }
+  if (lo == T.n_keys || T.word[lo] != w) return PB_SOLVE_MISS;
+  const uint32_t r = T.row[lo];
+  if (T.t[0][r] != a || T.t[1][r] != b || (T.t[3] && T.t[3][r] != tag)) return PB_SOLVE_MISS;
+  if (T.amb[lo]) return PB_SOLVE_AMBIGUOUS;
+  *c = T.t[2][r];
+  return PB_SOLVE_HIT;
 }
 
 }  // namespace pb200

@@ -13,7 +13,8 @@ so it can only match a row of its own table: merging an XOR and an AND table wit
 for XOR pass with an AND row.
 
 Here: the checks on a lookup argument as users give it, ``(q_K, (t1, t2, t3))`` or a list of them, shared by
-``Prover.from_arrays``, ``Setup.verification_key_arrays`` and ``synthetic.build_circuit``.  Out of scope, and
+``Prover.from_arrays``, ``Setup.verification_key_arrays``, ``synthetic.build_circuit`` and ``solve_wires``, and common
+table shapes (``range_table``, ``op_table``, ``xor_table``, ``and_table``).  Out of scope, and
 refused: zero knowledge with lookups, the sharded prover, tables wider than three columns."""
 from __future__ import annotations
 
@@ -100,3 +101,25 @@ def to_le_rows(ints) -> np.ndarray:
     """ints -> contiguous (m,32) uint8 little-endian"""
     raw = b"".join(int(x).to_bytes(32, "little") for x in ints)
     return np.frombuffer(raw, dtype=np.uint8).reshape(-1, 32).copy()
+
+
+# ---- common table shapes, as (t1, t2, t3) lists of ints ---------------------------------------------------------------
+def range_table(k: int):
+    """(v, 0, 0) for v < k: a lookup row (a, 0, 0) checks a < k"""
+    return [list(range(k)), [0] * k, [0] * k]
+
+
+def op_table(bits: int, op):
+    """(x, y, op(x, y)) for x, y < 2^bits, x-major"""
+    rows = [(x, y, op(x, y)) for x in range(1 << bits) for y in range(1 << bits)]
+    return [list(c) for c in zip(*rows)]
+
+
+def xor_table(bits: int):
+    """(x, y, x ^ y) for x, y < 2^bits"""
+    return op_table(bits, lambda x, y: x ^ y)
+
+
+def and_table(bits: int):
+    """(x, y, x & y) for x, y < 2^bits"""
+    return op_table(bits, lambda x, y: x & y)

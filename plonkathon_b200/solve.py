@@ -4,8 +4,29 @@
 custom terms -- the way the reference runs a program (compiler/program.py:161-192): a row r < n_constraints defines
 its O variable v when v is not -1, QO[r] != 0, no custom term whose selector is non-zero at r reads c or the next
 row, v is not an input and no earlier row defines v; it sets c = -(QL a + QR b + QM a b + QC + sum_k Q_k a^i b^j) / QO.
-Every other variable (lookup and shuffle rows, public inputs, rows whose terms involve c or the next row, hints)
-must come as an input.  The wires stay on the device if asked, for ``Prover.check_arrays`` and ``prove_arrays``."""
+
+With ``lookup=`` or ``lookups=`` the gate rule stays exactly as it is.  In addition, a row r < n_constraints defines
+its O variable from its table when all of these hold:
+
+* q_K[r] != 0 (with ``lookups=``, the table is the one whose q_k is 1 at r, with its tag k);
+* QO[r] = 0 (a row with QO != 0 keeps the gate rule, and its lookup is only checked when proving);
+* the O variable is not -1, not an input, and not defined by an earlier row (of either kind).
+
+Such a row sets c = t3 of the table row whose (t1, t2), and tag when tagged, equal (a, b) and the row's tag.  Within a
+table, t3 must be a function of (t1, t2); table rows that repeat the same (t1, t2, t3) are fine.  A range table
+(v, 0, 0) read as (a, -1, -1) defines nothing, so it stays a pure check.  The ``unset`` and ``order`` errors apply to
+table-defining rows exactly as to gate rows: an L or R operand must be the constant 0, an input, or defined by a
+strictly earlier row.  Two more error kinds can only be found while the rows are evaluated, so they only arise when
+``unset`` and ``order`` are both 0:
+
+* ``miss``: a table-defining row whose (tag, a, b) matches no row of its table;
+* ``ambiguous``: a table-defining row whose (tag, a, b) matches table rows with different t3.
+
+Each is an exact count with its lowest ``limit`` rows.  With any error, no wires are returned.
+
+Every other variable (shuffle out-rows, public inputs, rows whose terms involve c or the next row, hints, and lookup
+rows without a table argument) must come as an input.  The wires stay on the device if asked, for
+``Prover.check_arrays`` and ``prove_arrays``."""
 from __future__ import annotations
 
 import ctypes
@@ -16,6 +37,7 @@ import numpy as np
 from ._lib import check, default_context, lib
 from .custom_gates import padded, split_terms
 from .field import CURVE_ORDER
+from .lookup import check_lookup, check_lookups, to_le_rows
 from .wiring import MAX_ID, MAX_LOG_N, _wire
 
 WIRE = "LRO"
@@ -29,7 +51,10 @@ class WireSolution:
 
     * ``unset``: cells whose variable is neither an input nor defined by a row (``unset_cells``: cell = 3 row + col);
     * ``order``: L or R cells of a defining row whose variable that row or a later row defines (``order_cells``:
-      (cell, the defining row))."""
+      (cell, the defining row));
+    * ``miss``: rows that define from their table and whose (tag, a, b) matches no table row (``miss_rows``);
+    * ``ambiguous``: rows that define from their table and whose (tag, a, b) matches table rows with different t3
+      (``ambiguous_rows``)."""
     A: object
     B: object
     C: object
@@ -39,10 +64,30 @@ class WireSolution:
     order_cells: list
     limit: int
     _ids: np.ndarray = field(default=None, repr=False, compare=False)
+    miss: int = 0
+    ambiguous: int = 0
+    miss_rows: list = field(default_factory=list)
+    ambiguous_rows: list = field(default_factory=list)
+    # for the miss and ambiguous lines: {row: (a, b)}, and (Q_T per row or None, [t1, t2, t3(, t4)] as ints)
+    _operands: dict = field(default=None, repr=False, compare=False)
+    _table: tuple = field(default=None, repr=False, compare=False)
 
     @property
     def ok(self) -> bool:
-        return not (self.unset or self.order)
+        return not (self.unset or self.order or self.miss or self.ambiguous)
+
+    def _table_of(self, row) -> int:
+        qt = self._table[0] if self._table else None
+        return int(qt[row]) if qt is not None else 0
+
+    def _t3_values(self, tag, a, b) -> list:
+        """the distinct t3 of the table rows with key (tag, a, b), in table order"""
+        cols = self._table[1]
+        out = []
+        for r in range(len(cols[0])):
+            if cols[0][r] == a and cols[1][r] == b and (len(cols) < 4 or cols[3][r] == tag) and cols[2][r] not in out:
+                out.append(cols[2][r])
+        return out
 
     def lines(self) -> list:
         out = []
@@ -54,7 +99,17 @@ class WireSolution:
             row, col = divmod(c, 3)
             out.append("order: row %d reads variable %d (cell (%d, %s)), which row %d defines"
                        % (row, int(self._ids[c]), row, WIRE[col], d))
-        for k, listed in (("unset", self.unset_cells), ("order", self.order_cells)):
+        for r in self.miss_rows:
+            a, b = self._operands[r]
+            out.append("miss: row %d looks up (a, b) = (%d, %d) in table %d, which has no such row"
+                       % (r, a, b, self._table_of(r)))
+        for r in self.ambiguous_rows:
+            a, b = self._operands[r]
+            tag = self._table_of(r)
+            out.append("ambiguous: row %d looks up (a, b) = (%d, %d) in table %d, whose rows give %s"
+                       % (r, a, b, tag, " and ".join("c = %d" % c for c in self._t3_values(tag, a, b)[:2])))
+        for k, listed in (("unset", self.unset_cells), ("order", self.order_cells), ("miss", self.miss_rows),
+                          ("ambiguous", self.ambiguous_rows)):
             if getattr(self, k) > len(listed):
                 out.append("%s: %d more" % (k, getattr(self, k) - len(listed)))
         return out
@@ -62,8 +117,8 @@ class WireSolution:
     def __str__(self) -> str:
         if self.ok:
             return "wires solved"
-        head = "wires unsolved: " + ", ".join("%d %s" % (getattr(self, k), k) for k in ("unset", "order")
-                                              if getattr(self, k))
+        head = "wires unsolved: " + ", ".join("%d %s" % (getattr(self, k), k)
+                                              for k in ("unset", "order", "miss", "ambiguous") if getattr(self, k))
         return "\n".join([head] + ["  " + s for s in self.lines()])
 
 
@@ -80,6 +135,16 @@ def _column(name, col, n) -> np.ndarray:
     if any(not 0 <= v < CURVE_ORDER for v in vals):
         raise ValueError("%s holds a value not reduced below r" % name)
     return np.frombuffer(b"".join(v.to_bytes(32, "little") for v in vals), dtype=np.uint8).reshape(n, 32).copy()
+
+
+def _le_rows(ints) -> np.ndarray:
+    """ints in [0, r) -> contiguous (m, 32) uint8 little-endian; through numpy when they all fit 64 bits (q_K, Q_T and
+    small tables), else as lookup.to_le_rows"""
+    if not ints or max(ints) >= 1 << 64:
+        return to_le_rows(ints)
+    out = np.zeros((len(ints), 4), np.uint64)
+    out[:, 0] = np.array(ints, dtype=np.uint64)
+    return out.view(np.uint8).reshape(-1, 32)
 
 
 def _inputs(inputs):
@@ -127,7 +192,8 @@ def _inputs(inputs):
 
 
 def solve_wires(wire_L, wire_R, wire_O, pk: dict, inputs, group_order: int, n_constraints: int | None = None,
-                custom=(), device: bool = False, limit: int = 16, ctx=None) -> WireSolution:
+                custom=(), device: bool = False, limit: int = 16, ctx=None, lookup=None,
+                lookups=None) -> WireSolution:
     """-> ``WireSolution``: the wire values A, B, C of the circuit, each (n, 32) canonical little-endian, or its
     errors.
 
@@ -135,8 +201,10 @@ def solve_wires(wire_L, wire_R, wire_O, pk: dict, inputs, group_order: int, n_co
     QL QR QM QO QC (n ints or (n, 32) uint8 arrays).  ``inputs``: a dict variable id -> value, or a pair (ids,
     (k, 32) uint8 values).  ``custom``: the custom terms as ``Prover.from_arrays(custom=)`` takes them.  ``device``:
     A, B, C as (n, 32) uint8 CUDA tensors on the context's device (no copy to the host), else numpy arrays.
-    ``limit``: how many locations of each error kind to list.  Malformed arguments are a ValueError before the library
-    is called; the solve runs on the GPU of ``ctx`` (default: the default context)."""
+    ``limit``: how many locations of each error kind to list.  ``lookup`` = (q_K, (t1, t2, t3)) or ``lookups`` =
+    [(q_0, (t1, t2, t3)), ...], as ``Prover.from_arrays`` takes them: lookup rows then define from their table (the
+    module docstring has the rule).  Malformed arguments are a ValueError before the library is called; the solve runs
+    on the GPU of ``ctx`` (default: the default context)."""
     n = group_order
     if isinstance(n, bool) or not isinstance(n, (int, np.integer)) or n < 2 or n & (n - 1) or n > 1 << MAX_LOG_N:
         raise ValueError("group_order must be a power of two in [2, 2^%d], got %r" % (MAX_LOG_N, n))
@@ -158,6 +226,14 @@ def solve_wires(wire_L, wire_R, wire_O, pk: dict, inputs, group_order: int, n_co
     exps, ccols = split_terms(custom, n)
     cust = [_column("custom selector %r" % (e,), c, n) for e, c in zip(exps, ccols)]
     in_ids, in_vals = _inputs(inputs)
+    if lookup is not None and lookups is not None:
+        raise ValueError("pass either lookup= (one table) or lookups= (several tables), not both")
+    table = None
+    if lookup is not None:
+        qk, tcols, rows = check_lookup(lookup, n)
+        table = (qk, None, tcols, rows)
+    elif lookups is not None:
+        table = check_lookups(lookups, n)
     ctx = ctx or default_context()
 
     vp = ctypes.c_void_p
@@ -175,13 +251,42 @@ def solve_wires(wire_L, wire_R, wire_O, pk: dict, inputs, group_order: int, n_co
     else:
         out = [np.empty((n, 32), dtype=np.uint8) for _ in range(3)]
         ptrs = [a.ctypes.data for a in out]
-    check(lib().pb200_solve_wires(ctx.handle, ids.ctypes.data_as(vp), n.bit_length() - 1, m, sel_arr, len(exps),
-                                  ebytes, cust_arr, len(in_ids), in_ids.ctypes.data_as(vp), in_vals.ctypes.data_as(vp),
-                                  limit, counts, lists, (vp * 3)(*ptrs), 1 if device else 0))
+    if table is None:
+        check(lib().pb200_solve_wires(ctx.handle, ids.ctypes.data_as(vp), n.bit_length() - 1, m, sel_arr, len(exps),
+                                      ebytes, cust_arr, len(in_ids), in_ids.ctypes.data_as(vp),
+                                      in_vals.ctypes.data_as(vp), limit, counts, lists, (vp * 3)(*ptrs),
+                                      1 if device else 0))
+    else:
+        qk, qt, tcols, rows = table
+        qk_a = _le_rows(qk)
+        qt_a = _le_rows(qt) if qt is not None else None
+        tab = [_le_rows(c) for c in tcols]  # t1 t2 t3, and t4 with lookups=
+        counts = (ctypes.c_uint64 * 4)()
+        lists = (ctypes.c_uint32 * max(1, 5 * limit))()
+        operands = np.zeros((max(1, 4 * limit), 32), np.uint8)
+        col = lambda a: a.ctypes.data_as(vp) if a is not None else None  # noqa: E731
+        check(lib().pb200_solve_wires_lookup(ctx.handle, ids.ctypes.data_as(vp), n.bit_length() - 1, m, sel_arr,
+                                             len(exps), ebytes, cust_arr, len(in_ids), in_ids.ctypes.data_as(vp),
+                                             in_vals.ctypes.data_as(vp), col(qk_a), col(qt_a), col(tab[0]),
+                                             col(tab[1]), col(tab[2]), col(tab[3]) if len(tab) > 3 else None, rows,
+                                             limit, counts, lists, operands.ctypes.data_as(vp), (vp * 3)(*ptrs),
+                                             1 if device else 0))
     raw = [int(x) for x in lists[:3 * limit]]
     unset = [x for x in raw[:limit] if x != 0xffffffff]
     pairs = raw[limit:3 * limit]
     order = [(pairs[2 * k], pairs[2 * k + 1]) for k in range(limit) if pairs[2 * k] != 0xffffffff]
-    ok = not (counts[0] or counts[1])
+    ok = not any(counts)
     A, B, C = out if ok else (None, None, None)
-    return WireSolution(A, B, C, int(counts[0]), int(counts[1]), unset, order, limit, ids.reshape(-1))
+    sol = WireSolution(A, B, C, int(counts[0]), int(counts[1]), unset, order, limit, ids.reshape(-1))
+    if table is not None:
+        more = [int(x) for x in lists[3 * limit:5 * limit]]
+        sol.miss, sol.ambiguous = int(counts[2]), int(counts[3])
+        sol.miss_rows = [x for x in more[:limit] if x != 0xffffffff]
+        sol.ambiguous_rows = [x for x in more[limit:] if x != 0xffffffff]
+        ops = operands.reshape(-1, 32).tobytes()
+        val = lambda k: int.from_bytes(ops[32 * k:32 * k + 32], "little")  # noqa: E731
+        sol._operands = {r: (val(2 * k), val(2 * k + 1)) for k, r in enumerate(sol.miss_rows)}
+        sol._operands.update({r: (val(2 * limit + 2 * k), val(2 * limit + 2 * k + 1))
+                              for k, r in enumerate(sol.ambiguous_rows)})
+        sol._table = (table[1], table[2])
+    return sol

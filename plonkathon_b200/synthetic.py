@@ -248,6 +248,89 @@ def build_circuit(log_n: int, seed: int = 20260924, n_public: int = 2, fill: flo
                         (q_in, q_out) if shuffle else ())
 
 
+def table_circuit(log_n: int, bits: int = 4, chains: int = 1, tagged: bool = True, seed: int = 1) -> ArrayCircuit:
+    """A bit-manipulation circuit whose table rows read computed values and whose computed values come from tables:
+    ``chains`` independent chains, interleaved row by row (1: every row depends on the one before it; many: wide).
+
+    Each chain starts from two seeds x, y < 2^bits, the circuit's only free variables, and repeats a step while the
+    circuit has room for one more step of every chain.  With ``tagged`` (three tables: range(2^(2 bits)) as table 0,
+    XOR as table 1, AND as table 2, ``lookups=``) a step is six rows:
+      z = x ^ y (XOR row), w = x & z (AND row), nz = (2^bits - 1) - z (gate), u = 2^bits w + z (gate, recombination),
+      (u, 0, 0) in the range table (a pure check, O = -1), p = u nz (gate); then x, y = nz, w.
+    Without it (one XOR table, ``lookup=``) four rows: z = x ^ y, nz = (2^bits - 1) - z, u = 2^bits x + z, p = u nz;
+    then x, y = y, nz.  Lookup rows have every gate selector 0.  The values are computed here (``wires_values()``);
+    ``solve_wires(..., lookup(s)=)`` finds them from the seeds alone.  ValueError when the tables (3 * 2^(2 bits) or
+    2^(2 bits) rows) or one step of every chain do not fit 2^log_n rows."""
+    from .lookup import and_table, range_table, xor_table
+    n = 1 << log_n
+    mask = (1 << bits) - 1
+    if bits < 1:
+        raise ValueError("bits must be at least 1, got %r" % (bits,))
+    tabs = [range_table(1 << (2 * bits)), xor_table(bits), and_table(bits)] if tagged else [xor_table(bits)]
+    total = sum(len(t[0]) for t in tabs)
+    if total > n:
+        raise ValueError("the tables have %d rows in all, more than the circuit's %d" % (total, n))
+    per_step = 6 if tagged else 4
+    if chains < 1 or per_step * chains > n:
+        raise ValueError("%d chains of %d-row steps do not fit %d rows" % (chains, per_step, n))
+    steps = n // (per_step * chains)
+    m = steps * per_step * chains
+    rng = random.Random(seed)
+    values = []
+    for _ in range(2 * chains):
+        values.append(rng.randrange(1 << bits))
+    x = list(range(0, 2 * chains, 2))
+    y = list(range(1, 2 * chains, 2))
+    wL = np.full(n, -1, dtype=np.int64)
+    wR = np.full(n, -1, dtype=np.int64)
+    wO = np.full(n, -1, dtype=np.int64)
+    QL, QR, QM, QO, QC = ([0] * n for _ in range(5))
+    Q = [[0] * n for _ in tabs]
+    T_RANGE, T_XOR, T_AND = (0, 1, 2) if tagged else (None, 0, None)
+    row = 0
+
+    def new(v):
+        values.append(v)
+        return len(values) - 1
+
+    def put(a, b, o):
+        nonlocal row
+        wL[row], wR[row], wO[row] = a, b, o
+        row += 1
+        return row - 1
+
+    val = values.__getitem__
+    for _ in range(steps):
+        z = [new(val(x[k]) ^ val(y[k])) for k in range(chains)]
+        for k in range(chains):
+            Q[T_XOR][put(x[k], y[k], z[k])] = 1
+        if tagged:
+            w = [new(val(x[k]) & val(z[k])) for k in range(chains)]
+            for k in range(chains):
+                Q[T_AND][put(x[k], z[k], w[k])] = 1
+        nz = [new(mask - val(z[k])) for k in range(chains)]
+        for k in range(chains):
+            r = put(z[k], z[k], nz[k])
+            QL[r], QC[r], QO[r] = 1, (R - mask) % R, 1
+        hi = w if tagged else x
+        u = [new((val(hi[k]) << bits) + val(z[k])) for k in range(chains)]
+        for k in range(chains):
+            r = put(hi[k], z[k], u[k])
+            QL[r], QR[r], QO[r] = 1 << bits, 1, R - 1
+        if tagged:
+            for k in range(chains):
+                Q[T_RANGE][put(u[k], -1, -1)] = 1
+        p = [new(val(u[k]) * val(nz[k]) % R) for k in range(chains)]
+        for k in range(chains):
+            r = put(u[k], nz[k], p[k])
+            QM[r], QO[r] = R - 1, 1
+        x, y = (nz, w) if tagged else (y, nz)
+    assert row == m
+    lk = (Q[0], tuple(tabs[0])) if not tagged else ()
+    lks = tuple((q, tuple(t)) for q, t in zip(Q, tabs)) if tagged else ()
+    return ArrayCircuit(n, m, wL, wR, wO, QL, QR, QM, QO, QC, 0, values, [], [], lk, lks)
+
+
 def _custom_row(exps, Q, row, operands, k, values, wires, sel):
     """One row using the custom term a^i b^j c^l (selector column Q).  The wires of the monomial take the operands;
     the output goes on the first wire the term does not use:
