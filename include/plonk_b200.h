@@ -206,6 +206,32 @@ int pb200_solve_wires_lookup(pb200_ctx* ctx, const int64_t* h_ids, int log_n, ui
                              const uint8_t* h_t1, const uint8_t* h_t2, const uint8_t* h_t3, const uint8_t* h_t4,
                              uint64_t table_rows, uint32_t limit, uint64_t* h_counts, uint32_t* h_lists,
                              uint8_t* h_operands, void* const* out, int out_on_device);
+/* pb200_solve_wires for a circuit with a shuffle: the out-rows get the in-rows' tuples, sorted.  h_qin, h_qout (n x 32
+ * bytes, 0 or 1) as pb200_prover_set_shuffle takes them.  In-rows have q_in = 1 and q_out = 0, out-rows q_out = 1 and
+ * q_in = 0 (a row with both is an ordinary row); p is the first out-row.  Out-rows define nothing by the gate rule.
+ * The shuffle defines every variable on an out-row cell at row p: once every row below p is evaluated, the out-rows,
+ * ascending, take the in-rows' tuples in ascending lexicographic order of (a, b, c) as canonical integers.  To unset
+ * and order, out-row variables are defined at row p: a defining row at or below p that reads one is an order error
+ * naming row p.  h_counts[4]: unset and order as pb200_solve_wires counts them, then
+ *   late   in-row cells whose variable is defined at or after p (by the shuffle or by a row above p), not before it,
+ *   clash  out-row cells that cannot take the shuffled value;
+ * found before any row is evaluated.  h_lists (8 limit uint32): pb200_solve_wires' 3 limit entries, then `limit`
+ * (cell, defining row) pairs of late cells, then `limit` (cell, reason, row) triples of clash cells, ascending, unused
+ * entries 0xffffffff.  Reasons: 0 the cell has no variable (-1), 1 its variable is an input, 2 a row below p defines
+ * it (that row is the third entry, else 0xffffffff), 3 it is on another out-row cell too.  With any count non-zero
+ * nothing is written to `out`.  Without out-rows the call solves as pb200_solve_wires.  Refuses what pb200_solve_wires
+ * refuses and, before any device work, a null h_qin or h_qout, a value other than 0 or 1, and unequal numbers of ones.
+ * The shuffle's memory (3 bytes a row, 6 a cell, 128 an in-row) is counted against free memory and
+ * PB200_SOLVE_MAX_BYTES and freed before the call returns. */
+int pb200_solve_wires_shuffle(pb200_ctx* ctx, const int64_t* h_ids, int log_n, uint64_t n_constraints,
+                              const uint8_t* const* h_sel, unsigned n_custom, const uint8_t* h_exps,
+                              const uint8_t* const* h_custom, uint64_t n_inputs, const int64_t* h_input_ids,
+                              const uint8_t* h_input_values, const uint8_t* h_qin, const uint8_t* h_qout,
+                              uint32_t limit, uint64_t* h_counts, uint32_t* h_lists, void* const* out,
+                              int out_on_device);
+/* the last pb200_solve_wires_shuffle call on this thread that evaluated its rows: milliseconds of phase 1 (the
+ * defining rows below p), the shuffle step and phase 2 (the rest), from device events; count <= 3 */
+void pb200_solve_shuffle_stages(double* ms, int count);
 
 /* ---- Prover (prover.py:39-306) ---------------------------------------------------------------- */
 /* Proof layout.  A prover's proof is the plain 15 fields, then the fields of the blocks it has (next-row custom gate

@@ -124,6 +124,8 @@ def _load():
         "pb200_solve_wires": (I, [V, V, I, U64, V, U, V, V, U64, V, V, ctypes.c_uint32, V, V, V, I]),
         "pb200_solve_wires_lookup": (I, [V, V, I, U64, V, U, V, V, U64, V, V, V, V, V, V, V, V, U64,
                                          ctypes.c_uint32, V, V, V, V, I]),
+        "pb200_solve_wires_shuffle": (I, [V, V, I, U64, V, U, V, V, U64, V, V, V, V, ctypes.c_uint32, V, V, V, I]),
+        "pb200_solve_shuffle_stages": (None, [P(ctypes.c_double), I]),
         "pb200_prover_prove_device_lookup": (I, [V, V, V, V, V, U64, V]),
         "pb200_prover_prove_device_next_row": (I, [V, V, V, V, V, U64, V]),
         "pb200_prover_prove_device_shuffle": (I, [V, V, V, V, V, U64, V]),

@@ -72,7 +72,9 @@ void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constra
                int n_custom, const uint8_t* h_exps, const uint8_t* const* h_custom, uint64_t n_inputs,
                const int64_t* h_in_ids, const uint8_t* h_in_vals, uint32_t limit, uint64_t* h_counts,
                uint32_t* h_lists, void* const* out, bool out_on_device, const uint8_t* h_qk, const uint8_t* h_qtag,
-               const uint8_t* const* h_tab, uint64_t tab_rows, uint8_t* h_operands);
+               const uint8_t* const* h_tab, uint64_t tab_rows, uint8_t* h_operands, bool shuffle = false,
+               const uint8_t* h_qin = nullptr, const uint8_t* h_qout = nullptr);
+void solve_stages(double* out_ms, int count);
 // ptau.cu
 Srs* srs_create_ptau(Context* ctx, const uint8_t* h_g1, uint64_t count, const uint8_t* h_tau_g2, int precompute);
 Srs* srs_create_ptau_lagrange(Context* ctx, const uint8_t* h_block, uint64_t n, Srs* monomial, int precompute);
@@ -609,6 +611,19 @@ int pb200_solve_wires_lookup(pb200_ctx* ctx, const int64_t* h_ids, int log_n, ui
             h_operands);
   PB_API_END
 }
+int pb200_solve_wires_shuffle(pb200_ctx* ctx, const int64_t* h_ids, int log_n, uint64_t n_constraints,
+                              const uint8_t* const* h_sel, unsigned n_custom, const uint8_t* h_exps,
+                              const uint8_t* const* h_custom, uint64_t n_inputs, const int64_t* h_input_ids,
+                              const uint8_t* h_input_values, const uint8_t* h_qin, const uint8_t* h_qout,
+                              uint32_t limit, uint64_t* h_counts, uint32_t* h_lists, void* const* out,
+                              int out_on_device) {
+  PB_API_BEGIN PB_ON_CTX(C(ctx));
+  solve_run(C(ctx), h_ids, log_n, n_constraints, h_sel, (int)n_custom, h_exps, h_custom, n_inputs, h_input_ids,
+            h_input_values, limit, h_counts, h_lists, out, out_on_device != 0, nullptr, nullptr, nullptr, 0, nullptr,
+            true, h_qin, h_qout);
+  PB_API_END
+}
+void pb200_solve_shuffle_stages(double* ms, int count) { solve_stages(ms, count); }
 
 void pb200_prover_destroy(pb200_prover* p) { prover_destroy(reinterpret_cast<Prover*>(p)); }
 int pb200_prover_sliced(pb200_prover* p, int* out) {

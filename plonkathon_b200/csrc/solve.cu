@@ -23,6 +23,11 @@
 // through steps 2 and 4 as one ascending list.  Before step 4 the table index is built (solve_table_index: words of
 // the keys sorted, checked on full values, one entry per distinct key); k_solve_eval_lookup probes it (solve.cuh,
 // solve_probe) and flags miss and ambiguous rows, which still store 0 and release their flag.
+//
+// With a shuffle (pb200_solve_wires_shuffle) out-rows define nothing by the gate rule (k_solve_unqualify_out); their
+// variables are defined at the first out-row p (k_solve_claim_out), late and clash cells are flagged in step 2, and
+// step 4 runs in two phases, the defining rows below p and the rest, with the sorted in-row tuples written into the
+// out-rows between them (solve_shuffle).  DESIGN.md section 3 has the rule and the no-deadlock argument per phase.
 #include <algorithm>
 #include <cuda/atomic>
 #include <cub/device/device_radix_sort.cuh>
@@ -336,6 +341,139 @@ __global__ void __launch_bounds__(128) k_solve_eval_lookup(SolveSel s, SolveLk l
   }
 }
 
+// ---- the shuffle (pb200_solve_wires_shuffle) ---------------------------------------------------------------------------
+// side[r]: PB_SOLVE_IN for an in-row (q_in = 1, q_out = 0), PB_SOLVE_OUT for an out-row (q_out = 1, q_in = 0), else 0.
+// p: the first out-row.
+#define PB_SOLVE_IN 1
+#define PB_SOLVE_OUT 2
+
+// out-rows define nothing by the gate rule: their qualify flags cleared (after k_solve_qualify)
+__global__ void k_solve_unqualify_out(const uint8_t* side, uint64_t n_rows, uint8_t* qual) {
+  const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r < n_rows && side[r] == PB_SOLVE_OUT) qual[r] = 0;
+}
+
+// per out-row cell (after k_solve_vars): count the out-row cells of its variable, and let the shuffle define it at row p
+// unless it is the constant 0 or an input.  A row below p that defines it keeps it (a clash); a row above p does not.
+__global__ void k_solve_claim_out(const uint8_t* side, const uint32_t* var_of_cell, const uint32_t* inp, uint64_t n,
+                                  uint32_t p, uint32_t* out_cells, uint32_t* def_row) {
+  const uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= 3 * n || side[c / 3] != PB_SOLVE_OUT) return;
+  const uint32_t v = var_of_cell[c];
+  atomicAdd(out_cells + v, 1u);
+  if (inp[v] == PB_SOLVE_NONE) atomicMin(def_row + v, p);
+}
+
+// why an out-row cell cannot take the shuffled value, or PB_SOLVE_NONE when it can
+#define PB_SOLVE_CLASH_NO_VAR 0   // the cell has no variable (-1)
+#define PB_SOLVE_CLASH_INPUT 1    // its variable is an input
+#define PB_SOLVE_CLASH_DEFINED 2  // a row below p defines its variable
+#define PB_SOLVE_CLASH_SHARED 3   // its variable is on another out-row cell too
+__device__ __forceinline__ uint32_t solve_clash(uint32_t v, const uint32_t* inp, const uint32_t* def_row,
+                                                const uint32_t* out_cells, uint32_t p) {
+  if (inp[v] == PB_SOLVE_ZERO) return PB_SOLVE_CLASH_NO_VAR;
+  if (inp[v] != PB_SOLVE_NONE) return PB_SOLVE_CLASH_INPUT;
+  if (def_row[v] < p) return PB_SOLVE_CLASH_DEFINED;
+  if (out_cells[v] > 1) return PB_SOLVE_CLASH_SHARED;
+  return PB_SOLVE_NONE;
+}
+
+// per cell: late (an in-row cell whose variable is defined at or after p: by the shuffle or by a row above p) and
+// clash (an out-row cell that cannot take the shuffled value)
+__global__ void k_solve_shuffle_flags(const uint8_t* side, const uint32_t* var_of_cell, const uint32_t* inp,
+                                      const uint32_t* def_row, const uint32_t* out_cells, uint64_t n, uint32_t p,
+                                      uint8_t* late, uint8_t* clash) {
+  const uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= 3 * n) return;
+  const uint8_t sd = side[c / 3];
+  const uint32_t v = var_of_cell[c], d = def_row[v];
+  late[c] = (sd == PB_SOLVE_IN && inp[v] == PB_SOLVE_NONE && d != PB_SOLVE_NONE && d >= p) ? 1 : 0;
+  clash[c] = (sd == PB_SOLVE_OUT && solve_clash(v, inp, def_row, out_cells, p) != PB_SOLVE_NONE) ? 1 : 0;
+}
+
+// the clash list's second and third entries: the reason of each listed cell, and the row below p that defines its
+// variable (PB_SOLVE_NONE for the other reasons)
+__global__ void k_solve_clash_reasons(const uint32_t* cells, uint32_t count, const uint32_t* var_of_cell,
+                                      const uint32_t* inp, const uint32_t* def_row, const uint32_t* out_cells,
+                                      uint32_t p, uint32_t* out) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= count) return;
+  const uint32_t v = var_of_cell[cells[k]], why = solve_clash(v, inp, def_row, out_cells, p);
+  out[2 * k] = why;
+  out[2 * k + 1] = why == PB_SOLVE_CLASH_DEFINED ? def_row[v] : PB_SOLVE_NONE;
+}
+
+// the K in-rows' tuples, canonical, as twelve columns of K 64-bit words: word w (0..11) is limb w % 4 of a, b, c for
+// w / 4 = 0, 1, 2; and the starting positions 0..K-1
+__global__ void k_solve_shuffle_gather(const uint32_t* in_rows, uint64_t K, const uint32_t* var_of_cell, const Fr* val,
+                                       uint64_t* words, uint32_t* pos) {
+  const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= K) return;
+  const uint64_t r = in_rows[k];
+#pragma unroll
+  for (int col = 0; col < 3; col++) {
+    const Fr x = fp_from_mont(val[var_of_cell[3 * r + col]]);
+#pragma unroll
+    for (int l = 0; l < 4; l++) words[(uint64_t)(4 * col + l) * K + k] = (uint64_t)x.v[2 * l] | ((uint64_t)x.v[2 * l + 1] << 32);
+  }
+  pos[k] = (uint32_t)k;
+}
+
+// the OR (acc[w]) and the AND (acc[12 + w]) of every word over the in-rows (acc set to 0 and ~0 before)
+__global__ void __launch_bounds__(256) k_solve_shuffle_bits(const uint64_t* words, uint64_t K,
+                                                            unsigned long long* acc) {
+  __shared__ unsigned long long s_or[12], s_and[12];
+  if (threadIdx.x < 12) {
+    s_or[threadIdx.x] = 0;
+    s_and[threadIdx.x] = ~0ull;
+  }
+  __syncthreads();
+  unsigned long long o[12], a[12];
+#pragma unroll
+  for (int w = 0; w < 12; w++) o[w] = 0, a[w] = ~0ull;
+  for (uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; k < K; k += (uint64_t)gridDim.x * blockDim.x)
+#pragma unroll
+    for (int w = 0; w < 12; w++) {
+      const unsigned long long x = words[(uint64_t)w * K + k];
+      o[w] |= x;
+      a[w] &= x;
+    }
+#pragma unroll
+  for (int w = 0; w < 12; w++) {
+    for (int s = 16; s; s >>= 1) {
+      o[w] |= __shfl_xor_sync(0xffffffffu, o[w], s);
+      a[w] &= __shfl_xor_sync(0xffffffffu, a[w], s);
+    }
+    if ((threadIdx.x & 31) == 0) {
+      atomicOr(s_or + w, o[w]);
+      atomicAnd(s_and + w, a[w]);
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < 12) {
+    atomicOr(acc + threadIdx.x, s_or[threadIdx.x]);
+    atomicAnd(acc + 12 + threadIdx.x, s_and[threadIdx.x]);
+  }
+}
+
+// one LSD pass: the word of the tuple at each sorted position, the key of the pass's stable sort
+__global__ void k_solve_shuffle_key(const uint64_t* column, const uint32_t* pos, uint64_t K, uint64_t* key) {
+  const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < K) key[k] = column[pos[k]];
+}
+
+// out-row j (ascending) takes the tuple of in-row in_rows[pos[j]] (the j-th in sorted order): its three variables get
+// the in-row's values (Montgomery) and their ready flags
+__global__ void k_solve_shuffle_put(const uint32_t* in_rows, const uint32_t* out_rows, const uint32_t* pos, uint64_t K,
+                                    const uint32_t* var_of_cell, Fr* val, uint32_t* ready) {
+  const uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= 3 * K) return;
+  const uint64_t j = c / 3, col = c - 3 * j;
+  const uint32_t v = var_of_cell[3 * (uint64_t)out_rows[j] + col];
+  val[v] = val[var_of_cell[3 * (uint64_t)in_rows[pos[j]] + col]];
+  ready[v] = 1;
+}
+
 // a and b of each listed row, canonical, for the miss and ambiguous messages
 __global__ void k_solve_operands(const uint32_t* rows, uint32_t count, const uint32_t* var_of_cell, const Fr* val,
                                  Fr* out) {
@@ -430,6 +568,78 @@ static void solve_table_index(Context* ctx, SolveTable& T, uint64_t rows, DevBuf
   T.n_keys = keys_n;
 }
 
+// the shuffle step, between the two phases of the evaluation: out-row j (out_rows ascending) takes the tuple of the j-th
+// in-row in ascending (a, b, c) order, compared as canonical integers.  The positions 0..K-1 of the in-rows are sorted
+// LSD by the twelve 64-bit words of their tuple, c's lowest first and a's highest last, one stable SortPairs a word.  A
+// word equal on every in-row (OR = AND) is skipped, and the others sort only the bits from the lowest to the highest
+// one where OR and AND differ: small integers (addresses, counters) cost a pass or two, random field elements twelve.
+// temp: at least SortPairs' storage over K items; acc: 24 device words.
+static void solve_shuffle(Context* ctx, const uint32_t* in_rows, const uint32_t* out_rows, uint64_t K,
+                          const uint32_t* var_of_cell, Fr* val, uint32_t* ready, DevBuf& temp,
+                          unsigned long long* acc) {
+  cudaStream_t st = ctx->stream;
+  DevBuf words(K * 96), k1(K * 8), k2(K * 8), p1(K * 4), p2(K * 4);
+  k_solve_shuffle_gather<<<PB_SOLVE_GRID(K, 128), 0, st>>>(in_rows, K, var_of_cell, val, words.as<uint64_t>(),
+                                                           p1.as<uint32_t>());
+  solve_launched(ctx);
+  PB_CUDA(cudaMemsetAsync(acc, 0, 12 * 8, st));
+  PB_CUDA(cudaMemsetAsync(acc + 12, 0xff, 12 * 8, st));
+  const uint64_t blocks = std::min<uint64_t>((K + 255) / 256, 4 * (uint64_t)ctx->sm_count);
+  k_solve_shuffle_bits<<<(unsigned)blocks, 256, 0, st>>>(words.as<uint64_t>(), K, acc);
+  solve_launched(ctx);
+  unsigned long long bits[24];
+  PB_CUDA(cudaMemcpyAsync(bits, acc, sizeof bits, cudaMemcpyDeviceToHost, st));
+  PB_CUDA(cudaStreamSynchronize(st));
+  cub::DoubleBuffer<uint64_t> keys(k1.as<uint64_t>(), k2.as<uint64_t>());
+  cub::DoubleBuffer<uint32_t> pos(p1.as<uint32_t>(), p2.as<uint32_t>());
+  for (int t = 2; t >= 0; t--)  // c, b, a
+    for (int l = 0; l < 4; l++) {
+      const int w = 4 * t + l;
+      const unsigned long long diff = bits[w] ^ bits[12 + w];
+      if (!diff) continue;
+      k_solve_shuffle_key<<<PB_SOLVE_GRID(K, 256), 0, st>>>(words.as<uint64_t>() + (uint64_t)w * K, pos.Current(), K,
+                                                            keys.Current());
+      solve_launched(ctx);
+      size_t tb = temp.bytes;
+      PB_CUDA(cub::DeviceRadixSort::SortPairs(temp.p, tb, keys, pos, (int)K, __builtin_ctzll(diff),
+                                              64 - __builtin_clzll(diff), st));
+      ctx->launches++;
+    }
+  k_solve_shuffle_put<<<PB_SOLVE_GRID(3 * K, 256), 0, st>>>(in_rows, out_rows, pos.Current(), K, var_of_cell, val,
+                                                            ready);
+  solve_launched(ctx);
+  PB_CUDA(cudaStreamSynchronize(st));  // the sort's buffers die here
+}
+
+namespace {
+thread_local double g_solve_ms[3];  // the last shuffle solve: phase 1, the shuffle step, phase 2 (device events)
+}
+void solve_stages(double* out_ms, int count) {
+  for (int k = 0; k < count && k < 3; k++) out_ms[k] = g_solve_ms[k];
+}
+
+// q_in and q_out as pb200_prover_set_shuffle takes them, with its refusals (prover.cu, prover_set_shuffle) -> side[r]
+// (PB_SOLVE_IN, PB_SOLVE_OUT or 0)
+static std::vector<uint8_t> solve_require_shuffle(uint64_t n, const uint8_t* h_qin, const uint8_t* h_qout) {
+  PB_CHECK(h_qin && h_qout, "a shuffle needs q_in and q_out");
+  uint64_t ones[2] = {0, 0};
+  const uint8_t* sel[2] = {h_qin, h_qout};
+  for (int s = 0; s < 2; s++)
+    for (uint64_t i = 0; i < n; i++) {
+      const uint8_t* e = sel[s] + 32 * i;
+      bool ok = e[0] <= 1;
+      for (int k = 1; k < 32 && ok; k++) ok = e[k] == 0;
+      PB_CHECK(ok, s ? "q_out must be 0 or 1 on every row" : "q_in must be 0 or 1 on every row");
+      ones[s] += e[0];
+    }
+  PB_CHECK(ones[0] == ones[1], ("a shuffle needs as many q_in rows as q_out rows: " + std::to_string(ones[0]) +
+                                " and " + std::to_string(ones[1])).c_str());
+  std::vector<uint8_t> side(n);
+  for (uint64_t i = 0; i < n; i++)
+    side[i] = h_qin[32 * i] == h_qout[32 * i] ? 0 : h_qin[32 * i] ? PB_SOLVE_IN : PB_SOLVE_OUT;
+  return side;
+}
+
 // q_K, Q_T and the table as pb200_prover_set_lookup(_tagged) takes them, with its refusals (prover.cu,
 // prover_set_lookup)
 static void solve_require_lookup(uint64_t n, const uint8_t* h_qk, const uint8_t* h_qtag, const uint8_t* const* h_tab,
@@ -458,13 +668,15 @@ static void solve_require_lookup(uint64_t n, const uint8_t* h_qk, const uint8_t*
     }
 }
 
-// see plonk_b200.h (pb200_solve_wires, and pb200_solve_wires_lookup when h_tab is not null: then h_counts has four
-// entries and h_lists 5 limit)
+// see plonk_b200.h (pb200_solve_wires; pb200_solve_wires_lookup when h_tab is not null: then h_counts has four
+// entries and h_lists 5 limit; pb200_solve_wires_shuffle when `shuffle`: then h_counts has four entries and h_lists
+// 8 limit)
 void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constraints, const uint8_t* const* h_sel,
                int n_custom, const uint8_t* h_exps, const uint8_t* const* h_custom, uint64_t n_inputs,
                const int64_t* h_in_ids, const uint8_t* h_in_vals, uint32_t limit, uint64_t* h_counts,
                uint32_t* h_lists, void* const* out, bool out_on_device, const uint8_t* h_qk, const uint8_t* h_qtag,
-               const uint8_t* const* h_tab, uint64_t tab_rows, uint8_t* h_operands) {
+               const uint8_t* const* h_tab, uint64_t tab_rows, uint8_t* h_operands, bool shuffle,
+               const uint8_t* h_qin, const uint8_t* h_qout) {
   PB_CHECK(log_n >= 1 && log_n <= 26, "group order must be 2^k, 1 <= k <= 26 (the prover's range)");
   const uint64_t n = (uint64_t)1 << log_n, m = 3 * n;
   const bool lookup = h_tab != nullptr;
@@ -528,11 +740,24 @@ void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constra
     memcpy(&in_vals[32 * k], h_in_vals + 32 * order[k], 32);
   }
   if (lookup) solve_require_lookup(n, h_qk, h_qtag, h_tab, tab_rows);
+  // the shuffle: the rows of each side, K in-rows (as many out-rows), the first out-row p.  Without out-rows (q_in and
+  // q_out all 0, or both 1 on the same rows) the solve is the one without a shuffle.
+  std::vector<uint8_t> side;
+  uint64_t K = 0;
+  uint32_t p = PB_SOLVE_NONE;
+  if (shuffle) {
+    side = solve_require_shuffle(n, h_qin, h_qout);
+    for (uint64_t i = 0; i < n; i++) {
+      K += side[i] == PB_SOLVE_IN;
+      if (side[i] == PB_SOLVE_OUT && p == PB_SOLVE_NONE) p = (uint32_t)i;
+    }
+  }
+  const bool sh = K > 0;
 
   const int cb = perm_cell_bits(log_n);
   const int end_bit = perm_sort_bits(log_n, max_id);
   cudaStream_t st = ctx->stream;
-  size_t t_sort = 0, t_scan = 0, t_sel = 0, t_tab = 0;
+  size_t t_sort = 0, t_scan = 0, t_sel = 0, t_tab = 0, t_sh = 0;
   {
     cub::DoubleBuffer<uint64_t> d(nullptr, nullptr);
     PB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, t_sort, d, (int)m, 0, end_bit, st));
@@ -543,8 +768,12 @@ void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constra
       cub::DoubleBuffer<uint32_t> v(nullptr, nullptr);
       PB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t_tab, d, v, (int)tab_rows, 0, 64, st));
     }
+    if (sh) {
+      cub::DoubleBuffer<uint32_t> v(nullptr, nullptr);
+      PB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t_sh, d, v, (int)K, 0, 64, st));
+    }
   }
-  const uint64_t temp_bytes = std::max(std::max(t_sort, t_tab), std::max(t_scan, t_sel));
+  const uint64_t temp_bytes = std::max(std::max(std::max(t_sort, t_tab), std::max(t_scan, t_sel)), t_sh);
   // keys and alt (8 each), heads / run (4 each), var_of_cell, inp, def_row, ready (4 each), the values (32), the index
   // list (4), three flag bytes: per cell.  Selectors, 1 / QO and the custom selectors (32 each), the qualify and
   // defines flags: per row.  The inputs, the host outputs' staging and the sort's storage.
@@ -554,6 +783,10 @@ void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constra
   // (4 x 32), the sort's words and rows (2 x 8, 2 x 4), heads and runs (4 each), the split flag, the index (8 + 4 + 1);
   // the listed rows' operands
   if (lookup) need += n * (32 + 32 + 2) + tab_rows * (4 * 32 + 16 + 8 + 8 + 1 + 13) + (uint64_t)limit * 2 * 64 + 256;
+  // with a shuffle: the side and the in / out flags (1 each) per row; the out-row cell count (4) and the late and clash
+  // flags (1 each) per cell; per in-row its tuple (96), the sort's words and positions (2 x 8, 2 x 4) and the in-row and
+  // out-row lists (4 each); the listed cells' entries
+  if (sh) need += n * 3 + m * (4 + 2) + K * (96 + 16 + 8 + 8) + (uint64_t)limit * 5 * 4 + 256;
   size_t free_b = 0, total_b = 0;
   PB_CUDA(cudaMemGetInfo(&free_b, &total_b));
   // PB200_SOLVE_MAX_BYTES: the most device memory a solve may take (read per call), so it leaves room for other work
@@ -566,7 +799,8 @@ void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constra
   }
 
   DevBuf temp(temp_bytes), keys(m * 8), alt(m * 8), head(m * 4), run(m * 4), voc(m * 4), inp(m * 4), defr(m * 4),
-      ready(m * 4), val(m * 32), idx(m * 4), flags(3 * m), small(64), inids(n_inputs * 8 + 8), invals(n_inputs * 32 + 32),
+      ready(m * 4), val(m * 32), idx(m * 4), flags(3 * m), small(sh ? 32 + 24 * 8 : 64), inids(n_inputs * 8 + 8),
+      invals(n_inputs * 32 + 32),
       sel((6 + (uint64_t)n_custom) * n * 32), qual(n), defines(n);
   Fr* selp = sel.as<Fr>();
   const Fr* sel_col[5];
@@ -636,18 +870,41 @@ void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constra
   if (lookup) k_solve_qualify_lookup<<<PB_SOLVE_GRID(n, 256), 0, st>>>(s, qkb.as<Fr>(), n_constraints, qual.as<uint8_t>());
   else k_solve_qualify<<<PB_SOLVE_GRID(n, 256), 0, st>>>(s, n_constraints, qual.as<uint8_t>());
   solve_launched(ctx);
+  // the shuffle: per row its side, then the in-row and the out-row flags (for the row lists)
+  DevBuf sideb(sh ? 3 * n : 0), outc(sh ? m * 4 : 0), shf(sh ? 2 * m : 0);
+  if (sh) {
+    std::vector<uint8_t> fl(2 * n);
+    for (uint64_t i = 0; i < n; i++) {
+      fl[i] = side[i] == PB_SOLVE_IN;
+      fl[n + i] = side[i] == PB_SOLVE_OUT;
+    }
+    PB_CUDA(cudaMemcpyAsync(sideb.p, side.data(), n, cudaMemcpyHostToDevice, st));
+    PB_CUDA(cudaMemcpyAsync(sideb.as<uint8_t>() + n, fl.data(), 2 * n, cudaMemcpyHostToDevice, st));
+    k_solve_unqualify_out<<<PB_SOLVE_GRID(n, 256), 0, st>>>(sideb.as<uint8_t>(), n_constraints, qual.as<uint8_t>());
+    solve_launched(ctx);
+  }
   PB_CUDA(cudaMemsetAsync(defr.p, 0xff, m * 4, st));
   PB_CUDA(cudaMemsetAsync(inp.p, 0xff, m * 4, st));  // variables past the last run: no source
   k_solve_vars<<<PB_SOLVE_GRID(m, 256), 0, st>>>(sorted, run.as<uint32_t>(), m, cb, inids.as<uint64_t>(), n_inputs,
                                                 qual.as<uint8_t>(), voc.as<uint32_t>(), inp.as<uint32_t>(),
                                                 defr.as<uint32_t>());
   solve_launched(ctx);
+  if (sh) {  // out-row variables: defined at row p
+    PB_CUDA(cudaMemsetAsync(outc.p, 0, m * 4, st));
+    k_solve_claim_out<<<PB_SOLVE_GRID(m, 256), 0, st>>>(sideb.as<uint8_t>(), voc.as<uint32_t>(), inp.as<uint32_t>(), n,
+                                                       p, outc.as<uint32_t>(), defr.as<uint32_t>());
+    solve_launched(ctx);
+  }
   uint8_t* f_unset = flags.as<uint8_t>();
   uint8_t* f_order = f_unset + m;
   k_solve_flags<<<PB_SOLVE_GRID(m, 256), 0, st>>>(voc.as<uint32_t>(), inp.as<uint32_t>(), defr.as<uint32_t>(), n,
                                                  f_unset, f_order, defines.as<uint8_t>());
   solve_launched(ctx);
-  for (uint64_t k = 0; k < (lookup ? 5 : 3) * (uint64_t)limit; k++) h_lists[k] = 0xffffffffu;
+  if (sh) {  // row p defines nothing, though its O variable is defined at p: its flag and its operands' order flags off
+    PB_CUDA(cudaMemsetAsync(defines.as<uint8_t>() + p, 0, 1, st));
+    PB_CUDA(cudaMemsetAsync(f_order + 3 * (uint64_t)p, 0, 2, st));
+  }
+  for (uint64_t k = 0; k < (lookup ? 5 : shuffle ? 8 : 3) * (uint64_t)limit; k++) h_lists[k] = 0xffffffffu;
   uint32_t* num = small_u + 1;
   h_counts[0] = solve_compact(ctx, f_unset, m, temp, idx.as<uint32_t>(), num, limit, h_lists);
   std::vector<uint32_t> cells(limit);
@@ -668,7 +925,52 @@ void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constra
       h_lists[limit + 2 * (uint64_t)k + 1] = rows[k];
     }
   }
-  if (h_counts[0] || h_counts[1]) {
+  if (shuffle) h_counts[2] = h_counts[3] = 0;
+  if (sh) {  // late in-row cells and clashing out-row cells
+    uint8_t* f_late = shf.as<uint8_t>();
+    uint8_t* f_clash = f_late + m;
+    k_solve_shuffle_flags<<<PB_SOLVE_GRID(m, 256), 0, st>>>(sideb.as<uint8_t>(), voc.as<uint32_t>(), inp.as<uint32_t>(),
+                                                           defr.as<uint32_t>(), outc.as<uint32_t>(), n, p, f_late,
+                                                           f_clash);
+    solve_launched(ctx);
+    uint32_t* l_late = h_lists + 3 * (uint64_t)limit;
+    uint32_t* l_clash = l_late + 2 * (uint64_t)limit;
+    h_counts[2] = solve_compact(ctx, f_late, m, temp, idx.as<uint32_t>(), num, limit, cells.data());
+    const uint32_t n_late = (uint32_t)std::min<uint64_t>(h_counts[2], limit);
+    std::vector<uint32_t> ccells(limit);
+    h_counts[3] = solve_compact(ctx, f_clash, m, temp, idx.as<uint32_t>(), num, limit, ccells.data());
+    const uint32_t n_clash = (uint32_t)std::min<uint64_t>(h_counts[3], limit);
+    if (n_late + n_clash) {  // (late cell, the row defining its variable), (clash cell, reason, row)
+      DevBuf lst((size_t)(n_late + n_clash) * 4 * 4);
+      uint32_t* d = lst.as<uint32_t>();
+      PB_CUDA(cudaMemcpyAsync(d, cells.data(), (size_t)n_late * 4, cudaMemcpyHostToDevice, st));
+      PB_CUDA(cudaMemcpyAsync(d + n_late, ccells.data(), (size_t)n_clash * 4, cudaMemcpyHostToDevice, st));
+      uint32_t* o = d + n_late + n_clash;
+      if (n_late) {
+        k_solve_order_rows<<<PB_SOLVE_GRID(n_late, 128), 0, st>>>(d, n_late, voc.as<uint32_t>(), defr.as<uint32_t>(), o);
+        solve_launched(ctx);
+      }
+      if (n_clash) {
+        k_solve_clash_reasons<<<PB_SOLVE_GRID(n_clash, 128), 0, st>>>(d + n_late, n_clash, voc.as<uint32_t>(),
+                                                                       inp.as<uint32_t>(), defr.as<uint32_t>(),
+                                                                       outc.as<uint32_t>(), p, o + n_late);
+        solve_launched(ctx);
+      }
+      std::vector<uint32_t> got((size_t)n_late + 2 * (size_t)n_clash);
+      PB_CUDA(cudaMemcpyAsync(got.data(), o, got.size() * 4, cudaMemcpyDeviceToHost, st));
+      PB_CUDA(cudaStreamSynchronize(st));
+      for (uint32_t k = 0; k < n_late; k++) {
+        l_late[2 * k] = cells[k];
+        l_late[2 * k + 1] = got[k];
+      }
+      for (uint32_t k = 0; k < n_clash; k++) {
+        l_clash[3 * k] = ccells[k];
+        l_clash[3 * k + 1] = got[n_late + 2 * k];
+        l_clash[3 * k + 2] = got[n_late + 2 * k + 1];
+      }
+    }
+  }
+  if (h_counts[0] || h_counts[1] || (shuffle && (h_counts[2] || h_counts[3]))) {
     PB_CUDA(cudaStreamSynchronize(st));  // the call's buffers die here
     return;
   }
@@ -684,24 +986,54 @@ void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constra
     lk.T.amb = ix_amb.as<uint8_t>();
     solve_table_index(ctx, lk.T, tab_rows, temp, small_u + 6);
   }
+  // with a shuffle, phase 1 is the defining rows below p (the list's prefix idx[0, k)), phase 2 the rest
+  const uint64_t k_below = sh ? solve_compact(ctx, defines.as<uint8_t>(), p, temp, idx.as<uint32_t>(), num, 0, nullptr) : 0;
   const uint64_t n_def = solve_compact(ctx, defines.as<uint8_t>(), n, temp, idx.as<uint32_t>(), num, 0, nullptr);
-  if (n_def) {
+  auto evaluate = [&](const uint32_t* rows, uint64_t count) {
+    if (!count) return;
     int per_sm = 0;
     if (lookup) PB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_solve_eval_lookup, 128, 0));
     else PB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_solve_eval, 128, 0));
-    const uint64_t warps = (n_def + 31) / 32;
+    const uint64_t warps = (count + 31) / 32;
     const uint64_t blocks = std::min<uint64_t>((uint64_t)std::max(per_sm, 1) * ctx->sm_count, (warps + 3) / 4);
+    PB_CUDA(cudaMemsetAsync(small_u + 4, 0, 4, st));  // the ticket
     if (lookup)
-      k_solve_eval_lookup<<<(unsigned)blocks, 128, 0, st>>>(s, lk, idx.as<uint32_t>(), n_def, voc.as<uint32_t>(),
-                                                            val.as<Fr>(), ready.as<uint32_t>(), small_u + 4);
+      k_solve_eval_lookup<<<(unsigned)blocks, 128, 0, st>>>(s, lk, rows, count, voc.as<uint32_t>(), val.as<Fr>(),
+                                                            ready.as<uint32_t>(), small_u + 4);
     else
-      k_solve_eval<<<(unsigned)blocks, 128, 0, st>>>(s, idx.as<uint32_t>(), n_def, voc.as<uint32_t>(), val.as<Fr>(),
+      k_solve_eval<<<(unsigned)blocks, 128, 0, st>>>(s, rows, count, voc.as<uint32_t>(), val.as<Fr>(),
                                                      ready.as<uint32_t>(), small_u + 4);
     solve_launched(ctx);
     uint32_t stalled = 0;
     PB_CUDA(cudaMemcpyAsync(&stalled, small_u + 5, 4, cudaMemcpyDeviceToHost, st));
     PB_CUDA(cudaStreamSynchronize(st));
     PB_CHECK(stalled == 0, "solving the wires stalled: a defining row waited too long for its operands");
+  };
+  if (!sh) {
+    evaluate(idx.as<uint32_t>(), n_def);
+  } else {
+    DevBuf rowl(2 * K * 4);  // the in-rows, then the out-rows, ascending
+    const uint8_t* fl = sideb.as<uint8_t>() + n;
+    uint64_t got_in = solve_compact(ctx, fl, n, temp, rowl.as<uint32_t>(), num, 0, nullptr);
+    uint64_t got_out = solve_compact(ctx, fl + n, n, temp, rowl.as<uint32_t>() + K, num, 0, nullptr);
+    PB_CHECK(got_in == K && got_out == K, "solving the wires: the shuffle's row lists disagree with q_in and q_out");
+    cudaEvent_t ev[4];
+    for (auto& e : ev) PB_CUDA(cudaEventCreate(&e));
+    PB_CUDA(cudaEventRecord(ev[0], st));
+    evaluate(idx.as<uint32_t>(), k_below);
+    PB_CUDA(cudaEventRecord(ev[1], st));
+    solve_shuffle(ctx, rowl.as<uint32_t>(), rowl.as<uint32_t>() + K, K, voc.as<uint32_t>(), val.as<Fr>(),
+                  ready.as<uint32_t>(), temp, reinterpret_cast<unsigned long long*>(small_u + 8));
+    PB_CUDA(cudaEventRecord(ev[2], st));
+    evaluate(idx.as<uint32_t>() + k_below, n_def - k_below);
+    PB_CUDA(cudaEventRecord(ev[3], st));
+    PB_CUDA(cudaEventSynchronize(ev[3]));
+    for (int k = 0; k < 3; k++) {
+      float ms = 0;
+      PB_CUDA(cudaEventElapsedTime(&ms, ev[k], ev[k + 1]));
+      g_solve_ms[k] = ms;
+    }
+    for (auto& e : ev) PB_CUDA(cudaEventDestroy(e));
   }
   if (lookup) {  // miss and ambiguous: rows, and the operands a, b of the listed ones
     uint32_t* l_miss = h_lists + 3 * (uint64_t)limit;

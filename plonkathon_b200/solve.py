@@ -24,9 +24,30 @@ strictly earlier row.  Two more error kinds can only be found while the rows are
 
 Each is an exact count with its lowest ``limit`` rows.  With any error, no wires are returned.
 
-Every other variable (shuffle out-rows, public inputs, rows whose terms involve c or the next row, hints, and lookup
-rows without a table argument) must come as an input.  The wires stay on the device if asked, for
-``Prover.check_arrays`` and ``prove_arrays``."""
+With ``shuffle=(q_in, q_out)`` (as ``Prover.from_arrays`` takes it) the out-rows get their values from the shuffle.
+In-rows have q_in = 1 and q_out = 0, out-rows q_out = 1 and q_in = 0; a row with both selectors cancels out in the
+argument and is an ordinary row here.  p is the first out-row.  The rule:
+
+1. The shuffle defines every variable on an out-row cell, at row p: after every row below p is evaluated, the
+   out-rows, in ascending row order, take the in-rows' tuples in ascending lexicographic order of (a, b, c), compared
+   as canonical integers in [0, r), a first.  With a = address, b = time, c = value, that is a memory log sorted by
+   address and in time order within each address.  Out-rows define nothing by the gate rule or the table rule.  A
+   gate row above p with such a variable on its O cell only checks it.
+2. Every in-row cell must be known before p: its variable is -1, an input, or defined by a row below p.  Otherwise
+   the cell is ``late`` (also when it holds an out-row variable).
+3. Every out-row cell must be able to take the shuffled value.  Otherwise the cell is a ``clash``, for one of these
+   reasons: it has no variable (-1), its variable is an input, a gate or table row below p defines it, or the variable
+   is on another out-row cell too.
+4. ``unset`` and ``order`` keep their meaning, with out-row variables defined at row p: a defining row at or below p
+   that reads one is an ``order`` error "row r reads variable v (...), which row p defines".
+
+``late`` and ``clash`` are exact counts with their lowest ``limit`` cells, found before any row is evaluated, like
+``unset`` and ``order``.  Without out-rows the solve is the one without ``shuffle=``.  A shuffle does not combine with
+lookups.
+
+Every other variable (public inputs, rows whose terms involve c or the next row, hints, lookup rows without a table
+argument, and shuffle out-rows without ``shuffle=``) must come as an input.  The wires stay on the device if asked,
+for ``Prover.check_arrays`` and ``prove_arrays``."""
 from __future__ import annotations
 
 import ctypes
@@ -38,10 +59,13 @@ from ._lib import check, default_context, lib
 from .custom_gates import padded, split_terms
 from .field import CURVE_ORDER
 from .lookup import check_lookup, check_lookups, to_le_rows
+from .shuffle import check_shuffle
 from .wiring import MAX_ID, MAX_LOG_N, _wire
 
 WIRE = "LRO"
 SEL = ("QL", "QR", "QM", "QO", "QC")
+# why an out-row cell cannot take its shuffled value (pb200_solve_wires_shuffle's reason codes 0..3)
+CLASH_REASONS = ("no variable", "input", "defined", "shared")
 
 
 @dataclass
@@ -54,7 +78,11 @@ class WireSolution:
       (cell, the defining row));
     * ``miss``: rows that define from their table and whose (tag, a, b) matches no table row (``miss_rows``);
     * ``ambiguous``: rows that define from their table and whose (tag, a, b) matches table rows with different t3
-      (``ambiguous_rows``)."""
+      (``ambiguous_rows``);
+    * ``late``: in-row cells of a shuffle whose variable is defined at or after the first out-row (``late_cells``:
+      (cell, the defining row));
+    * ``clash``: out-row cells that cannot take the shuffled value (``clash_cells``: (cell, reason), the reason one of
+      ``CLASH_REASONS``)."""
     A: object
     B: object
     C: object
@@ -71,10 +99,17 @@ class WireSolution:
     # for the miss and ambiguous lines: {row: (a, b)}, and (Q_T per row or None, [t1, t2, t3(, t4)] as ints)
     _operands: dict = field(default=None, repr=False, compare=False)
     _table: tuple = field(default=None, repr=False, compare=False)
+    late: int = 0
+    clash: int = 0
+    late_cells: list = field(default_factory=list)
+    clash_cells: list = field(default_factory=list)
+    # for the late and clash lines: the first out-row, and {clash cell: the row below it defining its variable}
+    _first_out: int = field(default=None, repr=False, compare=False)
+    _clash_rows: dict = field(default=None, repr=False, compare=False)
 
     @property
     def ok(self) -> bool:
-        return not (self.unset or self.order or self.miss or self.ambiguous)
+        return not (self.unset or self.order or self.miss or self.ambiguous or self.late or self.clash)
 
     def _table_of(self, row) -> int:
         qt = self._table[0] if self._table else None
@@ -108,8 +143,27 @@ class WireSolution:
             tag = self._table_of(r)
             out.append("ambiguous: row %d looks up (a, b) = (%d, %d) in table %d, whose rows give %s"
                        % (r, a, b, tag, " and ".join("c = %d" % c for c in self._t3_values(tag, a, b)[:2])))
+        p = self._first_out
+        for c, d in self.late_cells:
+            row, col = divmod(c, 3)
+            out.append("late: in-row cell (row %d, %s) holds variable %d, which row %d defines, not before the first "
+                       "out-row %d" % (row, WIRE[col], int(self._ids[c]), d, p))
+        for c, why in self.clash_cells:
+            row, col = divmod(c, 3)
+            head = "clash: out-row cell (row %d, %s)" % (row, WIRE[col])
+            v = int(self._ids[c])
+            if why == "no variable":
+                out.append(head + " holds no variable (-1)")
+            elif why == "input":
+                out.append(head + " holds variable %d, an input" % v)
+            elif why == "defined":
+                out.append(head + " holds variable %d, which row %d defines, before the first out-row %d"
+                           % (v, self._clash_rows[c], p))
+            else:
+                out.append(head + " holds variable %d, which another out-row cell holds too" % v)
         for k, listed in (("unset", self.unset_cells), ("order", self.order_cells), ("miss", self.miss_rows),
-                          ("ambiguous", self.ambiguous_rows)):
+                          ("ambiguous", self.ambiguous_rows), ("late", self.late_cells),
+                          ("clash", self.clash_cells)):
             if getattr(self, k) > len(listed):
                 out.append("%s: %d more" % (k, getattr(self, k) - len(listed)))
         return out
@@ -118,7 +172,8 @@ class WireSolution:
         if self.ok:
             return "wires solved"
         head = "wires unsolved: " + ", ".join("%d %s" % (getattr(self, k), k)
-                                              for k in ("unset", "order", "miss", "ambiguous") if getattr(self, k))
+                                              for k in ("unset", "order", "miss", "ambiguous", "late", "clash")
+                                              if getattr(self, k))
         return "\n".join([head] + ["  " + s for s in self.lines()])
 
 
@@ -193,7 +248,7 @@ def _inputs(inputs):
 
 def solve_wires(wire_L, wire_R, wire_O, pk: dict, inputs, group_order: int, n_constraints: int | None = None,
                 custom=(), device: bool = False, limit: int = 16, ctx=None, lookup=None,
-                lookups=None) -> WireSolution:
+                lookups=None, shuffle=None) -> WireSolution:
     """-> ``WireSolution``: the wire values A, B, C of the circuit, each (n, 32) canonical little-endian, or its
     errors.
 
@@ -203,7 +258,8 @@ def solve_wires(wire_L, wire_R, wire_O, pk: dict, inputs, group_order: int, n_co
     A, B, C as (n, 32) uint8 CUDA tensors on the context's device (no copy to the host), else numpy arrays.
     ``limit``: how many locations of each error kind to list.  ``lookup`` = (q_K, (t1, t2, t3)) or ``lookups`` =
     [(q_0, (t1, t2, t3)), ...], as ``Prover.from_arrays`` takes them: lookup rows then define from their table (the
-    module docstring has the rule).  Malformed arguments are a ValueError before the library is called; the solve runs
+    module docstring has the rule).  ``shuffle`` = (q_in, q_out), as ``Prover.from_arrays`` takes it: the out-rows
+    then take the in-rows' tuples in sorted order (the module docstring has the rule).  Malformed arguments are a ValueError before the library is called; the solve runs
     on the GPU of ``ctx`` (default: the default context)."""
     n = group_order
     if isinstance(n, bool) or not isinstance(n, (int, np.integer)) or n < 2 or n & (n - 1) or n > 1 << MAX_LOG_N:
@@ -234,6 +290,12 @@ def solve_wires(wire_L, wire_R, wire_O, pk: dict, inputs, group_order: int, n_co
         table = (qk, None, tcols, rows)
     elif lookups is not None:
         table = check_lookups(lookups, n)
+    sh = None
+    if shuffle is not None:
+        if table is not None:
+            raise ValueError("shuffles do not combine with lookups")
+        q_in, q_out = check_shuffle(shuffle, n)
+        sh = [_le_rows(q) for q in (q_in, q_out)]
     ctx = ctx or default_context()
 
     vp = ctypes.c_void_p
@@ -251,7 +313,15 @@ def solve_wires(wire_L, wire_R, wire_O, pk: dict, inputs, group_order: int, n_co
     else:
         out = [np.empty((n, 32), dtype=np.uint8) for _ in range(3)]
         ptrs = [a.ctypes.data for a in out]
-    if table is None:
+    if sh is not None:
+        counts = (ctypes.c_uint64 * 4)()
+        lists = (ctypes.c_uint32 * max(1, 8 * limit))()
+        check(lib().pb200_solve_wires_shuffle(ctx.handle, ids.ctypes.data_as(vp), n.bit_length() - 1, m, sel_arr,
+                                              len(exps), ebytes, cust_arr, len(in_ids), in_ids.ctypes.data_as(vp),
+                                              in_vals.ctypes.data_as(vp), sh[0].ctypes.data_as(vp),
+                                              sh[1].ctypes.data_as(vp), limit, counts, lists, (vp * 3)(*ptrs),
+                                              1 if device else 0))
+    elif table is None:
         check(lib().pb200_solve_wires(ctx.handle, ids.ctypes.data_as(vp), n.bit_length() - 1, m, sel_arr, len(exps),
                                       ebytes, cust_arr, len(in_ids), in_ids.ctypes.data_as(vp),
                                       in_vals.ctypes.data_as(vp), limit, counts, lists, (vp * 3)(*ptrs),
@@ -289,4 +359,13 @@ def solve_wires(wire_L, wire_R, wire_O, pk: dict, inputs, group_order: int, n_co
         sol._operands.update({r: (val(2 * limit + 2 * k), val(2 * limit + 2 * k + 1))
                               for k, r in enumerate(sol.ambiguous_rows)})
         sol._table = (table[1], table[2])
+    if sh is not None:
+        more = [int(x) for x in lists[3 * limit:8 * limit]]
+        sol.late, sol.clash = int(counts[2]), int(counts[3])
+        sol.late_cells = [(more[2 * k], more[2 * k + 1]) for k in range(limit) if more[2 * k] != 0xffffffff]
+        trip = more[2 * limit:]
+        listed = [trip[3 * k:3 * k + 3] for k in range(limit) if trip[3 * k] != 0xffffffff]
+        sol.clash_cells = [(c, CLASH_REASONS[why]) for c, why, _ in listed]
+        sol._clash_rows = {c: d for c, _, d in listed}
+        sol._first_out = next((r for r in range(n) if q_out[r] and not q_in[r]), None)
     return sol

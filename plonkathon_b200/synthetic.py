@@ -403,6 +403,91 @@ def range_check_circuit(log_n: int, n_values: int, bits: int = 16, seed: int = 1
     return ArrayCircuit(n, m, wL, wR, wO, QL, QR, QM, QO, QC, 0, values, [], list(zip(RUNNING_SUM_TERMS, Q)))
 
 
+# the sorted-address gate over the next row: consecutive sorted addresses step by 0 or 1, (a' - a)(a' - a - 1) = 0,
+# i.e. a'^2 - 2 a a' + a^2 - a' + a = 0  (four custom terms and QL = 1)
+SORTED_STEP_TERMS = ((0, 0, 0, 2, 0, 0), (1, 0, 0, 1, 0, 0), (2, 0, 0, 0, 0, 0), (0, 0, 0, 1, 0, 0))
+
+
+def memory_circuit(log_n: int, n_addresses: int, seed: int = 1) -> ArrayCircuit:
+    """A memory-checking circuit: a log of memory records in execution order, the same log sorted by address, and gates
+    over the sorted side.  ``shuffle=`` lets ``solve_wires`` find its wires from its seeds alone.
+
+    The seeds (every free variable): a multiplier x, the addresses 0..n_addresses-1, each address's initial value and
+    a starting time.  Each of (n - 1) // 5 records is up to three rows: the time counter steps by one (an add-constant
+    gate), a write stores prev * x + k at its address (a gate; a read stores nothing and reuses the address's last
+    value variable), and a record row (address, time, value), every selector 0, q_in = 1.  The first n_addresses
+    records write to every address once, in a random order; the rest pick an address at random and write half the
+    time.  A contiguous block of out-rows (q_out = 1) follows, as fresh variables, holding the records sorted by
+    (address, time, value), with the sorted-address gate (SORTED_STEP_TERMS, QL = 1) on all but its last row, which
+    reads the next row (rows are cyclic).  After it, a running sum of the sorted values reads the out-rows' variables.
+    ``values`` is the builder's own witness, the sorted side sorted here.  ValueError when the records do not cover
+    the addresses."""
+    n = 1 << log_n
+    n_rec = (n - 1) // 5
+    if not 1 <= n_addresses <= n_rec:
+        raise ValueError("n_addresses must be in [1, %d] (one record each at least) for 2^%d rows, got %r"
+                         % (n_rec, log_n, n_addresses))
+    rng = random.Random(seed)
+    values = []
+    wL = np.full(n, -1, dtype=np.int64)
+    wR = np.full(n, -1, dtype=np.int64)
+    wO = np.full(n, -1, dtype=np.int64)
+    QL, QR, QM, QO, QC = ([0] * n for _ in range(5))
+    Q = [[0] * n for _ in SORTED_STEP_TERMS]
+    q_in, q_out = [0] * n, [0] * n
+    row = 0
+
+    def new(v):
+        values.append(v % R)
+        return len(values) - 1
+
+    def put(a, b, o):
+        nonlocal row
+        wL[row], wR[row], wO[row] = a, b, o
+        row += 1
+        return row - 1
+
+    x = new(rng.randrange(1, R))
+    addr = [new(a) for a in range(n_addresses)]
+    last = [new(rng.randrange(R)) for _ in range(n_addresses)]
+    t = new(rng.randrange(1 << 20))
+    first = list(range(n_addresses))
+    rng.shuffle(first)
+    records = []
+    for i in range(n_rec):
+        a = first[i] if i < n_addresses else rng.randrange(n_addresses)
+        nt = new(values[t] + 1)  # t <== t + 1 : L = -1, C = -1, O = 1
+        r = put(t, t, nt)
+        QL[r], QC[r], QO[r] = R - 1, R - 1, 1
+        t = nt
+        if i < n_addresses or rng.randrange(2):  # v <== prev * x + k : M = -1, C = -k, O = 1
+            k = rng.randrange(1, 1 << 30)
+            v = new(values[last[a]] * values[x] + k)
+            r = put(last[a], x, v)
+            QM[r], QC[r], QO[r] = R - 1, (R - k) % R, 1
+            last[a] = v
+        q_in[put(addr[a], t, last[a])] = 1
+        records.append((values[addr[a]], values[t], values[last[a]]))
+    records.sort()
+    sorted_v = []
+    for j, rec in enumerate(records):
+        r = put(*(new(w) for w in rec))
+        q_out[r] = 1
+        sorted_v.append(wO[r])
+        if j + 1 < len(records):
+            for q, wgt in zip(Q, (1, R - 2, 1, R - 1)):
+                q[r] = wgt
+            QL[r] = 1
+    s = -1
+    for v in sorted_v:  # s <== s + v : L = R = -1, O = 1 (the first s is the constant 0)
+        ns = new((values[s] if s >= 0 else 0) + values[v])
+        r = put(s, v, ns)
+        QL[r], QR[r], QO[r] = R - 1, R - 1, 1
+        s = ns
+    return ArrayCircuit(n, row, wL, wR, wO, QL, QR, QM, QO, QC, 0, values, [], list(zip(SORTED_STEP_TERMS, Q)),
+                        shuffle=(q_in, q_out))
+
+
 def circuit_arrays(c: ArrayCircuit):
     """-> (pk dict of (n,32) uint8 arrays, A, B, C arrays, public list) ready for Prover.from_arrays /
     prove_arrays."""
