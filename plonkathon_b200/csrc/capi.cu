@@ -8,6 +8,7 @@
 #include "msm_bucket.cuh"
 #include "prover.cuh"
 #include "pairing.cuh"
+#include "solve.cuh"
 #include "transcript.cuh"
 
 namespace pb200 {
@@ -68,12 +69,7 @@ void prover_check(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t
 // permutation.cu
 void permutation_run(Context* ctx, const int64_t* h_ids, int log_n, uint8_t* h_S);
 // solve.cu
-void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constraints, const uint8_t* const* h_sel,
-               int n_custom, const uint8_t* h_exps, const uint8_t* const* h_custom, uint64_t n_inputs,
-               const int64_t* h_in_ids, const uint8_t* h_in_vals, uint32_t limit, uint64_t* h_counts,
-               uint32_t* h_lists, void* const* out, bool out_on_device, const uint8_t* h_qk, const uint8_t* h_qtag,
-               const uint8_t* const* h_tab, uint64_t tab_rows, uint8_t* h_operands, bool shuffle = false,
-               const uint8_t* h_qin = nullptr, const uint8_t* h_qout = nullptr);
+void solve_run(Context* ctx, const SolveArgs& a, const SolveTableArgs* tb, const SolveShuffleArgs* sf);
 void solve_stages(double* out_ms, int count);
 // ptau.cu
 Srs* srs_create_ptau(Context* ctx, const uint8_t* h_g1, uint64_t count, const uint8_t* h_tau_g2, int precompute);
@@ -592,8 +588,9 @@ int pb200_solve_wires(pb200_ctx* ctx, const int64_t* h_ids, int log_n, uint64_t 
                       const uint8_t* h_input_values, uint32_t limit, uint64_t* h_counts, uint32_t* h_lists,
                       void* const* out, int out_on_device) {
   PB_API_BEGIN PB_ON_CTX(C(ctx));
-  solve_run(C(ctx), h_ids, log_n, n_constraints, h_sel, (int)n_custom, h_exps, h_custom, n_inputs, h_input_ids,
-            h_input_values, limit, h_counts, h_lists, out, out_on_device != 0, nullptr, nullptr, nullptr, 0, nullptr);
+  const SolveArgs a{h_ids, log_n, n_constraints, h_sel, (int)n_custom, h_exps, h_custom, n_inputs, h_input_ids,
+                    h_input_values, limit, h_counts, h_lists, out, out_on_device != 0};
+  solve_run(C(ctx), a, nullptr, nullptr);
   PB_API_END
 }
 int pb200_solve_wires_lookup(pb200_ctx* ctx, const int64_t* h_ids, int log_n, uint64_t n_constraints,
@@ -605,10 +602,10 @@ int pb200_solve_wires_lookup(pb200_ctx* ctx, const int64_t* h_ids, int log_n, ui
                              uint8_t* h_operands, void* const* out, int out_on_device) {
   PB_API_BEGIN PB_ON_CTX(C(ctx));
   PB_CHECK(!h_qtag == !h_t4, "tagged lookups need both Q_T and the table tag column t4");
-  const uint8_t* tab[4] = {h_t1, h_t2, h_t3, h_t4};
-  solve_run(C(ctx), h_ids, log_n, n_constraints, h_sel, (int)n_custom, h_exps, h_custom, n_inputs, h_input_ids,
-            h_input_values, limit, h_counts, h_lists, out, out_on_device != 0, h_qk, h_qtag, tab, table_rows,
-            h_operands);
+  const SolveArgs a{h_ids, log_n, n_constraints, h_sel, (int)n_custom, h_exps, h_custom, n_inputs, h_input_ids,
+                    h_input_values, limit, h_counts, h_lists, out, out_on_device != 0};
+  const SolveTableArgs tb{h_qk, h_qtag, {h_t1, h_t2, h_t3, h_t4}, table_rows, h_operands};
+  solve_run(C(ctx), a, &tb, nullptr);
   PB_API_END
 }
 int pb200_solve_wires_shuffle(pb200_ctx* ctx, const int64_t* h_ids, int log_n, uint64_t n_constraints,
@@ -618,9 +615,10 @@ int pb200_solve_wires_shuffle(pb200_ctx* ctx, const int64_t* h_ids, int log_n, u
                               uint32_t limit, uint64_t* h_counts, uint32_t* h_lists, void* const* out,
                               int out_on_device) {
   PB_API_BEGIN PB_ON_CTX(C(ctx));
-  solve_run(C(ctx), h_ids, log_n, n_constraints, h_sel, (int)n_custom, h_exps, h_custom, n_inputs, h_input_ids,
-            h_input_values, limit, h_counts, h_lists, out, out_on_device != 0, nullptr, nullptr, nullptr, 0, nullptr,
-            true, h_qin, h_qout);
+  const SolveArgs a{h_ids, log_n, n_constraints, h_sel, (int)n_custom, h_exps, h_custom, n_inputs, h_input_ids,
+                    h_input_values, limit, h_counts, h_lists, out, out_on_device != 0};
+  const SolveShuffleArgs sf{h_qin, h_qout};
+  solve_run(C(ctx), a, nullptr, &sf);
   PB_API_END
 }
 void pb200_solve_shuffle_stages(double* ms, int count) { solve_stages(ms, count); }

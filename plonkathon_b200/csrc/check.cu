@@ -39,16 +39,7 @@ __global__ void k_count_noncanonical(const Fr* v, uint64_t n, uint32_t* bad);
 
 #define PB_SIGMA_NONE 0xffffffffu
 #define PB_SIGMA_DUP 0x80000000u
-#define PB_CHECK_GRID(n, t) (unsigned)(((n) + (t)-1) / (t)), (t)
 
-__device__ __forceinline__ Fr chk_ld(const Fr* p) {
-  const uint4* q = reinterpret_cast<const uint4*>(p);
-  uint4 a = __ldg(q), b = __ldg(q + 1);
-  Fr r;
-  r.v[0] = a.x; r.v[1] = a.y; r.v[2] = a.z; r.v[3] = a.w;
-  r.v[4] = b.x; r.v[5] = b.y; r.v[6] = b.z; r.v[7] = b.w;
-  return r;
-}
 // 64-bit word w (0..3) of a value: limbs 2w and 2w + 1 (selected by value, so x stays in registers)
 __device__ __forceinline__ uint64_t chk_word(const Fr& x, int w) {
   const uint32_t lo = w == 0 ? x.v[0] : w == 1 ? x.v[2] : w == 2 ? x.v[4] : x.v[6];
@@ -58,7 +49,7 @@ __device__ __forceinline__ uint64_t chk_word(const Fr& x, int w) {
 // label of cell c = 3 row + col: omega^row (col + 1), Montgomery (roots: omega^i Montgomery)
 __device__ __forceinline__ Fr chk_label(const Fr* roots, uint32_t c) {
   const uint32_t row = c / 3, col = c - 3 * row;
-  const Fr w = chk_ld(roots + row);
+  const Fr w = ldg_fr(roots + row);
   Fr x = w;
   if (col >= 1) x = fp_add(x, w);
   if (col == 2) x = fp_add(x, w);
@@ -68,12 +59,12 @@ __device__ __forceinline__ Fr chk_label(const Fr* roots, uint32_t c) {
 struct SCols { const Fr* s[3]; };
 __device__ __forceinline__ Fr chk_s(const SCols& S, uint64_t n, uint32_t c) {
   const uint32_t row = c / 3, col = c - 3 * row;
-  return chk_ld((col == 0 ? S.s[0] : col == 1 ? S.s[1] : S.s[2]) + row);  // static indices: no local copy
+  return ldg_fr((col == 0 ? S.s[0] : col == 1 ? S.s[1] : S.s[2]) + row);  // static indices: no local copy
 }
 // value of cell c in the column-major wire copy W = A | B | C
 __device__ __forceinline__ Fr chk_v(const Fr* W, uint64_t n, uint32_t c) {
   const uint32_t row = c / 3, col = c - 3 * row;
-  return chk_ld(W + col * n + row);
+  return ldg_fr(W + col * n + row);
 }
 
 // ---- sigma ---------------------------------------------------------------------------------------------------------
@@ -135,16 +126,16 @@ __global__ void __launch_bounds__(128) k_check_gate(const Fr* W, const Fr* QL, c
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const Fr *A = W, *B = W + n, *C = W + 2 * n;
-  const Fr a = chk_ld(A + i), b = chk_ld(B + i), c = chk_ld(C + i);
-  Fr s = fp_mul(a, chk_ld(QL + i));
-  s = fp_add(s, fp_mul(b, chk_ld(QR + i)));
-  s = fp_add(s, fp_mul(fp_mul(a, b), chk_ld(QM + i)));
-  s = fp_add(s, fp_mul(c, chk_ld(QO + i)));
-  s = fp_add(s, chk_ld(QC + i));
-  if (i < n_public) s = fp_add(s, chk_ld(pub + i));
+  const Fr a = ldg_fr(A + i), b = ldg_fr(B + i), c = ldg_fr(C + i);
+  Fr s = fp_mul(a, ldg_fr(QL + i));
+  s = fp_add(s, fp_mul(b, ldg_fr(QR + i)));
+  s = fp_add(s, fp_mul(fp_mul(a, b), ldg_fr(QM + i)));
+  s = fp_add(s, fp_mul(c, ldg_fr(QO + i)));
+  s = fp_add(s, ldg_fr(QC + i));
+  if (i < n_public) s = fp_add(s, ldg_fr(pub + i));
   if constexpr (NEXT) {
     const uint64_t i1 = i + 1 == n ? 0 : i + 1;
-    s = custom_gate_sum_next(ct, i, a, b, c, chk_ld(A + i1), chk_ld(B + i1), chk_ld(C + i1), s);
+    s = custom_gate_sum_next(ct, i, a, b, c, ldg_fr(A + i1), ldg_fr(B + i1), ldg_fr(C + i1), s);
   } else {
     s = custom_gate_sum(ct, i, a, b, c, s);
   }
@@ -165,9 +156,9 @@ __global__ void __launch_bounds__(128) k_check_lookup(const Fr* W, const Fr* QK,
                                                       uint64_t rows, uint64_t n, uint8_t* flag) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  if (chk_ld(QK + i).is_zero()) { flag[i] = 0; return; }
+  if (ldg_fr(QK + i).is_zero()) { flag[i] = 0; return; }
   const int width = QT ? 4 : 3;
-  const Fr key[4] = {chk_ld(W + i), chk_ld(W + n + i), chk_ld(W + 2 * n + i), QT ? chk_ld(QT + i) : Fr::zero()};
+  const Fr key[4] = {ldg_fr(W + i), ldg_fr(W + n + i), ldg_fr(W + 2 * n + i), QT ? ldg_fr(QT + i) : Fr::zero()};
   uint64_t lo = 0, hi = rows;  // the prover's sorted table copy, in lookup_cmp's order
   while (lo < hi) {
     const uint64_t mid = (lo + hi) / 2;
@@ -181,7 +172,7 @@ __global__ void __launch_bounds__(128) k_check_lookup(const Fr* W, const Fr* QK,
 __global__ void k_check_sh_keys(const Fr* W, Fr theta, Fr theta2, uint64_t n, uint64_t* keys, uint32_t* rows) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const Fr f = fp_add(chk_ld(W + i), fp_add(fp_mul(theta, chk_ld(W + n + i)), fp_mul(theta2, chk_ld(W + 2 * n + i))));
+  const Fr f = fp_add(ldg_fr(W + i), fp_add(fp_mul(theta, ldg_fr(W + n + i)), fp_mul(theta2, ldg_fr(W + 2 * n + i))));
   keys[i] = chk_word(f, 0);
   rows[i] = (uint32_t)i;
 }
@@ -195,8 +186,8 @@ __global__ void k_check_sh_heads(const uint64_t* keys, const uint32_t* rows, con
   head[k] = start ? 1 : 0;
   if (!start) {
     const uint32_t r = rows[k], p = rows[k - 1];
-    if (chk_ld(W + r) != chk_ld(W + p) || chk_ld(W + n + r) != chk_ld(W + n + p) ||
-        chk_ld(W + 2 * n + r) != chk_ld(W + 2 * n + p))
+    if (ldg_fr(W + r) != ldg_fr(W + p) || ldg_fr(W + n + r) != ldg_fr(W + n + p) ||
+        ldg_fr(W + 2 * n + r) != ldg_fr(W + 2 * n + p))
       atomicAdd(impure, 1u);
   }
 }
@@ -209,8 +200,8 @@ __global__ void __launch_bounds__(256) k_check_sh_count(const uint32_t* run, con
   if (k < n) {
     const uint32_t r = rows[k];
     id = run[k] - 1;
-    in = chk_ld(QIN + r).is_zero() ? 0 : 1;
-    out = chk_ld(QOUT + r).is_zero() ? 0 : 1;
+    in = ldg_fr(QIN + r).is_zero() ? 0 : 1;
+    out = ldg_fr(QOUT + r).is_zero() ? 0 : 1;
   }
   const uint32_t peers = __match_any_sync(0xffffffffu, id);
   in = __reduce_add_sync(peers, in);
@@ -225,7 +216,7 @@ __global__ void k_check_sh_flag(const uint32_t* run, const uint32_t* rows, const
   if (k >= n) return;
   const uint32_t r = rows[k];
   const unsigned long long v = cnt[run[k] - 1];
-  const bool on = !chk_ld(QIN + r).is_zero() || !chk_ld(QOUT + r).is_zero();
+  const bool on = !ldg_fr(QIN + r).is_zero() || !ldg_fr(QOUT + r).is_zero();
   flag[r] = (on && (uint32_t)v != (uint32_t)(v >> 32)) ? 1 : 0;
 }
 // the copy list's pairs: (c, sigma(c)) for the `count` lowest failing cells
@@ -272,11 +263,6 @@ struct CheckTemp {
   }
 };
 
-static void launched(Context* ctx) {
-  ctx->launches++;
-  PB_CUDA(cudaGetLastError());
-}
-
 // sigma from the 3n labels and the 3n S entries, each sorted by its 64-bit word; the word is the first of the four
 // that no two labels share
 static void build_sigma(Prover* P, DevBuf& temp) {
@@ -291,7 +277,7 @@ static void build_sigma(Prover* P, DevBuf& temp) {
   int w = 0;
   for (;; w++) {
     PB_CHECK(w < 4, "witness check: every 64-bit word of the cell labels repeats among them");
-    k_check_label_keys<<<PB_CHECK_GRID(m, 256), 0, st>>>(P->roots.as<Fr>(), m, w, lk.as<uint64_t>(), lc.as<uint32_t>());
+    k_check_label_keys<<<PB_GRID(m, 256), 0, st>>>(P->roots.as<Fr>(), m, w, lk.as<uint64_t>(), lc.as<uint32_t>());
     launched(ctx);
     lkeys = cub::DoubleBuffer<uint64_t>(lk.as<uint64_t>(), lk2.as<uint64_t>());
     lcells = cub::DoubleBuffer<uint32_t>(lc.as<uint32_t>(), lc2.as<uint32_t>());
@@ -299,14 +285,14 @@ static void build_sigma(Prover* P, DevBuf& temp) {
     PB_CUDA(cub::DeviceRadixSort::SortPairs(temp.p, tb, lkeys, lcells, (int)m, 0, 64, st));
     launched(ctx);
     PB_CUDA(cudaMemsetAsync(equal.p, 0, 4, st));
-    k_check_adjacent<<<PB_CHECK_GRID(m, 256), 0, st>>>(lkeys.Current(), m, equal.as<uint32_t>());
+    k_check_adjacent<<<PB_GRID(m, 256), 0, st>>>(lkeys.Current(), m, equal.as<uint32_t>());
     launched(ctx);
     uint32_t eq = 0;
     PB_CUDA(cudaMemcpyAsync(&eq, equal.p, 4, cudaMemcpyDeviceToHost, st));
     PB_CUDA(cudaStreamSynchronize(st));
     if (eq == 0) break;
   }
-  k_check_s_keys<<<PB_CHECK_GRID(m, 256), 0, st>>>(S, n, m, w, sk.as<uint64_t>(), sc.as<uint32_t>());
+  k_check_s_keys<<<PB_GRID(m, 256), 0, st>>>(S, n, m, w, sk.as<uint64_t>(), sc.as<uint32_t>());
   launched(ctx);
   cub::DoubleBuffer<uint64_t> skeys(sk.as<uint64_t>(), sk2.as<uint64_t>());
   cub::DoubleBuffer<uint32_t> scells(sc.as<uint32_t>(), sc2.as<uint32_t>());
@@ -315,18 +301,20 @@ static void build_sigma(Prover* P, DevBuf& temp) {
   launched(ctx);
   DevBuf sigma(m * 4);
   PB_CUDA(cudaMemsetAsync(first.p, 0xff, m * 4, st));
-  k_check_sigma<<<PB_CHECK_GRID(m, 128), 0, st>>>(skeys.Current(), scells.Current(), lkeys.Current(), lcells.Current(), m,
+  k_check_sigma<<<PB_GRID(m, 128), 0, st>>>(skeys.Current(), scells.Current(), lkeys.Current(), lcells.Current(), m,
                                                   S, P->roots.as<Fr>(), n, sigma.as<uint32_t>(), first.as<uint32_t>());
   launched(ctx);
-  k_check_sigma_dups<<<PB_CHECK_GRID(m, 256), 0, st>>>(sigma.as<uint32_t>(), first.as<uint32_t>(), m);
+  k_check_sigma_dups<<<PB_GRID(m, 256), 0, st>>>(sigma.as<uint32_t>(), first.as<uint32_t>(), m);
   launched(ctx);
   PB_CUDA(cudaStreamSynchronize(st));  // the temporaries die here
   P->chk_sigma = std::move(sigma);
 }
 
-// flags[0, m) -> *count and the lowest min(count, limit) flagged indices at h_out
-static uint64_t compact(Context* ctx, const uint8_t* flags, uint64_t m, DevBuf& temp, uint32_t* d_idx, uint32_t* d_num,
-                        uint32_t limit, uint32_t* h_out) {
+// flags[0, m) -> the number of flagged indices, and the lowest min(count, limit) of them at h_out (null: the count
+// only).  d_idx: m words, d_num: one; temp: at least cub::DeviceSelect::Flagged's storage over m items.  The wire
+// solver lists its errors with it too.
+uint64_t compact_flagged(Context* ctx, const uint8_t* flags, uint64_t m, DevBuf& temp, uint32_t* d_idx,
+                         uint32_t* d_num, uint32_t limit, uint32_t* h_out) {
   cudaStream_t st = ctx->stream;
   size_t tb = temp.bytes;
   PB_CUDA(cub::DeviceSelect::Flagged(temp.p, tb, thrust::counting_iterator<uint32_t>(0), flags, d_idx, d_num, (int)m,
@@ -336,7 +324,7 @@ static uint64_t compact(Context* ctx, const uint8_t* flags, uint64_t m, DevBuf& 
   PB_CUDA(cudaMemcpyAsync(&num, d_num, 4, cudaMemcpyDeviceToHost, st));
   PB_CUDA(cudaStreamSynchronize(st));
   const uint32_t take = num < limit ? num : limit;
-  if (take) {
+  if (take && h_out) {
     PB_CUDA(cudaMemcpyAsync(h_out, d_idx, (size_t)take * 4, cudaMemcpyDeviceToHost, st));
     PB_CUDA(cudaStreamSynchronize(st));
   }
@@ -398,7 +386,7 @@ void prover_check(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t
   for (int k = 0; k < 3; k++) {
     Fr* w = W.as<Fr>() + k * n;
     PB_CUDA(cudaMemcpyAsync(w, src[k], n * 32, wires_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
-    k_count_noncanonical<<<PB_CHECK_GRID(n, 256), 0, st>>>(w, n, bad);
+    k_count_noncanonical<<<PB_GRID(n, 256), 0, st>>>(w, n, bad);
     launched(ctx);
     fr_to_mont(ctx, w, w, n);
   }
@@ -415,35 +403,35 @@ void prover_check(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t
   uint8_t* f = flags.as<uint8_t>();
   const Fr* Wp = W.as<Fr>();
   // gates
-  (P->next_row ? k_check_gate<true> : k_check_gate<false>)<<<PB_CHECK_GRID(n, 128), 0, st>>>(
+  (P->next_row ? k_check_gate<true> : k_check_gate<false>)<<<PB_GRID(n, 128), 0, st>>>(
       Wp, P->sel_lag[Prover::QL].as<Fr>(), P->sel_lag[Prover::QR].as<Fr>(), P->sel_lag[Prover::QM].as<Fr>(),
       P->sel_lag[Prover::QO].as<Fr>(), P->sel_lag[Prover::QC].as<Fr>(), pubd.as<Fr>(), n_public,
       P->custom_terms(P->sel_lag), n, f);
   launched(ctx);
-  h_counts[0] = compact(ctx, f, n, temp, idx.as<uint32_t>(), num, limit, l_gate);
+  h_counts[0] = compact_flagged(ctx, f, n, temp, idx.as<uint32_t>(), num, limit, l_gate);
   // copy constraints and the key
-  k_check_copy<<<PB_CHECK_GRID(m, 256), 0, st>>>(Wp, P->chk_sigma.as<uint32_t>(), n, m, f, f + m);
+  k_check_copy<<<PB_GRID(m, 256), 0, st>>>(Wp, P->chk_sigma.as<uint32_t>(), n, m, f, f + m);
   launched(ctx);
   std::vector<uint32_t> cells(limit);
-  h_counts[1] = compact(ctx, f, m, temp, idx.as<uint32_t>(), num, limit, cells.data());
+  h_counts[1] = compact_flagged(ctx, f, m, temp, idx.as<uint32_t>(), num, limit, cells.data());
   const uint32_t pairs = (uint32_t)std::min<uint64_t>(h_counts[1], limit);
   if (pairs) {  // (c, sigma(c)) of the listed cells
     DevBuf pb((size_t)pairs * 12);
     PB_CUDA(cudaMemcpyAsync(pb.p, cells.data(), (size_t)pairs * 4, cudaMemcpyHostToDevice, st));
-    k_check_pairs<<<PB_CHECK_GRID(pairs, 128), 0, st>>>(pb.as<uint32_t>(), pairs, P->chk_sigma.as<uint32_t>(),
+    k_check_pairs<<<PB_GRID(pairs, 128), 0, st>>>(pb.as<uint32_t>(), pairs, P->chk_sigma.as<uint32_t>(),
                                                         pb.as<uint32_t>() + pairs);
     launched(ctx);
     PB_CUDA(cudaMemcpyAsync(l_copy, pb.as<uint32_t>() + pairs, (size_t)pairs * 8, cudaMemcpyDeviceToHost, st));
     PB_CUDA(cudaStreamSynchronize(st));
   }
-  h_counts[2] = compact(ctx, f + m, m, temp, idx.as<uint32_t>(), num, limit, l_key);
+  h_counts[2] = compact_flagged(ctx, f + m, m, temp, idx.as<uint32_t>(), num, limit, l_key);
   // lookup rows
   if (P->lk) {
-    k_check_lookup<<<PB_CHECK_GRID(n, 128), 0, st>>>(Wp, P->lk_qk_lag.as<Fr>(),
+    k_check_lookup<<<PB_GRID(n, 128), 0, st>>>(Wp, P->lk_qk_lag.as<Fr>(),
                                                      P->lk_tagged ? P->lk_qt_lag.as<Fr>() : nullptr, P->lk_keys.as<Fr>(),
                                                      P->lk_rows, n, f);
     launched(ctx);
-    h_counts[3] = compact(ctx, f, n, temp, idx.as<uint32_t>(), num, limit, l_lookup);
+    h_counts[3] = compact_flagged(ctx, f, n, temp, idx.as<uint32_t>(), num, limit, l_lookup);
   }
   // shuffle rows: sort by the fingerprint's word, count both sides per run of equal words
   if (P->sh) {
@@ -455,7 +443,7 @@ void prover_check(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t
     for (int draw = 0;; draw++) {
       PB_CHECK(draw < 8, "witness check: eight shuffle fingerprints in a row had colliding words");
       const Fr theta = check_random_fr();
-      k_check_sh_keys<<<PB_CHECK_GRID(n, 128), 0, st>>>(Wp, theta, fp_sqr(theta), n, k1.as<uint64_t>(), r1.as<uint32_t>());
+      k_check_sh_keys<<<PB_GRID(n, 128), 0, st>>>(Wp, theta, fp_sqr(theta), n, k1.as<uint64_t>(), r1.as<uint32_t>());
       launched(ctx);
       keys = cub::DoubleBuffer<uint64_t>(k1.as<uint64_t>(), k2.as<uint64_t>());
       rows = cub::DoubleBuffer<uint32_t>(r1.as<uint32_t>(), r2.as<uint32_t>());
@@ -463,7 +451,7 @@ void prover_check(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t
       PB_CUDA(cub::DeviceRadixSort::SortPairs(temp.p, tb, keys, rows, (int)n, 0, 64, st));
       launched(ctx);
       PB_CUDA(cudaMemsetAsync(impure, 0, 4, st));
-      k_check_sh_heads<<<PB_CHECK_GRID(n, 256), 0, st>>>(keys.Current(), rows.Current(), Wp, n, run.as<uint32_t>(),
+      k_check_sh_heads<<<PB_GRID(n, 256), 0, st>>>(keys.Current(), rows.Current(), Wp, n, run.as<uint32_t>(),
                                                          impure);
       launched(ctx);
       uint32_t imp = 0;
@@ -477,13 +465,13 @@ void prover_check(Prover* P, const uint8_t* hA, const uint8_t* hB, const uint8_t
     PB_CUDA(cub::DeviceScan::InclusiveSum(temp.p, tb, run.as<uint32_t>(), run_id, (int)n, st));
     launched(ctx);
     PB_CUDA(cudaMemsetAsync(cnt.p, 0, n * 8, st));
-    k_check_sh_count<<<PB_CHECK_GRID(n, 256), 0, st>>>(run_id, rows.Current(), QIN, QOUT, n,
+    k_check_sh_count<<<PB_GRID(n, 256), 0, st>>>(run_id, rows.Current(), QIN, QOUT, n,
                                                        cnt.as<unsigned long long>());
     launched(ctx);
-    k_check_sh_flag<<<PB_CHECK_GRID(n, 256), 0, st>>>(run_id, rows.Current(), cnt.as<unsigned long long>(), QIN, QOUT,
+    k_check_sh_flag<<<PB_GRID(n, 256), 0, st>>>(run_id, rows.Current(), cnt.as<unsigned long long>(), QIN, QOUT,
                                                       n, f);
     launched(ctx);
-    h_counts[4] = compact(ctx, f, n, temp, idx.as<uint32_t>(), num, limit, l_shuffle);
+    h_counts[4] = compact_flagged(ctx, f, n, temp, idx.as<uint32_t>(), num, limit, l_shuffle);
   }
   PB_CUDA(cudaStreamSynchronize(st));  // the call's buffers die here
 }

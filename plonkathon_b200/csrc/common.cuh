@@ -110,6 +110,25 @@ struct Context {
 
 NttPlan* get_plan(Context* ctx, int log_n, bool inverse);
 
+// counts a kernel launched on `ctx` and reports a launch error
+inline void launched(Context* ctx) {
+  ctx->launches++;
+  PB_CUDA(cudaGetLastError());
+}
+
+// grid and block size of a launch with one thread per item: kernel<<<PB_GRID(n, t), ...>>>
+#define PB_GRID(n, t) (unsigned)(((n) + (t)-1) / (t)), (t)
+
+// a field element through the read-only data cache, as two 16-byte loads
+__device__ __forceinline__ Fr ldg_fr(const Fr* p) {
+  const uint4* q = reinterpret_cast<const uint4*>(p);
+  uint4 a = __ldg(q), b = __ldg(q + 1);
+  Fr r;
+  r.v[0] = a.x; r.v[1] = a.y; r.v[2] = a.z; r.v[3] = a.w;
+  r.v[4] = b.x; r.v[5] = b.y; r.v[6] = b.z; r.v[7] = b.w;
+  return r;
+}
+
 // `waiter` runs nothing enqueued after this call before everything enqueued on `producer` so far has finished
 inline void stream_join(Context* ctx, cudaStream_t waiter, cudaStream_t producer) {
   PB_CUDA(cudaEventRecord(ctx->join_ev, producer));

@@ -96,17 +96,6 @@ uint64_t srs_size(Srs* s);
 // ------------------------------------------------------------------------------------------
 // kernels
 // ------------------------------------------------------------------------------------------
-#define PB_GRID(n, t) (unsigned)(((n) + (t)-1) / (t)), (t)
-
-__device__ __forceinline__ Fr ldg_fr(const Fr* p) {
-  const uint4* q = reinterpret_cast<const uint4*>(p);
-  uint4 a = __ldg(q), b = __ldg(q + 1);
-  Fr r;
-  r.v[0] = a.x; r.v[1] = a.y; r.v[2] = a.z; r.v[3] = a.w;
-  r.v[4] = b.x; r.v[5] = b.y; r.v[6] = b.z; r.v[7] = b.w;
-  return r;
-}
-
 static Fr load_fr_checked(const uint8_t* h) {
   Fr a;
   memcpy(a.v, h, 32);
@@ -1108,6 +1097,36 @@ static ZkPatch zh_multiple(std::initializer_list<Fr> c) {
 // and z2(zeta w), and round 5 uses the blinded vectors.  deg T <= 3n + 5 still holds (the lookup products reach 2n + 6
 // after the division), so T is split as in plain zero-knowledge mode and the proof keeps its 1216 bytes.
 
+// q_K, Q_T and the table as prover_set_lookup takes them (and the wire solver, which reads the same table): refuses a
+// missing column, an empty table, more table rows than n, q_K not 0 or 1, Q_T not canonical or not 0 where q_K = 0,
+// and a table value not canonical, in that order.
+void lookup_require(uint64_t n, const uint8_t* h_qk, const uint8_t* h_qtag, const uint8_t* const* h_tab,
+                    uint64_t rows) {
+  const bool tagged = h_qtag != nullptr;
+  PB_CHECK(h_qk && h_tab && h_tab[0] && h_tab[1] && h_tab[2], "lookups need q_K and three table columns");
+  PB_CHECK(!tagged || h_tab[3], "tagged lookups need the table tag column t4");
+  PB_CHECK(rows >= 1, "the lookup table is empty");
+  PB_CHECK(rows <= n, "the lookup table has more rows than the circuit");
+  // q_K: 0 or 1 on every row; Q_T canonical and 0 where q_K = 0
+  for (uint64_t i = 0; i < n; i++) {
+    const uint8_t* e = h_qk + 32 * i;
+    bool ok = e[0] <= 1;
+    for (int k = 1; k < 32 && ok; k++) ok = e[k] == 0;
+    PB_CHECK(ok, "q_K must be 0 or 1 on every row");
+    if (!tagged) continue;
+    Fr x;
+    memcpy(x.v, h_qtag + 32 * i, 32);
+    PB_CHECK(fp_is_canonical(x), ("Q_T on row " + std::to_string(i) + " not reduced below the field modulus").c_str());
+    PB_CHECK(e[0] == 1 || x.is_zero(), ("Q_T must be 0 where q_K = 0: row " + std::to_string(i)).c_str());
+  }
+  for (int w = 0; w < (tagged ? 4 : 3); w++)
+    for (uint64_t r = 0; r < rows; r++) {
+      Fr x;
+      memcpy(x.v, h_tab[w] + 32 * r, 32);
+      PB_CHECK(fp_is_canonical(x), "lookup table value not reduced below the field modulus");
+    }
+}
+
 // h_qtag == nullptr: one untagged table of three columns (h_tab[3] unused).  Otherwise several tables concatenated: the
 // fourth column h_tab[3] holds each table row's table id and h_qtag = Q_T the id of the table each lookup row reads,
 // zero wherever q_K = 0.  The rows are matched on (a, b, c, Q_T) and compressed with eta^3 t4 (eta^3 Q_T in the
@@ -1125,22 +1144,7 @@ void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* h_qtag, co
   PB_CHECK(!P->zk, "lookups do not combine with zero-knowledge mode switched on first: set the table, then "
                    "pb200_prover_set_zk_lookup");
   PB_CHECK(!P->lk, "the lookup table is already set (set it once, before the first proof)");
-  PB_CHECK(h_qk && h_tab && h_tab[0] && h_tab[1] && h_tab[2], "lookups need q_K and three table columns");
-  PB_CHECK(!tagged || h_tab[3], "tagged lookups need the table tag column t4");
-  PB_CHECK(rows >= 1, "the lookup table is empty");
-  PB_CHECK(rows <= n, "the lookup table has more rows than the circuit");
-  // q_K: 0 or 1 on every row; Q_T canonical and 0 where q_K = 0
-  for (uint64_t i = 0; i < n; i++) {
-    const uint8_t* e = h_qk + 32 * i;
-    bool ok = e[0] <= 1;
-    for (int k = 1; k < 32 && ok; k++) ok = e[k] == 0;
-    PB_CHECK(ok, "q_K must be 0 or 1 on every row");
-    if (!tagged) continue;
-    Fr x;
-    memcpy(x.v, h_qtag + 32 * i, 32);
-    PB_CHECK(fp_is_canonical(x), ("Q_T on row " + std::to_string(i) + " not reduced below the field modulus").c_str());
-    PB_CHECK(e[0] == 1 || x.is_zero(), ("Q_T must be 0 where q_K = 0: row " + std::to_string(i)).c_str());
-  }
+  lookup_require(n, h_qk, h_qtag, h_tab, rows);
   // the table, padded to n rows by repeating its last row, in Montgomery form
   std::vector<Fr> tab[4];
   for (int w = 0; w < width; w++) {
@@ -1148,7 +1152,6 @@ void prover_set_lookup(Prover* P, const uint8_t* h_qk, const uint8_t* h_qtag, co
     for (uint64_t r = 0; r < n; r++) {
       Fr x;
       memcpy(x.v, h_tab[w] + 32 * std::min(r, rows - 1), 32);
-      PB_CHECK(fp_is_canonical(x), "lookup table value not reduced below the field modulus");
       tab[w][r] = fp_to_mont(x);
     }
   }
@@ -1316,17 +1319,9 @@ static void grand_product(Prover* P, Fr* num, const Fr* den, Fr* lag, Fr* coeff,
 // holds (the shuffle products reach 2n + 2, 2n + 3 next-row, after the division), so T is split as in zero-knowledge
 // mode and the proof keeps its 896 (992) bytes.
 
-// h_qin, h_qout: n x 32 bytes canonical, 0 or 1 on every row, with as many ones in each.  Every check comes before any
-// change, so a refused call leaves the prover as it was.
-void prover_set_shuffle(Prover* P, const uint8_t* h_qin, const uint8_t* h_qout) {
-  Context* ctx = P->ctx;
-  const uint64_t n = P->n;
-  PB_CHECK(P->world == 1, "shuffles are not available on the sharded prover (one GPU only)");
-  PB_CHECK(!P->sliced, PB_SLICED_WHY "the shuffle quotient needs the whole coset in round 3");
-  PB_CHECK(!P->lk, "shuffles do not combine with lookups");
-  PB_CHECK(!P->zk, "shuffles do not combine with zero-knowledge mode switched on first: set the shuffle, then "
-                   "pb200_prover_set_zk_shuffle");
-  PB_CHECK(!P->sh, "the shuffle selectors are already set (set them once, before the first proof)");
+// q_in and q_out as prover_set_shuffle takes them (and the wire solver): n x 32 bytes canonical, 0 or 1 on every row,
+// with as many ones in each
+void shuffle_require(uint64_t n, const uint8_t* h_qin, const uint8_t* h_qout) {
   PB_CHECK(h_qin && h_qout, "a shuffle needs q_in and q_out");
   uint64_t ones[2] = {0, 0};
   const uint8_t* sel[2] = {h_qin, h_qout};
@@ -1340,6 +1335,20 @@ void prover_set_shuffle(Prover* P, const uint8_t* h_qin, const uint8_t* h_qout) 
     }
   PB_CHECK(ones[0] == ones[1], ("a shuffle needs as many q_in rows as q_out rows: " + std::to_string(ones[0]) +
                                 " and " + std::to_string(ones[1])).c_str());
+}
+
+// Every check comes before any change, so a refused call leaves the prover as it was.
+void prover_set_shuffle(Prover* P, const uint8_t* h_qin, const uint8_t* h_qout) {
+  Context* ctx = P->ctx;
+  const uint64_t n = P->n;
+  PB_CHECK(P->world == 1, "shuffles are not available on the sharded prover (one GPU only)");
+  PB_CHECK(!P->sliced, PB_SLICED_WHY "the shuffle quotient needs the whole coset in round 3");
+  PB_CHECK(!P->lk, "shuffles do not combine with lookups");
+  PB_CHECK(!P->zk, "shuffles do not combine with zero-knowledge mode switched on first: set the shuffle, then "
+                   "pb200_prover_set_zk_shuffle");
+  PB_CHECK(!P->sh, "the shuffle selectors are already set (set them once, before the first proof)");
+  shuffle_require(n, h_qin, h_qout);
+  const uint8_t* sel[2] = {h_qin, h_qout};
   cudaStream_t st = ctx->stream;
   for (int s = 0; s < 2; s++) {  // as q_K: Lagrange values (round 2), coefficients (rounds 4, 5), the 4n coset (round 3)
     upload_mont(ctx, P->sh_lag[s], sel[s], n);

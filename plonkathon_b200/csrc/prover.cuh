@@ -25,12 +25,8 @@ __device__ __forceinline__ Fr custom_gate_sum(const CustomTerms& t, uint64_t i, 
 #pragma unroll
   for (int k = 0; k < PB_MAX_CUSTOM; k++) {
     if (k >= t.count) break;
-    const uint4* q = reinterpret_cast<const uint4*>(t.Q[k] + i);
-    uint4 lo = __ldg(q), hi = __ldg(q + 1);
-    Fr s;
-    s.v[0] = lo.x; s.v[1] = lo.y; s.v[2] = lo.z; s.v[3] = lo.w;
-    s.v[4] = hi.x; s.v[5] = hi.y; s.v[6] = hi.z; s.v[7] = hi.w;
-    acc = fp_add(acc, fp_mul(custom_monomial(a, b, c, t.f[k]), s));
+    const Fr q = ldg_fr(t.Q[k] + i);
+    acc = fp_add(acc, fp_mul(custom_monomial(a, b, c, t.f[k]), q));
   }
   return acc;
 }
@@ -40,12 +36,8 @@ __device__ __forceinline__ Fr custom_gate_sum_next(const CustomTerms& t, uint64_
 #pragma unroll
   for (int k = 0; k < PB_MAX_CUSTOM; k++) {
     if (k >= t.count) break;
-    const uint4* q = reinterpret_cast<const uint4*>(t.Q[k] + i);
-    uint4 lo = __ldg(q), hi = __ldg(q + 1);
-    Fr s;
-    s.v[0] = lo.x; s.v[1] = lo.y; s.v[2] = lo.z; s.v[3] = lo.w;
-    s.v[4] = hi.x; s.v[5] = hi.y; s.v[6] = hi.z; s.v[7] = hi.w;
-    acc = fp_add(acc, fp_mul(custom_monomial_next(a, b, c, an, bn, cn, t.f[k]), s));
+    const Fr q = ldg_fr(t.Q[k] + i);
+    acc = fp_add(acc, fp_mul(custom_monomial_next(a, b, c, an, bn, cn, t.f[k]), q));
   }
   return acc;
 }

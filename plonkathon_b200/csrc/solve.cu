@@ -10,7 +10,7 @@
 //                  order  an L or R cell of a defining row whose variable that row or a later one defines.
 //                Each kind is an exact count and its lowest `limit` cells (cub::DeviceSelect::Flagged, as check.cu).
 //   3. divisor:  1 / QO of every row by one batched inversion (k_batch_div); the body negates it.
-//   4. evaluate: k_solve_eval, persistent: each warp takes the next 32 defining rows in row order through one global
+//   4. evaluate: k_solve_eval<false>, persistent: each warp takes the next 32 defining rows in row order through one global
 //                ticket; a lane computes its row once the ready flags of its L and R variables are set (acquire), then
 //                stores c and sets its O variable's flag (release).  A lane whose operand a lower lane of its warp
 //                defines sees it on a later pass of the warp's loop.  Every wait is bounded: a warp that makes no
@@ -19,12 +19,12 @@
 // Device memory: about 430 bytes a row plus the outputs (DESIGN.md section 2), all freed before the call returns.
 //
 // With a table (pb200_solve_wires_lookup) a row with q_K != 0 and QO = 0 may also define its O variable, as t3 of the
-// table row matching its (tag, a, b).  k_solve_qualify_lookup flags it 2 beside the gate rows' 1, so both kinds go
-// through steps 2 and 4 as one ascending list.  Before step 4 the table index is built (solve_table_index: words of
-// the keys sorted, checked on full values, one entry per distinct key); k_solve_eval_lookup probes it (solve.cuh,
-// solve_probe) and flags miss and ambiguous rows, which still store 0 and release their flag.
+// table row matching its (tag, a, b).  k_solve_qualify flags it 2 beside the gate rows' 1, so both kinds go through
+// steps 2 and 4 as one ascending list.  Before step 4 the table index is built (solve_table_index: words of the keys
+// sorted, checked on full values, one entry per distinct key); k_solve_eval<true> probes it (solve.cuh, solve_probe)
+// and flags miss and ambiguous rows, which still store 0 and release their flag.
 //
-// With a shuffle (pb200_solve_wires_shuffle) out-rows define nothing by the gate rule (k_solve_unqualify_out); their
+// With a shuffle (pb200_solve_wires_shuffle) out-rows define nothing by the gate rule (k_solve_qualify); their
 // variables are defined at the first out-row p (k_solve_claim_out), late and clash cells are flagged in step 2, and
 // step 4 runs in two phases, the defining rows below p and the rest, with the sorted in-row tuples written into the
 // out-rows between them (solve_shuffle).  DESIGN.md section 3 has the rule and the no-deadlock argument per phase.
@@ -48,23 +48,19 @@ __global__ void k_batch_div(const Fr* num, const Fr* den, Fr* out, uint64_t n, u
 __global__ void k_count_noncanonical(const Fr* v, uint64_t n, uint32_t* bad);
 // check.cu
 Fr check_random_fr();
+uint64_t compact_flagged(Context* ctx, const uint8_t* flags, uint64_t m, DevBuf& temp, uint32_t* d_idx,
+                         uint32_t* d_num, uint32_t limit, uint32_t* h_out);
+// prover.cu
+void lookup_require(uint64_t n, const uint8_t* h_qk, const uint8_t* h_qtag, const uint8_t* const* h_tab,
+                    uint64_t rows);
+void shuffle_require(uint64_t n, const uint8_t* h_qin, const uint8_t* h_qout);
 // permutation.cu
 void perm_require_ids(const int64_t* h_ids, uint64_t m, int64_t* max_id);
 uint64_t* perm_sort_keys(Context* ctx, const int64_t* h_ids, uint64_t m, int cb, int end_bit, DevBuf& keys, DevBuf& alt,
                          DevBuf& temp, size_t temp_bytes, uint64_t m_ids);
 
-#define PB_SOLVE_GRID(n, t) (unsigned)(((n) + (t)-1) / (t)), (t)
 #define PB_SOLVE_BATCH_CH 16              // k_batch_div's chain length (PB_BATCH_CH)
 #define PB_SOLVE_STALL_NS 10000000000ull  // 10 s without progress of a warp: the evaluation has stalled
-
-__device__ __forceinline__ Fr sv_ld(const Fr* p) {
-  const uint4* q = reinterpret_cast<const uint4*>(p);
-  uint4 a = __ldg(q), b = __ldg(q + 1);
-  Fr r;
-  r.v[0] = a.x; r.v[1] = a.y; r.v[2] = a.z; r.v[3] = a.w;
-  r.v[4] = b.x; r.v[5] = b.y; r.v[6] = b.z; r.v[7] = b.w;
-  return r;
-}
 
 struct SolveSel {
   const Fr *ql, *qr, *qm, *qo, *qc, *inv_qo;  // Montgomery, n each
@@ -73,29 +69,25 @@ struct SolveSel {
   int n_custom;
 };
 
-// one flag per row: r < n_rows, QO != 0 and no term whose selector is non-zero at r reads c or the next row
-__global__ void k_solve_qualify(SolveSel s, uint64_t n_rows, uint8_t* qual) {
-  const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= n_rows) return;
-  bool ok = !sv_ld(s.qo + r).is_zero();
-#pragma unroll
-  for (int k = 0; k < PB_MAX_CUSTOM; k++)
-    if (k < s.n_custom && solve_term_reads_c(s.f[k]) && !sv_ld(s.q[k] + r).is_zero()) ok = false;
-  qual[r] = ok ? 1 : 0;
-}
+// side[r] of a shuffle: PB_SOLVE_IN for an in-row (q_in = 1, q_out = 0), PB_SOLVE_OUT for an out-row (q_out = 1,
+// q_in = 0), else 0
+#define PB_SOLVE_IN 1
+#define PB_SOLVE_OUT 2
 
-// with a table: 1 where a row defines by the gate rule (as k_solve_qualify), else 2 where it defines from its table:
-// q_K != 0 and QO = 0 (qk canonical)
+// one flag per row r < n_rows: 1 where it defines its O variable by the gate rule (QO != 0 and no term whose selector
+// is non-zero at r reads c or the next row), else PB_SOLVE_BY_TABLE where it defines from its table (qk not null:
+// q_K != 0 and QO = 0, qk canonical), else 0.  Out-rows of a shuffle (side not null) define nothing: 0.
 #define PB_SOLVE_BY_TABLE 2
-__global__ void k_solve_qualify_lookup(SolveSel s, const Fr* qk, uint64_t n_rows, uint8_t* qual) {
+__global__ void k_solve_qualify(SolveSel s, const Fr* qk, const uint8_t* side, uint64_t n_rows, uint8_t* qual) {
   const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n_rows) return;
-  const bool qo = !sv_ld(s.qo + r).is_zero();
+  const bool qo = !ldg_fr(s.qo + r).is_zero();
   bool ok = qo;
 #pragma unroll
   for (int k = 0; k < PB_MAX_CUSTOM; k++)
-    if (k < s.n_custom && solve_term_reads_c(s.f[k]) && !sv_ld(s.q[k] + r).is_zero()) ok = false;
-  qual[r] = ok ? 1 : (!qo && !sv_ld(qk + r).is_zero()) ? PB_SOLVE_BY_TABLE : 0;
+    if (k < s.n_custom && solve_term_reads_c(s.f[k]) && !ldg_fr(s.q[k] + r).is_zero()) ok = false;
+  const bool table = qk && !qo && !ldg_fr(qk + r).is_zero();
+  qual[r] = (side && side[r] == PB_SOLVE_OUT) ? 0 : ok ? 1 : table ? PB_SOLVE_BY_TABLE : 0;
 }
 
 // ---- the table index (solve.cuh, SolveTable) -----------------------------------------------------------------------
@@ -103,8 +95,8 @@ __global__ void k_solve_qualify_lookup(SolveSel s, const Fr* qk, uint64_t n_rows
 __global__ void k_solve_tab_keys(SolveTable T, uint64_t rows, uint64_t* keys, uint32_t* idx) {
   const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= rows) return;
-  const Fr tag = T.t[3] ? sv_ld(T.t[3] + k) : Fr::zero();
-  keys[k] = solve_table_word(tag, sv_ld(T.t[0] + k), sv_ld(T.t[1] + k), T.theta, T.theta2);
+  const Fr tag = T.t[3] ? ldg_fr(T.t[3] + k) : Fr::zero();
+  keys[k] = solve_table_word(tag, ldg_fr(T.t[0] + k), ldg_fr(T.t[1] + k), T.theta, T.theta2);
   idx[k] = (uint32_t)k;
 }
 // sorted position k: head[k] = 1 where a run of equal words starts; *impure counts neighbours with equal words and
@@ -118,10 +110,10 @@ __global__ void k_solve_tab_heads(SolveTable T, const uint64_t* keys, const uint
   bool differs = false;
   if (!start) {
     const uint32_t r = idx[k], p = idx[k - 1];
-    if (sv_ld(T.t[0] + r) != sv_ld(T.t[0] + p) || sv_ld(T.t[1] + r) != sv_ld(T.t[1] + p) ||
-        (T.t[3] && sv_ld(T.t[3] + r) != sv_ld(T.t[3] + p)))
+    if (ldg_fr(T.t[0] + r) != ldg_fr(T.t[0] + p) || ldg_fr(T.t[1] + r) != ldg_fr(T.t[1] + p) ||
+        (T.t[3] && ldg_fr(T.t[3] + r) != ldg_fr(T.t[3] + p)))
       atomicAdd(impure, 1u);
-    differs = sv_ld(T.t[2] + r) != sv_ld(T.t[2] + p);
+    differs = ldg_fr(T.t[2] + r) != ldg_fr(T.t[2] + p);
   }
   split[k] = differs ? 1 : 0;
 }
@@ -192,7 +184,7 @@ __global__ void k_solve_init(const uint32_t* inp, const Fr* in_vals, uint64_t n_
   if (v >= n_vars) return;
   const uint32_t s = inp[v];
   if (s == PB_SOLVE_ZERO) val[v] = Fr::zero();
-  else if (s != PB_SOLVE_NONE) val[v] = fp_to_mont(sv_ld(in_vals + s));
+  else if (s != PB_SOLVE_NONE) val[v] = fp_to_mont(ldg_fr(in_vals + s));
   ready[v] = s != PB_SOLVE_NONE ? 1 : 0;
 }
 
@@ -212,67 +204,13 @@ struct SolveLk {
 };
 
 // the defining rows rows[0, n_def), ascending, in dependency order (see the file comment).  status[0]: the ticket,
-// status[1]: set when a warp stalled.
+// status[1]: set when a warp stalled.  kTable: a row flagged PB_SOLVE_BY_TABLE probes the index (solve.cuh,
+// solve_probe) instead of running the gate body; a miss or an ambiguous key sets the row's flag and still stores c = 0
+// and the ready flag, so the rows that depend on it finish.  lk is read only then.
+template <bool kTable>
 __global__ void __launch_bounds__(128) k_solve_eval(SolveSel s, const uint32_t* rows, uint64_t n_def,
                                                     const uint32_t* var_of_cell, Fr* val, uint32_t* ready,
-                                                    uint32_t* status) {
-  const uint32_t lane = threadIdx.x & 31;
-  cuda::atomic_ref<uint32_t, cuda::thread_scope_device> stalled(status[1]);
-  for (;;) {
-    uint32_t t = 0;
-    if (lane == 0) t = atomicAdd(status, 1u);
-    t = __shfl_sync(0xffffffffu, t, 0);
-    const uint64_t i = (uint64_t)t * 32 + lane;
-    if ((uint64_t)t * 32 >= n_def) return;
-    bool done = i >= n_def;
-    uint32_t vl = 0, vr = 0, vo = 0;
-    SolveRow sr;
-    if (!done) {
-      const uint64_t r = rows[i];
-      vl = var_of_cell[3 * r];
-      vr = var_of_cell[3 * r + 1];
-      vo = var_of_cell[3 * r + 2];
-      sr.ql = sv_ld(s.ql + r);
-      sr.qr = sv_ld(s.qr + r);
-      sr.qm = sv_ld(s.qm + r);
-      sr.qc = sv_ld(s.qc + r);
-      sr.neg_inv_qo = fp_neg(sv_ld(s.inv_qo + r));
-#pragma unroll
-      for (int k = 0; k < PB_MAX_CUSTOM; k++) sr.q[k] = k < s.n_custom ? sv_ld(s.q[k] + r) : Fr::zero();
-    }
-    uint64_t since = sv_now();
-    while (!__all_sync(0xffffffffu, done)) {
-      bool moved = false;
-      if (!done) {
-        cuda::atomic_ref<uint32_t, cuda::thread_scope_device> rl(ready[vl]), rr(ready[vr]);
-        if (rl.load(cuda::memory_order_acquire) && rr.load(cuda::memory_order_acquire)) {
-          const Fr a = val[vl], b = val[vr];
-          val[vo] = solve_gate(sr, s.f, s.n_custom, a, b);
-          cuda::atomic_ref<uint32_t, cuda::thread_scope_device>(ready[vo]).store(1, cuda::memory_order_release);
-          done = moved = true;
-        }
-      }
-      if (__any_sync(0xffffffffu, moved)) {
-        since = sv_now();
-        continue;
-      }
-      // leave together: the decisions are the warp's, so no lane is left in a later __all_sync alone
-      if (__any_sync(0xffffffffu, lane == 0 && stalled.load(cuda::memory_order_relaxed))) return;
-      if (__any_sync(0xffffffffu, lane == 0 && sv_now() - since > PB_SOLVE_STALL_NS)) {
-        if (lane == 0) stalled.store(1, cuda::memory_order_relaxed);
-        return;
-      }
-      __nanosleep(64);
-    }
-  }
-}
-
-// k_solve_eval with rows that define from their table: a row flagged PB_SOLVE_BY_TABLE probes the index (solve_probe)
-// instead of running the gate body.  A miss or an ambiguous key sets the row's flag and still stores c = 0 and the
-// ready flag, so the rows that depend on it finish.  (A kernel of its own, so that k_solve_eval stays as it was.)
-__global__ void __launch_bounds__(128) k_solve_eval_lookup(SolveSel s, SolveLk lk, const uint32_t* rows,
-                                                           uint64_t n_def, const uint32_t* var_of_cell, Fr* val,
-                                                           uint32_t* ready, uint32_t* status) {
+                                                    uint32_t* status, SolveLk lk) {
   const uint32_t lane = threadIdx.x & 31;
   cuda::atomic_ref<uint32_t, cuda::thread_scope_device> stalled(status[1]);
   for (;;) {
@@ -292,18 +230,19 @@ __global__ void __launch_bounds__(128) k_solve_eval_lookup(SolveSel s, SolveLk l
       vl = var_of_cell[3 * r];
       vr = var_of_cell[3 * r + 1];
       vo = var_of_cell[3 * r + 2];
-      row = r;
-      table = lk.qual[r] == PB_SOLVE_BY_TABLE;
-      if (table) {
-        tag = lk.qt ? sv_ld(lk.qt + r) : Fr::zero();
-      } else {
-        sr.ql = sv_ld(s.ql + r);
-        sr.qr = sv_ld(s.qr + r);
-        sr.qm = sv_ld(s.qm + r);
-        sr.qc = sv_ld(s.qc + r);
-        sr.neg_inv_qo = fp_neg(sv_ld(s.inv_qo + r));
+      if constexpr (kTable) {
+        row = r;
+        table = lk.qual[r] == PB_SOLVE_BY_TABLE;
+        if (table) tag = lk.qt ? ldg_fr(lk.qt + r) : Fr::zero();
+      }
+      if (!table) {
+        sr.ql = ldg_fr(s.ql + r);
+        sr.qr = ldg_fr(s.qr + r);
+        sr.qm = ldg_fr(s.qm + r);
+        sr.qc = ldg_fr(s.qc + r);
+        sr.neg_inv_qo = fp_neg(ldg_fr(s.inv_qo + r));
 #pragma unroll
-        for (int k = 0; k < PB_MAX_CUSTOM; k++) sr.q[k] = k < s.n_custom ? sv_ld(s.q[k] + r) : Fr::zero();
+        for (int k = 0; k < PB_MAX_CUSTOM; k++) sr.q[k] = k < s.n_custom ? ldg_fr(s.q[k] + r) : Fr::zero();
       }
     }
     uint64_t since = sv_now();
@@ -342,16 +281,7 @@ __global__ void __launch_bounds__(128) k_solve_eval_lookup(SolveSel s, SolveLk l
 }
 
 // ---- the shuffle (pb200_solve_wires_shuffle) ---------------------------------------------------------------------------
-// side[r]: PB_SOLVE_IN for an in-row (q_in = 1, q_out = 0), PB_SOLVE_OUT for an out-row (q_out = 1, q_in = 0), else 0.
-// p: the first out-row.
-#define PB_SOLVE_IN 1
-#define PB_SOLVE_OUT 2
-
-// out-rows define nothing by the gate rule: their qualify flags cleared (after k_solve_qualify)
-__global__ void k_solve_unqualify_out(const uint8_t* side, uint64_t n_rows, uint8_t* qual) {
-  const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r < n_rows && side[r] == PB_SOLVE_OUT) qual[r] = 0;
-}
+// side[r] as k_solve_qualify reads it; p: the first out-row.
 
 // per out-row cell (after k_solve_vars): count the out-row cells of its variable, and let the shuffle define it at row p
 // unless it is the constant 0 or an input.  A row below p that defines it keeps it (a clash); a row above p does not.
@@ -500,30 +430,6 @@ __global__ void k_solve_order_rows(const uint32_t* cells, uint32_t count, const 
   if (k < count) out[k] = def_row[var_of_cell[cells[k]]];
 }
 
-// flags[0, m) -> *count and the lowest min(count, limit) flagged indices at h_out
-static uint64_t solve_compact(Context* ctx, const uint8_t* flags, uint64_t m, DevBuf& temp, uint32_t* d_idx,
-                              uint32_t* d_num, uint32_t limit, uint32_t* h_out) {
-  cudaStream_t st = ctx->stream;
-  size_t tb = temp.bytes;
-  PB_CUDA(cub::DeviceSelect::Flagged(temp.p, tb, thrust::counting_iterator<uint32_t>(0), flags, d_idx, d_num, (int)m,
-                                     st));
-  ctx->launches++;
-  uint32_t num = 0;
-  PB_CUDA(cudaMemcpyAsync(&num, d_num, 4, cudaMemcpyDeviceToHost, st));
-  PB_CUDA(cudaStreamSynchronize(st));
-  const uint32_t take = num < limit ? num : limit;
-  if (take && h_out) {
-    PB_CUDA(cudaMemcpyAsync(h_out, d_idx, (size_t)take * 4, cudaMemcpyDeviceToHost, st));
-    PB_CUDA(cudaStreamSynchronize(st));
-  }
-  return num;
-}
-
-static void solve_launched(Context* ctx) {
-  ctx->launches++;
-  PB_CUDA(cudaGetLastError());
-}
-
 // the table index of T's columns (rows table rows) into T.word / T.row / T.amb; sets T.theta, T.theta2 and T.n_keys.
 // The (word, row) pairs are sorted; neighbours with equal words must have equal keys, else theta is drawn again.  The
 // runs of equal words are then the distinct keys, in ascending word order.  temp: at least SortPairs' storage over rows
@@ -537,17 +443,17 @@ static void solve_table_index(Context* ctx, SolveTable& T, uint64_t rows, DevBuf
     PB_CHECK(draw < 8, "solving the wires: eight table words in a row had colliding keys");
     T.theta = check_random_fr();
     T.theta2 = fp_sqr(T.theta);
-    k_solve_tab_keys<<<PB_SOLVE_GRID(rows, 128), 0, st>>>(T, rows, k1.as<uint64_t>(), r1.as<uint32_t>());
-    solve_launched(ctx);
+    k_solve_tab_keys<<<PB_GRID(rows, 128), 0, st>>>(T, rows, k1.as<uint64_t>(), r1.as<uint32_t>());
+    launched(ctx);
     keys = cub::DoubleBuffer<uint64_t>(k1.as<uint64_t>(), k2.as<uint64_t>());
     idx = cub::DoubleBuffer<uint32_t>(r1.as<uint32_t>(), r2.as<uint32_t>());
     size_t tb = temp.bytes;
     PB_CUDA(cub::DeviceRadixSort::SortPairs(temp.p, tb, keys, idx, (int)rows, 0, 64, st));
     ctx->launches++;
     PB_CUDA(cudaMemsetAsync(impure, 0, 4, st));
-    k_solve_tab_heads<<<PB_SOLVE_GRID(rows, 256), 0, st>>>(T, keys.Current(), idx.Current(), rows, head.as<uint32_t>(),
+    k_solve_tab_heads<<<PB_GRID(rows, 256), 0, st>>>(T, keys.Current(), idx.Current(), rows, head.as<uint32_t>(),
                                                            split.as<uint8_t>(), impure);
-    solve_launched(ctx);
+    launched(ctx);
     uint32_t imp = 0;
     PB_CUDA(cudaMemcpyAsync(&imp, impure, 4, cudaMemcpyDeviceToHost, st));
     PB_CUDA(cudaStreamSynchronize(st));
@@ -557,11 +463,11 @@ static void solve_table_index(Context* ctx, SolveTable& T, uint64_t rows, DevBuf
   PB_CUDA(cub::DeviceScan::InclusiveSum(temp.p, tb, head.as<uint32_t>(), run.as<uint32_t>(), (int)rows, st));
   ctx->launches++;
   PB_CUDA(cudaMemsetAsync(const_cast<uint8_t*>(T.amb), 0, rows, st));
-  k_solve_tab_unique<<<PB_SOLVE_GRID(rows, 256), 0, st>>>(keys.Current(), idx.Current(), head.as<uint32_t>(),
+  k_solve_tab_unique<<<PB_GRID(rows, 256), 0, st>>>(keys.Current(), idx.Current(), head.as<uint32_t>(),
                                                           run.as<uint32_t>(), split.as<uint8_t>(), rows,
                                                           const_cast<uint64_t*>(T.word), const_cast<uint32_t*>(T.row),
                                                           const_cast<uint8_t*>(T.amb));
-  solve_launched(ctx);
+  launched(ctx);
   uint32_t keys_n = 0;
   PB_CUDA(cudaMemcpyAsync(&keys_n, run.as<uint32_t>() + rows - 1, 4, cudaMemcpyDeviceToHost, st));
   PB_CUDA(cudaStreamSynchronize(st));  // the index's temporaries die here
@@ -579,14 +485,14 @@ static void solve_shuffle(Context* ctx, const uint32_t* in_rows, const uint32_t*
                           unsigned long long* acc) {
   cudaStream_t st = ctx->stream;
   DevBuf words(K * 96), k1(K * 8), k2(K * 8), p1(K * 4), p2(K * 4);
-  k_solve_shuffle_gather<<<PB_SOLVE_GRID(K, 128), 0, st>>>(in_rows, K, var_of_cell, val, words.as<uint64_t>(),
+  k_solve_shuffle_gather<<<PB_GRID(K, 128), 0, st>>>(in_rows, K, var_of_cell, val, words.as<uint64_t>(),
                                                            p1.as<uint32_t>());
-  solve_launched(ctx);
+  launched(ctx);
   PB_CUDA(cudaMemsetAsync(acc, 0, 12 * 8, st));
   PB_CUDA(cudaMemsetAsync(acc + 12, 0xff, 12 * 8, st));
   const uint64_t blocks = std::min<uint64_t>((K + 255) / 256, 4 * (uint64_t)ctx->sm_count);
   k_solve_shuffle_bits<<<(unsigned)blocks, 256, 0, st>>>(words.as<uint64_t>(), K, acc);
-  solve_launched(ctx);
+  launched(ctx);
   unsigned long long bits[24];
   PB_CUDA(cudaMemcpyAsync(bits, acc, sizeof bits, cudaMemcpyDeviceToHost, st));
   PB_CUDA(cudaStreamSynchronize(st));
@@ -597,17 +503,17 @@ static void solve_shuffle(Context* ctx, const uint32_t* in_rows, const uint32_t*
       const int w = 4 * t + l;
       const unsigned long long diff = bits[w] ^ bits[12 + w];
       if (!diff) continue;
-      k_solve_shuffle_key<<<PB_SOLVE_GRID(K, 256), 0, st>>>(words.as<uint64_t>() + (uint64_t)w * K, pos.Current(), K,
+      k_solve_shuffle_key<<<PB_GRID(K, 256), 0, st>>>(words.as<uint64_t>() + (uint64_t)w * K, pos.Current(), K,
                                                             keys.Current());
-      solve_launched(ctx);
+      launched(ctx);
       size_t tb = temp.bytes;
       PB_CUDA(cub::DeviceRadixSort::SortPairs(temp.p, tb, keys, pos, (int)K, __builtin_ctzll(diff),
                                               64 - __builtin_clzll(diff), st));
       ctx->launches++;
     }
-  k_solve_shuffle_put<<<PB_SOLVE_GRID(3 * K, 256), 0, st>>>(in_rows, out_rows, pos.Current(), K, var_of_cell, val,
+  k_solve_shuffle_put<<<PB_GRID(3 * K, 256), 0, st>>>(in_rows, out_rows, pos.Current(), K, var_of_cell, val,
                                                             ready);
-  solve_launched(ctx);
+  launched(ctx);
   PB_CUDA(cudaStreamSynchronize(st));  // the sort's buffers die here
 }
 
@@ -618,414 +524,379 @@ void solve_stages(double* out_ms, int count) {
   for (int k = 0; k < count && k < 3; k++) out_ms[k] = g_solve_ms[k];
 }
 
-// q_in and q_out as pb200_prover_set_shuffle takes them, with its refusals (prover.cu, prover_set_shuffle) -> side[r]
-// (PB_SOLVE_IN, PB_SOLVE_OUT or 0)
-static std::vector<uint8_t> solve_require_shuffle(uint64_t n, const uint8_t* h_qin, const uint8_t* h_qout) {
-  PB_CHECK(h_qin && h_qout, "a shuffle needs q_in and q_out");
-  uint64_t ones[2] = {0, 0};
-  const uint8_t* sel[2] = {h_qin, h_qout};
-  for (int s = 0; s < 2; s++)
-    for (uint64_t i = 0; i < n; i++) {
-      const uint8_t* e = sel[s] + 32 * i;
-      bool ok = e[0] <= 1;
-      for (int k = 1; k < 32 && ok; k++) ok = e[k] == 0;
-      PB_CHECK(ok, s ? "q_out must be 0 or 1 on every row" : "q_in must be 0 or 1 on every row");
-      ones[s] += e[0];
-    }
-  PB_CHECK(ones[0] == ones[1], ("a shuffle needs as many q_in rows as q_out rows: " + std::to_string(ones[0]) +
-                                " and " + std::to_string(ones[1])).c_str());
-  std::vector<uint8_t> side(n);
-  for (uint64_t i = 0; i < n; i++)
-    side[i] = h_qin[32 * i] == h_qout[32 * i] ? 0 : h_qin[32 * i] ? PB_SOLVE_IN : PB_SOLVE_OUT;
-  return side;
-}
-
-// q_K, Q_T and the table as pb200_prover_set_lookup(_tagged) takes them, with its refusals (prover.cu,
-// prover_set_lookup)
-static void solve_require_lookup(uint64_t n, const uint8_t* h_qk, const uint8_t* h_qtag, const uint8_t* const* h_tab,
-                                 uint64_t rows) {
-  const bool tagged = h_qtag != nullptr;
-  PB_CHECK(h_qk && h_tab[0] && h_tab[1] && h_tab[2], "lookups need q_K and three table columns");
-  PB_CHECK(!tagged || h_tab[3], "tagged lookups need the table tag column t4");
-  PB_CHECK(rows >= 1, "the lookup table is empty");
-  PB_CHECK(rows <= n, "the lookup table has more rows than the circuit");
-  for (uint64_t i = 0; i < n; i++) {
-    const uint8_t* e = h_qk + 32 * i;
-    bool ok = e[0] <= 1;
-    for (int k = 1; k < 32 && ok; k++) ok = e[k] == 0;
-    PB_CHECK(ok, "q_K must be 0 or 1 on every row");
-    if (!tagged) continue;
-    Fr x;
-    memcpy(x.v, h_qtag + 32 * i, 32);
-    PB_CHECK(fp_is_canonical(x), ("Q_T on row " + std::to_string(i) + " not reduced below the field modulus").c_str());
-    PB_CHECK(e[0] == 1 || x.is_zero(), ("Q_T must be 0 where q_K = 0: row " + std::to_string(i)).c_str());
-  }
-  for (int w = 0; w < (tagged ? 4 : 3); w++)
-    for (uint64_t r = 0; r < rows; r++) {
-      Fr x;
-      memcpy(x.v, h_tab[w] + 32 * r, 32);
-      PB_CHECK(fp_is_canonical(x), "lookup table value not reduced below the field modulus");
-    }
-}
-
-// see plonk_b200.h (pb200_solve_wires; pb200_solve_wires_lookup when h_tab is not null: then h_counts has four
-// entries and h_lists 5 limit; pb200_solve_wires_shuffle when `shuffle`: then h_counts has four entries and h_lists
-// 8 limit)
-void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constraints, const uint8_t* const* h_sel,
-               int n_custom, const uint8_t* h_exps, const uint8_t* const* h_custom, uint64_t n_inputs,
-               const int64_t* h_in_ids, const uint8_t* h_in_vals, uint32_t limit, uint64_t* h_counts,
-               uint32_t* h_lists, void* const* out, bool out_on_device, const uint8_t* h_qk, const uint8_t* h_qtag,
-               const uint8_t* const* h_tab, uint64_t tab_rows, uint8_t* h_operands, bool shuffle,
-               const uint8_t* h_qin, const uint8_t* h_qout) {
-  PB_CHECK(log_n >= 1 && log_n <= 26, "group order must be 2^k, 1 <= k <= 26 (the prover's range)");
-  const uint64_t n = (uint64_t)1 << log_n, m = 3 * n;
-  const bool lookup = h_tab != nullptr;
-  const bool tagged = lookup && h_qtag != nullptr;
-  PB_CHECK(n_constraints <= n, "n_constraints above the group order");
-  PB_CHECK(h_ids && h_sel && h_counts && (h_lists || limit == 0) && out && (h_in_ids || n_inputs == 0) &&
-               (h_in_vals || n_inputs == 0),
-           "solving the wires needs the ids, the selectors, the inputs and the outputs");
-  for (int k = 0; k < 5; k++) PB_CHECK(h_sel[k], "solving the wires needs QL, QR, QM, QO and QC");
-  for (int k = 0; k < 3; k++) PB_CHECK(out[k], "solving the wires needs three output buffers");
-  PB_CHECK(limit <= m, "limit above 3n, the most entries a list can have");
-  PB_CHECK(n_custom >= 0 && n_custom <= PB_MAX_CUSTOM, "at most 4 custom gate terms");
-  PB_CHECK(n_custom == 0 || (h_exps && h_custom), "custom gate terms need their exponents and selectors");
+namespace {
+// one call of solve_run: its arguments, what the host checks made of them, and the device buffers of the steps
+struct Solve {
+  Context* ctx;
+  cudaStream_t st;
+  const SolveArgs& a;
+  const SolveTableArgs* tb;    // null without a table
+  const SolveShuffleArgs* sf;  // null without a shuffle
+  uint64_t n = 0, m = 0;
   SolveSel s = {};
-  s.n_custom = n_custom;
-  for (int k = 0; k < n_custom; k++) {
-    const uint8_t* e = h_exps + 6 * k;
-    const int deg = e[0] + e[1] + e[2] + e[3] + e[4] + e[5];
-    PB_CHECK(deg >= 1 && deg <= 3, "custom gate term must have total degree 1, 2 or 3");
-    PB_CHECK(h_custom[k], "custom gate term without its selector");
-    int f = 0;
-    for (int w = 0; w < 6; w++)
-      for (int t = 0; t < e[w]; t++) s.f[k][f++] = (uint8_t)w;
-    while (f < 3) s.f[k][f++] = PB_FACTOR_ONE;
-  }
-  // ids (only rows below n_constraints are read), inputs and their values, before any device work
   int64_t max_id = -1;
-  perm_require_ids(h_ids, 3 * n_constraints, &max_id);
-  std::vector<uint64_t> order(n_inputs);
-  for (uint64_t k = 0; k < n_inputs; k++) {
-    const int64_t id = h_in_ids[k];
-    if (id < 0 || id > PB_PERM_MAX_ID) {
-      char b[256];
-      snprintf(b, sizeof b, "input %llu: variable id %lld is outside [0, 2^32 - 2]", (unsigned long long)k,
-               (long long)id);
-      throw Error(b);
-    }
-    Fr x;
-    memcpy(x.v, h_in_vals + 32 * k, 32);
-    if (!fp_is_canonical(x)) {
-      char b[256];
-      snprintf(b, sizeof b, "input %llu (variable %lld): value not reduced below the field modulus",
-               (unsigned long long)k, (long long)id);
-      throw Error(b);
-    }
-    order[k] = k;
-  }
-  std::sort(order.begin(), order.end(), [&](uint64_t a, uint64_t b) {
-    return h_in_ids[a] != h_in_ids[b] ? h_in_ids[a] < h_in_ids[b] : a < b;
-  });
-  std::vector<uint64_t> in_keys(n_inputs);
-  std::vector<uint8_t> in_vals(n_inputs * 32);
-  for (uint64_t k = 0; k < n_inputs; k++) {
-    if (k > 0 && h_in_ids[order[k]] == h_in_ids[order[k - 1]]) {
-      char b[256];
-      snprintf(b, sizeof b, "inputs %llu and %llu both name variable %lld", (unsigned long long)order[k - 1],
-               (unsigned long long)order[k], (long long)h_in_ids[order[k]]);
-      throw Error(b);
-    }
-    in_keys[k] = (uint64_t)(h_in_ids[order[k]] + 1);
-    memcpy(&in_vals[32 * k], h_in_vals + 32 * order[k], 32);
-  }
-  if (lookup) solve_require_lookup(n, h_qk, h_qtag, h_tab, tab_rows);
-  // the shuffle: the rows of each side, K in-rows (as many out-rows), the first out-row p.  Without out-rows (q_in and
-  // q_out all 0, or both 1 on the same rows) the solve is the one without a shuffle.
+  std::vector<uint64_t> in_keys;  // the inputs' ids + 1, ascending, and their values in that order
+  std::vector<uint8_t> in_vals;
+  // the shuffle: per row its side, K in-rows (as many out-rows), the first out-row p.  Without out-rows (q_in and q_out
+  // all 0, or both 1 on the same rows) the solve is the one without a shuffle.
   std::vector<uint8_t> side;
   uint64_t K = 0;
   uint32_t p = PB_SOLVE_NONE;
-  if (shuffle) {
-    side = solve_require_shuffle(n, h_qin, h_qout);
-    for (uint64_t i = 0; i < n; i++) {
-      K += side[i] == PB_SOLVE_IN;
-      if (side[i] == PB_SOLVE_OUT && p == PB_SOLVE_NONE) p = (uint32_t)i;
-    }
-  }
-  const bool sh = K > 0;
+  bool out_rows = false;
+  uint64_t temp_bytes = 0;
+  DevBuf temp, keys, alt, head, run, voc, inp, defr, ready, val, idx, flags, small, inids, invals, sel, qual, defines;
+  DevBuf qkb, qtb, tabb, errf, ix_word, ix_row, ix_amb;  // the table
+  DevBuf sideb, outc, shf;                                // the shuffle
+  SolveLk lk = {};
+  uint32_t *small_u = nullptr, *num = nullptr;
 
-  const int cb = perm_cell_bits(log_n);
-  const int end_bit = perm_sort_bits(log_n, max_id);
-  cudaStream_t st = ctx->stream;
-  size_t t_sort = 0, t_scan = 0, t_sel = 0, t_tab = 0, t_sh = 0;
-  {
+  Solve(Context* c, const SolveArgs& args, const SolveTableArgs* t, const SolveShuffleArgs* f)
+      : ctx(c), st(c->stream), a(args), tb(t), sf(f) {}
+
+  // the arguments, before any device work
+  void require() {
+    PB_CHECK(a.log_n >= 1 && a.log_n <= 26, "group order must be 2^k, 1 <= k <= 26 (the prover's range)");
+    n = (uint64_t)1 << a.log_n;
+    m = 3 * n;
+    PB_CHECK(a.n_constraints <= n, "n_constraints above the group order");
+    PB_CHECK(a.ids && a.sel && a.counts && (a.lists || a.limit == 0) && a.out && (a.in_ids || a.n_inputs == 0) &&
+                 (a.in_vals || a.n_inputs == 0),
+             "solving the wires needs the ids, the selectors, the inputs and the outputs");
+    for (int k = 0; k < 5; k++) PB_CHECK(a.sel[k], "solving the wires needs QL, QR, QM, QO and QC");
+    for (int k = 0; k < 3; k++) PB_CHECK(a.out[k], "solving the wires needs three output buffers");
+    PB_CHECK(a.limit <= m, "limit above 3n, the most entries a list can have");
+    PB_CHECK(a.n_custom >= 0 && a.n_custom <= PB_MAX_CUSTOM, "at most 4 custom gate terms");
+    PB_CHECK(a.n_custom == 0 || (a.exps && a.custom), "custom gate terms need their exponents and selectors");
+    s.n_custom = a.n_custom;
+    for (int k = 0; k < a.n_custom; k++) {
+      const uint8_t* e = a.exps + 6 * k;
+      const int deg = e[0] + e[1] + e[2] + e[3] + e[4] + e[5];
+      PB_CHECK(deg >= 1 && deg <= 3, "custom gate term must have total degree 1, 2 or 3");
+      PB_CHECK(a.custom[k], "custom gate term without its selector");
+      int f = 0;
+      for (int w = 0; w < 6; w++)
+        for (int t = 0; t < e[w]; t++) s.f[k][f++] = (uint8_t)w;
+      while (f < 3) s.f[k][f++] = PB_FACTOR_ONE;
+    }
+    // ids (only rows below n_constraints are read), inputs and their values
+    perm_require_ids(a.ids, 3 * a.n_constraints, &max_id);
+    std::vector<uint64_t> order(a.n_inputs);
+    for (uint64_t k = 0; k < a.n_inputs; k++) {
+      const int64_t id = a.in_ids[k];
+      if (id < 0 || id > PB_PERM_MAX_ID) {
+        char b[256];
+        snprintf(b, sizeof b, "input %llu: variable id %lld is outside [0, 2^32 - 2]", (unsigned long long)k,
+                 (long long)id);
+        throw Error(b);
+      }
+      Fr x;
+      memcpy(x.v, a.in_vals + 32 * k, 32);
+      if (!fp_is_canonical(x)) {
+        char b[256];
+        snprintf(b, sizeof b, "input %llu (variable %lld): value not reduced below the field modulus",
+                 (unsigned long long)k, (long long)id);
+        throw Error(b);
+      }
+      order[k] = k;
+    }
+    const int64_t* ids = a.in_ids;
+    std::sort(order.begin(), order.end(),
+              [ids](uint64_t x, uint64_t y) { return ids[x] != ids[y] ? ids[x] < ids[y] : x < y; });
+    in_keys.resize(a.n_inputs);
+    in_vals.resize(a.n_inputs * 32);
+    for (uint64_t k = 0; k < a.n_inputs; k++) {
+      if (k > 0 && a.in_ids[order[k]] == a.in_ids[order[k - 1]]) {
+        char b[256];
+        snprintf(b, sizeof b, "inputs %llu and %llu both name variable %lld", (unsigned long long)order[k - 1],
+                 (unsigned long long)order[k], (long long)a.in_ids[order[k]]);
+        throw Error(b);
+      }
+      in_keys[k] = (uint64_t)(a.in_ids[order[k]] + 1);
+      memcpy(&in_vals[32 * k], a.in_vals + 32 * order[k], 32);
+    }
+    if (tb) lookup_require(n, tb->qk, tb->qtag, tb->tab, tb->rows);
+    if (sf) {
+      shuffle_require(n, sf->qin, sf->qout);
+      side.resize(n);
+      for (uint64_t i = 0; i < n; i++) {
+        const uint8_t in = sf->qin[32 * i], out = sf->qout[32 * i];
+        side[i] = in == out ? 0 : in ? PB_SOLVE_IN : PB_SOLVE_OUT;
+        K += side[i] == PB_SOLVE_IN;
+        if (side[i] == PB_SOLVE_OUT && p == PB_SOLVE_NONE) p = (uint32_t)i;
+      }
+    }
+    out_rows = K > 0;
+  }
+
+  // the device memory the call needs, refused when more than is free; then the buffers
+  void reserve() {
+    const int end_bit = perm_sort_bits(a.log_n, max_id);
+    const uint64_t rows = tb ? tb->rows : 0;
+    size_t t_sort = 0, t_scan = 0, t_sel = 0, t_tab = 0, t_sh = 0;
     cub::DoubleBuffer<uint64_t> d(nullptr, nullptr);
+    cub::DoubleBuffer<uint32_t> v(nullptr, nullptr);
     PB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, t_sort, d, (int)m, 0, end_bit, st));
     PB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, t_scan, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)m, st));
     PB_CUDA(cub::DeviceSelect::Flagged(nullptr, t_sel, thrust::counting_iterator<uint32_t>(0), (const uint8_t*)nullptr,
                                        (uint32_t*)nullptr, (uint32_t*)nullptr, (int)m, st));
-    if (lookup) {
-      cub::DoubleBuffer<uint32_t> v(nullptr, nullptr);
-      PB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t_tab, d, v, (int)tab_rows, 0, 64, st));
+    if (tb) PB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t_tab, d, v, (int)rows, 0, 64, st));
+    if (out_rows) PB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t_sh, d, v, (int)K, 0, 64, st));
+    temp_bytes = std::max(std::max(std::max(t_sort, t_tab), std::max(t_scan, t_sel)), t_sh);
+    // keys and alt (8 each), heads / run (4 each), var_of_cell, inp, def_row, ready (4 each), the values (32), the
+    // index list (4), three flag bytes: per cell.  Selectors, 1 / QO and the custom selectors (32 each), the qualify
+    // and defines flags: per row.  The inputs, the host outputs' staging and the sort's storage.
+    const uint64_t limit = a.limit, n_custom = (uint64_t)a.n_custom;
+    uint64_t need = m * (8 + 8 + 4 + 4 + 4 * 4 + 32 + 4 + 3) + n * (32 * (6 + n_custom) + 2) + a.n_inputs * 40 +
+                    (a.out_on_device ? 0 : m * 32) + temp_bytes + 256;
+    // with a table: q_K and Q_T (32 each) and the miss and ambiguous flags (1 each) per row; per table row its columns
+    // (4 x 32), the sort's words and rows (2 x 8, 2 x 4), heads and runs (4 each), the split flag, the index
+    // (8 + 4 + 1); the listed rows' operands
+    if (tb) need += n * (32 + 32 + 2) + rows * (4 * 32 + 16 + 8 + 8 + 1 + 13) + limit * 2 * 64 + 256;
+    // with a shuffle: the side and the in / out flags (1 each) per row; the out-row cell count (4) and the late and
+    // clash flags (1 each) per cell; per in-row its tuple (96), the sort's words and positions (2 x 8, 2 x 4) and the
+    // in-row and out-row lists (4 each); the listed cells' entries
+    if (out_rows) need += n * 3 + m * (4 + 2) + K * (96 + 16 + 8 + 8) + limit * 5 * 4 + 256;
+    size_t free_b = 0, total_b = 0;
+    PB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    // PB200_SOLVE_MAX_BYTES: the most device memory a solve may take (read per call), so it leaves room for other work
+    if (const char* e = getenv("PB200_SOLVE_MAX_BYTES")) free_b = std::min<size_t>(free_b, strtoull(e, nullptr, 10));
+    if (need > free_b) {
+      char b[256];
+      snprintf(b, sizeof b, "solving the wires of 2^%d rows needs %llu bytes of device memory, %llu are free", a.log_n,
+               (unsigned long long)need, (unsigned long long)free_b);
+      throw Error(b);
     }
-    if (sh) {
-      cub::DoubleBuffer<uint32_t> v(nullptr, nullptr);
-      PB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t_sh, d, v, (int)K, 0, 64, st));
+    for (DevBuf* b : {&keys, &alt}) b->alloc(m * 8);
+    for (DevBuf* b : {&head, &run, &voc, &inp, &defr, &ready, &idx}) b->alloc(m * 4);
+    temp.alloc(temp_bytes);
+    val.alloc(m * 32);
+    flags.alloc(3 * m);
+    small.alloc(out_rows ? 32 + 24 * 8 : 64);
+    inids.alloc(a.n_inputs * 8 + 8);
+    invals.alloc(a.n_inputs * 32 + 32);
+    sel.alloc((6 + n_custom) * n * 32);
+    qual.alloc(n);
+    defines.alloc(n);
+    small_u = small.as<uint32_t>();
+    num = small_u + 1;
+    if (tb) {
+      qkb.alloc(n * 32);
+      if (tb->qtag) qtb.alloc(n * 32);
+      tabb.alloc((tb->qtag ? 4 : 3) * rows * 32);
+      errf.alloc(2 * n);
     }
-  }
-  const uint64_t temp_bytes = std::max(std::max(std::max(t_sort, t_tab), std::max(t_scan, t_sel)), t_sh);
-  // keys and alt (8 each), heads / run (4 each), var_of_cell, inp, def_row, ready (4 each), the values (32), the index
-  // list (4), three flag bytes: per cell.  Selectors, 1 / QO and the custom selectors (32 each), the qualify and
-  // defines flags: per row.  The inputs, the host outputs' staging and the sort's storage.
-  uint64_t need = m * (8 + 8 + 4 + 4 + 4 * 4 + 32 + 4 + 3) + n * (32 * (6 + (uint64_t)n_custom) + 2) +
-                  n_inputs * 40 + (out_on_device ? 0 : m * 32) + temp_bytes + 256;
-  // with a table: q_K and Q_T (32 each) and the miss and ambiguous flags (1 each) per row; per table row its columns
-  // (4 x 32), the sort's words and rows (2 x 8, 2 x 4), heads and runs (4 each), the split flag, the index (8 + 4 + 1);
-  // the listed rows' operands
-  if (lookup) need += n * (32 + 32 + 2) + tab_rows * (4 * 32 + 16 + 8 + 8 + 1 + 13) + (uint64_t)limit * 2 * 64 + 256;
-  // with a shuffle: the side and the in / out flags (1 each) per row; the out-row cell count (4) and the late and clash
-  // flags (1 each) per cell; per in-row its tuple (96), the sort's words and positions (2 x 8, 2 x 4) and the in-row and
-  // out-row lists (4 each); the listed cells' entries
-  if (sh) need += n * 3 + m * (4 + 2) + K * (96 + 16 + 8 + 8) + (uint64_t)limit * 5 * 4 + 256;
-  size_t free_b = 0, total_b = 0;
-  PB_CUDA(cudaMemGetInfo(&free_b, &total_b));
-  // PB200_SOLVE_MAX_BYTES: the most device memory a solve may take (read per call), so it leaves room for other work
-  if (const char* e = getenv("PB200_SOLVE_MAX_BYTES")) free_b = std::min<size_t>(free_b, strtoull(e, nullptr, 10));
-  if (need > free_b) {
-    char b[256];
-    snprintf(b, sizeof b, "solving the wires of 2^%d rows needs %llu bytes of device memory, %llu are free", log_n,
-             (unsigned long long)need, (unsigned long long)free_b);
-    throw Error(b);
+    if (out_rows) {
+      sideb.alloc(3 * n);
+      outc.alloc(m * 4);
+      shf.alloc(2 * m);
+    }
   }
 
-  DevBuf temp(temp_bytes), keys(m * 8), alt(m * 8), head(m * 4), run(m * 4), voc(m * 4), inp(m * 4), defr(m * 4),
-      ready(m * 4), val(m * 32), idx(m * 4), flags(3 * m), small(sh ? 32 + 24 * 8 : 64), inids(n_inputs * 8 + 8),
-      invals(n_inputs * 32 + 32),
-      sel((6 + (uint64_t)n_custom) * n * 32), qual(n), defines(n);
-  Fr* selp = sel.as<Fr>();
-  const Fr* sel_col[5];
-  for (int k = 0; k < 5 + n_custom; k++) {
-    Fr* col = selp + (uint64_t)k * n;
-    PB_CUDA(cudaMemcpyAsync(col, k < 5 ? h_sel[k] : h_custom[k - 5], n * 32, cudaMemcpyHostToDevice, st));
-    if (k < 5) sel_col[k] = col;
-    else s.q[k - 5] = col;
-  }
-  uint32_t* small_u = small.as<uint32_t>();
-  PB_CUDA(cudaMemsetAsync(small.p, 0, 64, st));
-  k_count_noncanonical<<<PB_SOLVE_GRID((5 + (uint64_t)n_custom) * n, 256), 0, st>>>(selp, (5 + (uint64_t)n_custom) * n,
-                                                                                   small_u + 2);
-  solve_launched(ctx);
-  fr_to_mont(ctx, selp, selp, (5 + (uint64_t)n_custom) * n);
-  s.ql = sel_col[0];
-  s.qr = sel_col[1];
-  s.qm = sel_col[2];
-  s.qo = sel_col[3];
-  s.qc = sel_col[4];
-  Fr* inv = selp + (5 + (uint64_t)n_custom) * n;
-  s.inv_qo = inv;
-  const uint64_t T = (n + PB_SOLVE_BATCH_CH - 1) / PB_SOLVE_BATCH_CH;
-  k_batch_div<<<PB_SOLVE_GRID(T, 128), 0, st>>>(nullptr, s.qo, inv, n, T);
-  solve_launched(ctx);
-  uint32_t bad_sel = 0;
-  PB_CUDA(cudaMemcpyAsync(&bad_sel, small_u + 2, 4, cudaMemcpyDeviceToHost, st));
-  PB_CUDA(cudaStreamSynchronize(st));
-  PB_CHECK(bad_sel == 0, "selector value not reduced below the field modulus");
-  if (n_inputs) {
-    PB_CUDA(cudaMemcpyAsync(inids.p, in_keys.data(), n_inputs * 8, cudaMemcpyHostToDevice, st));
-    PB_CUDA(cudaMemcpyAsync(invals.p, in_vals.data(), n_inputs * 32, cudaMemcpyHostToDevice, st));
-  }
-  // the table: q_K (canonical), Q_T and the table columns (Montgomery), the per-row error flags
-  const int width = tagged ? 4 : 3;
-  DevBuf qkb(lookup ? n * 32 : 0), qtb(tagged ? n * 32 : 0), tabb(lookup ? width * tab_rows * 32 : 0),
-      errf(lookup ? 2 * n : 0);
-  SolveLk lk = {};
-  if (lookup) {
-    PB_CUDA(cudaMemcpyAsync(qkb.p, h_qk, n * 32, cudaMemcpyHostToDevice, st));
-    if (tagged) {
-      PB_CUDA(cudaMemcpyAsync(qtb.p, h_qtag, n * 32, cudaMemcpyHostToDevice, st));
-      fr_to_mont(ctx, qtb.as<Fr>(), qtb.as<Fr>(), n);
+  // the selectors, the inputs, the table and the shuffle's sides on the device; 1. group; 2. sources
+  void sources() {
+    Fr* selp = sel.as<Fr>();
+    const uint64_t n_sel = (5 + (uint64_t)a.n_custom) * n;
+    const Fr* sel_col[5];
+    for (int k = 0; k < 5 + a.n_custom; k++) {
+      Fr* col = selp + (uint64_t)k * n;
+      PB_CUDA(cudaMemcpyAsync(col, k < 5 ? a.sel[k] : a.custom[k - 5], n * 32, cudaMemcpyHostToDevice, st));
+      if (k < 5) sel_col[k] = col;
+      else s.q[k - 5] = col;
     }
-    for (int w = 0; w < width; w++) {
-      lk.T.t[w] = tabb.as<Fr>() + (uint64_t)w * tab_rows;
-      PB_CUDA(cudaMemcpyAsync(tabb.as<Fr>() + (uint64_t)w * tab_rows, h_tab[w], tab_rows * 32, cudaMemcpyHostToDevice,
-                              st));
-    }
-    fr_to_mont(ctx, tabb.as<Fr>(), tabb.as<Fr>(), width * tab_rows);
-    PB_CUDA(cudaMemsetAsync(errf.p, 0, 2 * n, st));
-    lk.qual = qual.as<uint8_t>();
-    lk.qt = tagged ? qtb.as<Fr>() : nullptr;
-    lk.miss = errf.as<uint8_t>();
-    lk.amb = lk.miss + n;
-    h_counts[2] = h_counts[3] = 0;
-  }
-
-  // 1. group
-  const uint64_t* sorted = perm_sort_keys(ctx, h_ids, m, cb, end_bit, keys, alt, temp, temp_bytes, 3 * n_constraints);
-  k_solve_heads<<<PB_SOLVE_GRID(m, 256), 0, st>>>(sorted, m, cb, head.as<uint32_t>());
-  solve_launched(ctx);
-  size_t tb = temp.bytes;
-  PB_CUDA(cub::DeviceScan::InclusiveSum(temp.p, tb, head.as<uint32_t>(), run.as<uint32_t>(), (int)m, st));
-  ctx->launches++;
-  // 2. sources and errors
-  if (lookup) k_solve_qualify_lookup<<<PB_SOLVE_GRID(n, 256), 0, st>>>(s, qkb.as<Fr>(), n_constraints, qual.as<uint8_t>());
-  else k_solve_qualify<<<PB_SOLVE_GRID(n, 256), 0, st>>>(s, n_constraints, qual.as<uint8_t>());
-  solve_launched(ctx);
-  // the shuffle: per row its side, then the in-row and the out-row flags (for the row lists)
-  DevBuf sideb(sh ? 3 * n : 0), outc(sh ? m * 4 : 0), shf(sh ? 2 * m : 0);
-  if (sh) {
-    std::vector<uint8_t> fl(2 * n);
-    for (uint64_t i = 0; i < n; i++) {
-      fl[i] = side[i] == PB_SOLVE_IN;
-      fl[n + i] = side[i] == PB_SOLVE_OUT;
-    }
-    PB_CUDA(cudaMemcpyAsync(sideb.p, side.data(), n, cudaMemcpyHostToDevice, st));
-    PB_CUDA(cudaMemcpyAsync(sideb.as<uint8_t>() + n, fl.data(), 2 * n, cudaMemcpyHostToDevice, st));
-    k_solve_unqualify_out<<<PB_SOLVE_GRID(n, 256), 0, st>>>(sideb.as<uint8_t>(), n_constraints, qual.as<uint8_t>());
-    solve_launched(ctx);
-  }
-  PB_CUDA(cudaMemsetAsync(defr.p, 0xff, m * 4, st));
-  PB_CUDA(cudaMemsetAsync(inp.p, 0xff, m * 4, st));  // variables past the last run: no source
-  k_solve_vars<<<PB_SOLVE_GRID(m, 256), 0, st>>>(sorted, run.as<uint32_t>(), m, cb, inids.as<uint64_t>(), n_inputs,
-                                                qual.as<uint8_t>(), voc.as<uint32_t>(), inp.as<uint32_t>(),
-                                                defr.as<uint32_t>());
-  solve_launched(ctx);
-  if (sh) {  // out-row variables: defined at row p
-    PB_CUDA(cudaMemsetAsync(outc.p, 0, m * 4, st));
-    k_solve_claim_out<<<PB_SOLVE_GRID(m, 256), 0, st>>>(sideb.as<uint8_t>(), voc.as<uint32_t>(), inp.as<uint32_t>(), n,
-                                                       p, outc.as<uint32_t>(), defr.as<uint32_t>());
-    solve_launched(ctx);
-  }
-  uint8_t* f_unset = flags.as<uint8_t>();
-  uint8_t* f_order = f_unset + m;
-  k_solve_flags<<<PB_SOLVE_GRID(m, 256), 0, st>>>(voc.as<uint32_t>(), inp.as<uint32_t>(), defr.as<uint32_t>(), n,
-                                                 f_unset, f_order, defines.as<uint8_t>());
-  solve_launched(ctx);
-  if (sh) {  // row p defines nothing, though its O variable is defined at p: its flag and its operands' order flags off
-    PB_CUDA(cudaMemsetAsync(defines.as<uint8_t>() + p, 0, 1, st));
-    PB_CUDA(cudaMemsetAsync(f_order + 3 * (uint64_t)p, 0, 2, st));
-  }
-  for (uint64_t k = 0; k < (lookup ? 5 : shuffle ? 8 : 3) * (uint64_t)limit; k++) h_lists[k] = 0xffffffffu;
-  uint32_t* num = small_u + 1;
-  h_counts[0] = solve_compact(ctx, f_unset, m, temp, idx.as<uint32_t>(), num, limit, h_lists);
-  std::vector<uint32_t> cells(limit);
-  h_counts[1] = solve_compact(ctx, f_order, m, temp, idx.as<uint32_t>(), num, limit, cells.data());
-  const uint32_t listed = (uint32_t)std::min<uint64_t>(h_counts[1], limit);
-  if (listed) {  // (cell, the row defining its variable)
-    DevBuf pairs((size_t)listed * 8);
-    PB_CUDA(cudaMemcpyAsync(pairs.p, cells.data(), (size_t)listed * 4, cudaMemcpyHostToDevice, st));
-    k_solve_order_rows<<<PB_SOLVE_GRID(listed, 128), 0, st>>>(pairs.as<uint32_t>(), listed, voc.as<uint32_t>(),
-                                                              defr.as<uint32_t>(), pairs.as<uint32_t>() + listed);
-    solve_launched(ctx);
-    std::vector<uint32_t> rows(listed);
-    PB_CUDA(cudaMemcpyAsync(rows.data(), pairs.as<uint32_t>() + listed, (size_t)listed * 4, cudaMemcpyDeviceToHost,
-                            st));
+    PB_CUDA(cudaMemsetAsync(small.p, 0, 64, st));
+    k_count_noncanonical<<<PB_GRID(n_sel, 256), 0, st>>>(selp, n_sel, small_u + 2);
+    launched(ctx);
+    fr_to_mont(ctx, selp, selp, n_sel);
+    s.ql = sel_col[0];
+    s.qr = sel_col[1];
+    s.qm = sel_col[2];
+    s.qo = sel_col[3];
+    s.qc = sel_col[4];
+    s.inv_qo = selp + n_sel;
+    const uint64_t T = (n + PB_SOLVE_BATCH_CH - 1) / PB_SOLVE_BATCH_CH;
+    k_batch_div<<<PB_GRID(T, 128), 0, st>>>(nullptr, s.qo, selp + n_sel, n, T);
+    launched(ctx);
+    uint32_t bad_sel = 0;
+    PB_CUDA(cudaMemcpyAsync(&bad_sel, small_u + 2, 4, cudaMemcpyDeviceToHost, st));
     PB_CUDA(cudaStreamSynchronize(st));
-    for (uint32_t k = 0; k < listed; k++) {
-      h_lists[limit + 2 * (uint64_t)k] = cells[k];
-      h_lists[limit + 2 * (uint64_t)k + 1] = rows[k];
+    PB_CHECK(bad_sel == 0, "selector value not reduced below the field modulus");
+    if (a.n_inputs) {
+      PB_CUDA(cudaMemcpyAsync(inids.p, in_keys.data(), a.n_inputs * 8, cudaMemcpyHostToDevice, st));
+      PB_CUDA(cudaMemcpyAsync(invals.p, in_vals.data(), a.n_inputs * 32, cudaMemcpyHostToDevice, st));
     }
-  }
-  if (shuffle) h_counts[2] = h_counts[3] = 0;
-  if (sh) {  // late in-row cells and clashing out-row cells
-    uint8_t* f_late = shf.as<uint8_t>();
-    uint8_t* f_clash = f_late + m;
-    k_solve_shuffle_flags<<<PB_SOLVE_GRID(m, 256), 0, st>>>(sideb.as<uint8_t>(), voc.as<uint32_t>(), inp.as<uint32_t>(),
-                                                           defr.as<uint32_t>(), outc.as<uint32_t>(), n, p, f_late,
-                                                           f_clash);
-    solve_launched(ctx);
-    uint32_t* l_late = h_lists + 3 * (uint64_t)limit;
-    uint32_t* l_clash = l_late + 2 * (uint64_t)limit;
-    h_counts[2] = solve_compact(ctx, f_late, m, temp, idx.as<uint32_t>(), num, limit, cells.data());
-    const uint32_t n_late = (uint32_t)std::min<uint64_t>(h_counts[2], limit);
-    std::vector<uint32_t> ccells(limit);
-    h_counts[3] = solve_compact(ctx, f_clash, m, temp, idx.as<uint32_t>(), num, limit, ccells.data());
-    const uint32_t n_clash = (uint32_t)std::min<uint64_t>(h_counts[3], limit);
-    if (n_late + n_clash) {  // (late cell, the row defining its variable), (clash cell, reason, row)
-      DevBuf lst((size_t)(n_late + n_clash) * 4 * 4);
-      uint32_t* d = lst.as<uint32_t>();
-      PB_CUDA(cudaMemcpyAsync(d, cells.data(), (size_t)n_late * 4, cudaMemcpyHostToDevice, st));
-      PB_CUDA(cudaMemcpyAsync(d + n_late, ccells.data(), (size_t)n_clash * 4, cudaMemcpyHostToDevice, st));
-      uint32_t* o = d + n_late + n_clash;
-      if (n_late) {
-        k_solve_order_rows<<<PB_SOLVE_GRID(n_late, 128), 0, st>>>(d, n_late, voc.as<uint32_t>(), defr.as<uint32_t>(), o);
-        solve_launched(ctx);
+    if (tb) {  // q_K (canonical), Q_T and the table columns (Montgomery), the per-row error flags
+      const uint64_t rows = tb->rows;
+      const int width = tb->qtag ? 4 : 3;
+      PB_CUDA(cudaMemcpyAsync(qkb.p, tb->qk, n * 32, cudaMemcpyHostToDevice, st));
+      if (tb->qtag) {
+        PB_CUDA(cudaMemcpyAsync(qtb.p, tb->qtag, n * 32, cudaMemcpyHostToDevice, st));
+        fr_to_mont(ctx, qtb.as<Fr>(), qtb.as<Fr>(), n);
       }
-      if (n_clash) {
-        k_solve_clash_reasons<<<PB_SOLVE_GRID(n_clash, 128), 0, st>>>(d + n_late, n_clash, voc.as<uint32_t>(),
-                                                                       inp.as<uint32_t>(), defr.as<uint32_t>(),
-                                                                       outc.as<uint32_t>(), p, o + n_late);
-        solve_launched(ctx);
+      for (int w = 0; w < width; w++) {
+        lk.T.t[w] = tabb.as<Fr>() + (uint64_t)w * rows;
+        PB_CUDA(cudaMemcpyAsync(tabb.as<Fr>() + (uint64_t)w * rows, tb->tab[w], rows * 32, cudaMemcpyHostToDevice, st));
       }
-      std::vector<uint32_t> got((size_t)n_late + 2 * (size_t)n_clash);
-      PB_CUDA(cudaMemcpyAsync(got.data(), o, got.size() * 4, cudaMemcpyDeviceToHost, st));
-      PB_CUDA(cudaStreamSynchronize(st));
-      for (uint32_t k = 0; k < n_late; k++) {
-        l_late[2 * k] = cells[k];
-        l_late[2 * k + 1] = got[k];
-      }
-      for (uint32_t k = 0; k < n_clash; k++) {
-        l_clash[3 * k] = ccells[k];
-        l_clash[3 * k + 1] = got[n_late + 2 * k];
-        l_clash[3 * k + 2] = got[n_late + 2 * k + 1];
-      }
+      fr_to_mont(ctx, tabb.as<Fr>(), tabb.as<Fr>(), width * rows);
+      PB_CUDA(cudaMemsetAsync(errf.p, 0, 2 * n, st));
+      lk.qual = qual.as<uint8_t>();
+      lk.qt = tb->qtag ? qtb.as<Fr>() : nullptr;
+      lk.miss = errf.as<uint8_t>();
+      lk.amb = lk.miss + n;
     }
-  }
-  if (h_counts[0] || h_counts[1] || (shuffle && (h_counts[2] || h_counts[3]))) {
-    PB_CUDA(cudaStreamSynchronize(st));  // the call's buffers die here
-    return;
+    if (out_rows) {  // per row its side, then the in-row and the out-row flags (for the row lists)
+      std::vector<uint8_t> fl(2 * n);
+      for (uint64_t i = 0; i < n; i++) {
+        fl[i] = side[i] == PB_SOLVE_IN;
+        fl[n + i] = side[i] == PB_SOLVE_OUT;
+      }
+      PB_CUDA(cudaMemcpyAsync(sideb.p, side.data(), n, cudaMemcpyHostToDevice, st));
+      PB_CUDA(cudaMemcpyAsync(sideb.as<uint8_t>() + n, fl.data(), 2 * n, cudaMemcpyHostToDevice, st));
+    }
+
+    // 1. group
+    const int cb = perm_cell_bits(a.log_n);
+    const uint64_t* sorted = perm_sort_keys(ctx, a.ids, m, cb, perm_sort_bits(a.log_n, max_id), keys, alt, temp,
+                                            temp_bytes, 3 * a.n_constraints);
+    k_solve_heads<<<PB_GRID(m, 256), 0, st>>>(sorted, m, cb, head.as<uint32_t>());
+    launched(ctx);
+    size_t tb_bytes = temp.bytes;
+    PB_CUDA(cub::DeviceScan::InclusiveSum(temp.p, tb_bytes, head.as<uint32_t>(), run.as<uint32_t>(), (int)m, st));
+    ctx->launches++;
+    // 2. sources
+    k_solve_qualify<<<PB_GRID(n, 256), 0, st>>>(s, tb ? qkb.as<Fr>() : nullptr,
+                                                out_rows ? sideb.as<uint8_t>() : nullptr, a.n_constraints,
+                                                qual.as<uint8_t>());
+    launched(ctx);
+    PB_CUDA(cudaMemsetAsync(defr.p, 0xff, m * 4, st));
+    PB_CUDA(cudaMemsetAsync(inp.p, 0xff, m * 4, st));  // variables past the last run: no source
+    k_solve_vars<<<PB_GRID(m, 256), 0, st>>>(sorted, run.as<uint32_t>(), m, cb, inids.as<uint64_t>(), a.n_inputs,
+                                             qual.as<uint8_t>(), voc.as<uint32_t>(), inp.as<uint32_t>(),
+                                             defr.as<uint32_t>());
+    launched(ctx);
+    if (out_rows) {  // out-row variables: defined at row p
+      PB_CUDA(cudaMemsetAsync(outc.p, 0, m * 4, st));
+      k_solve_claim_out<<<PB_GRID(m, 256), 0, st>>>(sideb.as<uint8_t>(), voc.as<uint32_t>(), inp.as<uint32_t>(), n, p,
+                                                    outc.as<uint32_t>(), defr.as<uint32_t>());
+      launched(ctx);
+    }
+    k_solve_flags<<<PB_GRID(m, 256), 0, st>>>(voc.as<uint32_t>(), inp.as<uint32_t>(), defr.as<uint32_t>(), n,
+                                              flags.as<uint8_t>(), flags.as<uint8_t>() + m, defines.as<uint8_t>());
+    launched(ctx);
+    if (out_rows) {  // row p defines nothing, though its O variable is defined at p: its flag and its operands' order
+                     // flags off
+      PB_CUDA(cudaMemsetAsync(defines.as<uint8_t>() + p, 0, 1, st));
+      PB_CUDA(cudaMemsetAsync(flags.as<uint8_t>() + m + 3 * (uint64_t)p, 0, 2, st));
+    }
   }
 
-  // 3.-4. the defining rows in row order, evaluated
-  k_solve_init<<<PB_SOLVE_GRID(m, 256), 0, st>>>(inp.as<uint32_t>(), invals.as<Fr>(), m, val.as<Fr>(),
-                                                ready.as<uint32_t>());
-  solve_launched(ctx);
-  DevBuf ix_word(lookup ? tab_rows * 8 : 0), ix_row(lookup ? tab_rows * 4 : 0), ix_amb(lookup ? tab_rows : 0);
-  if (lookup) {
-    lk.T.word = ix_word.as<uint64_t>();
-    lk.T.row = ix_row.as<uint32_t>();
-    lk.T.amb = ix_amb.as<uint8_t>();
-    solve_table_index(ctx, lk.T, tab_rows, temp, small_u + 6);
+  // the cells flagged in f (m of them): their count, and at out the lowest `limit` of them, each followed by `extra`
+  // entries that fill(d_cells, listed, d_entries) computes on the device
+  template <class Fill>
+  uint64_t list_cells(const uint8_t* f, uint32_t* out, int extra, Fill fill) {
+    std::vector<uint32_t> cells(a.limit);
+    const uint64_t count = compact_flagged(ctx, f, m, temp, idx.as<uint32_t>(), num, a.limit, cells.data());
+    const uint32_t listed = (uint32_t)std::min<uint64_t>(count, a.limit);
+    if (listed) {
+      DevBuf d((size_t)listed * (1 + extra) * 4);
+      PB_CUDA(cudaMemcpyAsync(d.p, cells.data(), (size_t)listed * 4, cudaMemcpyHostToDevice, st));
+      fill(d.as<uint32_t>(), listed, d.as<uint32_t>() + listed);
+      launched(ctx);
+      std::vector<uint32_t> got((size_t)listed * extra);
+      PB_CUDA(cudaMemcpyAsync(got.data(), d.as<uint32_t>() + listed, got.size() * 4, cudaMemcpyDeviceToHost, st));
+      PB_CUDA(cudaStreamSynchronize(st));
+      for (uint32_t k = 0; k < listed; k++) {
+        out[(1 + extra) * (uint64_t)k] = cells[k];
+        for (int j = 0; j < extra; j++) out[(1 + extra) * (uint64_t)k + 1 + j] = got[(uint64_t)extra * k + j];
+      }
+    }
+    return count;
   }
-  // with a shuffle, phase 1 is the defining rows below p (the list's prefix idx[0, k)), phase 2 the rest
-  const uint64_t k_below = sh ? solve_compact(ctx, defines.as<uint8_t>(), p, temp, idx.as<uint32_t>(), num, 0, nullptr) : 0;
-  const uint64_t n_def = solve_compact(ctx, defines.as<uint8_t>(), n, temp, idx.as<uint32_t>(), num, 0, nullptr);
-  auto evaluate = [&](const uint32_t* rows, uint64_t count) {
+  // the cells flagged in f, each with the row defining its variable
+  uint64_t list_with_rows(const uint8_t* f, uint32_t* out) {
+    return list_cells(f, out, 1, [&](const uint32_t* cells, uint32_t count, uint32_t* rows) {
+      k_solve_order_rows<<<PB_GRID(count, 128), 0, st>>>(cells, count, voc.as<uint32_t>(), defr.as<uint32_t>(), rows);
+    });
+  }
+
+  // the errors found before any row is evaluated: unset and order, and with out-rows late and clash; true with any
+  bool errors() {
+    const uint64_t limit = a.limit;
+    uint64_t* counts = a.counts;
+    for (uint64_t k = 0; k < (tb ? 5 : sf ? 8 : 3) * limit; k++) a.lists[k] = 0xffffffffu;
+    counts[0] = compact_flagged(ctx, flags.as<uint8_t>(), m, temp, idx.as<uint32_t>(), num, a.limit, a.lists);
+    counts[1] = list_with_rows(flags.as<uint8_t>() + m, a.lists + limit);
+    if (tb || sf) counts[2] = counts[3] = 0;
+    if (out_rows) {  // late in-row cells (with their defining row), clashing out-row cells (with reason and row)
+      uint8_t* f_late = shf.as<uint8_t>();
+      uint8_t* f_clash = f_late + m;
+      k_solve_shuffle_flags<<<PB_GRID(m, 256), 0, st>>>(sideb.as<uint8_t>(), voc.as<uint32_t>(), inp.as<uint32_t>(),
+                                                        defr.as<uint32_t>(), outc.as<uint32_t>(), n, p, f_late,
+                                                        f_clash);
+      launched(ctx);
+      counts[2] = list_with_rows(f_late, a.lists + 3 * limit);
+      counts[3] = list_cells(f_clash, a.lists + 5 * limit, 2, [&](const uint32_t* cells, uint32_t count, uint32_t* o) {
+        k_solve_clash_reasons<<<PB_GRID(count, 128), 0, st>>>(cells, count, voc.as<uint32_t>(), inp.as<uint32_t>(),
+                                                              defr.as<uint32_t>(), outc.as<uint32_t>(), p, o);
+      });
+    }
+    return counts[0] || counts[1] || (sf && (counts[2] || counts[3]));
+  }
+
+  // the rows[0, count) through k_solve_eval, as many warps as fit on the device
+  void evaluate(const uint32_t* rows, uint64_t count) {
     if (!count) return;
+    const auto kernel = tb ? k_solve_eval<true> : k_solve_eval<false>;
     int per_sm = 0;
-    if (lookup) PB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_solve_eval_lookup, 128, 0));
-    else PB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_solve_eval, 128, 0));
+    PB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, 128, 0));
     const uint64_t warps = (count + 31) / 32;
     const uint64_t blocks = std::min<uint64_t>((uint64_t)std::max(per_sm, 1) * ctx->sm_count, (warps + 3) / 4);
     PB_CUDA(cudaMemsetAsync(small_u + 4, 0, 4, st));  // the ticket
-    if (lookup)
-      k_solve_eval_lookup<<<(unsigned)blocks, 128, 0, st>>>(s, lk, rows, count, voc.as<uint32_t>(), val.as<Fr>(),
-                                                            ready.as<uint32_t>(), small_u + 4);
-    else
-      k_solve_eval<<<(unsigned)blocks, 128, 0, st>>>(s, rows, count, voc.as<uint32_t>(), val.as<Fr>(),
-                                                     ready.as<uint32_t>(), small_u + 4);
-    solve_launched(ctx);
+    kernel<<<(unsigned)blocks, 128, 0, st>>>(s, rows, count, voc.as<uint32_t>(), val.as<Fr>(), ready.as<uint32_t>(),
+                                             small_u + 4, lk);
+    launched(ctx);
     uint32_t stalled = 0;
     PB_CUDA(cudaMemcpyAsync(&stalled, small_u + 5, 4, cudaMemcpyDeviceToHost, st));
     PB_CUDA(cudaStreamSynchronize(st));
     PB_CHECK(stalled == 0, "solving the wires stalled: a defining row waited too long for its operands");
-  };
-  if (!sh) {
-    evaluate(idx.as<uint32_t>(), n_def);
-  } else {
+  }
+
+  // 3.-4. the defining rows in row order, evaluated: one phase, or with out-rows the defining rows below p (the
+  // list's prefix idx[0, k_below)), the shuffle step and the rest
+  void evaluate_all() {
+    k_solve_init<<<PB_GRID(m, 256), 0, st>>>(inp.as<uint32_t>(), invals.as<Fr>(), m, val.as<Fr>(),
+                                             ready.as<uint32_t>());
+    launched(ctx);
+    if (tb) {
+      ix_word.alloc(tb->rows * 8);
+      ix_row.alloc(tb->rows * 4);
+      ix_amb.alloc(tb->rows);
+      lk.T.word = ix_word.as<uint64_t>();
+      lk.T.row = ix_row.as<uint32_t>();
+      lk.T.amb = ix_amb.as<uint8_t>();
+      solve_table_index(ctx, lk.T, tb->rows, temp, small_u + 6);
+    }
+    uint32_t* list = idx.as<uint32_t>();
+    const uint8_t* def = defines.as<uint8_t>();
+    const uint64_t k_below = out_rows ? compact_flagged(ctx, def, p, temp, list, num, 0, nullptr) : 0;
+    const uint64_t n_def = compact_flagged(ctx, def, n, temp, list, num, 0, nullptr);
+    if (!out_rows) {
+      evaluate(list, n_def);
+      return;
+    }
     DevBuf rowl(2 * K * 4);  // the in-rows, then the out-rows, ascending
     const uint8_t* fl = sideb.as<uint8_t>() + n;
-    uint64_t got_in = solve_compact(ctx, fl, n, temp, rowl.as<uint32_t>(), num, 0, nullptr);
-    uint64_t got_out = solve_compact(ctx, fl + n, n, temp, rowl.as<uint32_t>() + K, num, 0, nullptr);
+    const uint64_t got_in = compact_flagged(ctx, fl, n, temp, rowl.as<uint32_t>(), num, 0, nullptr);
+    const uint64_t got_out = compact_flagged(ctx, fl + n, n, temp, rowl.as<uint32_t>() + K, num, 0, nullptr);
     PB_CHECK(got_in == K && got_out == K, "solving the wires: the shuffle's row lists disagree with q_in and q_out");
     cudaEvent_t ev[4];
     for (auto& e : ev) PB_CUDA(cudaEventCreate(&e));
     PB_CUDA(cudaEventRecord(ev[0], st));
-    evaluate(idx.as<uint32_t>(), k_below);
+    evaluate(list, k_below);
     PB_CUDA(cudaEventRecord(ev[1], st));
     solve_shuffle(ctx, rowl.as<uint32_t>(), rowl.as<uint32_t>() + K, K, voc.as<uint32_t>(), val.as<Fr>(),
                   ready.as<uint32_t>(), temp, reinterpret_cast<unsigned long long*>(small_u + 8));
     PB_CUDA(cudaEventRecord(ev[2], st));
-    evaluate(idx.as<uint32_t>() + k_below, n_def - k_below);
+    evaluate(list + k_below, n_def - k_below);
     PB_CUDA(cudaEventRecord(ev[3], st));
     PB_CUDA(cudaEventSynchronize(ev[3]));
     for (int k = 0; k < 3; k++) {
@@ -1035,41 +906,60 @@ void solve_run(Context* ctx, const int64_t* h_ids, int log_n, uint64_t n_constra
     }
     for (auto& e : ev) PB_CUDA(cudaEventDestroy(e));
   }
-  if (lookup) {  // miss and ambiguous: rows, and the operands a, b of the listed ones
-    uint32_t* l_miss = h_lists + 3 * (uint64_t)limit;
+
+  // with a table, the errors found while evaluating: miss and ambiguous rows, and the operands a, b of the listed
+  // ones; true with any
+  bool table_errors() {
+    if (!tb) return false;
+    const uint64_t limit = a.limit;
+    uint64_t* counts = a.counts;
+    uint32_t* l_miss = a.lists + 3 * limit;
     uint32_t* l_amb = l_miss + limit;
-    h_counts[2] = solve_compact(ctx, lk.miss, n, temp, idx.as<uint32_t>(), num, limit, l_miss);
-    h_counts[3] = solve_compact(ctx, lk.amb, n, temp, idx.as<uint32_t>(), num, limit, l_amb);
-    const uint32_t take[2] = {(uint32_t)std::min<uint64_t>(h_counts[2], limit),
-                              (uint32_t)std::min<uint64_t>(h_counts[3], limit)};
-    if (h_operands && take[0] + take[1]) {
+    counts[2] = compact_flagged(ctx, lk.miss, n, temp, idx.as<uint32_t>(), num, a.limit, l_miss);
+    counts[3] = compact_flagged(ctx, lk.amb, n, temp, idx.as<uint32_t>(), num, a.limit, l_amb);
+    const uint32_t take[2] = {(uint32_t)std::min<uint64_t>(counts[2], limit),
+                              (uint32_t)std::min<uint64_t>(counts[3], limit)};
+    if (tb->operands && take[0] + take[1]) {
       DevBuf lrows((size_t)(take[0] + take[1]) * 4), ops((size_t)(take[0] + take[1]) * 64);
       PB_CUDA(cudaMemcpyAsync(lrows.p, l_miss, (size_t)take[0] * 4, cudaMemcpyHostToDevice, st));
       PB_CUDA(cudaMemcpyAsync(lrows.as<uint32_t>() + take[0], l_amb, (size_t)take[1] * 4, cudaMemcpyHostToDevice, st));
-      k_solve_operands<<<PB_SOLVE_GRID(take[0] + take[1], 128), 0, st>>>(lrows.as<uint32_t>(), take[0] + take[1],
-                                                                          voc.as<uint32_t>(), val.as<Fr>(), ops.as<Fr>());
-      solve_launched(ctx);
-      PB_CUDA(cudaMemcpyAsync(h_operands, ops.p, (size_t)take[0] * 64, cudaMemcpyDeviceToHost, st));
-      PB_CUDA(cudaMemcpyAsync(h_operands + (uint64_t)limit * 64, ops.as<uint8_t>() + (size_t)take[0] * 64,
+      k_solve_operands<<<PB_GRID(take[0] + take[1], 128), 0, st>>>(lrows.as<uint32_t>(), take[0] + take[1],
+                                                                   voc.as<uint32_t>(), val.as<Fr>(), ops.as<Fr>());
+      launched(ctx);
+      PB_CUDA(cudaMemcpyAsync(tb->operands, ops.p, (size_t)take[0] * 64, cudaMemcpyDeviceToHost, st));
+      PB_CUDA(cudaMemcpyAsync(tb->operands + limit * 64, ops.as<uint8_t>() + (size_t)take[0] * 64,
                               (size_t)take[1] * 64, cudaMemcpyDeviceToHost, st));
       PB_CUDA(cudaStreamSynchronize(st));
     }
-    if (h_counts[2] || h_counts[3]) {
-      PB_CUDA(cudaStreamSynchronize(st));  // the call's buffers die here
-      return;
-    }
+    return counts[2] || counts[3];
   }
-  // 5. write
-  DevBuf staging(out_on_device ? 0 : m * 32);
-  Fr* W[3];
-  for (int k = 0; k < 3; k++)
-    W[k] = out_on_device ? reinterpret_cast<Fr*>(out[k]) : staging.as<Fr>() + (uint64_t)k * n;
-  k_solve_write<<<PB_SOLVE_GRID(m, 256), 0, st>>>(voc.as<uint32_t>(), val.as<Fr>(), n, W[0], W[1], W[2]);
-  solve_launched(ctx);
-  if (!out_on_device)
+
+  // 5. every cell's value into A, B, C
+  void write() {
+    DevBuf staging(a.out_on_device ? 0 : m * 32);
+    Fr* W[3];
     for (int k = 0; k < 3; k++)
-      PB_CUDA(cudaMemcpyAsync(out[k], W[k], n * 32, cudaMemcpyDeviceToHost, st));
-  PB_CUDA(cudaStreamSynchronize(st));
+      W[k] = a.out_on_device ? reinterpret_cast<Fr*>(a.out[k]) : staging.as<Fr>() + (uint64_t)k * n;
+    k_solve_write<<<PB_GRID(m, 256), 0, st>>>(voc.as<uint32_t>(), val.as<Fr>(), n, W[0], W[1], W[2]);
+    launched(ctx);
+    if (!a.out_on_device)
+      for (int k = 0; k < 3; k++) PB_CUDA(cudaMemcpyAsync(a.out[k], W[k], n * 32, cudaMemcpyDeviceToHost, st));
+    PB_CUDA(cudaStreamSynchronize(st));
+  }
+};
+}  // namespace
+
+// see plonk_b200.h: pb200_solve_wires, with `tb` pb200_solve_wires_lookup, with `sf` pb200_solve_wires_shuffle
+void solve_run(Context* ctx, const SolveArgs& a, const SolveTableArgs* tb, const SolveShuffleArgs* sf) {
+  Solve S(ctx, a, tb, sf);
+  S.require();
+  S.reserve();
+  S.sources();
+  if (!S.errors()) {
+    S.evaluate_all();
+    if (!S.table_errors()) S.write();
+  }
+  PB_CUDA(cudaStreamSynchronize(ctx->stream));  // the call's buffers die here
 }
 
 }  // namespace pb200

@@ -12,6 +12,41 @@ namespace pb200 {
 
 #define PB_SOLVE_NONE 0xffffffffu  // no defining row / no input
 
+// ---- the arguments of solve_run (plonk_b200.h has their meaning) -----------------------------------------------------
+// the circuit, its inputs and the outputs, as pb200_solve_wires takes them; lists holds 3, 5 (table) or 8 (shuffle)
+// times limit entries, counts 2 or 4
+struct SolveArgs {
+  const int64_t* ids;
+  int log_n;
+  uint64_t n_constraints;
+  const uint8_t* const* sel;  // QL QR QM QO QC
+  int n_custom;
+  const uint8_t* exps;
+  const uint8_t* const* custom;
+  uint64_t n_inputs;
+  const int64_t* in_ids;
+  const uint8_t* in_vals;
+  uint32_t limit;
+  uint64_t* counts;
+  uint32_t* lists;
+  void* const* out;
+  bool out_on_device;
+};
+// rows that define from their table (pb200_solve_wires_lookup): q_K, Q_T and t4 (both null for one untagged table),
+// t1 t2 t3, the table's rows, and where the listed miss and ambiguous rows' operands go (or null)
+struct SolveTableArgs {
+  const uint8_t* qk;
+  const uint8_t* qtag;
+  const uint8_t* tab[4];
+  uint64_t rows;
+  uint8_t* operands;
+};
+// a shuffle (pb200_solve_wires_shuffle): q_in and q_out
+struct SolveShuffleArgs {
+  const uint8_t* qin;
+  const uint8_t* qout;
+};
+
 // the selectors of one row, Montgomery; neg_inv_qo = -1 / QO
 struct SolveRow {
   Fr ql, qr, qm, qc, neg_inv_qo;

@@ -302,8 +302,6 @@ def solve_wires(wire_L, wire_R, wire_O, pk: dict, inputs, group_order: int, n_co
     sel_arr = (vp * 5)(*[s.ctypes.data for s in sel])
     cust_arr = (vp * max(1, len(cust)))(*[c.ctypes.data for c in cust])
     ebytes = bytes(x for e in exps for x in padded(e)) or b"\0"
-    counts = (ctypes.c_uint64 * 2)()
-    lists = (ctypes.c_uint32 * max(1, 3 * limit))()
     if device:
         import torch
         dev = torch.device("cuda", ctx.device)
@@ -313,46 +311,39 @@ def solve_wires(wire_L, wire_R, wire_O, pk: dict, inputs, group_order: int, n_co
     else:
         out = [np.empty((n, 32), dtype=np.uint8) for _ in range(3)]
         ptrs = [a.ctypes.data for a in out]
+    # the mode's entry point, its own arguments, and the entries per listed location of each error kind
+    col = lambda a: a.ctypes.data_as(vp) if a is not None else None  # noqa: E731
+    extra = ()
     if sh is not None:
-        counts = (ctypes.c_uint64 * 4)()
-        lists = (ctypes.c_uint32 * max(1, 8 * limit))()
-        check(lib().pb200_solve_wires_shuffle(ctx.handle, ids.ctypes.data_as(vp), n.bit_length() - 1, m, sel_arr,
-                                              len(exps), ebytes, cust_arr, len(in_ids), in_ids.ctypes.data_as(vp),
-                                              in_vals.ctypes.data_as(vp), sh[0].ctypes.data_as(vp),
-                                              sh[1].ctypes.data_as(vp), limit, counts, lists, (vp * 3)(*ptrs),
-                                              1 if device else 0))
+        call, args, arity = lib().pb200_solve_wires_shuffle, (col(sh[0]), col(sh[1])), (1, 2, 2, 3)
     elif table is None:
-        check(lib().pb200_solve_wires(ctx.handle, ids.ctypes.data_as(vp), n.bit_length() - 1, m, sel_arr, len(exps),
-                                      ebytes, cust_arr, len(in_ids), in_ids.ctypes.data_as(vp),
-                                      in_vals.ctypes.data_as(vp), limit, counts, lists, (vp * 3)(*ptrs),
-                                      1 if device else 0))
+        call, args, arity = lib().pb200_solve_wires, (), (1, 2)
     else:
         qk, qt, tcols, rows = table
-        qk_a = _le_rows(qk)
-        qt_a = _le_rows(qt) if qt is not None else None
         tab = [_le_rows(c) for c in tcols]  # t1 t2 t3, and t4 with lookups=
-        counts = (ctypes.c_uint64 * 4)()
-        lists = (ctypes.c_uint32 * max(1, 5 * limit))()
+        args = (col(_le_rows(qk)), col(_le_rows(qt) if qt is not None else None), col(tab[0]), col(tab[1]),
+                col(tab[2]), col(tab[3]) if len(tab) > 3 else None, rows)
+        call, arity = lib().pb200_solve_wires_lookup, (1, 2, 1, 1)
         operands = np.zeros((max(1, 4 * limit), 32), np.uint8)
-        col = lambda a: a.ctypes.data_as(vp) if a is not None else None  # noqa: E731
-        check(lib().pb200_solve_wires_lookup(ctx.handle, ids.ctypes.data_as(vp), n.bit_length() - 1, m, sel_arr,
-                                             len(exps), ebytes, cust_arr, len(in_ids), in_ids.ctypes.data_as(vp),
-                                             in_vals.ctypes.data_as(vp), col(qk_a), col(qt_a), col(tab[0]),
-                                             col(tab[1]), col(tab[2]), col(tab[3]) if len(tab) > 3 else None, rows,
-                                             limit, counts, lists, operands.ctypes.data_as(vp), (vp * 3)(*ptrs),
-                                             1 if device else 0))
-    raw = [int(x) for x in lists[:3 * limit]]
-    unset = [x for x in raw[:limit] if x != 0xffffffff]
-    pairs = raw[limit:3 * limit]
-    order = [(pairs[2 * k], pairs[2 * k + 1]) for k in range(limit) if pairs[2 * k] != 0xffffffff]
+        extra = (operands.ctypes.data_as(vp),)
+    counts = (ctypes.c_uint64 * len(arity))()
+    lists = (ctypes.c_uint32 * max(1, sum(arity) * limit))()
+    check(call(ctx.handle, ids.ctypes.data_as(vp), n.bit_length() - 1, m, sel_arr, len(exps), ebytes, cust_arr,
+               len(in_ids), in_ids.ctypes.data_as(vp), in_vals.ctypes.data_as(vp), *args, limit, counts, lists, *extra,
+               (vp * 3)(*ptrs), 1 if device else 0))
+    # each kind's `limit` slots of `a` entries, a used slot's first entry not 0xffffffff
+    raw = [int(x) for x in lists[:sum(arity) * limit]]
+    listed, at = [], 0
+    for a in arity:
+        slots = [tuple(raw[at + a * k:at + a * k + a]) for k in range(limit)]
+        listed.append([e[0] if a == 1 else e for e in slots if e[0] != 0xffffffff])
+        at += a * limit
     ok = not any(counts)
     A, B, C = out if ok else (None, None, None)
-    sol = WireSolution(A, B, C, int(counts[0]), int(counts[1]), unset, order, limit, ids.reshape(-1))
+    sol = WireSolution(A, B, C, int(counts[0]), int(counts[1]), listed[0], listed[1], limit, ids.reshape(-1))
     if table is not None:
-        more = [int(x) for x in lists[3 * limit:5 * limit]]
         sol.miss, sol.ambiguous = int(counts[2]), int(counts[3])
-        sol.miss_rows = [x for x in more[:limit] if x != 0xffffffff]
-        sol.ambiguous_rows = [x for x in more[limit:] if x != 0xffffffff]
+        sol.miss_rows, sol.ambiguous_rows = listed[2], listed[3]
         ops = operands.reshape(-1, 32).tobytes()
         val = lambda k: int.from_bytes(ops[32 * k:32 * k + 32], "little")  # noqa: E731
         sol._operands = {r: (val(2 * k), val(2 * k + 1)) for k, r in enumerate(sol.miss_rows)}
@@ -360,12 +351,9 @@ def solve_wires(wire_L, wire_R, wire_O, pk: dict, inputs, group_order: int, n_co
                               for k, r in enumerate(sol.ambiguous_rows)})
         sol._table = (table[1], table[2])
     if sh is not None:
-        more = [int(x) for x in lists[3 * limit:8 * limit]]
         sol.late, sol.clash = int(counts[2]), int(counts[3])
-        sol.late_cells = [(more[2 * k], more[2 * k + 1]) for k in range(limit) if more[2 * k] != 0xffffffff]
-        trip = more[2 * limit:]
-        listed = [trip[3 * k:3 * k + 3] for k in range(limit) if trip[3 * k] != 0xffffffff]
-        sol.clash_cells = [(c, CLASH_REASONS[why]) for c, why, _ in listed]
-        sol._clash_rows = {c: d for c, _, d in listed}
+        sol.late_cells = listed[2]
+        sol.clash_cells = [(c, CLASH_REASONS[why]) for c, why, _ in listed[3]]
+        sol._clash_rows = {c: d for c, _, d in listed[3]}
         sol._first_out = next((r for r in range(n) if q_out[r] and not q_in[r]), None)
     return sol
